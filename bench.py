@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- the driver's measurement contract for the pairwise-contraction hot path.
+"""bench.py -- measurement of the pairwise-contraction hot path.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]
 
 Workload (BASELINE.json: "pairwise contractions/sec + effective ZGEMM TFLOP/s on random-circuit network"; north star:
 the 36-qubit random-circuit amplitude network): `random_circuit(36 qubits, 10 rounds, p1 = p2 = 0.5, Sycamore coupling,
@@ -26,6 +26,10 @@ through `contract_tensor_network`.
 Extra objects: "roofline" (the dominant kernel crt_gemm_kernel: int8 tensor pipe, timed live with CUDA events on every
 launch inside the timed region), "pair_c2" (BASELINE configs[1], the single 4096^3 pair: engines side by side, host
 pipeline), "cpu_baseline", "clocks", "gpu_launches".
+
+--dump-outputs DIR: after the timed steps, rank 0 writes what the last timed step returned -- the network's amplitude --
+as DIR/amplitude.npy (float64 [re, im]).  The network is built from a fixed seed, so two builds of the project run on the
+same inputs and their dumps compare output for output.
 """
 from __future__ import annotations
 
@@ -46,13 +50,10 @@ METRIC = "pairwise contractions/sec (effective ZGEMM TFLOP/s in zgemm_tflops)"
 NET = {"qubits": 36, "rounds": 10, "p1": 0.5, "p2": 0.5, "seed": 1}
 WORKLOAD = ("36-qubit random-circuit amplitude network (10 rounds, p1=p2=0.5, Sycamore coupling, seed 1; 489 leaves, "
             "488 pairs) through contract_tensor_network")
-# Measured on this pool's B200 with tools/fp64_peak.cu (profiles/r01_fp64_peak_microbench.txt):
-# DMMA m8n8k4 sustained, = 148 SM x 64 FMA/clk x 2 x 1.965 GHz.  tcgen05 has no f64 kind.
-FP64_TENSOR_PEAK_TFLOPS = 37.2
-INT8_NOMINAL_TOPS = 4500.0   # dense int8 tcgen05 (kind::i8), 2 x the nominal bf16 figure
-# Measured on this pool's B200 with tools/i8_peak.cu (profiles/r02_i8_peak.txt): back-to-back UMMA kind::i8 cta_group::2 from
-# resident shared memory, 4533 TOP/s sustained over 274 ms (4592 over 54 ms) -- the int8 tensor pipe at ~1.88 GHz.
-INT8_MEASURED_TOPS = 4533.0
+# Roofline denominators: NVIDIA's data sheet for the H100 SXM (700 W), dense.  Data-sheet figures, not reached rates:
+# tools/fp64_peak.cu and tools/i8_peak.cu measure what a given card sustains.
+FP64_TENSOR_PEAK_TFLOPS = 67.0
+INT8_PEAK_TOPS = 1979.0
 
 
 # ------------------------------------------------------------------------------------------------ inputs
@@ -147,7 +148,7 @@ def pinned_complex(shape, rng):
 
 # ------------------------------------------------------------------------------------------------ helpers
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     FIELDS = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
               "clocks_event_reasons.sw_power_cap")
@@ -212,30 +213,6 @@ def effective_cpus() -> int:
         except Exception:
             pass
     return n
-
-
-def _peak(key, fallback):
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)[key])
-    except Exception:
-        return fallback  # B200_PROFILING.md fallback
-
-
-def _captured_traffic():
-    """DRAM bytes per launch of the dominant kernel on C2 from the committed ncu summary of this round (a capture of the
-    same command, never measured under the timer); None if no r02 capture is committed."""
-    import re
-    for name in ("r02_ncu_crt_gemm_summary.txt",):
-        try:
-            txt = open(os.path.join(ROOT, "profiles", name)).read()
-            rd = re.search(r"^dram__bytes_read\.sum\s+([0-9.]+)\s+(\w+)", txt, re.M)
-            wr = re.search(r"^dram__bytes_write\.sum\s+([0-9.]+)\s+(\w+)", txt, re.M)
-            scale = {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}
-            return float(rd.group(1)) * scale[rd.group(2)] + float(wr.group(1)) * scale[wr.group(2)], name
-        except Exception:
-            continue
-    return None, None
 
 
 def oracle_network_seconds(tn, path, repeats, warm=1):
@@ -335,7 +312,7 @@ def pair_c2(tb, ctx, torch, stream, steps):
     ctx.set_tcgen05_slices(0)
     ms, g = timed(5)
     out["engines"]["dmma_fp64"] = {"ms_per_pair": ms, "gemm_kernel_ms": g, "zgemm_tflops": flops / ms * 1e-9,
-                                   "frac_of_measured_fp64_peak": flops / g * 1e-9 / FP64_TENSOR_PEAK_TFLOPS}
+                                   "frac_of_fp64_peak": flops / g * 1e-9 / FP64_TENSOR_PEAK_TFLOPS}
     ctx.set_tcgen05_slices(8)
     # end to end with host buffers: H2D of both operands, the pair, D2H of the result
     def e2e_step():
@@ -466,8 +443,12 @@ def run_ours(args):
     ms_per_step = total_ms / args.steps
     value = pairs / (ms_per_step * 1e-3)
 
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "amplitude.npy"), np.array([amp.real, amp.imag], dtype=np.float64))
+
     # ---- e2e: the public call from host leaves, device->host read of the amplitude inside -----------------
-    e2e_steps = max(3, min(args.steps, 10))
+    e2e_steps = args.steps
     for _ in range(warmup):       # W >= 3 like the resident form: the library compiles its plan on the SECOND sighting of a structure
         read_amp(step_e2e())
     barrier()
@@ -485,15 +466,14 @@ def run_ours(args):
 
     line = None
     if rank == 0:
-        bf16_meas = _peak("bf16_tflops", 1590.0)
         line = {
             "metric": METRIC, "value": value, "unit": "contractions/s", "n_gpus": world, "steps": args.steps, "warmup": warmup,
             "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
-            "dtype": "f64", "dtype_note": "complex128 in, complex128 out; GEMM-like pairs run as 16-17 exact int8 modular GEMMs on tcgen05 + CRT "
+            "dtype": "f64", "dtype_note": "complex128 in, complex128 out; GEMM-like pairs run as 16-17 exact int8 modular GEMMs on the tensor cores (wgmma) + CRT "
                                           "(guaranteed normwise bound 2^-49 K max|b| max|a|, measured 1e-15: FP64-GEMM-equivalent), all other pairs in FP64",
             "data": "synthetic", "zgemm_tflops": flops / (ms_per_step * 1e-3) * 1e-12,
             "config": {"workload": WORKLOAD, "path": mode, "pairs": pairs, "flops_8mnk": flops,
-                       "l2": "every step re-reads its operands from HBM: the dominant pairs move 0.3-6 GB each (> 126 MB L2)",
+                       "l2": "every step re-reads its operands from HBM: the dominant pairs move 0.3-6 GB each (> 50 MB L2)",
                        "engines_per_step": {k: v // max(1, args.steps) for k, v in ec.items() if v}},
             "clocks": clocks,
             "e2e": {"value": e2e_val, "unit": "contractions/s", "h2d_bytes_per_step": leaf_bytes(net), "d2h_bytes_per_step": 16,
@@ -506,26 +486,21 @@ def run_ours(args):
             line["config"]["partitioning"] = facts
         if gt["launches"]:
             ach = gt["int8_ops"] / (gt["ms"] * 1e-3) * 1e-12
-            traffic, tfile = _captured_traffic()
             line["roofline"] = {
-                "bound": "tensor", "kernel": "crt_gemm_kernel (tcgen05.mma.cta_group::2.kind::i8, TMA, TMEM; one int8 GEMM per modulus)",
-                "achieved": ach, "peak": INT8_MEASURED_TOPS, "unit": "int8 TOP/s", "frac": ach / INT8_MEASURED_TOPS,
-                "peak_source": "int8 tensor-pipe peak measured on this pool with tools/i8_peak.cu (profiles/r02_i8_peak.txt, sustained); MEASURED_PEAKS.json "
-                               f"has no int8 entry: against its bf16 burst x 2 = {2.0 * bf16_meas:.0f} the fraction is {ach / (2.0 * bf16_meas):.3f}, against nominal 4500 "
-                               f"{ach / INT8_NOMINAL_TOPS:.3f}; ncu on the C2 launch: 96 % of the per-cycle pipe peak at a power-capped 1.50 GHz (profiles/r02_ncu_crt_gemm_summary.txt)",
+                "bound": "tensor", "kernel": "crt_gemm_kernel (wgmma.m64n256k32.s32.s8.s8, TMA; one int8 GEMM per modulus)",
+                "achieved": ach, "peak": INT8_PEAK_TOPS, "unit": "int8 TOP/s", "frac": ach / INT8_PEAK_TOPS,
+                "peak_source": "H100 SXM data sheet, dense int8 at 700 W (tools/i8_peak.cu measures the sustained rate of a card)",
                 "how": f"CUDA events around every one of the {gt['launches']} launches of the kernel inside the timed region (sum of durations "
-                       f"{gt['ms']:.3f} ms = {gt['ms'] / total_ms:.2f} of it); executed int8 ops = 2 x (4, or 3 from K >= 4096) x moduli x Np x Mp x Kp (padded tiles)",
+                       f"{gt['ms']:.3f} ms = {gt['ms'] / total_ms:.2f} of it); executed int8 ops = 2 x (4, or 3 from K >= 2048) x moduli x Np x Mp x Kp (padded tiles)",
                 "kernel_ms_per_step": gt["ms"] / args.steps, "launches_per_step": gt["launches"] / args.steps,
                 "executed_int8_ops_per_step": gt["int8_ops"] / args.steps,
-                "traffic": traffic, "traffic_note": (f"dram read+write of ONE launch on the C2 pair from profiles/{tfile} (ncu --set full of this kernel; not a "
-                                                     "measurement of the timed run)") if traffic else "no ncu capture committed yet",
                 "algorithmic_flops_per_step": flops,
             }
     # ---- extra objects (never fatal) ------------------------------------------------------------------------
     extras = {}
     try:
         if world == 1 and not args.no_pair:
-            extras["pair_c2"] = pair_c2(tb, ctx, torch, stream, 10)
+            extras["pair_c2"] = pair_c2(tb, ctx, torch, stream, args.steps)
         if world == 1 and not args.no_extras:
             # the same network on the FP64 pipe only, and with a better tree (random-greedy, 64 trials)
             ctx.set_tcgen05_slices(0)
@@ -586,8 +561,8 @@ def run_ours(args):
 
 
 CONFIG5_PATH = os.path.join("bench_inputs", "sycamore53_d12.json")
-# amplitude <0^53| C |0^53> of the Sycamore-53 depth-12 circuit (seed 1), measured with two independent paths / slicings on
-# a B200 (profiles/r02_config5_sycamore53_d12.jsonl: they agree to 2e-15); regression reference of the config5 object
+# amplitude <0^53| C |0^53> of the Sycamore-53 depth-12 circuit (seed 1), computed with two independent paths / slicings
+# (they agree to 2e-15); regression reference of the config5 object
 CONFIG5_AMPLITUDE = complex(-6.148484459425177e-09, -5.130555022162778e-09)
 
 
@@ -635,8 +610,7 @@ def config5_sycamore(tb, ctx, dist, rank, world, max_over_ranks, all_ranks_ok, s
             "seconds": sec, "seconds_all": [round(t, 4) for t in ts], "setup_seconds_untimed": setup,
             "contractions_per_s": pairs5 / sec, "zgemm_tflops": flops_slice * n_slices / sec * 1e-12,
             "amplitude": [amp5.real, amp5.imag], "rel_diff_vs_committed_amplitude": abs(amp5 - CONFIG5_AMPLITUDE) / abs(CONFIG5_AMPLITUDE),
-            "cpu_baseline": "oracle port, 1 of 64 slices of the same path: 87.3 s on 16 cores -> 5586 s extrapolated (tools/bench_sliced.py --cpu-slices 1, "
-                            "profiles/r02_config5_sycamore53_d12.jsonl)"}
+            "cpu_baseline": "not measured here: tools/bench_sliced.py --cpu-slices 1 times one slice of the same path on the CPU oracle"}
 
 
 def parity_and_modes(tb, ctx, dist, torch, stream, tn, fpath, net, path, amp_fanin, rank, world, local, meta_group, max_over_ranks, all_ranks_ok):
@@ -693,7 +667,9 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-pair", action="store_true", help="skip the pair_c2 object")
     ap.add_argument("--no-extras", action="store_true", help="skip the extra objects")
-    ap.add_argument("--no-config5", action="store_true", help="skip the Sycamore-53 depth-12 object (about 30 s at N = 1)")
+    ap.add_argument("--no-config5", action="store_true", help="skip the Sycamore-53 depth-12 object")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's result (the amplitude) as DIR/amplitude.npy, float64 [re, im]")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

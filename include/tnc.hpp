@@ -42,7 +42,7 @@ class Context {
   Context(const Context&) = delete;
   Context& operator=(const Context&) = delete;
   tncb_ctx* get() const { return h_; }
-  // requested normwise tolerance of the tcgen05 engine (0 = full FP64 mantissa), see tncb_ctx_set_tolerance
+  // requested normwise tolerance of the int8 engine (0 = full FP64 mantissa), see tncb_ctx_set_tolerance
   void set_tolerance(double rel) { check(tncb_ctx_set_tolerance(h_, rel)); }
   void synchronize() { check(tncb_ctx_synchronize(h_)); }
  private:

@@ -1,5 +1,5 @@
 /*
- * tncb.h -- C ABI of libtncb200: the B200-native pairwise tensor-contraction hot
+ * tncb.h -- C ABI of libtncb200: the H100-native pairwise tensor-contraction hot
  * path of qc-tum/TNC (tnc v1.0.0 @ 5dd62b3).
  *
  * This is the drop-in boundary.  TNC reaches its numeric kernel through plain
@@ -70,15 +70,15 @@ void* tncb_ctx_stream(tncb_ctx* ctx);
 /* Counters since creation / last reset: kernels launched by this library, arena peak. */
 /* Give device memory back to the driver: synchronises, then cudaFree's every arena slab that holds no live block (the
  * arena otherwise keeps what it reserved for reuse).  For processes that switch between workloads of very different
- * footprints (e.g. a flat network, then a sliced one with a 64 GiB workspace).  The internal plan cache of
+ * footprints (e.g. a flat network, then a sliced one with a tens-of-GiB workspace).  The internal plan cache of
  * tncb_contract_tensor_network is dropped as well; plans created with tncb_plan_create keep their workspaces until they
  * are destroyed. */
 int tncb_ctx_trim(tncb_ctx* ctx, uint64_t* freed_bytes, uint64_t* reserved_bytes);
 int tncb_ctx_stats(tncb_ctx* ctx, uint64_t* kernel_launches, uint64_t* arena_peak_bytes,
                    uint64_t* arena_live_bytes);
 int tncb_ctx_reset_stats(tncb_ctx* ctx);
-/* Dense-GEMM engine for large GEMM-like pairs (M, N >= 128, K >= 256, M*N*K >= 2^28): K1', the tcgen05 int8
- * tensor pipe (tcgen05.mma has no f64 kind).  Default engine = integer modular (CRT) emulation: every operand row
+/* Dense-GEMM engine for large GEMM-like pairs (M, N >= 128, K >= 256, M*N*K >= 2^28): K1', the int8
+ * tensor cores (wgmma has no f64 kind; the API keeps its historical tcgen05 names).  Default engine = integer modular (CRT) emulation: every operand row
  * is scaled by a power of two and truncated to an `a`-bit integer (a = 53 by default = the whole mantissa of the
  * row's largest element), one int8 GEMM per coprime modulus (16 moduli for a = 53, K <= 2^13), exact CRT
  * reconstruction.  GUARANTEED bound (not "exact"):
@@ -104,8 +104,8 @@ int tncb_ctx_set_tcgen05_moduli(tncb_ctx* ctx, int n_moduli);
 /* Real int8 GEMMs per modulus behind one complex product: 4 (re = ArBr - AiBi, im = ArBi + AiBr) or 3 (Karatsuba:
  * k1 = ArBr, k2 = AiBi, k3 = (Ar+Ai)(Br+Bi); re = k1 - k2, im = k3 - k1 - k2 -- the operand sums are taken on the residues,
  * i.e. exactly, so both forms reconstruct the same integers and differ only in the last rounding of the reconstruction).
- * 25 % fewer int8 operations for one more operand plane per side and one more residue plane, which pays from K ~ 4096
- * (profiles/r02_engine_sweep.jsonl): 0 (default) = 3 when K >= min_k3 (default 4096), else 4; min_k3 <= 0 keeps the
+ * 25 % fewer int8 operations for one more operand plane per side and one more residue plane, which pays for long K.
+ * 0 (default) = 3 when K >= min_k3 (default 2048), else 4; min_k3 <= 0 keeps the
  * current threshold. */
 int tncb_ctx_set_tcgen05_products(tncb_ctx* ctx, int products, long long min_k3);
 /* What K1' would do for contraction length k (no GPU): modulus count, operand bits and the guaranteed factor
@@ -120,7 +120,7 @@ int tncb_ctx_set_tcgen05_workspace(tncb_ctx* ctx, size_t bytes);
  * and min_tiles == 1 drops the M*N*K >= 2^28 requirement (used by the parity tests). */
 int tncb_ctx_set_tcgen05_threshold(tncb_ctx* ctx, long long min_tiles, long long min_k);
 /* Pairs executed per engine since the last tncb_ctx_reset_stats: [0] K0, [1] K0 split-K, [2] K1 (DMMA),
- * [3] K1 split-K, [4] K1' (tcgen05), [5] K2, [6] permute, [7] reserved. */
+ * [3] K1 split-K, [4] K1' (int8 tensor cores), [5] K2, [6] permute, [7] reserved. */
 int tncb_ctx_engine_counts(tncb_ctx* ctx, uint64_t counts[8]);
 /* int8 operations (2 x MAC) executed by the GEMM kernels of the last K1' pair and its modulus count. */
 int tncb_ctx_last_tcgen05_info(tncb_ctx* ctx, double* int8_ops, int* n_moduli);
@@ -130,7 +130,7 @@ int tncb_ctx_last_tcgen05_products(tncb_ctx* ctx, int* products);
  * with CUDA events on the ctx stream; tncb_ctx_last_gemm_ms synchronises and returns the last one. */
 int tncb_ctx_time_gemm(tncb_ctx* ctx, int enable);
 int tncb_ctx_last_gemm_ms(tncb_ctx* ctx, float* ms);
-/* enable = 2: every launch of the tcgen05 GEMM kernel is bracketed; tncb_ctx_gemm_totals synchronises, returns the
+/* enable = 2: every launch of the int8 GEMM kernel is bracketed; tncb_ctx_gemm_totals synchronises, returns the
  * summed device time, the executed int8 operations (2 x MAC, padded tiles) and the launch count, and resets. */
 int tncb_ctx_gemm_totals(tncb_ctx* ctx, double* ms, double* int8_ops, uint64_t* launches);
 
@@ -183,7 +183,7 @@ int tncb_pair_out_legs(int n_a, const uint64_t* a_legs, const uint64_t* a_dims,
                        int* n_out, uint64_t* out_legs, uint64_t* out_dims,
                        uint64_t* m, uint64_t* n, uint64_t* k);
 /* Which kernel class the planner would pick for that pair (no GPU):
- * 0 = K0 strided/warp-reduce kernel, 1 = K1 fused gather ZGEMM (DMMA, or tcgen05 K1' above the size
+ * 0 = K0 strided/warp-reduce kernel, 1 = K1 fused gather ZGEMM (DMMA, or the int8 K1' above the size
  * threshold), 2 = K2 streaming kernel (big tensor x tiny tensor, HBM-bound). */
 int tncb_pair_kernel_class(int n_a, const uint64_t* a_legs, const uint64_t* a_dims,
                            int n_b, const uint64_t* b_legs, const uint64_t* b_dims);

@@ -1,5 +1,6 @@
 """bench.py's accounting (no GPU): the pair count, the 8MNK flop total and the host->device bytes it reports for the headline
-network are the values the committed bench lines carry, and the flop total agrees with two independent counters -- the mirror
+network are the values the committed bench line carries (tests/golden/bench_n1.json: one H100 80GB HBM3 at a 400 W power
+limit), and the flop total agrees with two independent counters -- the mirror
 of the reference's cost model (contraction_cost.rs:26-32: (2(K-1) + 6K) M N per pair = 8MNK - 2MN) and the oracle's per-pair
 statistics on a network it can contract in seconds."""
 import json
@@ -18,7 +19,7 @@ def test_headline_network_accounting(built_lib):
     tn = bench.build_network()
     path = bench.greedy_path(tn)
     pairs, flops = bench.count_pairs(path), bench.path_flops(tn, path)
-    line = json.load(open(os.path.join(ROOT, "profiles", "r02_bench_n1.json")))
+    line = json.load(open(os.path.join(ROOT, "tests", "golden", "bench_n1.json")))
     assert pairs == 488 == line["config"]["pairs"] and len(tn.tensors) == 489
     assert flops == line["config"]["flops_8mnk"] == line["roofline"]["algorithmic_flops_per_step"]
     assert bench.leaf_bytes(tn) == line["e2e"]["h2d_bytes_per_step"]

@@ -1,10 +1,10 @@
-"""tnc_b200 -- B200-native pairwise tensor-contraction hot path of qc-tum/TNC.
+"""tnc_b200 -- H100-native pairwise tensor-contraction hot path of qc-tum/TNC.
 
 Host-side mirror (Python, over the C ABI in include/tncb.h) of the reference's interface for
 this path: `tensornetwork.tensor.Tensor`, `tensornetwork.tensordata.TensorData`,
 `contractionpath.ContractionPath`, `tensornetwork.contraction.contract_tensor_network`,
 `builders.circuit_builder.Circuit` / `Permutor`, and `dist.communication` for the
-partitioned fan-in (tnc::mpi::communication).  All numerics run in libtncb200 (CUDA, sm_100a);
+partitioned fan-in (tnc::mpi::communication).  All numerics run in libtncb200 (CUDA, sm_90a);
 nothing here computes on the CPU.
 """
 from __future__ import annotations
@@ -42,7 +42,7 @@ class Context:
         return {"kernel_launches": a.value, "arena_peak_bytes": b.value, "arena_live_bytes": c.value}
 
     def set_tcgen05_slices(self, slices: int) -> None:
-        """0: FP64 tensor pipe (DMMA).  2..8: tcgen05 int8 digit slicing (K1') for large pairs."""
+        """0: FP64 tensor pipe (DMMA) for every pair.  2..8: the int8 tensor-core engine (K1') takes large pairs."""
         check(self._l.tncb_ctx_set_tcgen05_slices(self.handle, int(slices)))
 
     def set_tcgen05_engine(self, engine: int) -> None:
@@ -86,7 +86,7 @@ class Context:
         check(self._l.tncb_ctx_set_tcgen05_threshold(self.handle, int(min_tiles), int(min_k)))
 
     def time_gemm(self, enable=True) -> None:
-        """False/0 off, True/1 last launch of the dominant GEMM kernel, 2 accumulate every tcgen05 GEMM launch."""
+        """False/0 off, True/1 last launch of the dominant GEMM kernel, 2 accumulate every int8 GEMM launch."""
         check(self._l.tncb_ctx_time_gemm(self.handle, int(enable)))
 
     def gemm_totals(self) -> dict:

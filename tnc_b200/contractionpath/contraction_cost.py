@@ -120,15 +120,17 @@ def communication_path_op_costs(inputs: Sequence[Tensor], path, only_count_ops: 
 
 
 # ---- planning-only device time model (NOT in the reference) -------------------------------------------------------
-# The reference scores partitionings by operation counts (contract_op_cost_tensors); on a B200 the pairs that dominate a
+# The reference scores partitionings by operation counts (contract_op_cost_tensors); on a GPU the pairs that dominate a
 # partitioned or sliced contraction are as often bandwidth-bound (tensors of 2^28..2^30 elements meeting tiny ones) as
-# compute-bound, and the fan-in moves them over NVLink.  `gpu_time_tensors` is a two-roof estimate per pair from measured
-# rates of this repo's kernels (profiles/r02_engine_sweep.jsonl, r02_trace_part*.txt, r02_trace_sycamore_d12_slice.txt):
-#   * FP64 kernels (K1 DMMA, K2, K0): 34 TFLOP/s x K/(K+24)  (35 at K = 2^23; 12.5-18.5 at K = 16; gate-sized K stay HBM-bound);
-#   * K1' (int8 engine; M, N >= 128, 256 <= K <= 2^20, MNK >= 2^28): 160 K/(K+600) TFLOP/s-equivalent (48 at K=256, 74 at 512,
-#     124 at 2048, 140 at 4096: the residue / reconstruction passes do not shrink with K) plus the operand conversion,
-#     40 bytes of residue planes per operand element (what makes M = N = 128, K = 2^20 cost 3 ms more than its GEMM);
-#   * ~5 TB/s of HBM traffic, ~5 us per launch.
+# compute-bound, and the fan-in moves them over NVLink.  `gpu_time_tensors` is a two-roof estimate per pair.  Its rates were
+# fitted on the GPU generation this project targeted before the H100 and have NOT been re-measured on the H100; they are
+# planning parameters (the committed paths in bench_inputs/ were ranked with them), and only the ranking of candidate
+# trees depends on them:
+#   * FP64 kernels (K1 DMMA, K2, K0): 34 TFLOP/s x K/(K+24) (short K loses to the per-chunk overheads; gate-sized K stay
+#     HBM-bound);
+#   * K1' (int8 engine; M, N >= 128, 256 <= K <= 2^20, MNK >= 2^28): 160 K/(K+600) TFLOP/s-equivalent (the residue /
+#     reconstruction passes do not shrink with K) plus the operand conversion, 40 bytes of residue planes per operand element;
+#   * 5 TB/s of HBM traffic, 5 us per launch.
 # Used by tools/plan_partitions.py (partitionings) and csrc/reconf.cpp via tools/search_path.py (trees + slices): the C++
 # Objective::pair restates exactly this function and tests/test_tree_reconfiguration.py pins the two against each other.
 GPU_RATES = {"crt_flops": 160e12, "crt_k_half": 600.0, "dmma_flops": 34e12, "hbm_bytes": 5e12, "launch_s": 5e-6,

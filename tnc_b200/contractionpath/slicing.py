@@ -50,7 +50,7 @@ def path_cost(tensors: Sequence[Tuple[Sequence[int], Sequence[int]]], path: Cont
 
 def path_time(tensors: Sequence[Tuple[Sequence[int], Sequence[int]]], path: ContractionPath, sliced: Iterable[int] = ()) -> float:
     """Predicted device seconds of one slice (contraction_cost.gpu_time_tensors per pair): unlike the flop count it
-    sees that halving K of the dominant pair costs the tcgen05 engine efficiency while halving M or N does not."""
+    sees that halving K of the dominant pair costs the int8 engine efficiency while halving M or N does not."""
     from ..tensornetwork.tensor import Tensor as _T
     from .contraction_cost import gpu_time_tensors
     sl = set(sliced)

@@ -1,14 +1,14 @@
-// K1' -- the dense contraction on the 5th-gen tensor cores (tcgen05) through an integer modular
+// K1' -- the dense contraction on the int8 tensor cores (Hopper wgmma) through an integer modular
 // (Chinese-remainder) emulation of the complex128 GEMM.
 //
-// tcgen05.mma has no f64 kind.  The FP64 contraction C[n,m] = sum_k Bt[n,k] * At[m,k] reaches the int8
+// The tensor cores have no f64 wgmma.  The FP64 contraction C[n,m] = sum_k Bt[n,k] * At[m,k] reaches the int8
 // tensor pipe like this (all arithmetic below is exact until the last conversion):
 //   1. every row of the K-major operands is scaled by a power of two and truncated to an integer,
 //        X' = trunc(x * 2^(a - e_row)),   |X'| < 2^a,  a <= 53   (e_row: max(|re|,|im|) of the row < 2^e_row)
 //   2. for N pairwise coprime moduli m_i <= 256 the residues X' mod m_i (symmetric, int8) are written as
 //      K-major planes -- the leg permutation of the reference's TTGT is fused into this pass (gather
 //      through the plan's offset tables);
-//   3. per modulus ONE int8 GEMM on tcgen05.mma.kind::i8 (int32 accumulators in TMEM) gives
+//   3. per modulus ONE int8 GEMM on wgmma.mma_async.s32.s8.s8 (int32 accumulators in registers) gives
 //      C' mod m_i for the exact integer product C' = sum_k B'[n,k] A'[m,k]; the GEMM epilogue reduces the
 //      accumulator mod m_i and stores one int8 per real output;
 //   4. a reconstruction pass evaluates the CRT in split double precision,
@@ -22,16 +22,11 @@
 // published "Ozaki scheme II" (integer modular technique for GEMM emulation); this is an independent
 // implementation for complex operands with the TTGT gather fused in.
 //
-// GEMM kernel (crt_gemm_kernel): persistent CTA pairs (cluster 2x1, tcgen05 cta_group::2), work item =
-// (modulus, K chunk, 256x128 complex tile), items ordered modulus-major with a grouped tile raster so that the
-// ~74 pairs resident at any time share a few operand row bands of ONE modulus in L2.
-//   warp 0  TMA producer (cp.async.bulk.tensor 2D, SWIZZLE_128B, 3 stages x 64 KB)
-//   warp 1  (leader CTA) single-thread tcgen05.mma issuer: 2 UMMAs (M=256 N=256 K=32) per 32-byte K step,
-//           Br x [Ar;Ai]^T and Bi x [-Ai;Ar]^T into one 256-column accumulator (cols 0-127 re, 128-255 im)
-//   warps 2-9 epilogue (two per TMEM lane quarter: real / imaginary columns): tcgen05.ld -> (acc mod m_i) -> byte ->
-//           shared-memory staging -> coalesced global stores; TMEM holds two accumulators, so the epilogue of item j
-//           overlaps the MMAs of item j+1.
+// GEMM kernel (crt_gemm_kernel, main loop in sm90.h): persistent CTAs of three warpgroups, work item = (modulus, K chunk,
+// 128 x 128 complex tile; three products: 128 x 256 of one product), items ordered modulus-major with a grouped tile
+// raster so that the CTAs resident at any time share a few operand row bands of ONE modulus in L2.
 #include "internal.h"
+#include "sm90.h"
 #include <cuda.h>
 #include <algorithm>
 #include <cmath>
@@ -47,17 +42,12 @@ static const int kModuli[CRT_MAX_MOD] = {256, 253, 251, 249, 247, 245, 241, 239,
                                          227, 223, 211, 199, 197, 193, 191, 181, 179, 173};
 constexpr int CRT_BT = 128;        // tile rows per CTA (n) = tile cols (m)
 constexpr int CRT_BKB = 128;       // K bytes per stage row (one 128-byte swizzle row)
-constexpr int CRT_TILE = CRT_BT * CRT_BKB;      // 16 KB
-// shared-memory ring of the GEMM kernel: 192 KB either way
+// stage ring of the GEMM kernel (stage layouts in sm90.h): four products 2 x 80 KB, three products 3 x 48 KB
 template <bool KARA> struct CrtRing {
-  static constexpr int TILES = KARA ? 2 : 4;            // four products: Br, Bi, X (Ar | Ai), Y (-Ai | Ar); three: B_p, A_p
-  static constexpr int STAGE_BYTES = TILES * CRT_TILE;
-  static constexpr int STAGES = KARA ? 6 : 3;
+  static constexpr int STAGES = KARA ? 3 : 2;
 };
-constexpr int CRT_RING_BYTES = 3 * 4 * CRT_TILE;
-constexpr int CRT_THREADS = 320;                // warp 0 TMA, warp 1 MMA, warps 2-9 epilogue (two per TMEM lane quarter)
-constexpr int CRT_STG_ROW = CRT_BT;              // row of the epilogue staging tile (bytes; 16-byte chunks XOR-swizzled by row)
-constexpr int CRT_STG_BYTES = 32 * CRT_STG_ROW;  // per epilogue warp: 32 rows x 128 residue bytes of one component
+constexpr int CRT_STG_ROW = 2 * CRT_BT + 16;     // row of a consumer's epilogue staging tile: 256 residue bytes + 16 of padding
+constexpr int CRT_STG_BYTES = 64 * CRT_STG_ROW;  // per consumer warpgroup: 64 rows
 constexpr int CRT_KCHUNK_MAX = 32768;           // 2 * K * 128 * 128 < 2^31 for K <= 2^15
 constexpr int CRT_G = 34;                       // fixed-point bits of the leading CRT weight
 
@@ -326,76 +316,15 @@ crt_residue_kernel(const double2* __restrict__ src, const long long* __restrict_
   }
 }
 
-// ---- tcgen05 helpers -------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t c_smem(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void c_mbar_init(uint64_t* bar, int count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(c_smem(bar)), "r"(count)); }
-__device__ __forceinline__ void c_mbar_expect_tx(uint64_t* bar, uint32_t bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(c_smem(bar)), "r"(bytes) : "memory"); }
-__device__ __forceinline__ void c_mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred P1;\n\t"
-      "CRT_WAIT:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
-      "@P1 bra CRT_DONE;\n\t"
-      "bra CRT_WAIT;\n\t"
-      "CRT_DONE:\n\t}" ::"r"(c_smem(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void c_cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// K-major SWIZZLE_128B canonical layout (UMMA shared-memory descriptor): LBO = 1, SBO = 1024 B, version 1
-__device__ __forceinline__ uint64_t c_desc(const void* smem) {
-  uint64_t d = 0;
-  d |= (uint64_t)((c_smem(smem) >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// both CTAs' loads signal the LEADER's barrier (peer bit of the shared::cluster address cleared)
-__device__ __forceinline__ void c_tma_2d_2sm(const CUtensorMap* map, uint64_t* bar, void* smem, int c0, int c1) {
-  const uint32_t leader_bar = c_smem(bar) & 0xFEFFFFFFu;
-  asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-               ::"r"(c_smem(smem)), "l"(map), "r"(leader_bar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void c_umma_i8_2sm(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::i8 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void c_commit_2sm(uint64_t* bar) {   // arrives on `bar` in both CTAs of the pair
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(c_smem(bar)), "h"((uint16_t)3) : "memory");
-}
-// arrive on `bar` of cluster CTA `cta`.  Default semantics (release at CTA scope), NOT .release.cluster: the only thing
-// the waiter depends on is that this warp's TMEM reads are done (tcgen05.wait::ld + tcgen05.fence::before_thread_sync);
-// a cluster-scope release compiles to MEMBAR.ALL.GPU + ERRBAR and stalls until every residue byte this warp just stored
-// has reached L2 -- 2-3 thousand cycles per item, which paced all short-K items (ncu: top stall of the kernel).
-__device__ __forceinline__ void c_mbar_arrive_cta(uint64_t* bar, uint32_t cta) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(c_smem(bar)), "r"(cta));
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-__device__ __forceinline__ void c_tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-}
-
+// ---- GEMM kernel -----------------------------------------------------------------------------------
 struct CrtGemmArgs {
   int8_t* R;          // residues + 128 as bytes: [((mod * nkc + kc) * NPL + plane) * Np + n] * Mp + m
                       //   four products: NPL = 2 (re, im);  three products: NPL = 3 (k1, k2, k3; re = k1 + k3, im = k1 + k2)
-  int Np, Mp;         // padded plane rows of this panel (Np % 256 == 0, Mp % tile_m == 0)
-  int pairs_n, tiles_m, tile_m;   // tile_m: 128 (four products: 128 re + 128 im columns) or 256 (three products)
+  int Np, Mp;         // padded plane rows of this panel (Np % 128 == 0, Mp % tile_m == 0)
+  int tiles_n, tiles_m, tile_m;   // tile_m: 128 (four products: 128 re + 128 im columns) or 256 (three products)
   int nmod, nkc, kb_per_chunk, num_kb;
   int total_items;
-  int group;          // n-pairs per raster band
+  int group;          // n-tiles per raster band
   int negmod[CRT_MAX_MOD];   // -m_i (kept as data so that the epilogue's a - q m is ONE multiply-add)
   int magic[CRT_MAX_MOD];
 };
@@ -403,190 +332,118 @@ struct CrtGemmArgs {
 struct CrtItem { int mod_i, prod, kc, n0, m0; };
 template <bool KARA>
 __device__ __forceinline__ CrtItem crt_decode(const CrtGemmArgs& p, int item) {
-  const int tiles = p.pairs_n * p.tiles_m;
+  const int tiles = p.tiles_n * p.tiles_m;
   const int mk = item / tiles, t = item - mk * tiles;
   CrtItem it;
   const int mp = mk / p.nkc;            // (modulus, product) major, K chunk minor
   it.kc = mk - mp * p.nkc;
   it.mod_i = KARA ? mp / 3 : mp; it.prod = KARA ? mp - it.mod_i * 3 : 0;
-  // grouped raster: bands of `group` n-pairs x all m-tiles; concurrently running pairs (consecutive items)
-  // share `group` Bt row bands and ~(#pairs / group) At tiles
+  // grouped raster: bands of `group` n-tiles x all m-tiles; concurrently running CTAs (consecutive items)
+  // share `group` Bt row bands and ~(#CTAs / group) At tiles
   const int per_band = p.group * p.tiles_m;
   const int band = t / per_band, first = band * p.group;
-  const int gsize = min(p.group, p.pairs_n - first);
+  const int gsize = min(p.group, p.tiles_n - first);
   const int r = t - band * per_band;
-  it.n0 = (first + r % gsize) * (2 * CRT_BT);
+  it.n0 = (first + r % gsize) * CRT_BT;
   it.m0 = (r / gsize) * p.tile_m;
   return it;
 }
 
+// Persistent CTAs, work item = (modulus, K chunk, 128 x 128 complex tile), items ordered modulus-major with a grouped tile
+// raster.  Warpgroup 0 streams the operand tiles (TMA), warpgroups 1-2 run the wgmma main loop (sm90.h) on 64 Bt rows each
+// and then their epilogue: accumulator mod m_i -> one offset byte -> shared-memory staging -> coalesced 16-byte stores.
+// The producer runs ahead into the next item while the consumers are in their epilogue.
 template <bool KARA>
-__global__ void __launch_bounds__(CRT_THREADS, 1)
+__global__ void __launch_bounds__(WG_THREADS, 1)
 crt_gemm_kernel(const __grid_constant__ CUtensorMap mapB, const __grid_constant__ CUtensorMap mapA,
                 const __grid_constant__ CrtGemmArgs p) {
-  constexpr int CRT_STAGES = CrtRing<KARA>::STAGES, CRT_STAGE_BYTES = CrtRing<KARA>::STAGE_BYTES;
+  constexpr int STAGES = CrtRing<KARA>::STAGES;
   extern __shared__ __align__(1024) uint8_t crt_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(crt_smem_raw) + 1023) & ~(uintptr_t)1023);
-  __shared__ uint64_t full_bar[CRT_STAGES], empty_bar[CRT_STAGES], tfull_bar[2], tempty_bar[2];
-  __shared__ uint32_t tmem_base_smem;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint32_t crank;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(crank));   // cluster dims (2,1,1)
-  const bool leader = crank == 0;
-  const int cluster_id = blockIdx.x >> 1, n_clusters = gridDim.x >> 1;
+  __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES];
+  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < CRT_STAGES; s++) { c_mbar_init(&full_bar[s], 1); c_mbar_init(&empty_bar[s], 1); }
-    for (int b = 0; b < 2; b++) { c_mbar_init(&tfull_bar[b], 1); c_mbar_init(&tempty_bar[b], 16); }   // 8 epilogue warps x 2 CTAs
+    for (int s = 0; s < STAGES; s++) { wg_mbar_init(&full_bar[s], 1); wg_mbar_init(&empty_bar[s], 2); }   // 2 consumer warpgroups
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {   // both CTAs, same warp id, same smem destination
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(c_smem(&tmem_base_smem)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  c_cluster_sync();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = tmem_base_smem;
 
-  if (warp == 0 && lane == 0) {
-    // ================= TMA producer (both CTAs) =================
+  if (wg == 0) {
+    // ================= TMA producer =================
+    wg_setmaxnreg_producer();
+    if (tid != 0) return;
     int it = 0;
-    for (int item = cluster_id; item < p.total_items; item += n_clusters) {
+    for (int item = blockIdx.x; item < p.total_items; item += gridDim.x) {
       const CrtItem w = crt_decode<KARA>(p, item);
       const int kb0 = w.kc * p.kb_per_chunk, kb1 = min(p.num_kb, kb0 + p.kb_per_chunk);
-      // own 128 of the pair's 256 Bt rows; three products: plane `prod` of both operands, own 128 of the 256 At rows
-      const int rowB = (KARA ? w.mod_i * 3 + w.prod : w.mod_i * 2) * p.Np + w.n0 + (int)crank * CRT_BT;
-      const int rowA = (KARA ? (w.mod_i * 3 + w.prod) * p.Mp + w.m0 + (int)crank * CRT_BT : (w.mod_i * 3) * p.Mp + w.m0);
+      // three products: plane `prod` of both operands (256 At rows); four: Br, Bi and the three At planes (-Ai, Ar, Ai)
+      const int rowB = (KARA ? w.mod_i * 3 + w.prod : w.mod_i * 2) * p.Np + w.n0;
+      const int rowA = (KARA ? w.mod_i * 3 + w.prod : w.mod_i * 3) * p.Mp + w.m0;
       for (int kb = kb0; kb < kb1; kb++, it++) {
-        const int s = it % CRT_STAGES;
-        if (it >= CRT_STAGES) c_mbar_wait(&empty_bar[s], ((it / CRT_STAGES) - 1) & 1);
-        uint8_t* st = smem + s * CRT_STAGE_BYTES;
-        if (leader) c_mbar_expect_tx(&full_bar[s], 2 * CRT_STAGE_BYTES);   // bytes of both CTAs land on the leader's barrier
+        uint8_t* st = wg_produce_begin<STAGES, KARA>(smem, full_bar, empty_bar, it);
+        uint64_t* bar = &full_bar[it % STAGES];
         const int kx = kb * CRT_BKB;
+        uint8_t* a = st + WgStage<KARA>::A;
+        wg_tma_2d(&mapB, bar, st, kx, rowB);
         if (KARA) {
-          c_tma_2d_2sm(&mapB, &full_bar[s], st + 0 * CRT_TILE, kx, rowB);           // B_p
-          c_tma_2d_2sm(&mapA, &full_bar[s], st + 1 * CRT_TILE, kx, rowA);           // A_p (N rows 128 crank ...)
-          continue;
-        }
-        c_tma_2d_2sm(&mapB, &full_bar[s], st + 0 * CRT_TILE, kx, rowB);             // Br
-        c_tma_2d_2sm(&mapB, &full_bar[s], st + 1 * CRT_TILE, kx, rowB + p.Np);      // Bi
-        if (leader) {
-          c_tma_2d_2sm(&mapA, &full_bar[s], st + 2 * CRT_TILE, kx, rowA + p.Mp);    // X: Ar   (N rows   0..127)
-          c_tma_2d_2sm(&mapA, &full_bar[s], st + 3 * CRT_TILE, kx, rowA);           // Y: -Ai
+          wg_tma_2d(&mapA, bar, a, kx, rowA);
+          wg_tma_2d(&mapA, bar, a + WG_TILE, kx, rowA + WG_ROWS);
         } else {
-          c_tma_2d_2sm(&mapA, &full_bar[s], st + 2 * CRT_TILE, kx, rowA + 2 * p.Mp);// X: Ai   (N rows 128..255)
-          c_tma_2d_2sm(&mapA, &full_bar[s], st + 3 * CRT_TILE, kx, rowA + p.Mp);    // Y: Ar
+          wg_tma_2d(&mapB, bar, st + WgStage<KARA>::B1, kx, rowB + p.Np);
+          wg_tma_2d(&mapA, bar, a, kx, rowA);
+          wg_tma_2d(&mapA, bar, a + WG_TILE, kx, rowA + p.Mp);
+          wg_tma_2d(&mapA, bar, a + 2 * WG_TILE, kx, rowA + 2 * p.Mp);
         }
       }
     }
-  } else if (warp == 1 && lane == 0 && leader) {
-    // ================= MMA issuer (leader CTA only) =================
-    // idesc: D = S32 (2)@4, A/B signed int8 (1)@7,@10, both K-major, N = 256 (>>3)@17, M = 256 (>>4)@24
-    const uint32_t idesc = (2u << 4) | (1u << 7) | (1u << 10) | ((256u >> 3) << 17) | ((256u >> 4) << 24);
-    int it = 0, f = 0;
-    for (int item = cluster_id; item < p.total_items; item += n_clusters, f++) {
+  } else {
+    // ================= consumers: wgmma main loop + epilogue (own 64 Bt rows) =================
+    wg_setmaxnreg_consumer();
+    const int c = wg - 1, wq = tid >> 5, lane = tid & 31;
+    WgRing<STAGES, KARA> ring{smem, full_bar, empty_bar};
+    uint8_t* stg = smem + STAGES * WgStage<KARA>::BYTES + c * CRT_STG_BYTES;
+    uint32_t acc[128];
+#pragma unroll
+    for (int i = 0; i < 128; i++) acc[i] = 0u;
+    for (int item = blockIdx.x; item < p.total_items; item += gridDim.x) {
       const CrtItem w = crt_decode<KARA>(p, item);
       const int kb0 = w.kc * p.kb_per_chunk, kb1 = min(p.num_kb, kb0 + p.kb_per_chunk);
-      const int buf = f & 1;
-      if (f >= 2) { c_mbar_wait(&tempty_bar[buf], ((f >> 1) - 1) & 1); asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-      const uint32_t acc = tmem_base + (uint32_t)(buf * 256);
       bool first = true;
-      for (int kb = kb0; kb < kb1; kb++, it++) {
-        const int s = it % CRT_STAGES;
-        c_mbar_wait(&full_bar[s], (it / CRT_STAGES) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint8_t* st = smem + s * CRT_STAGE_BYTES;
-        if (KARA) {
-          const uint64_t d_b = c_desc(st), d_a = c_desc(st + CRT_TILE);
-#pragma unroll
-          for (int k = 0; k < CRT_BKB / 32; k++) {
-            c_umma_i8_2sm(acc, d_b + (uint64_t)(k * 32 >> 4), d_a + (uint64_t)(k * 32 >> 4), idesc, first ? 0u : 1u);   // B_p x A_p (256 At rows)
-            first = false;
-          }
-        } else {
-          const uint64_t d_br = c_desc(st), d_bi = c_desc(st + CRT_TILE), d_x = c_desc(st + 2 * CRT_TILE), d_y = c_desc(st + 3 * CRT_TILE);
-#pragma unroll
-          for (int k = 0; k < CRT_BKB / 32; k++) {
-            const uint64_t ko = (uint64_t)(k * 32 >> 4);
-            c_umma_i8_2sm(acc, d_br + ko, d_x + ko, idesc, first ? 0u : 1u);   // Br x [Ar ; Ai]
-            first = false;
-            c_umma_i8_2sm(acc, d_bi + ko, d_y + ko, idesc, 1u);               // Bi x [-Ai ; Ar]
-          }
-        }
-        c_commit_2sm(&empty_bar[s]);
-      }
-      c_commit_2sm(&tfull_bar[buf]);
-    }
-  } else if (warp >= 2) {
-    // ================= epilogue (both CTAs; own 128 rows): acc mod m_i -> one (offset) byte =================
-    // Eight warps: warp w reads TMEM lanes 32 (w % 4) ..., warps 2-5 take the real columns 0-127, warps 6-9 the imaginary
-    // columns 128-255.  Two warps per scheduler hide each other's dependency stalls and keep all four TMEM read ports busy
-    // (ncu r02 with four warps: issue slots 35 % busy, the epilogue -- not the MMA -- paced every item with K <= 1024).
-    const int q = warp & 3;              // TMEM lane quarter this warp may read
-    const int comp = (warp - 2) >> 2;    // 0: real, 1: imaginary (three products: At rows 0-127 / 128-255 of the tile)
-    int f = 0;
-    for (int item = cluster_id; item < p.total_items; item += n_clusters, f++) {
-      const CrtItem w = crt_decode<KARA>(p, item);
-      const int buf = f & 1;
+      for (int kb = kb0; kb < kb1; kb++) ring.mma_stage(acc, c, first, tid == 0);
+      ring.drain(tid == 0);
       const int negm = p.negmod[w.mod_i], magic = p.magic[w.mod_i];
-      const long long row0 = (long long)w.n0 + (int)crank * CRT_BT + q * 32;     // first of this warp's 32 rows
-      int8_t* dst = KARA ? p.R + ((long long)((w.mod_i * p.nkc + w.kc) * 3 + w.prod) * p.Np + row0) * p.Mp + w.m0 + comp * CRT_BT
-                         : p.R + ((long long)((w.mod_i * p.nkc + w.kc) * 2 + comp) * p.Np + row0) * p.Mp + w.m0;
-      c_mbar_wait(&tfull_bar[buf], (f >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t tbase = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * 256 + comp * CRT_BT);
-      // 32 columns at a time; the TMEM load of chunk c+1 is in flight while chunk c is reduced (tcgen05.wait::ld waits for
-      // every outstanding load of the thread, so it sits before the NEXT issue).  A thread owns a ROW of the accumulator,
-      // so direct stores would scatter 32 x 16 bytes over 32 lines per instruction: the 32 x 128 bytes are parked in a
-      // per-warp shared-memory tile (16-byte chunks XOR-swizzled by row) and written out 4 full 128-byte rows at a time.
-      uint8_t* stg = smem + CRT_STAGES * CRT_STAGE_BYTES + (warp - 2) * CRT_STG_BYTES;
-      uint32_t va[32], vb[32];
-      c_tmem_ld32(tbase, va);
+      wg_bar_sync(1 + c);     // the previous item's copy-out has read the staging tile
 #pragma unroll
-      for (int ch = 0; ch < 4; ch++) {
-        uint32_t (&v)[32] = (ch & 1) == 0 ? va : vb;
-        uint32_t (&nx)[32] = (ch & 1) == 0 ? vb : va;
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (ch < 3) c_tmem_ld32(tbase + (uint32_t)(32 * (ch + 1)), nx);
-        uint32_t wds[8];
+      for (int j = 0; j < 32; j++) {
 #pragma unroll
-        for (int j = 0; j < 32; j++) {
-          const int a = (int)v[j];
-          // q = floor(a * magic / 2^32) in [a/m - 1.25, a/m + 0.25] (|a| < 2^31, |magic / 2^32 - 1/m| <= 2^-33), so
-          // t = a - q m lies in [-0.25 m, 1.25 m] = [-64, 320]: one conditional subtraction of m leaves a representative in
-          // [-128, 127]; its low byte, with the top bit flipped (once per packed word), is the OFFSET byte residue + 128.
-          // (-m is passed in, the condition is a predicate: IMAD.HI + IMAD are the only multiplier-pipe instructions --
-          // ncu r02, K = 512: that pipe was 68 % busy and paced the item, see profiles/r02_ncu_crt_gemm_k512.txt)
-          int t = __mulhi(a, magic) * negm + a;
-          if (t > 127) t += negm;
-          constexpr uint32_t sel[4] = {0x3214u, 0x3240u, 0x3410u, 0x4210u};
-          if ((j & 3) == 0) wds[j >> 2] = 0;
-          wds[j >> 2] = __byte_perm(wds[j >> 2], (uint32_t)t, sel[j & 3]);
+        for (int h = 0; h < 2; h++) {
+          uint32_t b = 0;
+#pragma unroll
+          for (int e = 0; e < 2; e++) {
+            const int a = (int)acc[4 * j + 2 * h + e];
+            // q = floor(a * magic / 2^32) in [a/m - 1.25, a/m + 0.25] (|a| < 2^31, |magic / 2^32 - 1/m| <= 2^-33), so
+            // t = a - q m lies in [-0.25 m, 1.25 m] = [-64, 320]: one conditional subtraction of m leaves a representative in
+            // [-128, 127]; its low byte with the top bit flipped is the OFFSET byte residue + 128.
+            int t = __mulhi(a, magic) * negm + a;
+            if (t > 127) t += negm;
+            b |= ((uint32_t)t & 0xffu) << (8 * e);
+          }
+          const int r = wq * 16 + (lane >> 2) + 8 * h, col = 8 * j + 2 * (lane & 3);
+          *reinterpret_cast<uint16_t*>(stg + r * CRT_STG_ROW + col) = (uint16_t)(b ^ 0x8080u);
         }
-#pragma unroll
-        for (int j = 0; j < 8; j++) wds[j] ^= 0x80808080u;
-        uint8_t* srow = stg + lane * CRT_STG_ROW;
-        *reinterpret_cast<uint4*>(srow + (((2 * ch) ^ (lane & 7)) << 4)) = make_uint4(wds[0], wds[1], wds[2], wds[3]);
-        *reinterpret_cast<uint4*>(srow + (((2 * ch + 1) ^ (lane & 7)) << 4)) = make_uint4(wds[4], wds[5], wds[6], wds[7]);
       }
-      __syncwarp();
+      wg_bar_sync(1 + c);
+      const long long nrow0 = (long long)w.n0 + c * 64;
 #pragma unroll
       for (int i = 0; i < 8; i++) {
-        const int r = i * 4 + (lane >> 3), c16 = lane & 7;
-        *reinterpret_cast<uint4*>(dst + (long long)r * p.Mp + c16 * 16) = *reinterpret_cast<const uint4*>(stg + r * CRT_STG_ROW + ((c16 ^ (r & 7)) << 4));
+        const int q = i * 128 + tid, row = q >> 4, c16 = q & 15;
+        int8_t* dst = KARA ? p.R + ((long long)((w.mod_i * p.nkc + w.kc) * 3 + w.prod) * p.Np + nrow0 + row) * p.Mp + w.m0 + c16 * 16
+                           : p.R + ((long long)((w.mod_i * p.nkc + w.kc) * 2 + (c16 >> 3)) * p.Np + nrow0 + row) * p.Mp + w.m0 + (c16 & 7) * 16;
+        *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(stg + row * CRT_STG_ROW + c16 * 16);
       }
-      __syncwarp();
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) c_mbar_arrive_cta(&tempty_bar[buf], 0);   // the leader's MMA issuer waits for all 8 epilogue warps
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  c_cluster_sync();
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
 }
 
 // ---- CRT reconstruction -------------------------------------------------------------------------------
@@ -691,7 +548,7 @@ crt_reconstruct_kernel(const __grid_constant__ CrtReconArgs a, const __grid_cons
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn crt_get_encode() {
+static EncodeTiledFn get_encode() {
   static EncodeTiledFn fn = nullptr;
   static bool tried = false;
   if (!tried) {
@@ -702,12 +559,12 @@ static EncodeTiledFn crt_get_encode() {
   }
   return fn;
 }
-static int crt_make_map(CUtensorMap* m, void* ptr, uint64_t rows, uint64_t kbytes) {
-  EncodeTiledFn enc = crt_get_encode();
+int wg_make_map(CUtensorMap* m, void* ptr, uint64_t rows, uint64_t kbytes) {
+  EncodeTiledFn enc = get_encode();
   if (!enc) return fail(TNCB_ERR_CUDA, "cuTensorMapEncodeTiled is not available");
   cuuint64_t dims[2] = {kbytes, rows};
   cuuint64_t strides[1] = {kbytes};
-  cuuint32_t box[2] = {(cuuint32_t)CRT_BKB, (cuuint32_t)CRT_BT};
+  cuuint32_t box[2] = {(cuuint32_t)WG_BKB, (cuuint32_t)WG_ROWS};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -729,20 +586,21 @@ int launch_k1_crt(tncb_ctx* ctx, const PairPlan& P, const double2* A, const doub
   cudaStream_t st = ctx->stream;
   const long long Kp = round_up_ll(P.K, CRT_BKB);
   const int num_kb = (int)(Kp / CRT_BKB);
-  const int n_clusters_max = std::max(1, ctx->sm_count / 2);
+  const int ctas_max = std::max(1, ctx->sm_count);
   // three real products per complex product (Karatsuba; sums of residues are exact mod m_i) instead of four: 25 % fewer int8
   // operations for one more operand plane per side and one more residue plane.  An item then carries half the MMA work per
-  // accumulator, so short K (where the epilogue paces the item) keeps the four-product form: measured break-even K ~ 4096.
+  // accumulator, so short K (where the epilogue paces the item) keeps the four-product form.  Measured on an H100
+  // (profiles/h100_engine_sweep.jsonl, 4096 x 4096 x K): three products win by 18 % at K = 2048 and by ~2 % (noise) at K = 1024.
   const bool kara = ctx->crt_products == 3 || (ctx->crt_products == 0 && Kp >= ctx->crt_kara_min_k);
   const int TM = kara ? 2 * CRT_BT : CRT_BT;        // At rows per tile
   const int NPB = kara ? 3 : 2, NPR = kara ? 3 : 2;  // Bt operand planes, residue planes per modulus
   // K chunks: int32-safe length, and more chunks when there are too few tiles to fill the machine (split-K:
   // the reconstruction adds the chunk residues)
-  const long long tiles_total = round_up_ll(P.N, 2 * CRT_BT) / (2 * CRT_BT) * (round_up_ll(P.M, TM) / TM);
+  const long long tiles_total = round_up_ll(P.N, CRT_BT) / CRT_BT * (round_up_ll(P.M, TM) / TM);
   int nkc = (int)((Kp + CRT_KCHUNK_MAX - 1) / CRT_KCHUNK_MAX);
   {
     const long long items = tiles_total * nmod * (kara ? 3 : 1);
-    const long long want = 2LL * n_clusters_max;
+    const long long want = ctas_max;
     if (items * nkc < want) nkc = (int)std::min<long long>((want + items - 1) / items, std::max(1, num_kb / 8));
     nkc = std::max(1, std::min(nkc, 32));      // exactness of the reconstruction: sum of <= 32 chunk residues
   }
@@ -752,13 +610,13 @@ int launch_k1_crt(tncb_ctx* ctx, const PairPlan& P, const double2* A, const doub
 
   // ---- panels: bound the workspace (planes + residues) ----
   const size_t budget = ctx->crt_ws_bytes;
-  long long pn = round_up_ll(P.N, 2 * CRT_BT), pm = round_up_ll(P.M, TM);   // panel extents (padded)
+  long long pn = round_up_ll(P.N, CRT_BT), pm = round_up_ll(P.M, TM);   // panel extents (padded)
   auto ws_bytes = [&](long long n_, long long m_) {
     return (size_t)nmod * (size_t)Kp * (size_t)(NPB * n_ + 3 * m_) + (size_t)nmod * nkc * NPR * (size_t)n_ * (size_t)m_;
   };
-  while (ws_bytes(pn, pm) > budget && (pm > TM || pn > 2 * CRT_BT)) {
+  while (ws_bytes(pn, pm) > budget && (pm > TM || pn > CRT_BT)) {
     if (pm >= pn && pm > TM) pm = round_up_ll(pm / 2, TM);
-    else if (pn > 2 * CRT_BT) pn = round_up_ll(pn / 2, 2 * CRT_BT);
+    else if (pn > CRT_BT) pn = round_up_ll(pn / 2, CRT_BT);
     else pm = round_up_ll(pm / 2, TM);
   }
   const size_t bytesB = (size_t)nmod * NPB * pn * Kp, bytesA = (size_t)nmod * 3 * pm * Kp;
@@ -776,11 +634,12 @@ int launch_k1_crt(tncb_ctx* ctx, const PairPlan& P, const double2* A, const doub
 
   static bool attr_done_dev[64] = {false};          // cudaFuncSetAttribute is per device
   bool& attr_done = attr_done_dev[ctx->device & 63];
-  const int smem_gemm = CRT_RING_BYTES + 8 * CRT_STG_BYTES + 1024;
+  const int smem_gemm4 = CrtRing<false>::STAGES * WgStage<false>::BYTES + 2 * CRT_STG_BYTES + 1024;
+  const int smem_gemm3 = CrtRing<true>::STAGES * WgStage<true>::BYTES + 2 * CRT_STG_BYTES + 1024;
   const int smem_res = RES_ROWS * RES_RS * (int)sizeof(double2);
   if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(crt_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_gemm);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(crt_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_gemm);
+    cudaError_t e = cudaFuncSetAttribute(crt_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_gemm4);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(crt_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_gemm3);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(crt_residue_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_res);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(crt_residue_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_res);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(crt_residue_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_res);
@@ -804,7 +663,7 @@ int launch_k1_crt(tncb_ctx* ctx, const PairPlan& P, const double2* A, const doub
 
   for (long long n0 = 0; n0 < P.N; n0 += pn) {
     const long long nrows = std::min(pn, P.N - n0);
-    const long long Np = round_up_ll(nrows, 2 * CRT_BT);
+    const long long Np = round_up_ll(nrows, CRT_BT);
     // ---- Bt panel: exponents + residues (padding rows / K tail must be zero residues) ----
     if (Np != nrows) cudaMemsetAsync(pb, 0, (size_t)nmod * NPB * Np * Kp, st);
     cudaMemsetAsync(max_n, 0, (size_t)nrows * sizeof(unsigned long long), st);
@@ -816,7 +675,7 @@ int launch_k1_crt(tncb_ctx* ctx, const PairPlan& P, const double2* A, const doub
     }
     ctx->launches += 2;
     CUtensorMap mapB;
-    if ((rc = crt_make_map(&mapB, pb, (uint64_t)nmod * NPB * Np, (uint64_t)Kp))) { cleanup(); return rc; }
+    if ((rc = wg_make_map(&mapB, pb, (uint64_t)nmod * NPB * Np, (uint64_t)Kp))) { cleanup(); return rc; }
     for (long long m0 = 0; m0 < P.M; m0 += pm) {
       const long long mcols = std::min(pm, P.M - m0);
       const long long Mp = round_up_ll(mcols, TM);
@@ -830,29 +689,23 @@ int launch_k1_crt(tncb_ctx* ctx, const PairPlan& P, const double2* A, const doub
       }
       ctx->launches += 2;
       CUtensorMap mapA;
-      if ((rc = crt_make_map(&mapA, pa, (uint64_t)nmod * 3 * Mp, (uint64_t)Kp))) { cleanup(); return rc; }
+      if ((rc = wg_make_map(&mapA, pa, (uint64_t)nmod * 3 * Mp, (uint64_t)Kp))) { cleanup(); return rc; }
       CrtGemmArgs g;
       g.R = (int8_t*)pr; g.Np = (int)Np; g.Mp = (int)Mp;
-      g.pairs_n = (int)(Np / (2 * CRT_BT)); g.tiles_m = (int)(Mp / TM); g.tile_m = TM;
+      g.tiles_n = (int)(Np / CRT_BT); g.tiles_m = (int)(Mp / TM); g.tile_m = TM;
       g.nmod = nmod; g.nkc = nkc; g.kb_per_chunk = kb_per_chunk; g.num_kb = num_kb;
-      const long long items = (long long)g.pairs_n * g.tiles_m * nmod * nkc * (kara ? 3 : 1);
+      const long long items = (long long)g.tiles_n * g.tiles_m * nmod * nkc * (kara ? 3 : 1);
       if (items > 0x7fffffffLL) { cleanup(); return fail(TNCB_ERR_UNSUPPORTED, "too many work items"); }
       g.total_items = (int)items;
       g.group = ctx->crt_group;
       for (int i = 0; i < CRT_MAX_MOD; i++) { g.negmod[i] = -T.mod[i]; g.magic[i] = T.magic[i]; }
-      const int n_clusters = (int)std::min<long long>(n_clusters_max, items);
-      cudaLaunchConfig_t cfg{};
-      cfg.gridDim = dim3((unsigned)(2 * n_clusters)); cfg.blockDim = dim3(CRT_THREADS);
-      cfg.dynamicSmemBytes = smem_gemm; cfg.stream = st;
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeClusterDimension;
-      attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-      cfg.attrs = attr; cfg.numAttrs = 1;
+      const unsigned grid = (unsigned)std::min<long long>(ctas_max, items);
       const double ops = 2.0 * (kara ? 3.0 : 4.0) * (double)nmod * (double)Np * (double)Mp * (double)Kp;
       const bool time_this = ctx->time_gemm == 2 || (ctx->time_gemm == 1 && !timed);
       if (time_this) gemm_timer_begin(ctx);
-      cudaError_t e = kara ? cudaLaunchKernelEx(&cfg, crt_gemm_kernel<true>, mapB, mapA, g)
-                           : cudaLaunchKernelEx(&cfg, crt_gemm_kernel<false>, mapB, mapA, g);
+      if (kara) crt_gemm_kernel<true><<<grid, WG_THREADS, smem_gemm3, st>>>(mapB, mapA, g);
+      else crt_gemm_kernel<false><<<grid, WG_THREADS, smem_gemm4, st>>>(mapB, mapA, g);
+      cudaError_t e = cudaGetLastError();
       if (time_this) { gemm_timer_end(ctx, ops); timed = true; }
       if (e != cudaSuccess) { cleanup(); return fail(TNCB_ERR_CUDA, std::string("crt_gemm_kernel launch: ") + cudaGetErrorString(e)); }
       ctx->last_int8_ops += ops;

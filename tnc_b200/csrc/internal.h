@@ -77,7 +77,7 @@ struct tncb_ctx {
   cudaStream_t stream = nullptr;
   tncb::Arena arena;
   uint64_t launches = 0;
-  int oz_slices = 8;  // 0 = DMMA only; otherwise the tcgen05 int8 engine (K1') takes large pairs (digit-slicing engine: #slices)
+  int oz_slices = 8;  // 0 = DMMA only; otherwise the int8 tensor-core engine (K1') takes large pairs (digit-slicing engine: #slices)
   int oz_engine = 0;  // 0 = CRT / modular engine (crt.cu, default), 1 = 7-bit digit slicing (ozaki.cu, kept for A/B)
   long long oz_min_tiles = 96, oz_min_k = 1536;   // thresholds of the digit-slicing engine
   // CRT engine: operand bits (53 = full mantissa) or a requested tolerance, forced modulus count, thresholds, workspace
@@ -86,12 +86,12 @@ struct tncb_ctx {
   size_t crt_ws_bytes = (size_t)12 << 30; int crt_group = 8;
   double last_int8_ops = 0.0; int last_nmod = 0; int last_products = 0;
   int crt_products = 0;            // real int8 products per complex product: 0 = auto (3 when K >= crt_kara_min_k), 3, 4
-  long long crt_kara_min_k = 4096;
-  uint64_t engine_count[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // K0, K0 split-K, K1 DMMA, K1 DMMA split-K, K1' tcgen05, K2, permute, -
+  long long crt_kara_min_k = 2048;
+  uint64_t engine_count[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // K0, K0 split-K, K1 DMMA, K1 DMMA split-K, K1' int8, K2, permute, -
   // dominant-kernel timing: 0 off, 1 keep the last launch (gemm_ev0/1), 2 accumulate every launch (event pool)
   int time_gemm = 0; cudaEvent_t gemm_ev0 = nullptr, gemm_ev1 = nullptr; bool gemm_ev_valid = false;
   std::vector<cudaEvent_t> gemm_pool; size_t gemm_used = 0; std::vector<double> gemm_ops;
-  int sm_count = 148;
+  int sm_count = 132;
   // pinned staging for leaf uploads
   void* stage_host = nullptr; size_t stage_bytes = 0;
   // K1 offset-table workspace (grown on demand, stream-ordered reuse)
@@ -127,11 +127,11 @@ int launch_permute(tncb_ctx* ctx, const double2* in, double2* out, int rank,
 int launch_conj(tncb_ctx* ctx, double2* data, uint64_t elems);
 int launch_add(tncb_ctx* ctx, double2* dst, const double2* src, uint64_t elems);
 int ensure_tab(tncb_ctx* ctx, size_t elems);
-// K1': tcgen05 int8-sliced ZGEMM (ozaki.cu); tables as built by launch_k1
+// K1': int8 digit-sliced ZGEMM on wgmma (ozaki.cu); tables as built by launch_k1
 int launch_k1_ozaki(tncb_ctx* ctx, const PairPlan& p, const double2* A, const double2* B, double2* C, int S,
                     const long long* offAm, const long long* offBn, const long long* offAk, const long long* offBk);
 
-// K1' default engine: tcgen05 int8 GEMMs over coprime moduli + CRT reconstruction (crt.cu)
+// K1' default engine: wgmma int8 GEMMs over coprime moduli + CRT reconstruction (crt.cu)
 int launch_k1_crt(tncb_ctx* ctx, const PairPlan& p, const double2* A, const double2* B, double2* C,
                   const long long* offAm, const long long* offBn, const long long* offAk, const long long* offBk);
 void crt_choose(long long K, int want_bits, int nmod_force, int* nmod, int* bits_a, int* bits_b);

@@ -1,4 +1,4 @@
-// sm_100a kernels of the pairwise-contraction hot path (replaces tetra::contract, called at
+// sm_90a kernels of the pairwise-contraction hot path (replaces tetra::contract, called at
 // tnc/src/tensornetwork/contraction.rs:78-84, i.e. HPTT transposes + faer/MKL ZGEMM).
 //
 //   C[n, m] = sum_k Bt[n, k] * At[k, m]      (complex128, C row-major [N][M])
@@ -10,9 +10,9 @@
 //   K0  strided kernel: G lanes per output element cooperate over K (shuffle reduction),
 //       optional deterministic split-K; for tiny and for low-intensity pairs.
 //   K1  fused gather + ZGEMM: cp.async 16-byte gathers into a fragment-ordered shared-memory
-//       ring, FP64 tensor-core DMMA (mma.sync.m8n8k4.f64, 4 real MMAs per complex tile).
-//       tcgen05.mma has no f64 kind, so the FP64 tensor path on sm_100a is DMMA; measured
-//       peak 37.2 TFLOP/s (profiles/r01_fp64_peak_microbench.txt).
+//       ring, FP64 tensor-core DMMA (mma.sync.m16n8k4.f64, 4 real MMAs per complex tile).
+//       wgmma has no f64 kind, so the FP64 tensor path on sm_90a is DMMA (H100 SXM data sheet:
+//       67 TFLOP/s FP64 tensor core; tools/fp64_peak.cu measures a card).
 #include "internal.h"
 #include <algorithm>
 #include <cstdio>
@@ -162,10 +162,13 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N_>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N_)); }
 
-__device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b) {
-  asm("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-      : "+d"(c0), "+d"(c1)
-      : "d"(a), "d"(b));
+// D[16x8] += A[16x4] . B[4x8]: on sm_90 the m16n8k* shapes run at the full FP64 tensor rate, m8n8k4 at half of it.
+// Fragments: a0 / a1 = rows lane/4 and lane/4 + 8 (col lane%4), b = row lane%4 (col lane/4), c0,c1 / c2,c3 = rows lane/4 and
+// lane/4 + 8 (cols 2 (lane%4) + {0,1}) -- i.e. two stacked m8n8k4 fragments, so the 8-row fragment order below serves both.
+__device__ __forceinline__ void dmma1684(double& c0, double& c1, double& c2, double& c3, double a0, double a1, double b) {
+  asm("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+      : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3)
+      : "d"(a0), "d"(a1), "d"(b));
 }
 
 constexpr int K1_BK = 16;
@@ -207,6 +210,7 @@ k1_kernel(const __grid_constant__ K1Args p) {
   constexpr int TJ = BM / WARPS_M / 8; // 8-col blocks per warp
   constexpr int KPW = BK / NW;         // kk per warp in !KFAST mode
   static_assert(BK % NW == 0 && BN % 32 == 0 && BM % 32 == 0 && NT % BK == 0, "tile/threads mismatch");
+  static_assert(TI % 2 == 0, "m16n8k4 pairs 8-row blocks");
   constexpr int B_ROWS = B_KFAST ? BN / (NT / BK) : BN / 32; // free-index positions per thread
   constexpr int A_COLS = A_KFAST ? BM / (NT / BK) : BM / 32;
   constexpr int B_KO = B_KFAST ? 1 : KPW;                    // K positions per thread
@@ -325,20 +329,20 @@ k1_kernel(const __grid_constant__ K1Args p) {
     for (int i = 0; i < TI; i++) bf[i] = sB[((wn * TI + i) * (BK / 4) + kb) * 32 + lane];
 #pragma unroll
     for (int j = 0; j < TJ; j++) af[j] = sA[(kb * (BM / 8) + wm * TJ + j) * 32 + lane];
-    // four passes so that the two DMMAs feeding one accumulator are TI*TJ*2 issues apart
+    // two passes so that the two DMMAs feeding one accumulator are TI*TJ issues apart; one m16n8k4 covers 8-row blocks i, i+1
 #pragma unroll
-    for (int i = 0; i < TI; i++)
+    for (int i = 0; i < TI; i += 2)
 #pragma unroll
       for (int j = 0; j < TJ; j++) {
-        dmma884(cr[i][j][0], cr[i][j][1], bf[i].x, af[j].x);
-        dmma884(ci[i][j][0], ci[i][j][1], bf[i].x, af[j].y);
+        dmma1684(cr[i][j][0], cr[i][j][1], cr[i + 1][j][0], cr[i + 1][j][1], bf[i].x, bf[i + 1].x, af[j].x);
+        dmma1684(ci[i][j][0], ci[i][j][1], ci[i + 1][j][0], ci[i + 1][j][1], bf[i].x, bf[i + 1].x, af[j].y);
       }
 #pragma unroll
-    for (int i = 0; i < TI; i++)
+    for (int i = 0; i < TI; i += 2)
 #pragma unroll
       for (int j = 0; j < TJ; j++) {
-        dmma884(cr[i][j][0], cr[i][j][1], -bf[i].y, af[j].y); // SASS DMMA negates the operand for free
-        dmma884(ci[i][j][0], ci[i][j][1], bf[i].y, af[j].x);
+        dmma1684(cr[i][j][0], cr[i][j][1], cr[i + 1][j][0], cr[i + 1][j][1], -bf[i].y, -bf[i + 1].y, af[j].y);   // negated for free
+        dmma1684(ci[i][j][0], ci[i][j][1], ci[i + 1][j][0], ci[i + 1][j][1], bf[i].y, bf[i + 1].y, af[j].x);
       }
   };
 
@@ -662,8 +666,8 @@ static int launch_k1(tncb_ctx* ctx, const PairPlan& P, const double2* A, const d
       }
     } else if (P.M >= 256 && P.N >= 256 && P.K >= 256) {
       const long long tiles = ((P.M + 127) / 128) * ((P.N + 127) / 128);
-      // crossover measured on B200 (profiles/r01_engine_sweep.txt): short K is dominated by the S
-      // FP64 read-modify-write flushes per tile, few tiles leave SMs idle (1 CTA per 128x128 tile)
+      // short K is dominated by the S FP64 read-modify-write flushes per tile, few tiles leave SMs
+      // idle (1 CTA per 128x128 tile)
       if (force || (tiles >= ctx->oz_min_tiles && P.K >= ctx->oz_min_k) || (tiles >= 1024 && P.K >= 1024)) {
         int rc = launch_k1_ozaki(ctx, P, A, B, C, ctx->oz_slices, a.offAm, a.offBn, a.offAk, a.offBk);
         if (rc == TNCB_OK) ctx->engine_count[4]++;
@@ -671,10 +675,9 @@ static int launch_k1(tncb_ctx* ctx, const PairPlan& P, const double2* A, const d
       }
     }
   }
-  // Tile choice (A/B-measured on B200, C2 pair, profiles/r01_k1_tile_ab.txt): 64x64 tiles with a
-  // 2-stage ring and 2 co-resident CTAs per SM reach ~90 % of the DMMA peak (independent CTAs
-  // hide each other's per-chunk barrier/gather bubbles); 128x64 with 3-4 stages and 1 CTA/SM
-  // stays at 75-81 %.  Skinny outputs use a 32-wide tile on the narrow side.
+  // Tile choice: 64x64 tiles with a 2-stage ring and 2 co-resident CTAs per SM (independent CTAs
+  // hide each other's per-chunk barrier/gather bubbles); TNCB_K1_VARIANT=1 selects 128x64 with
+  // 4 stages and 1 CTA/SM.  Skinny outputs use a 32-wide tile on the narrow side.
   static const int variant = std::getenv("TNCB_K1_VARIANT") ? atoi(std::getenv("TNCB_K1_VARIANT")) : 0;
   if (variant == 1) return launch_k1_modes<128, 64, 4, 2, 4, 1>(ctx, a, P.b_kfast, P.a_kfast, true);
   if (P.N <= 32 && P.M > 32) return launch_k1_modes<32, 64, 1, 2, 2, 2>(ctx, a, P.b_kfast, P.a_kfast, true);
@@ -686,11 +689,8 @@ static int launch_k1(tncb_ctx* ctx, const PairPlan& P, const double2* A, const d
 // K2: streaming kernel for big x tiny pairs (HBM-bound).  thread <-> one index x of the big free
 // side; the tiny operand sits in shared memory as S[s][k]; every thread reads its K elements of the
 // big operand once and writes its NS outputs.  Algorithmic traffic 16*(BIG*K + BIG*SMALL) bytes.
-// Gate-sized tiny operands (K, NS <= 4) stream at 5.8-6.1 TB/s.  With K = NS = 16 (the stem steps of the Sycamore-53 depth-12
-// slices: 16 input and 16 output streams GBs apart per block) it stays at 3.2 TB/s / 35 % of the FP64 pipe although DRAM
-// moves exactly the algorithmic bytes in full sectors (profiles/r02_ncu_k2_summary.txt).  Two fixes for "not enough loads
-// in flight" were measured and removed again: four loads per trip (11.0 vs 10.8 ms) and a 3-stage cp.async ring in shared
-// memory with 48 loads in flight per thread (11.7-13.5 ms) -- so the limit is not load latency under this access pattern.
+// With K = NS = 16 (the stem steps of the Sycamore-53 depth-12 slices) every block reads 16 input and writes 16 output streams
+// that lie GBs apart; the kernel's rate on the H100 at those shapes has not been measured.
 // ------------------------------------------------------------------------------------------
 struct K2Args {
   LegList big;     // free legs of the big operand (strides in the big operand)

@@ -408,9 +408,10 @@ static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) 
     }
   }
   P->ws_bytes = A.top;
-  // one workspace for all intermediates of a run: at most 64 GiB or 0.62 of the device (B200: ~110 GiB; leaves room for the
-  // int8 engine's 12 GiB of planes and the staged leaves), whichever is larger; TNCB_PLAN_WS_GB overrides
-  size_t limit = std::max((size_t)64 << 30, (size_t)(0.62 * (double)device_bytes));
+  // one workspace for all intermediates of a run: at most 0.62 of the device (H100 80 GB: ~46 GiB; leaves room for the
+  // int8 engine's 12 GiB of planes and the staged leaves), 46 GiB when the device size is unknown (plan created without a
+  // context); TNCB_PLAN_WS_GB overrides
+  size_t limit = device_bytes ? (size_t)(0.62 * (double)device_bytes) : (size_t)46 << 30;
   if (const char* e = std::getenv("TNCB_PLAN_WS_GB")) limit = (size_t)std::max(1, atoi(e)) << 30;
   if (P->ws_bytes > limit) { P->is_static = false; return; }
   // ---- batch descriptors ----
@@ -650,7 +651,7 @@ int tncb_plan_create(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, tn
   if (rc) { delete p; return rc; }
   size_t dev_free = 0, dev_total = 0;
   if (ctx) { cudaSetDevice(ctx->device); if (cudaMemGetInfo(&dev_free, &dev_total) != cudaSuccess) { dev_total = 0; cudaGetLastError(); } }
-  tncb::plan_static_layout(p, ctx ? ctx->sm_count : 148, dev_total);
+  tncb::plan_static_layout(p, ctx ? ctx->sm_count : 132, dev_total);
   *out = p;
   return TNCB_OK;
 }

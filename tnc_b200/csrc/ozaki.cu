@@ -1,11 +1,11 @@
 // K1' (LEGACY engine, round 1; selectable with tncb_ctx_set_tcgen05_engine(ctx, 1) for A/B measurements -- the default
 // engine is the modular / CRT emulation in crt.cu, which needs 16 int8 GEMM sweeps where this one needs 36).
 //
-// The dense contraction on the 5th-gen tensor cores (tcgen05) by 7-bit digit slicing (Ozaki scheme I): every real operand
+// The dense contraction on the int8 tensor cores (Hopper wgmma) by 7-bit digit slicing (Ozaki scheme I): every real operand
 // row is scaled by a power of two and cut into S signed 7-bit digit planes,
 //     x * 2^-e = sum_{p<S} d_p * 128^-(p+1) + r,   |d_p| <= 127,  |r| < 128^-S,
-// and  C ~= sum_{t<S} 128^-(t+2) * sum_{p+q=t} (D^B_p . D^A_q)  with every D.D an exact int8 GEMM (int32 accumulation in
-// TMEM, K chunked so it cannot overflow) and the recombination in FP64.  NOT exact: the digit products with p + q >= S are
+// and  C ~= sum_{t<S} 128^-(t+2) * sum_{p+q=t} (D^B_p . D^A_q)  with every D.D an exact int8 GEMM (int32 accumulation,
+// K chunked so it cannot overflow) and the recombination in FP64.  NOT exact: the digit products with p + q >= S are
 // dropped, so |C - C_exact|[n,m] <= (S+1) K 2^(-7S) * 4 max|b[n,:]| max|a[m,:]| (S = 8: measured 1e-15..7e-15 of max|C|),
 // rows containing NaN / Inf give unspecified finite values (the CRT engine poisons them with NaN), and there is no tolerance
 // control beyond the digit count.  The leg permutation of the reference's TTGT is fused into the slicing pass (gather
@@ -14,15 +14,14 @@
 // Complex arithmetic without int negation in the MMA: planes Br, Bi for Bt and nAi(=-Ai), Ar, Ai
 // for At; in shared memory the At planes sit as [nAi | Ar | Ai] so that
 //     Br x [Ar ; Ai]^T  -> (real | imag) columns,    Bi x [nAi ; Ar]^T -> (real | imag) columns
-// are two N=256 UMMAs into one 256-column accumulator (cols 0..127 real, 128..255 imag).
+// are two N=256 wgmmas into one 256-column accumulator (cols 0..127 real, 128..255 imag): the four-product stage of sm90.h.
 //
-// Kernel structure (one CTA per 128x128 complex output tile, 192 threads; oz_gemm2_kernel: CTA pairs, cta_group::2):
-//   warp 0  TMA producer (cp.async.bulk.tensor, SWIZZLE_128B, mbarrier complete_tx)
-//   warp 1  TMEM allocator + single-thread tcgen05.mma.kind::i8 issuer
-//   warps 2-5 epilogue: tcgen05.ld -> int32 -> FP64 * 2^(e_n + e_m - 7(t+2)) -> C (+=)
-// TMEM holds two 256-column accumulators so the epilogue of digit level t overlaps the MMAs
-// of level t+1.
+// Kernel structure (one CTA per 128x128 complex output tile, three warpgroups, main loop in sm90.h):
+//   warpgroup 0    TMA producer
+//   warpgroups 1-2 wgmma on 64 Bt rows each, then the epilogue of digit level t and K chunk kc:
+//                  int32 -> FP64 * 2^(e_n + e_m - 7(t+2)) -> C (+=)
 #include "internal.h"
+#include "sm90.h"
 #include <cuda.h>
 #include <algorithm>
 #include <cstdio>
@@ -32,10 +31,7 @@ namespace tncb {
 
 constexpr int OZ_BT = 128;      // tile rows (n) = tile cols (m)
 constexpr int OZ_BKB = 128;     // K bytes per stage row (one 128-byte swizzle row)
-constexpr int OZ_STAGES = 2;
-constexpr int OZ_TILE = OZ_BT * OZ_BKB;           // 16 KB
-constexpr int OZ_STAGE_BYTES = 5 * OZ_TILE;       // Br, Bi, nAi, Ar, Ai
-constexpr int OZ_THREADS = 192;
+constexpr int OZ_STAGES = 2;    // 2 x 80 KB
 constexpr int OZ_KCHUNK = 8192;                   // int32-safe: 2*(t+1)*K*127^2 < 2^31 for t <= 7
 constexpr int OZ_MAX_S = 8;
 
@@ -113,64 +109,6 @@ __global__ void oz_slice_kernel(const double2* __restrict__ src, const long long
   }
 }
 
-// ---- tcgen05 helpers ------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t oz_smem(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void oz_mbar_init(uint64_t* bar, int count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(oz_smem(bar)), "r"(count)); }
-__device__ __forceinline__ void oz_mbar_expect_tx(uint64_t* bar, uint32_t bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(oz_smem(bar)), "r"(bytes) : "memory"); }
-__device__ __forceinline__ void oz_mbar_arrive(uint64_t* bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(oz_smem(bar)) : "memory"); }
-__device__ __forceinline__ void oz_mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred P1;\n\t"
-      "OZ_WAIT:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
-      "@P1 bra OZ_DONE;\n\t"
-      "bra OZ_WAIT;\n\t"
-      "OZ_DONE:\n\t}" ::"r"(oz_smem(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void oz_tma_2d(const CUtensorMap* map, uint64_t* bar, void* smem, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-               ::"r"(oz_smem(smem)), "l"(map), "r"(oz_smem(bar)), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void oz_tma_2d_mc(const CUtensorMap* map, uint64_t* bar, void* smem, int c0, int c1, uint16_t mask) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
-               ::"r"(oz_smem(smem)), "l"(map), "r"(oz_smem(bar)), "r"(c0), "r"(c1), "h"(mask) : "memory");
-}
-__device__ __forceinline__ void oz_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(oz_smem(bar)), "h"(mask) : "memory");
-}
-__device__ __forceinline__ void oz_cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// K-major SWIZZLE_128B canonical layout (cute UMMA SmemDescriptor): LBO=1, SBO=1024 B, version 1
-__device__ __forceinline__ uint64_t oz_desc(const void* smem) {
-  uint64_t d = 0;
-  d |= (uint64_t)((oz_smem(smem) >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-__device__ __forceinline__ void oz_umma_i8(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void oz_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(oz_smem(bar)) : "memory");
-}
-__device__ __forceinline__ void oz_tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-}
-
 struct OzArgs {
   double2* C;
   const int* exp_n;   // per Bt row
@@ -179,55 +117,35 @@ struct OzArgs {
   int Np, Mp;         // padded plane rows
   int num_kb;         // Kp / 128
   int S;
-  int flags;          // bit 0: grouped tile raster (L2 reuse), bit 1: streaming (evict-first) accesses for the C read-modify-write
 };
 
-// CL = true: launched as 2x2 thread-block clusters.  The two CTAs of a cluster row work on the same
-// 128 Bt rows and the two of a column on the same 128 At rows, so every CTA loads only half of each
-// operand tile (64 rows) and TMA-multicasts it to its peer: L2->SM operand traffic per CTA drops
-// from 80 KB to 40 KB per stage (the non-cluster kernel is bound by exactly that traffic).
-template <bool CL>
-__global__ void __launch_bounds__(OZ_THREADS, 1)
+__global__ void __launch_bounds__(WG_THREADS, 1)
 oz_gemm_kernel(const __grid_constant__ CUtensorMap mapB, const __grid_constant__ CUtensorMap mapA,
                const __grid_constant__ OzArgs p) {
   extern __shared__ __align__(1024) uint8_t oz_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(oz_smem_raw) + 1023) & ~(uintptr_t)1023);
-  __shared__ uint64_t full_bar[OZ_STAGES], empty_bar[OZ_STAGES], tfull_bar[2], tempty_bar[2];
-  __shared__ uint32_t tmem_base_smem;
+  __shared__ uint64_t full_bar[OZ_STAGES], empty_bar[OZ_STAGES];
   __shared__ double col_scale[OZ_BT];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   const int n0 = blockIdx.y * OZ_BT, m0 = blockIdx.x * OZ_BT;
   const int S = p.S;
   const int kb_per_chunk = OZ_KCHUNK / OZ_BKB;
   const int nkc = (p.num_kb + kb_per_chunk - 1) / kb_per_chunk;
 
-  uint32_t crank = 0;
-  if (CL) asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(crank));
-  const int cx = crank & 1, cy = (crank >> 1) & 1;   // cluster dims (2,2,1): rank = x + 2*y
-  // a stage may be refilled once this CTA *and* the peers that multicast into it... no: once every
-  // CTA that this CTA's producer writes to has consumed it: self, the x-peer (Bt halves), the y-peer (At halves)
-  const uint16_t free_mask = CL ? (uint16_t)((1u << crank) | (1u << (crank ^ 1)) | (1u << (crank ^ 2))) : 0;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < OZ_STAGES; s++) { oz_mbar_init(&full_bar[s], 1); oz_mbar_init(&empty_bar[s], CL ? 3 : 1); }
-    for (int b = 0; b < 2; b++) { oz_mbar_init(&tfull_bar[b], 1); oz_mbar_init(&tempty_bar[b], 4); }
+    for (int s = 0; s < OZ_STAGES; s++) { wg_mbar_init(&full_bar[s], 1); wg_mbar_init(&empty_bar[s], 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (threadIdx.x < OZ_BT) {
     const long long gm = (long long)m0 + threadIdx.x;
     col_scale[threadIdx.x] = gm < p.M ? scalbn(1.0, p.exp_m[gm]) : 0.0;
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(oz_smem(&tmem_base_smem)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  if (CL) oz_cluster_sync();   // peers' barriers are initialised before any multicast / remote arrive
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = tmem_base_smem;
 
-  if (warp == 0 && lane == 0) {
+  if (wg == 0) {
     // ================= TMA producer =================
+    wg_setmaxnreg_producer();
+    if (tid != 0) return;
     int it = 0;
     for (int t = 0; t < S; t++)
       for (int kc = 0; kc < nkc; kc++) {
@@ -235,341 +153,74 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapB, const __grid_constant__
         for (int pp = 0; pp <= t; pp++) {
           const int qq = t - pp;
           for (int kb = kb0; kb < kb1; kb++, it++) {
-            const int s = it % OZ_STAGES;
-            if (it >= OZ_STAGES) oz_mbar_wait(&empty_bar[s], ((it / OZ_STAGES) - 1) & 1);
-            uint8_t* st = smem + s * OZ_STAGE_BYTES;
-            oz_mbar_expect_tx(&full_bar[s], OZ_STAGE_BYTES);
+            uint8_t* st = wg_produce_begin<OZ_STAGES, false>(smem, full_bar, empty_bar, it);
+            uint64_t* bar = &full_bar[it % OZ_STAGES];
+            uint8_t* a = st + WgStage<false>::A;
             const int kx = kb * OZ_BKB;
-            if (!CL) {
-              oz_tma_2d(&mapB, &full_bar[s], st + 0 * OZ_TILE, kx, (0 * S + pp) * p.Np + n0);  // Br_p
-              oz_tma_2d(&mapB, &full_bar[s], st + 1 * OZ_TILE, kx, (1 * S + pp) * p.Np + n0);  // Bi_p
-              oz_tma_2d(&mapA, &full_bar[s], st + 2 * OZ_TILE, kx, (0 * S + qq) * p.Mp + m0);  // nAi_q
-              oz_tma_2d(&mapA, &full_bar[s], st + 3 * OZ_TILE, kx, (1 * S + qq) * p.Mp + m0);  // Ar_q
-              oz_tma_2d(&mapA, &full_bar[s], st + 4 * OZ_TILE, kx, (2 * S + qq) * p.Mp + m0);  // Ai_q
-            } else {
-              // 64-row halves (box = 64 x 128 B); the SW128 layout keeps rows 0-63 / 64-127 in the first / second 8 KB
-              const uint16_t row_mask = (uint16_t)(0x3u << (2 * cy));                 // CTAs with the same n-tile
-              const uint16_t col_mask = (uint16_t)((1u << cx) | (1u << (cx + 2)));    // CTAs with the same m-tile
-              const int hb = cx * 64, ha = cy * 64;
-              oz_tma_2d_mc(&mapB, &full_bar[s], st + 0 * OZ_TILE + hb * OZ_BKB, kx, (0 * S + pp) * p.Np + n0 + hb, row_mask);
-              oz_tma_2d_mc(&mapB, &full_bar[s], st + 1 * OZ_TILE + hb * OZ_BKB, kx, (1 * S + pp) * p.Np + n0 + hb, row_mask);
-              oz_tma_2d_mc(&mapA, &full_bar[s], st + 2 * OZ_TILE + ha * OZ_BKB, kx, (0 * S + qq) * p.Mp + m0 + ha, col_mask);
-              oz_tma_2d_mc(&mapA, &full_bar[s], st + 3 * OZ_TILE + ha * OZ_BKB, kx, (1 * S + qq) * p.Mp + m0 + ha, col_mask);
-              oz_tma_2d_mc(&mapA, &full_bar[s], st + 4 * OZ_TILE + ha * OZ_BKB, kx, (2 * S + qq) * p.Mp + m0 + ha, col_mask);
-            }
+            wg_tma_2d(&mapB, bar, st, kx, (0 * S + pp) * p.Np + n0);                      // Br_p
+            wg_tma_2d(&mapB, bar, st + WgStage<false>::B1, kx, (1 * S + pp) * p.Np + n0); // Bi_p
+            wg_tma_2d(&mapA, bar, a, kx, (0 * S + qq) * p.Mp + m0);                       // nAi_q
+            wg_tma_2d(&mapA, bar, a + WG_TILE, kx, (1 * S + qq) * p.Mp + m0);             // Ar_q
+            wg_tma_2d(&mapA, bar, a + 2 * WG_TILE, kx, (2 * S + qq) * p.Mp + m0);         // Ai_q
           }
         }
       }
-  } else if (warp == 1 && lane == 0) {
-    // ================= MMA issuer =================
-    // idesc: D=S32 (2)@4, A/B signed int8 (1)@7,@10, both K-major, N=256 (>>3)@17, M=128 (>>4)@24
-    const uint32_t idesc = (2u << 4) | (1u << 7) | (1u << 10) | ((256u >> 3) << 17) | ((128u >> 4) << 24);
-    int it = 0, f = 0;
-    for (int t = 0; t < S; t++)
+  } else {
+    // ================= consumers: wgmma + epilogue (own 64 Bt rows) =================
+    wg_setmaxnreg_consumer();
+    const int c = wg - 1, wq = tid >> 5, lane = tid & 31;
+    WgRing<OZ_STAGES, false> ring{smem, full_bar, empty_bar};
+    long long gn[2];
+    bool row_ok[2];
+    int en[2];
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      gn[h] = (long long)n0 + c * 64 + wq * 16 + (lane >> 2) + 8 * h;
+      row_ok[h] = gn[h] < p.N;
+      en[h] = row_ok[h] ? p.exp_n[gn[h]] : 0;
+    }
+    uint32_t acc[128];
+#pragma unroll
+    for (int i = 0; i < 128; i++) acc[i] = 0u;
+    int f = 0;
+    for (int t = 0; t < S; t++) {
+      const double rs[2] = {scalbn(1.0, en[0] - 7 * (t + 2)), scalbn(1.0, en[1] - 7 * (t + 2))};
       for (int kc = 0; kc < nkc; kc++, f++) {
-        const int buf = f & 1;
-        if (f >= 2) { oz_mbar_wait(&tempty_bar[buf], ((f >> 1) - 1) & 1); asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-        const uint32_t acc = tmem_base + (uint32_t)(buf * 256);
         const int kb0 = kc * kb_per_chunk, kb1 = min(p.num_kb, kb0 + kb_per_chunk);
         bool first = true;
         for (int pp = 0; pp <= t; pp++)
-          for (int kb = kb0; kb < kb1; kb++, it++) {
-            const int s = it % OZ_STAGES;
-            oz_mbar_wait(&full_bar[s], (it / OZ_STAGES) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint8_t* st = smem + s * OZ_STAGE_BYTES;
-            const uint64_t d_br = oz_desc(st), d_bi = oz_desc(st + OZ_TILE);
-            const uint64_t d_nai_ar = oz_desc(st + 2 * OZ_TILE), d_ar_ai = oz_desc(st + 3 * OZ_TILE);
+          for (int kb = kb0; kb < kb1; kb++) ring.mma_stage(acc, c, first, tid == 0);
+        ring.drain(tid == 0);
 #pragma unroll
-            for (int k = 0; k < OZ_BKB / 32; k++) {
-              const uint64_t ko = (uint64_t)(k * 32 >> 4);
-              oz_umma_i8(acc, d_br + ko, d_ar_ai + ko, idesc, first ? 0u : 1u);   // (Br.Ar | Br.Ai)
-              first = false;
-              oz_umma_i8(acc, d_bi + ko, d_nai_ar + ko, idesc, 1u);               // (-Bi.Ai | Bi.Ar)
-            }
-            if (CL) oz_commit_mc(&empty_bar[s], free_mask); else oz_commit(&empty_bar[s]);
-          }
-        oz_commit(&tfull_bar[buf]);
-      }
-  } else if (warp >= 2) {
-    // ================= epilogue =================
-    const int q = warp & 3;
-    const long long gn = (long long)n0 + q * 32 + lane;
-    const bool row_ok = gn < p.N;
-    const int en = row_ok ? p.exp_n[gn] : 0;
-    double2* crow = p.C + gn * p.M + m0;
-    int f = 0;
-    for (int t = 0; t < S; t++) {
-      const double rs = scalbn(1.0, en - 7 * (t + 2));
-      for (int kc = 0; kc < nkc; kc++, f++) {
-        const int buf = f & 1;
-        oz_mbar_wait(&tfull_bar[buf], (f >> 1) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tbase = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * 256);
-#pragma unroll 1
-        for (int c0 = 0; c0 < OZ_BT; c0 += 32) {
-          uint32_t vr[32], vi[32];
-          oz_tmem_ld32(tbase + (uint32_t)c0, vr);
-          oz_tmem_ld32(tbase + (uint32_t)(128 + c0), vi);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          if (row_ok) {
+        for (int h = 0; h < 2; h++) {
+          if (!row_ok[h]) continue;
+          double2* crow = p.C + gn[h] * p.M + m0;
 #pragma unroll
-            for (int j = 0; j < 32; j++) {
-              const long long gm = (long long)m0 + c0 + j;
-              if (gm < p.M) {
-                const double sc = rs * col_scale[c0 + j];
-                double2 acc2 = make_double2((double)(int)vr[j] * sc, (double)(int)vi[j] * sc);
-                if (f != 0) { const double2 old = crow[c0 + j]; acc2.x += old.x; acc2.y += old.y; }
-                crow[c0 + j] = acc2;
+          for (int j = 0; j < 16; j++) {
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+              const int col = 8 * j + 2 * (lane & 3) + e;
+              if ((long long)m0 + col < p.M) {
+                const double sc = rs[h] * col_scale[col];
+                double2 v = make_double2((double)(int)acc[4 * j + 2 * h + e] * sc, (double)(int)acc[4 * (j + 16) + 2 * h + e] * sc);
+                if (f != 0) { const double2 old = crow[col]; v.x += old.x; v.y += old.y; }
+                crow[col] = v;
               }
             }
           }
         }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) oz_mbar_arrive(&tempty_bar[buf]);
       }
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (CL) oz_cluster_sync();   // nobody leaves while a peer may still multicast into / signal this CTA
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
-}
-
-// ---- 2-CTA variant: tcgen05.mma.cta_group::2 (M = 256 over a CTA pair) ---------------------------
-// The 1-CTA kernel is bound by shared-memory bandwidth (profiles/r01_tcgen05_cluster_ab.txt): per
-// K-step it reads 24 KB of UMMA operands and takes 20 KB of TMA fills.  With cta_group::2 the pair
-// computes a 256 (n) x 128 (m) complex tile: every CTA supplies its own 128 Bt rows and only HALF of
-// the N = 256 operand (CTA0: Ar and nAi, CTA1: Ai and Ar), i.e. 16 KB reads + 16 KB fills per K-step,
-// and a stage shrinks from 80 KB to 64 KB (3 stages fit).  Protocol as in CUTLASS' 2-SM kernels: both
-// CTAs' TMA loads signal the leader's full barrier (peer bit cleared), only the leader issues the MMA,
-// commits are multicast to both CTAs, epilogues of both CTAs arrive on the leader's tmem-empty barrier.
-constexpr int OZ2_STAGES = 3;
-constexpr int OZ2_STAGE_BYTES = 4 * OZ_TILE;   // Br, Bi, X (Ar | Ai), Y (nAi | Ar)
-
-__device__ __forceinline__ void oz_tma_2d_2sm(const CUtensorMap* map, uint64_t* bar, void* smem, int c0, int c1) {
-  const uint32_t leader_bar = oz_smem(bar) & 0xFEFFFFFFu;   // Sm100MmaPeerBitMask: CTA0's barrier
-  asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-               ::"r"(oz_smem(smem)), "l"(map), "r"(leader_bar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void oz_umma_i8_2sm(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::i8 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void oz_commit_2sm(uint64_t* bar) {   // arrives on `bar` in both CTAs of the pair
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(oz_smem(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void oz_mbar_arrive_cta(uint64_t* bar, uint32_t cta) {   // arrive on `bar` of cluster CTA `cta`
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(oz_smem(bar)), "r"(cta));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-
-__global__ void __launch_bounds__(OZ_THREADS, 1)
-oz_gemm2_kernel(const __grid_constant__ CUtensorMap mapB, const __grid_constant__ CUtensorMap mapA,
-                const __grid_constant__ OzArgs p) {
-  extern __shared__ __align__(1024) uint8_t oz_smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(oz_smem_raw) + 1023) & ~(uintptr_t)1023);
-  __shared__ uint64_t full_bar[OZ2_STAGES], empty_bar[OZ2_STAGES], tfull_bar[2], tempty_bar[2];
-  __shared__ uint32_t tmem_base_smem;
-  __shared__ double col_scale[OZ_BT];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint32_t crank;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(crank));   // cluster dims (2,1,1): rank = blockIdx.x & 1 (CTA pairs form along x)
-  const bool leader = crank == 0;
-  int tile_n = blockIdx.x, tile_m = blockIdx.y;                // n on x so that a pair covers 256 Bt rows
-  if (p.flags & 1) {
-    // grouped raster: consecutive CTA pairs sweep bands of 8 n-pairs x all m-tiles, so that the ~74 pairs
-    // resident at a time share 8 Bt row-pairs and ~9 At tiles instead of all 16 row-pairs and ~5 At tiles
-    const int pairs_n = gridDim.x >> 1, tiles_m = gridDim.y, GROUP = 8;
-    const int L = (blockIdx.x >> 1) + pairs_n * blockIdx.y;    // linear pair id in launch order
-    const int per_band = GROUP * tiles_m;
-    const int band = L / per_band, first = band * GROUP;
-    const int gsize = min(GROUP, pairs_n - first);
-    const int r = L - band * per_band;
-    tile_n = ((first + r % gsize) << 1) | (blockIdx.x & 1);
-    tile_m = r / gsize;
-  }
-  const int n0 = tile_n * OZ_BT, m0 = tile_m * OZ_BT;
-  const int S = p.S;
-  const int kb_per_chunk = OZ_KCHUNK / OZ_BKB;
-  const int nkc = (p.num_kb + kb_per_chunk - 1) / kb_per_chunk;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < OZ2_STAGES; s++) { oz_mbar_init(&full_bar[s], 1); oz_mbar_init(&empty_bar[s], 1); }
-    for (int b = 0; b < 2; b++) { oz_mbar_init(&tfull_bar[b], 1); oz_mbar_init(&tempty_bar[b], 8); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (threadIdx.x < OZ_BT) {
-    const long long gm = (long long)m0 + threadIdx.x;
-    col_scale[threadIdx.x] = gm < p.M ? scalbn(1.0, p.exp_m[gm]) : 0.0;
-  }
-  if (warp == 1) {   // both CTAs, same warp id, same smem destination
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(oz_smem(&tmem_base_smem)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  oz_cluster_sync();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = tmem_base_smem;
-
-  if (warp == 0 && lane == 0) {
-    // ================= TMA producer (both CTAs) =================
-    int it = 0;
-    for (int t = 0; t < S; t++)
-      for (int kc = 0; kc < nkc; kc++) {
-        const int kb0 = kc * kb_per_chunk, kb1 = min(p.num_kb, kb0 + kb_per_chunk);
-        for (int pp = 0; pp <= t; pp++) {
-          const int qq = t - pp;
-          for (int kb = kb0; kb < kb1; kb++, it++) {
-            const int s = it % OZ2_STAGES;
-            if (it >= OZ2_STAGES) oz_mbar_wait(&empty_bar[s], ((it / OZ2_STAGES) - 1) & 1);
-            uint8_t* st = smem + s * OZ2_STAGE_BYTES;
-            if (leader) oz_mbar_expect_tx(&full_bar[s], 2 * OZ2_STAGE_BYTES);   // bytes of both CTAs land on the leader's barrier
-            const int kx = kb * OZ_BKB;
-            oz_tma_2d_2sm(&mapB, &full_bar[s], st + 0 * OZ_TILE, kx, (0 * S + pp) * p.Np + n0);   // Br_p, own rows
-            oz_tma_2d_2sm(&mapB, &full_bar[s], st + 1 * OZ_TILE, kx, (1 * S + pp) * p.Np + n0);   // Bi_p
-            if (leader) {
-              oz_tma_2d_2sm(&mapA, &full_bar[s], st + 2 * OZ_TILE, kx, (1 * S + qq) * p.Mp + m0); // X: Ar  (N rows   0..127)
-              oz_tma_2d_2sm(&mapA, &full_bar[s], st + 3 * OZ_TILE, kx, (0 * S + qq) * p.Mp + m0); // Y: nAi
-            } else {
-              oz_tma_2d_2sm(&mapA, &full_bar[s], st + 2 * OZ_TILE, kx, (2 * S + qq) * p.Mp + m0); // X: Ai  (N rows 128..255)
-              oz_tma_2d_2sm(&mapA, &full_bar[s], st + 3 * OZ_TILE, kx, (1 * S + qq) * p.Mp + m0); // Y: Ar
-            }
-          }
-        }
-      }
-  } else if (warp == 1 && lane == 0 && leader) {
-    // ================= MMA issuer (leader CTA only) =================
-    // idesc: D=S32, A/B signed int8, K-major, N=256, M=256 (cta_group::2)
-    const uint32_t idesc = (2u << 4) | (1u << 7) | (1u << 10) | ((256u >> 3) << 17) | ((256u >> 4) << 24);
-    int it = 0, f = 0;
-    for (int t = 0; t < S; t++)
-      for (int kc = 0; kc < nkc; kc++, f++) {
-        const int buf = f & 1;
-        if (f >= 2) { oz_mbar_wait(&tempty_bar[buf], ((f >> 1) - 1) & 1); asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-        const uint32_t acc = tmem_base + (uint32_t)(buf * 256);
-        const int kb0 = kc * kb_per_chunk, kb1 = min(p.num_kb, kb0 + kb_per_chunk);
-        bool first = true;
-        for (int pp = 0; pp <= t; pp++)
-          for (int kb = kb0; kb < kb1; kb++, it++) {
-            const int s = it % OZ2_STAGES;
-            oz_mbar_wait(&full_bar[s], (it / OZ2_STAGES) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint8_t* st = smem + s * OZ2_STAGE_BYTES;
-            const uint64_t d_br = oz_desc(st), d_bi = oz_desc(st + OZ_TILE), d_x = oz_desc(st + 2 * OZ_TILE), d_y = oz_desc(st + 3 * OZ_TILE);
-#pragma unroll
-            for (int k = 0; k < OZ_BKB / 32; k++) {
-              const uint64_t ko = (uint64_t)(k * 32 >> 4);
-              oz_umma_i8_2sm(acc, d_br + ko, d_x + ko, idesc, first ? 0u : 1u);   // Br x [Ar ; Ai]
-              first = false;
-              oz_umma_i8_2sm(acc, d_bi + ko, d_y + ko, idesc, 1u);               // Bi x [nAi ; Ar]
-            }
-            oz_commit_2sm(&empty_bar[s]);
-          }
-        oz_commit_2sm(&tfull_bar[buf]);
-      }
-  } else if (warp >= 2) {
-    // ================= epilogue (both CTAs; own 128 rows) =================
-    const int q = warp & 3;
-    const long long gn = (long long)n0 + q * 32 + lane;
-    const bool row_ok = gn < p.N;
-    const int en = row_ok ? p.exp_n[gn] : 0;
-    double2* crow = p.C + gn * p.M + m0;
-    int f = 0;
-    for (int t = 0; t < S; t++) {
-      const double rs = scalbn(1.0, en - 7 * (t + 2));
-      for (int kc = 0; kc < nkc; kc++, f++) {
-        const int buf = f & 1;
-        oz_mbar_wait(&tfull_bar[buf], (f >> 1) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tbase = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * 256);
-#pragma unroll 1
-        for (int c0 = 0; c0 < OZ_BT; c0 += 32) {
-          uint32_t vr[32], vi[32];
-          oz_tmem_ld32(tbase + (uint32_t)c0, vr);
-          oz_tmem_ld32(tbase + (uint32_t)(128 + c0), vi);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          if (row_ok) {
-#pragma unroll
-            for (int j = 0; j < 32; j++) {
-              const long long gm = (long long)m0 + c0 + j;
-              if (gm < p.M) {
-                const double sc = rs * col_scale[c0 + j];
-                double2 acc2 = make_double2((double)(int)vr[j] * sc, (double)(int)vi[j] * sc);
-                if (p.flags & 2) {   // C is touched once per digit level: keep it out of the L2's way
-                  if (f != 0) { const double2 old = __ldcs(crow + c0 + j); acc2.x += old.x; acc2.y += old.y; }
-                  __stcs(crow + c0 + j, acc2);
-                } else {
-                  if (f != 0) { const double2 old = crow[c0 + j]; acc2.x += old.x; acc2.y += old.y; }
-                  crow[c0 + j] = acc2;
-                }
-              }
-            }
-          }
-        }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) oz_mbar_arrive_cta(&tempty_bar[buf], 0);   // the leader's MMA issuer waits for all 8 epilogue warps
-      }
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  oz_cluster_sync();
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
 }
 
 // ---- host side --------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    cudaDriverEntryPointQueryResult q;
-    void* p = nullptr;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess) fn = (EncodeTiledFn)p;
-  }
-  return fn;
-}
-
-static int make_map(CUtensorMap* m, void* ptr, uint64_t rows, uint64_t kbytes, uint32_t box_rows) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return fail(TNCB_ERR_CUDA, "cuTensorMapEncodeTiled is not available");
-  cuuint64_t dims[2] = {kbytes, rows};
-  cuuint64_t strides[1] = {kbytes};
-  cuuint32_t box[2] = {(cuuint32_t)OZ_BKB, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(TNCB_ERR_CUDA, "cuTensorMapEncodeTiled failed: " + std::to_string((int)r));
-  return TNCB_OK;
-}
-
 // tables: offAm[M], offBn[N], offAk[K], offBk[K] (built by the caller, see kernels.cu)
 int launch_k1_ozaki(tncb_ctx* ctx, const PairPlan& P, const double2* A, const double2* B, double2* C, int S,
                     const long long* offAm, const long long* offBn, const long long* offAk, const long long* offBk) {
   if (S < 2) S = 2;
   if (S > OZ_MAX_S) S = OZ_MAX_S;
-  // The 2x2 multicast variant is kept for the record but is OFF by default: measured on C2 it is
-  // slower (GEMM 10.3 ms vs 8.85 ms) although it halves the L2->SM operand traffic -- the kernel is
-  // bound by shared-memory bandwidth (UMMA operand reads 24 KB + TMA writes 20 KB per K-step = 172 B/clk
-  // against 128 B/clk), which multicast does not change; see profiles/r01_tcgen05_cluster_ab.txt.
-  static const bool cl = std::getenv("TNCB_OZ_CLUSTER") != nullptr;
-  // default: the cta_group::2 kernel (oz_gemm2_kernel); TNCB_OZ_1CTA=1 selects the 1-CTA kernel
-  static const bool two_cta = std::getenv("TNCB_OZ_1CTA") == nullptr && !cl;
-  const long long pad = cl ? 2 * OZ_BT : OZ_BT;   // 2x2 clusters need an even number of tiles per dimension
-  const long long pad_n = two_cta ? 2 * OZ_BT : pad;                    // CTA pairs split 256 Bt rows
-  const long long Np = (P.N + pad_n - 1) / pad_n * pad_n, Mp = (P.M + pad - 1) / pad * pad;
+  const long long Np = (P.N + OZ_BT - 1) / OZ_BT * OZ_BT, Mp = (P.M + OZ_BT - 1) / OZ_BT * OZ_BT;
   const long long Kp = (P.K + OZ_BKB - 1) / OZ_BKB * OZ_BKB;
   const size_t bytesB = (size_t)2 * S * Np * Kp, bytesA = (size_t)3 * S * Mp * Kp;
   const size_t bytesE = (size_t)(Np + Mp) * sizeof(int);
@@ -594,55 +245,18 @@ int launch_k1_ozaki(tncb_ctx* ctx, const PairPlan& P, const double2* A, const do
   }
   ctx->launches += 4;
   CUtensorMap mapB, mapA;
-  const uint32_t box_rows = (cl && !two_cta) ? OZ_BT / 2 : OZ_BT;
-  if ((rc = make_map(&mapB, pb, (uint64_t)2 * S * Np, (uint64_t)Kp, box_rows)) || (rc = make_map(&mapA, pa, (uint64_t)3 * S * Mp, (uint64_t)Kp, box_rows))) { cleanup(); return rc; }
+  if ((rc = wg_make_map(&mapB, pb, (uint64_t)2 * S * Np, (uint64_t)Kp)) || (rc = wg_make_map(&mapA, pa, (uint64_t)3 * S * Mp, (uint64_t)Kp))) { cleanup(); return rc; }
   OzArgs a;
   a.C = C; a.exp_n = exp_n; a.exp_m = exp_m; a.M = P.M; a.N = P.N; a.Np = (int)Np; a.Mp = (int)Mp;
   a.num_kb = (int)(Kp / OZ_BKB); a.S = S;
-  // default 1 = grouped raster (A/B on C2, same box: GEMM 7.62 ms vs 8.14-8.26 ms; streaming C accesses, bit 1,
-  // measured slower: 9.04 ms) -- profiles/r01_tcgen05_cluster_ab.txt
-  static const int tune = std::getenv("TNCB_OZ_TUNE") ? atoi(std::getenv("TNCB_OZ_TUNE")) : 1;
-  a.flags = tune;
-  const int smem_bytes = OZ_STAGES * OZ_STAGE_BYTES + 1024;
-  dim3 grid((unsigned)(Mp / OZ_BT), (unsigned)(Np / OZ_BT));
-  if (two_cta) {
-    const int smem2 = OZ2_STAGES * OZ2_STAGE_BYTES + 1024;
-    cudaError_t e2 = cudaFuncSetAttribute(oz_gemm2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem2);
-    if (e2 != cudaSuccess) { cleanup(); return fail(TNCB_ERR_CUDA, cudaGetErrorString(e2)); }
-    const double ops2 = 2.0 * 4.0 * (S * (S + 1) / 2) * (double)Np * (double)Mp * (double)Kp;
-    if (ctx->time_gemm) gemm_timer_begin(ctx);
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)(Np / OZ_BT), (unsigned)(Mp / OZ_BT));   // n tiles on x
-    cfg.blockDim = dim3(OZ_THREADS); cfg.dynamicSmemBytes = smem2; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    e2 = cudaLaunchKernelEx(&cfg, oz_gemm2_kernel, mapB, mapA, a);
-    if (ctx->time_gemm) gemm_timer_end(ctx, ops2);
-    ctx->last_int8_ops = ops2; ctx->last_nmod = 0;
-    ctx->launches++;
-    cleanup();
-    if (e2 != cudaSuccess) return fail(TNCB_ERR_CUDA, std::string("2-CTA launch: ") + cudaGetErrorString(e2));
-    return TNCB_OK;
-  }
-  auto kern = cl ? oz_gemm_kernel<true> : oz_gemm_kernel<false>;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
+  const int smem_bytes = OZ_STAGES * WgStage<false>::BYTES + 1024;
+  cudaError_t e = cudaFuncSetAttribute(oz_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
   if (e != cudaSuccess) { cleanup(); return fail(TNCB_ERR_CUDA, cudaGetErrorString(e)); }
+  const double ops = 2.0 * 4.0 * (S * (S + 1) / 2) * (double)Np * (double)Mp * (double)Kp;
   if (ctx->time_gemm) gemm_timer_begin(ctx);
-  if (cl) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid; cfg.blockDim = dim3(OZ_THREADS); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 2; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    e = cudaLaunchKernelEx(&cfg, kern, mapB, mapA, a);
-    if (e != cudaSuccess) { cleanup(); return fail(TNCB_ERR_CUDA, std::string("cluster launch: ") + cudaGetErrorString(e)); }
-  } else {
-    kern<<<grid, OZ_THREADS, smem_bytes, st>>>(mapB, mapA, a);
-  }
-  if (ctx->time_gemm) gemm_timer_end(ctx, 2.0 * 4.0 * (S * (S + 1) / 2) * (double)Np * (double)Mp * (double)Kp);
+  oz_gemm_kernel<<<dim3((unsigned)(Mp / OZ_BT), (unsigned)(Np / OZ_BT)), WG_THREADS, smem_bytes, st>>>(mapB, mapA, a);
+  if (ctx->time_gemm) gemm_timer_end(ctx, ops);
+  ctx->last_int8_ops = ops; ctx->last_nmod = 0;
   ctx->launches++;
   e = cudaGetLastError();
   cleanup();  // stream-ordered reuse: later allocations are only touched by later kernels

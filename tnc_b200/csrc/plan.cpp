@@ -129,7 +129,7 @@ const char* tncb_strerror(int status) {
   }
 }
 
-const char* tncb_version(void) { return "libtncb200 0.2 (sm_100a; K0 strided/split-K, K1 gather+DMMA ZGEMM, K1' tcgen05 int8 digit slicing, K2 streaming)"; }
+const char* tncb_version(void) { return "libtncb200 0.3 (sm_90a; K0 strided/split-K, K1 gather+DMMA ZGEMM, K1' wgmma int8 modular / digit slicing, K2 streaming)"; }
 
 int tncb_pair_out_legs(int n_a, const uint64_t* a_legs, const uint64_t* a_dims,
                        int n_b, const uint64_t* b_legs, const uint64_t* b_dims,

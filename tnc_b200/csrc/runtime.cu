@@ -142,9 +142,9 @@ int tncb_ctx_create(int device, size_t arena_bytes, tncb_ctx** out) {
   TNCB_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   TNCB_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major < 10)
+  if (prop.major != 9 || prop.minor != 0)   // sm_90a code (wgmma, setmaxnreg) runs on compute capability 9.0 only
     return fail(TNCB_ERR_CUDA, std::string("device is sm_") + std::to_string(prop.major * 10 + prop.minor) +
-                                   ", libtncb200 is built for sm_100a only");
+                                   ", libtncb200 is built for sm_90a only");
   tncb_ctx* ctx = new tncb_ctx();
   ctx->device = device;
   ctx->sm_count = prop.multiProcessorCount;

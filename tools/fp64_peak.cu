@@ -1,5 +1,5 @@
-// Microbenchmark: FP64 pipe peaks on sm_100a (DFMA vs DMMA mma.sync f64 shapes).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/fp64_peak tools/fp64_peak.cu
+// Microbenchmark: FP64 pipe peaks on sm_90a (DFMA vs DMMA mma.sync f64 shapes).
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/fp64_peak tools/fp64_peak.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #define CK(x) do{cudaError_t e=(x); if(e!=cudaSuccess){printf("CUDA %s @%d\n",cudaGetErrorString(e),__LINE__);return 1;}}while(0)
@@ -35,6 +35,24 @@ __global__ void k_dmma884(double* out, int iters, double s) {
   double r=0;
 #pragma unroll
   for (int i=0;i<ILP;i++) r+=c[i][0]+c[i][1];
+  out[blockIdx.x*blockDim.x+threadIdx.x]=r;
+}
+
+template<int ILP>
+__global__ void k_dmma1684(double* out, int iters, double s) {
+  double c[ILP][4];
+#pragma unroll
+  for (int i=0;i<ILP;i++){c[i][0]=0;c[i][1]=0;c[i][2]=0;c[i][3]=0;}
+  double a0 = s + threadIdx.x*1e-6, a1=a0*0.5, b = 1.0 - s*1e-3;
+  for (int it=0; it<iters; ++it) {
+#pragma unroll
+    for (int i=0;i<ILP;i++)
+      asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+        : "+d"(c[i][0]), "+d"(c[i][1]), "+d"(c[i][2]), "+d"(c[i][3]) : "d"(a0),"d"(a1),"d"(b));
+  }
+  double r=0;
+#pragma unroll
+  for (int i=0;i<ILP;i++) r+=c[i][0]+c[i][1]+c[i][2]+c[i][3];
   out[blockIdx.x*blockDim.x+threadIdx.x]=r;
 }
 
@@ -83,6 +101,7 @@ template<typename F>
 int timeit(const char* name, F launch, double flop_per_launch) {
   cudaEvent_t e0,e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   launch(); launch(); CK(cudaDeviceSynchronize());
+  if (cudaGetLastError() != cudaSuccess) { printf("%-28s launch failed (too many registers for this block size)\n", name); return 0; }
   float best=1e30f, tot=0;
   for (int r=0;r<5;r++){ cudaEventRecord(e0); launch(); cudaEventRecord(e1); CK(cudaEventSynchronize(e1)); float ms; cudaEventElapsedTime(&ms,e0,e1); if(ms<best)best=ms; tot+=ms; }
   printf("%-28s best %8.3f ms  %7.2f TFLOP/s   (mean %7.2f TFLOP/s)\n", name, best, flop_per_launch/best*1e-9, flop_per_launch/(tot/5)*1e-9);
@@ -104,6 +123,8 @@ int main(){
     double warps=thr_tot/32;
     snprintf(nm,64,"dmma884 ilp8 b%d t%d",bps,thr);
     timeit(nm,[&]{k_dmma884<8><<<grid,thr>>>(out,iters,0.5);}, warps*iters*8*(8*8*4*2.0));
+    snprintf(nm,64,"dmma1684 ilp4 b%d t%d",bps,thr);
+    timeit(nm,[&]{k_dmma1684<4><<<grid,thr>>>(out,iters,0.5);}, warps*iters*4*(16*8*4*2.0));
     snprintf(nm,64,"dmma1688 ilp4 b%d t%d",bps,thr);
     timeit(nm,[&]{k_dmma1688<4><<<grid,thr>>>(out,iters,0.5);}, warps*iters*4*(16*8*8*2.0));
     snprintf(nm,64,"dmma16816 ilp4 b%d t%d",bps,thr);

@@ -2,7 +2,7 @@
 //   g++ -std=c++17 -g -O1 -fsanitize=address,undefined -I/usr/local/cuda/include tools/hdf5_fuzz.cpp tnc_b200/csrc/hdf5io.cpp -lz -o /tmp/hdf5_fuzz
 //   /tmp/hdf5_fuzz seed.h5 20000
 // Mutates the seed file (byte flips, truncations, wild 8-byte words) and drives open / shape / attr / read on every
-// mutant; any out-of-bounds access aborts.  Result of the last run: profiles/r02_hdf5_fuzz.txt.
+// mutant; any out-of-bounds access aborts.
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>

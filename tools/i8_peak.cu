@@ -1,100 +1,66 @@
-// int8 tensor-pipe peak of this GPU (tcgen05.mma.cta_group::2.kind::i8, M=256 N=256 K=32), measured the way
-// tools/fp64_peak.cu measures the FP64 pipe: no memory traffic at all.  Every CTA pair keeps ONE operand stage in
-// shared memory (content irrelevant) and the leader issues back-to-back UMMAs into a TMEM accumulator; this is the
-// denominator of the int8 roofline in bench.py (replaces the "2 x cuBLAS bf16" proxy of round 1).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/i8_peak tools/i8_peak.cu && tools/i8_peak
+// int8 tensor-pipe peak of this GPU (wgmma.mma_async.m64n256k32.s32.s8.s8), measured the way tools/fp64_peak.cu
+// measures the FP64 pipe: no memory traffic at all.  Every CTA keeps ONE operand stage in shared memory (content
+// irrelevant) and two warpgroups issue back-to-back wgmmas into register accumulators; this is the denominator of the
+// int8 roofline in bench.py.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/i8_peak tools/i8_peak.cu && tools/i8_peak
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>
+#include "../tnc_b200/csrc/sm90.h"
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ uint64_t make_desc(const void* smem) {   // K-major SWIZZLE_128B: LBO = 1, SBO = 1024 B, version 1
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_u32(smem) >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred P1;\n\tW:\n\tmbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t@P1 bra D;\n\tbra W;\n\tD:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
+using namespace tncb;
 
-__global__ void __launch_bounds__(128, 1) i8_peak_kernel(int iters) {
+__global__ void __launch_bounds__(256, 1) i8_peak_kernel(int iters, int* sink) {
   extern __shared__ __align__(1024) uint8_t raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~(uintptr_t)1023);
-  __shared__ uint64_t bar;
-  __shared__ uint32_t tmem_base_smem;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint32_t crank;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(crank));
-  for (int i = threadIdx.x; i < 32768 / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(smem)[i] = 0x01010101u * (uint32_t)(i & 3);
-  if (threadIdx.x == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(&bar)), "r"(1));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_smem)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
+  for (int i = threadIdx.x; i < 49152 / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(smem)[i] = 0x01010101u * (uint32_t)(i & 3);
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy smem writes -> visible to the tensor core
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = tmem_base_smem;
-  if (crank == 0 && warp == 0 && lane == 0) {
-    const uint32_t idesc = (2u << 4) | (1u << 7) | (1u << 10) | ((256u >> 3) << 17) | ((256u >> 4) << 24);
-    const uint64_t da = make_desc(smem), db = make_desc(smem + 16384);
-    for (int it = 0; it < iters; it++) {
+  const int wg = threadIdx.x >> 7;
+  const uint64_t da = wg_desc(smem + wg * 64 * 128), db = wg_desc(smem + 16384);
+  uint32_t acc[128];
 #pragma unroll
-      for (int k = 0; k < 4; k++) {
-        const uint64_t ko = (uint64_t)(k * 32 >> 4);
-        const uint32_t acc = tmem_base + (uint32_t)((it & 1) * 256);
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::2.kind::i8 [%0], %1, %2, %3, p;\n\t}"
-                     ::"r"(acc), "l"(da + ko), "l"(db + ko), "r"(idesc), "r"(1u) : "memory");
-      }
-    }
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(&bar)), "h"((uint16_t)3) : "memory");
+  for (int i = 0; i < 128; i++) acc[i] = 0u;
+  for (int it = 0; it < iters; it++) {
+    wg_fence();
+#pragma unroll
+    for (int k = 0; k < 4; k++) wg_mma_s8_m64n256k32(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1u);
+    wg_commit();
+    wg_wait<1>();
   }
-  if (warp == 0 && lane == 0) mbar_wait(&bar, 0);   // both CTAs: all MMAs have completed
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
+  wg_wait<0>();
+  int s = 0;
+#pragma unroll
+  for (int i = 0; i < 128; i++) s += (int)acc[i];
+  if (s == 0x7fffffff) sink[threadIdx.x] = s;   // keeps the accumulators alive
 }
 
-int main(int argc, char** argv) {
+int main() {
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, 0);
   const int sms = prop.multiProcessorCount;
-  const int smem = 32768 + 1024;
+  const int smem = 49152 + 1024;
   cudaFuncSetAttribute(i8_peak_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(sms / 2 * 2)); cfg.blockDim = dim3(128); cfg.dynamicSmemBytes = smem;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
+  int* sink = nullptr;
+  cudaMalloc(&sink, 256 * sizeof(int));
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0); cudaEventCreate(&e1);
-  printf("%s, %d SMs, %d CTA pairs; UMMA kind::i8 cta_group::2 M=256 N=256 K=32, operands resident in shared memory\n", prop.name, sms, sms / 2);
-  for (int iters : {2000, 20000, 200000, 1000000}) {
-    cudaLaunchKernelEx(&cfg, i8_peak_kernel, 100);   // warm
+  printf("%s, %d SMs; wgmma m64n256k32 s8, two warpgroups per SM, operands resident in shared memory\n", prop.name, sms);
+  for (int iters : {2000, 20000, 200000}) {
+    i8_peak_kernel<<<sms, 256, smem>>>(100, sink);   // warm
     cudaDeviceSynchronize();
     cudaEventRecord(e0);
-    cudaError_t e = cudaLaunchKernelEx(&cfg, i8_peak_kernel, iters);
+    i8_peak_kernel<<<sms, 256, smem>>>(iters, sink);
     cudaEventRecord(e1);
     cudaEventSynchronize(e1);
-    if (e != cudaSuccess || cudaGetLastError() != cudaSuccess) { printf("launch failed: %s\n", cudaGetErrorString(e)); return 1; }
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { printf("launch failed: %s\n", cudaGetErrorString(e)); return 1; }
     float ms = 0;
     cudaEventElapsedTime(&ms, e0, e1);
-    const double ops = 2.0 * 256.0 * 256.0 * 32.0 * 4.0 * (double)iters * (double)(sms / 2);
-    printf("iters %8d  %9.3f ms  %8.1f int8 TOP/s  (%.3f of nominal 4500)\n", iters, ms, ops / (ms * 1e-3) * 1e-12, ops / (ms * 1e-3) * 1e-12 / 4500.0);
+    const double ops = 2.0 * 64.0 * 256.0 * 32.0 * 4.0 * 2.0 * (double)iters * (double)sms;
+    printf("iters %8d  %9.3f ms  %8.1f int8 TOP/s\n", iters, ms, ops / (ms * 1e-3) * 1e-12);
   }
+  cudaFree(sink);
   return 0;
 }

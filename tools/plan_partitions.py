@@ -6,7 +6,7 @@ Pipeline (all seeded, metadata only): FM bisection -> 400-evaluation simulated a
 (contractionpath/repartitioning.py, the step-budget restatement of the reference's SA balancer) -> the resulting
 nested path flattened into one contraction tree -> tree_cut(N) (contractionpath/tree_partition.py): N subtrees +
 the N-1 top nodes as the fan-in path -> 6 seeded SA chains of 1500 evaluations per N started from that cut, scored by
-the predicted critical-path time on B200s (two-roof pair model + NVLink transfer of the fan-in operands); the
+the predicted critical-path time on GPUs (two-roof pair model + NVLink transfer of the fan-in operands); the
 candidate with the smallest predicted time is kept."""
 import hashlib
 import json
@@ -95,7 +95,7 @@ def _sa_job(args):
 def plan(tn, parts_list=(2, 4, 8), sa_steps=400, seed=1, refine_steps=1500, refine_seeds=(1, 2, 3, 4, 5, 6), workers=0):
     """Per rank count N: start = tree-cut(N) of the 2-part SA tree (op-count objective, like the reference), refined by
     `refine_seeds` independent seeded SA chains of `refine_steps` evaluations whose objective is the predicted
-    critical-path TIME on B200s (contraction_cost.gpu_time_tensors: two-roof pair times + NVLink transfer of every
+    critical-path TIME on GPUs (contraction_cost.gpu_time_tensors: two-roof pair times + NVLink transfer of every
     fan-in operand); the reference anneals 48 chains for minutes on an op-count objective
     (simulated_annealing.rs:406-592).  The candidate with the smallest predicted time wins.  Deterministic."""
     import multiprocessing as mp

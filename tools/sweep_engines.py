@@ -1,4 +1,4 @@
-"""DMMA (K1) vs the tcgen05 int8 engines (K1': modular/CRT with several modulus counts, legacy digit slicing) over GEMM
+"""DMMA (K1) vs the int8 tensor-core engines (K1': modular/CRT with several modulus counts, legacy digit slicing) over GEMM
 shapes: device time per pair on the same box, error against the DMMA result.
 usage: python tools/sweep_engines.py [MxNxK ...]"""
 import json
