@@ -27,6 +27,71 @@ def tc_ctx(built_lib, request):
     c.close()
 
 
+ENGINES = [("4prod", 0, 4), ("3prod", 0, 3), ("digits", 1, 0)]
+
+
+@pytest.fixture(params=ENGINES, ids=[e[0] for e in ENGINES])
+def int8_ctx(built_lib, request):
+    """The modular engine in its 4- and 3-product forms, and the digit-slicing engine (engine 1, S = 8 digits)."""
+    import tnc_b200 as tb
+    _, engine, products = request.param
+    c = tb.Context(0)
+    c.set_tcgen05_slices(8)
+    c.set_tcgen05_threshold(1, 128)
+    c.set_tcgen05_engine(engine)
+    if engine == 0:
+        c.set_tcgen05_products(products)
+    c.engine, c.products, c.slices = engine, products, 8
+    yield c
+    c.close()
+
+
+def digit_bound(K, S):
+    """Engine 1's guarantee (ozaki.cu): |C - C_exact|[n,m] <= (S+1) K 2^(-7S) * 4 max|b[n,:]| max|a[m,:]|."""
+    return (S + 1) * K * 2.0 ** (-7 * S) * 4
+
+
+def engine_bound(ctx, K):
+    import tnc_b200 as tb
+    return tb.tcgen05_bound(K)["bound"] if ctx.engine == 0 else digit_bound(K, ctx.slices)
+
+
+def absmax(x, axis):
+    """max(|re|, |im|) along axis: the magnitude both engines scale a row by"""
+    return np.maximum(np.abs(x.real).max(axis=axis), np.abs(x.imag).max(axis=axis))
+
+
+def gemm_view(a_legs, a, b_legs, b):
+    """Bt [N, K] and At [K, M] with C = Bt At, legs ordered as in oracle.contract_pair."""
+    shared = [l for l in a_legs if l in b_legs]
+    bf = [i for i, l in enumerate(b_legs) if l not in a_legs]
+    af = [i for i, l in enumerate(a_legs) if l not in b_legs]
+    bk = [b_legs.index(l) for l in shared]
+    ak = [a_legs.index(l) for l in shared]
+    N, M, K = (int(np.prod([x.shape[i] for i in ix], dtype=np.int64)) for x, ix in ((b, bf), (a, af), (a, ak)))
+    return np.transpose(b, bf + bk).reshape(N, K), np.transpose(a, ak + af).reshape(K, M)
+
+
+def edge_sample(rng, n, count=24):
+    """first/last index, 63/64, 127/128, 255/256 where they exist, filled up with random indices"""
+    idx = {i for i in (0, 63, 64, 127, 128, 255, 256, n - 1) if i < n}
+    rest = [int(i) for i in rng.permutation(n) if int(i) not in idx]
+    return np.array(sorted(idx) + rest[:max(0, count - len(idx))])
+
+
+def check_bound(ctx, rng, got, a_legs, a, b_legs, b):
+    """sampled entries (tile edges included) against a long-double reference, in units of the engine's own bound"""
+    bt, at = gemm_view(a_legs, a, b_legs, b)
+    N, K = bt.shape
+    M = at.shape[1]
+    ns, ms = edge_sample(rng, N), edge_sample(rng, M)
+    ref = bt[ns].astype(np.clongdouble) @ at[:, ms].astype(np.clongdouble)
+    scale = absmax(bt[ns], 1)[:, None] * absmax(at[:, ms], 0)[None, :]
+    err = np.abs(got.reshape(N, M)[np.ix_(ns, ms)] - ref)
+    ratio = float((err / (engine_bound(ctx, K) * scale)).max())
+    assert ratio <= 1.0, ratio
+
+
 @pytest.fixture()
 def dmma_ctx(built_lib):
     import tnc_b200 as tb
@@ -37,7 +102,14 @@ def dmma_ctx(built_lib):
 
 
 def check(ctx, rng, a_legs, a_dims, b_legs, b_dims, tol=1e-12, scale_rows=False, engine="k1_tcgen05"):
+    """With the digit-slicing engine (engine 1), only pairs it takes (M, N, K >= 256) run, and they are also checked against
+    that engine's own bound; the smaller cases are the modular engine's."""
     import tnc_b200 as tb
+    M = int(np.prod([d for l, d in zip(a_legs, a_dims) if l not in b_legs]))
+    N = int(np.prod([d for l, d in zip(b_legs, b_dims) if l not in a_legs]))
+    K = int(np.prod([d for l, d in zip(a_legs, a_dims) if l in b_legs]))
+    if getattr(ctx, "engine", 0) == 1 and min(M, N, K) < 256:
+        return None, None
     a, b = rand_c(rng, a_dims), rand_c(rng, b_dims)
     if scale_rows:  # wildly different magnitudes per slice of the leading free legs -> per-row exponents matter
         a = a * np.exp(rng.uniform(-40, 40, size=[a_dims[0]] + [1] * (len(a_dims) - 1)))
@@ -49,6 +121,8 @@ def check(ctx, rng, a_legs, a_dims, b_legs, b_dims, tol=1e-12, scale_rows=False,
     assert legs == ref_legs and got.shape == ref.shape
     err = np.abs(got - ref).max()
     assert err <= tol * max(1.0, np.abs(ref).max()), err
+    if getattr(ctx, "engine", 0) == 1 and engine == "k1_tcgen05":
+        check_bound(ctx, rng, got, a_legs, a, b_legs, b)
     return got, ref
 
 
@@ -121,48 +195,78 @@ def test_tcgen05_square(tc_ctx):
     check(tc_ctx, rng, [0, 1], [128, 128], [1, 2], [128, 128])      # one tile pair, half of it padding
 
 
-def test_tcgen05_ragged(tc_ctx):
+def test_tcgen05_ragged(int8_ctx):
     rng = np.random.default_rng(2)
-    check(tc_ctx, rng, [0, 1], [300, 333], [1, 2], [333, 260])      # M, N, K not multiples of 128
-    check(tc_ctx, rng, [0, 1, 2], [7, 41, 300], [2, 3, 1], [300, 257, 41], engine="k0_splitk")  # M = 7: too thin for tcgen05 -> K0 split-K
-    check(tc_ctx, rng, [0, 1, 2], [133, 41, 30], [2, 3, 1], [30, 257, 41])   # permuted K legs (K = 1230), ragged everywhere
-    check(tc_ctx, rng, [0, 1], [130, 129], [1, 2], [129, 131])
+    check(int8_ctx, rng, [0, 1], [300, 333], [1, 2], [333, 260])      # M, N, K not multiples of 128
+    check(int8_ctx, rng, [0, 1, 2], [7, 41, 300], [2, 3, 1], [300, 257, 41], engine="k0_splitk")  # M = 7: too thin for tcgen05 -> K0 split-K
+    check(int8_ctx, rng, [0, 1, 2], [133, 41, 30], [2, 3, 1], [30, 257, 41])   # permuted K legs (K = 1230), ragged everywhere
+    check(int8_ctx, rng, [0, 1], [130, 129], [1, 2], [129, 131])
+    check(int8_ctx, rng, [0, 1, 2], [257, 20, 15], [2, 3, 1], [15, 511, 20])   # one row past a tile, one short of it
 
 
-def test_tcgen05_permuted_circuit_like(tc_ctx):
+def test_tcgen05_permuted_circuit_like(int8_ctx):
     rng = np.random.default_rng(3)
     sh = list(range(100, 109)); af = list(range(9)); bf = list(range(50, 59))
     a_legs = [x for p in zip(af, sh) for x in p]
     b_legs = [x for p in zip(reversed(sh), bf) for x in p]
-    check(tc_ctx, rng, a_legs, [2] * 18, b_legs, [2] * 18)           # M = N = K = 512, all dims 2, interleaved
+    check(int8_ctx, rng, a_legs, [2] * 18, b_legs, [2] * 18)           # M = N = K = 512, all dims 2, interleaved
     # shared legs leading in a, trailing in b: both loader modes (row-fast / k-fast) of the preparation kernels
-    check(tc_ctx, rng, [0, 1, 2, 3], [16, 16, 16, 16], [4, 5, 0, 1], [16, 16, 16, 16])
-    check(tc_ctx, rng, [2, 3, 0, 1], [16, 16, 16, 16], [0, 1, 4, 5], [16, 16, 16, 16])
+    check(int8_ctx, rng, [0, 1, 2, 3], [16, 16, 16, 16], [4, 5, 0, 1], [16, 16, 16, 16])
+    check(int8_ctx, rng, [2, 3, 0, 1], [16, 16, 16, 16], [0, 1, 4, 5], [16, 16, 16, 16])
     # C2 in small: dim-4 legs, shared legs interleaved with the free ones in both operands (M = N = K = 256): the warp
     # lanes of the preparation kernels are split 4 along k x 8 along rows (a) and 8 x 4 (b)
-    check(tc_ctx, rng, list(range(8)), [4] * 8, [7, 8, 5, 9, 3, 10, 1, 11], [4] * 8)
-    check(tc_ctx, rng, [0, 1, 2], [160, 64, 48], [2, 3, 1], [48, 130, 64])       # fastest K leg of a is 48 long (lk = 5), of b 64
+    check(int8_ctx, rng, list(range(8)), [4] * 8, [7, 8, 5, 9, 3, 10, 1, 11], [4] * 8)
+    check(int8_ctx, rng, [0, 1, 2], [160, 64, 48], [2, 3, 1], [48, 130, 64])       # fastest K leg of a is 48 long (lk = 5), of b 64
 
 
-def test_tcgen05_row_scaling(tc_ctx):
+def test_tcgen05_row_scaling(int8_ctx):
     rng = np.random.default_rng(4)
     # relative tolerance per output row group: compare in scaled units
     import tnc_b200 as tb
     a = rand_c(rng, [256, 256]); b = rand_c(rng, [256, 256])
     ra = np.exp(rng.uniform(-30, 30, size=(256, 1))); rb = np.exp(rng.uniform(-30, 30, size=(1, 256)))
     a2, b2 = a * ra, b * rb                                            # a rows (M) and b columns (N) scaled
-    legs, got = tb.contract_pair(tc_ctx, [0, 1], a2, [1, 2], b2)
+    int8_ctx.reset_stats()
+    legs, got = tb.contract_pair(int8_ctx, [0, 1], a2, [1, 2], b2)
+    assert int8_ctx.engine_counts()["k1_tcgen05"] == 1
     _, ref = orc.contract_pair([0, 1], a2, [1, 2], b2)
     rel = np.abs(got - ref) / (rb.T * ra.T * 16.0 * np.ones_like(np.abs(ref)))
     assert rel.max() <= 1e-12, rel.max()
+    check_bound(int8_ctx, rng, got, [0, 1], a2, [1, 2], b2)
 
 
-def test_tcgen05_long_k_split(tc_ctx):
-    """K = 20000 with one tile pair: the engine splits K over CTA pairs (chunk residues add up in the reconstruction);
+def test_tcgen05_long_k_split(int8_ctx):
+    """K = 20000 with one tile pair: the modular engine splits K over CTAs (chunk residues add up in the reconstruction),
+    the digit-slicing engine runs three int32-safe K chunks of 8192 (the epilogue adds each chunk into C);
     K = 70000 > 32768 needs several int32-safe chunks in any case."""
     rng = np.random.default_rng(5)
-    check(tc_ctx, rng, [0, 1], [256, 20000], [1, 2], [20000, 256])
-    check(tc_ctx, rng, [0, 1], [128, 70000], [1, 2], [70000, 128], tol=3e-12)
+    check(int8_ctx, rng, [0, 1], [256, 20000], [1, 2], [20000, 256])
+    check(int8_ctx, rng, [0, 1], [128, 70000], [1, 2], [70000, 128], tol=3e-12)
+
+
+@pytest.mark.parametrize("S", [2, 4, 8])
+def test_digit_slicing_digit_counts(built_lib, S):
+    """The digit-slicing engine with S = 2, 4 and 8 digits, each against its own bound, on a ragged pair with per-row
+    exponents.  The int8 operation count, 8 * S(S+1)/2 * Np Mp Kp, shows that S digits were used."""
+    import tnc_b200 as tb
+    rng = np.random.default_rng(100 + S)
+    ctx = tb.Context(0)
+    try:
+        ctx.set_tcgen05_threshold(1, 128)
+        ctx.set_tcgen05_engine(1)
+        ctx.set_tcgen05_slices(S)
+        ctx.engine, ctx.slices = 1, S
+        M, N, K = 385, 300, 1000
+        a = rand_c(rng, (M, K)) * np.exp(rng.uniform(-8, 8, size=(M, 1)))
+        b = rand_c(rng, (K, N)) * np.exp(rng.uniform(-8, 8, size=(1, N)))
+        ctx.reset_stats()
+        _, got = tb.contract_pair(ctx, [0, 1], a, [1, 2], b)
+        assert ctx.engine_counts()["k1_tcgen05"] == 1
+        padded = lambda x: -(-x // 128) * 128
+        assert ctx.last_tcgen05_info()["int8_ops"] == 8 * (S * (S + 1) // 2) * padded(N) * padded(M) * padded(K)
+        check_bound(ctx, rng, got, [0, 1], a, [1, 2], b)
+    finally:
+        ctx.close()
 
 
 def bound_check(ctx, rng, M, N, K, rel=0.0, n_mod=0, zero_row=False):
@@ -237,31 +341,47 @@ def test_nonfinite_rows_poison_their_outputs(tc_ctx):
     assert np.abs(got[~bad] - ref[~bad]).max() <= 1e-12 * np.abs(ref).max()
 
 
-def test_extreme_exponents(tc_ctx):
-    """Rows near the ends of the double range: maxima of 2^-1040 (denormal: the scale exponent is clamped at -1000, the row
-    keeps ABSOLUTE accuracy 2^(-1000-53)), 2^-900, 1 and 2^+900 against columns of 2^-100 .. 2^+20; every finite product is
-    within the bound relative to max|b row| * max(|a row|, 2^-1000)."""
+def extreme_pair(ctx, a2, b2):
+    """C = b2^T a2^T on the int8 engine: every entry finite and within the engine's bound relative to
+    max(|b col|, 2^-1001) * max(|a row|, 2^-1001) (the scale exponents are clamped at -1000)."""
     import tnc_b200 as tb
+    ctx.reset_stats()
+    _, got = tb.contract_pair(ctx, [0, 1], a2, [1, 2], b2)
+    assert ctx.engine_counts()["k1_tcgen05"] == 1
+    ref = b2.T.astype(np.clongdouble) @ a2.T.astype(np.clongdouble)
+    assert np.all(np.isfinite(got.real)) and np.all(np.isfinite(got.imag))
+    mxa = np.maximum(absmax(a2, 1), 2.0 ** -1001)
+    mxb = np.maximum(absmax(b2, 0), 2.0 ** -1001)
+    # outputs below 2^-1022 are denormal doubles: no FP64 result (the reference's included) can be closer than 2^-1075
+    allowed = engine_bound(ctx, a2.shape[1]) * (mxb[:, None].astype(np.longdouble) * mxa[None, :].astype(np.longdouble)) + np.longdouble(2.0) ** -1070
+    assert np.all(np.abs(got - ref) <= allowed), float((np.abs(got - ref) / allowed).max())
+    return got, ref
+
+
+def test_extreme_exponents(int8_ctx):
+    """Rows near the ends of the double range.  First pair: a rows with maxima of 2^-1040 (denormal: the scale exponent is
+    clamped at -1000, the row keeps ABSOLUTE accuracy 2^(-1000-53)), 2^-900, 1 and 2^+900 against b columns of
+    2^-100 .. 2^+20.  Second pair: the other ends, a rows with maxima in [2^1023, 2^1024) (the largest scale exponent a finite
+    row can have, 1024) against b columns of 2^-1040 and of 2^-100 .. 2^-70, and rows of 2^-60 against all of them; every
+    product is finite."""
     rng = np.random.default_rng(9)
-    M, N, K = 256, 128, 384
+    M, N, K = 256, 256, 384
     a, b = rand_c(rng, (M, K)), rand_c(rng, (K, N))
     ea = np.zeros(M, dtype=int); ea[:64] = -1040; ea[64:128] = -900; ea[192:] = 900
     eb = rng.integers(-100, 20, size=N)
     a2 = np.ldexp(a.real, ea[:, None]) + 1j * np.ldexp(a.imag, ea[:, None])
     b2 = np.ldexp(b.real, eb[None, :]) + 1j * np.ldexp(b.imag, eb[None, :])
-    tc_ctx.reset_stats()
-    _, got = tb.contract_pair(tc_ctx, [0, 1], a2, [1, 2], b2)
-    assert tc_ctx.engine_counts()["k1_tcgen05"] == 1
-    ref = b2.T.astype(np.clongdouble) @ a2.T.astype(np.clongdouble)
-    assert np.all(np.isfinite(got.real)) and np.all(np.isfinite(got.imag))
-    mxa = np.maximum(np.maximum(np.abs(a2.real), np.abs(a2.imag)).max(axis=1), 2.0 ** -1001)
-    mxb = np.maximum(np.abs(b2.real), np.abs(b2.imag)).max(axis=0)
-    bound = tb.tcgen05_bound(K)["bound"]
-    # outputs below 2^-1022 are denormal doubles: no FP64 result (the reference's included) can be closer than 2^-1075
-    allowed = bound * (mxb[:, None].astype(np.longdouble) * mxa[None, :].astype(np.longdouble)) + np.longdouble(2.0) ** -1070
-    assert np.all(np.abs(got - ref) <= allowed), float((np.abs(got - ref) / allowed).max())
+    got, ref = extreme_pair(int8_ctx, a2, b2)
     rel = (np.abs(got - ref)[:, 128:] / np.abs(ref)[:, 128:]).astype(np.float64)    # rows of ordinary magnitude: relative accuracy as usual
     assert np.median(rel) < 1e-14
+
+    a, b = rand_c(rng, (M, K)), rand_c(rng, (K, N))
+    a3 = a * 2.0 ** -60
+    a3[:8] = a[:8] / absmax(a[:8], 1)[:, None] * (1.5 * 2.0 ** 1023)     # max(|re|, |im|) of the row = 1.5 * 2^1023
+    eb = rng.integers(-100, -70, size=N); eb[:64] = -1040
+    b3 = np.ldexp(b.real, eb[None, :]) + 1j * np.ldexp(b.imag, eb[None, :])
+    assert absmax(a3[:8], 1).min() >= 2.0 ** 1023
+    extreme_pair(int8_ctx, a3, b3)
 
 
 def test_panels_when_the_workspace_is_small(tc_ctx):

@@ -7,8 +7,12 @@
 // and  C ~= sum_{t<S} 128^-(t+2) * sum_{p+q=t} (D^B_p . D^A_q)  with every D.D an exact int8 GEMM (int32 accumulation,
 // K chunked so it cannot overflow) and the recombination in FP64.  NOT exact: the digit products with p + q >= S are
 // dropped, so |C - C_exact|[n,m] <= (S+1) K 2^(-7S) * 4 max|b[n,:]| max|a[m,:]| (S = 8: measured 1e-15..7e-15 of max|C|),
-// rows containing NaN / Inf give unspecified finite values (the CRT engine poisons them with NaN), and there is no tolerance
-// control beyond the digit count.  The leg permutation of the reference's TTGT is fused into the slicing pass (gather
+// with max|.| = max(|re|, |im|) over the row.  The bound holds over the whole double range: a row's scale exponent
+// e = ilogb(max) + 1 is clamped below at kOzExpMin = -1000 (rows under 2^-1001, denormal ones included, keep ABSOLUTE
+// accuracy: read max|.| as max(max|.|, 2^-1001) in the bound), and e <= 1024 for any finite row, so 2^-e is finite and
+// non-zero; the output scale 2^(e_n + e_m - 7(t+2)) is applied as one scalbn, so no partial scale overflows or underflows.
+// Rows containing NaN / Inf give unspecified finite values (the CRT engine poisons them with NaN), and there is no
+// tolerance control beyond the digit count.  The leg permutation of the reference's TTGT is fused into the slicing pass (gather
 // through the plan's offset tables), which writes K-major int8 planes that TMA can stream.
 //
 // Complex arithmetic without int negation in the MMA: planes Br, Bi for Bt and nAi(=-Ai), Ar, Ai
@@ -19,7 +23,7 @@
 // Kernel structure (one CTA per 128x128 complex output tile, three warpgroups, main loop in sm90.h):
 //   warpgroup 0    TMA producer
 //   warpgroups 1-2 wgmma on 64 Bt rows each, then the epilogue of digit level t and K chunk kc:
-//                  int32 -> FP64 * 2^(e_n + e_m - 7(t+2)) -> C (+=)
+//                  scalbn(int32 -> FP64, e_n + e_m - 7(t+2)) -> C (+=)
 #include "internal.h"
 #include "sm90.h"
 #include <cuda.h>
@@ -34,9 +38,11 @@ constexpr int OZ_BKB = 128;     // K bytes per stage row (one 128-byte swizzle r
 constexpr int OZ_STAGES = 2;    // 2 x 80 KB
 constexpr int OZ_KCHUNK = 8192;                   // int32-safe: 2*(t+1)*K*127^2 < 2^31 for t <= 7
 constexpr int OZ_MAX_S = 8;
+constexpr int kOzExpMin = -1000;                  // as crt.cu's kExpMin: 2^-e stays finite for every row
 
 // ---- operand preparation --------------------------------------------------------------------
-// exponent e (per row of the K-major operand) with max(|re|,|im|) * 2^-e in [0.5, 1)
+// exponent e (per row of the K-major operand) with max(|re|,|im|) * 2^-e in [0.5, 1), clamped at kOzExpMin (then the
+// scaled row is below 0.5); e <= 1024 for a finite maximum
 __global__ void oz_rowexp_kernel(const double2* __restrict__ src, const long long* __restrict__ off_row,
                                  const long long* __restrict__ off_k, long long rows, long long K, int* __restrict__ exps) {
   const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -50,7 +56,7 @@ __global__ void oz_rowexp_kernel(const double2* __restrict__ src, const long lon
   }
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, d));
-  if (lane == 0) exps[row] = (m > 0.0 && isfinite(m)) ? (ilogb(m) + 1) : 0;
+  if (lane == 0) exps[row] = (m > 0.0 && isfinite(m)) ? max(ilogb(m) + 1, kOzExpMin) : 0;
 }
 
 // One thread: 16 consecutive k of one row -> 16 bytes of every digit plane.
@@ -125,7 +131,7 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapB, const __grid_constant__
   extern __shared__ __align__(1024) uint8_t oz_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(oz_smem_raw) + 1023) & ~(uintptr_t)1023);
   __shared__ uint64_t full_bar[OZ_STAGES], empty_bar[OZ_STAGES];
-  __shared__ double col_scale[OZ_BT];
+  __shared__ int col_exp[OZ_BT];
   const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   const int n0 = blockIdx.y * OZ_BT, m0 = blockIdx.x * OZ_BT;
   const int S = p.S;
@@ -138,7 +144,7 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapB, const __grid_constant__
   }
   if (threadIdx.x < OZ_BT) {
     const long long gm = (long long)m0 + threadIdx.x;
-    col_scale[threadIdx.x] = gm < p.M ? scalbn(1.0, p.exp_m[gm]) : 0.0;
+    col_exp[threadIdx.x] = gm < p.M ? p.exp_m[gm] : 0;
   }
   __syncthreads();
 
@@ -184,7 +190,7 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapB, const __grid_constant__
     for (int i = 0; i < 128; i++) acc[i] = 0u;
     int f = 0;
     for (int t = 0; t < S; t++) {
-      const double rs[2] = {scalbn(1.0, en[0] - 7 * (t + 2)), scalbn(1.0, en[1] - 7 * (t + 2))};
+      const int row_exp[2] = {en[0] - 7 * (t + 2), en[1] - 7 * (t + 2)};
       for (int kc = 0; kc < nkc; kc++, f++) {
         const int kb0 = kc * kb_per_chunk, kb1 = min(p.num_kb, kb0 + kb_per_chunk);
         bool first = true;
@@ -201,8 +207,8 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapB, const __grid_constant__
             for (int e = 0; e < 2; e++) {
               const int col = 8 * j + 2 * (lane & 3) + e;
               if ((long long)m0 + col < p.M) {
-                const double sc = rs[h] * col_scale[col];
-                double2 v = make_double2((double)(int)acc[4 * j + 2 * h + e] * sc, (double)(int)acc[4 * (j + 16) + 2 * h + e] * sc);
+                const int sc = row_exp[h] + col_exp[col];   // one scalbn: 2^(e_n + e_m - 7(t+2)) may lie outside the double range
+                double2 v = make_double2(scalbn((double)(int)acc[4 * j + 2 * h + e], sc), scalbn((double)(int)acc[4 * (j + 16) + 2 * h + e], sc));
                 if (f != 0) { const double2 old = crow[col]; v.x += old.x; v.y += old.y; }
                 crow[col] = v;
               }
