@@ -154,21 +154,26 @@ def test_sycamore_small_vs_oracle(ctx):
     assert abs(got - ref) <= 1e-9 * abs(ref) + 1e-14
 
 
-def test_plan_graph_replay_matches_eager(ctx):
-    """K0-only plans replay as one CUDA graph; results must equal the eager executor bit for bit
-    (same kernels, same order) for every payload."""
+def test_plan_graph_replay_matches_eager(ctx, monkeypatch):
+    """K0-only plans replay as one CUDA graph; results must equal the eager pair-by-pair executor bit for bit
+    (same kernels, same order) for every payload.  The eager side is a plan created with TNCB_NO_STATIC=1, which never
+    gets a static layout (the plan cache behind contract_tensor_network would serve later calls with a graph too)."""
     from tnc_b200.builders import random_circuit_builder
-    from tnc_b200.tensornetwork import NetworkPlan, contract_tensor_network
+    from tnc_b200.tensornetwork import NetworkPlan
     c = random_circuit_builder(12, 6, 0.5, 0.5, np.random.default_rng(9))
     tn0, _ = c.into_amplitude_network("0" * 12)
     path = greedy(tn0)
+    monkeypatch.setenv("TNCB_NO_STATIC", "1")
+    eager = NetworkPlan(tn0, path, ctx=ctx)
+    monkeypatch.delenv("TNCB_NO_STATIC")
     plan = NetworkPlan(tn0, path, ctx=ctx)
     for bits in ["0" * 12, "1" * 12, "010101010101", "000011110000"]:
         c2 = random_circuit_builder(12, 6, 0.5, 0.5, np.random.default_rng(9))
         tn, _ = c2.into_amplitude_network(bits)
-        a = complex(plan.execute(tn).to_numpy())
-        b = complex(contract_tensor_network(tn, path, ctx=ctx).to_numpy())
+        ctx.reset_stats(); a = complex(plan.execute(tn).to_numpy()); la = ctx.stats()["kernel_launches"]
+        ctx.reset_stats(); b = complex(eager.execute(tn).to_numpy()); lb = ctx.stats()["kernel_launches"]
         assert a == b, (bits, a, b)
+        assert lb >= len(path.toplevel) > la, (la, lb)                   # eager: one launch per pair; graph: batched levels
 
 
 def test_sliced_equals_flat(ctx):
