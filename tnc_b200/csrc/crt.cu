@@ -41,13 +41,31 @@ constexpr int CRT_MAX_MOD = 20;
 static const int kModuli[CRT_MAX_MOD] = {256, 253, 251, 249, 247, 245, 241, 239, 233, 229,
                                          227, 223, 211, 199, 197, 193, 191, 181, 179, 173};
 constexpr int CRT_BT = 128;        // tile rows per CTA (n) = tile cols (m)
-constexpr int CRT_BKB = 128;       // K bytes per stage row (one 128-byte swizzle row)
-// stage ring of the GEMM kernel (stage layouts in sm90.h): four products 2 x 80 KB, three products 3 x 48 KB
+constexpr int CRT_BKB = WG_BKB;    // K padding of the operand planes (one 128-byte swizzle row); a K block is 128 / BK stages
+// Stage ring of the GEMM kernel (stage layouts in sm90.h), one configuration per form: STAGES slots of BK K bytes each.
+// Chosen from tools/crt_gemm_sweep.py at the benchmark network's pairs (profiles/h100_crt_ring.jsonl, H100 80GB HBM3 at a
+// 400 W power limit): three products keep 3 x 48 KB (2 slots: ~10 % slower; 4 x 48 KB: no faster; 8 x 24 KB, two wgmmas
+// per stage: 25-35 % slower); four products take 5 x 40 KB of 64-byte stages (3-6 % faster than 2 x 80 KB).
+// The -D overrides exist for that sweep, which builds each ring variant as a separate copy of the library.
+#ifndef CRT_RING3_STAGES
+#define CRT_RING3_STAGES 3
+#endif
+#ifndef CRT_RING3_BK
+#define CRT_RING3_BK 128
+#endif
+#ifndef CRT_RING4_STAGES
+#define CRT_RING4_STAGES 5
+#endif
+#ifndef CRT_RING4_BK
+#define CRT_RING4_BK 64
+#endif
 template <bool KARA> struct CrtRing {
-  static constexpr int STAGES = KARA ? 3 : 2;
+  static constexpr int STAGES = KARA ? CRT_RING3_STAGES : CRT_RING4_STAGES;
+  static constexpr int BK = KARA ? CRT_RING3_BK : CRT_RING4_BK;
+  using Stage = WgStage<KARA, BK>;
+  static constexpr int SMEM = STAGES * Stage::BYTES + 1024;   // + the 1024-byte alignment pad of the dynamic shared memory
+  static_assert(SMEM <= 232448 - 1024, "stage ring exceeds the per-block shared memory of sm_90");
 };
-constexpr int CRT_STG_ROW = 2 * CRT_BT + 16;     // row of a consumer's epilogue staging tile: 256 residue bytes + 16 of padding
-constexpr int CRT_STG_BYTES = 64 * CRT_STG_ROW;  // per consumer warpgroup: 64 rows
 constexpr int CRT_KCHUNK_MAX = 32768;           // 2 * K * 128 * 128 < 2^31 for K <= 2^15
 constexpr int CRT_G = 34;                       // fixed-point bits of the leading CRT weight
 
@@ -351,13 +369,15 @@ __device__ __forceinline__ CrtItem crt_decode(const CrtGemmArgs& p, int item) {
 
 // Persistent CTAs, work item = (modulus, K chunk, 128 x 128 complex tile), items ordered modulus-major with a grouped tile
 // raster.  Warpgroup 0 streams the operand tiles (TMA), warpgroups 1-2 run the wgmma main loop (sm90.h) on 64 Bt rows each
-// and then their epilogue: accumulator mod m_i -> one offset byte -> shared-memory staging -> coalesced 16-byte stores.
-// The producer runs ahead into the next item while the consumers are in their epilogue.
+// and then their epilogue: accumulator mod m_i -> one offset byte -> a transpose of 32-bit words inside each lane quad
+// (shuffles, no shared memory) -> 16-byte stores.  The producer runs ahead into the next item, up to the ring's depth,
+// while the consumers are in their epilogue.
 template <bool KARA>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 crt_gemm_kernel(const __grid_constant__ CUtensorMap mapB, const __grid_constant__ CUtensorMap mapA,
                 const __grid_constant__ CrtGemmArgs p) {
-  constexpr int STAGES = CrtRing<KARA>::STAGES;
+  constexpr int STAGES = CrtRing<KARA>::STAGES, BK = CrtRing<KARA>::BK, SUB = CRT_BKB / BK;
+  using Stage = typename CrtRing<KARA>::Stage;
   extern __shared__ __align__(1024) uint8_t crt_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(crt_smem_raw) + 1023) & ~(uintptr_t)1023);
   __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES];
@@ -380,20 +400,20 @@ crt_gemm_kernel(const __grid_constant__ CUtensorMap mapB, const __grid_constant_
       // three products: plane `prod` of both operands (256 At rows); four: Br, Bi and the three At planes (-Ai, Ar, Ai)
       const int rowB = (KARA ? w.mod_i * 3 + w.prod : w.mod_i * 2) * p.Np + w.n0;
       const int rowA = (KARA ? w.mod_i * 3 + w.prod : w.mod_i * 3) * p.Mp + w.m0;
-      for (int kb = kb0; kb < kb1; kb++, it++) {
-        uint8_t* st = wg_produce_begin<STAGES, KARA>(smem, full_bar, empty_bar, it);
+      for (int ks = kb0 * SUB; ks < kb1 * SUB; ks++, it++) {
+        uint8_t* st = wg_produce_begin<STAGES, KARA, BK>(smem, full_bar, empty_bar, it);
         uint64_t* bar = &full_bar[it % STAGES];
-        const int kx = kb * CRT_BKB;
-        uint8_t* a = st + WgStage<KARA>::A;
+        const int kx = ks * BK;
+        uint8_t* a = st + Stage::A;
         wg_tma_2d(&mapB, bar, st, kx, rowB);
         if (KARA) {
           wg_tma_2d(&mapA, bar, a, kx, rowA);
-          wg_tma_2d(&mapA, bar, a + WG_TILE, kx, rowA + WG_ROWS);
+          wg_tma_2d(&mapA, bar, a + Stage::TILE, kx, rowA + WG_ROWS);
         } else {
-          wg_tma_2d(&mapB, bar, st + WgStage<KARA>::B1, kx, rowB + p.Np);
+          wg_tma_2d(&mapB, bar, st + Stage::B1, kx, rowB + p.Np);
           wg_tma_2d(&mapA, bar, a, kx, rowA);
-          wg_tma_2d(&mapA, bar, a + WG_TILE, kx, rowA + p.Mp);
-          wg_tma_2d(&mapA, bar, a + 2 * WG_TILE, kx, rowA + 2 * p.Mp);
+          wg_tma_2d(&mapA, bar, a + Stage::TILE, kx, rowA + p.Mp);
+          wg_tma_2d(&mapA, bar, a + 2 * Stage::TILE, kx, rowA + 2 * p.Mp);
         }
       }
     }
@@ -401,8 +421,9 @@ crt_gemm_kernel(const __grid_constant__ CUtensorMap mapB, const __grid_constant_
     // ================= consumers: wgmma main loop + epilogue (own 64 Bt rows) =================
     wg_setmaxnreg_consumer();
     const int c = wg - 1, wq = tid >> 5, lane = tid & 31;
-    WgRing<STAGES, KARA> ring{smem, full_bar, empty_bar};
-    uint8_t* stg = smem + STAGES * WgStage<KARA>::BYTES + c * CRT_STG_BYTES;
+    const int q = lane & 3;
+    const bool q0 = q & 1, q1 = q & 2;
+    WgRing<STAGES, KARA, BK> ring{smem, full_bar, empty_bar};
     uint32_t acc[128];
 #pragma unroll
     for (int i = 0; i < 128; i++) acc[i] = 0u;
@@ -410,37 +431,64 @@ crt_gemm_kernel(const __grid_constant__ CUtensorMap mapB, const __grid_constant_
       const CrtItem w = crt_decode<KARA>(p, item);
       const int kb0 = w.kc * p.kb_per_chunk, kb1 = min(p.num_kb, kb0 + p.kb_per_chunk);
       bool first = true;
-      for (int kb = kb0; kb < kb1; kb++) ring.mma_stage(acc, c, first, tid == 0);
+      for (int ks = kb0 * SUB; ks < kb1 * SUB; ks++) ring.mma_stage(acc, c, first, tid == 0);
       ring.drain(tid == 0);
       const int negm = p.negmod[w.mod_i], magic = p.magic[w.mod_i];
-      wg_bar_sync(1 + c);     // the previous item's copy-out has read the staging tile
+      // A lane quad (same lane / 4) holds 256 consecutive residue bytes of each of its two rows h: lane q has the two bytes at
+      // columns 8 j + 2 q (+1) for every j.  Per 16-byte chunk c (columns 16 c .. 16 c + 15) lane q packs its four bytes into
+      // one word u = (j = 2c: 2 bytes | j = 2c + 1: 2 bytes).  Chunk c is made of word c of all four lanes; per group of four
+      // chunks (i), a 4 x 4 transpose of words inside the quad (two butterfly rounds of shuffles) gives lane q the four words
+      // of chunk 4 i + q, so the quad stores 64 contiguous bytes of its row per instruction.
+      int8_t* row_base[2];
 #pragma unroll
-      for (int j = 0; j < 32; j++) {
+      for (int h = 0; h < 2; h++) {
+        const long long n = (long long)w.n0 + c * 64 + wq * 16 + (lane >> 2) + 8 * h;
+        row_base[h] = KARA ? p.R + ((long long)((w.mod_i * p.nkc + w.kc) * 3 + w.prod) * p.Np + n) * p.Mp + w.m0
+                           : p.R + ((long long)((w.mod_i * p.nkc + w.kc) * 2) * p.Np + n) * p.Mp + w.m0;
+      }
+#pragma unroll
+      for (int i = 0; i < 4; i++) {
 #pragma unroll
         for (int h = 0; h < 2; h++) {
-          uint32_t b = 0;
+          uint32_t x[4];            // x[k]: this lane's word of chunk 4 i + k
 #pragma unroll
-          for (int e = 0; e < 2; e++) {
-            const int a = (int)acc[4 * j + 2 * h + e];
-            // q = floor(a * magic / 2^32) in [a/m - 1.25, a/m + 0.25] (|a| < 2^31, |magic / 2^32 - 1/m| <= 2^-33), so
-            // t = a - q m lies in [-0.25 m, 1.25 m] = [-64, 320]: one conditional subtraction of m leaves a representative in
-            // [-128, 127]; its low byte with the top bit flipped is the OFFSET byte residue + 128.
-            int t = __mulhi(a, magic) * negm + a;
-            if (t > 127) t += negm;
-            b |= ((uint32_t)t & 0xffu) << (8 * e);
+          for (int k = 0; k < 4; k++) {
+            uint32_t u = 0;
+#pragma unroll
+            for (int jj = 0; jj < 2; jj++) {
+#pragma unroll
+              for (int e = 0; e < 2; e++) {
+                const int a = (int)acc[4 * (8 * i + 2 * k + jj) + 2 * h + e];
+                // q = floor(a * magic / 2^32) in [a/m - 1.25, a/m + 0.25] (|a| < 2^31, |magic / 2^32 - 1/m| <= 2^-33), so
+                // t = a - q m lies in [-0.25 m, 1.25 m] = [-64, 320]: one conditional subtraction of m leaves a representative
+                // in [-128, 127]; its low byte with the top bit flipped is the OFFSET byte residue + 128.
+                int t = __mulhi(a, magic) * negm + a;
+                if (t > 127) t += negm;
+                u |= (((uint32_t)t & 0xffu) ^ 0x80u) << (8 * (2 * jj + e));
+              }
+            }
+            x[k] = u;
           }
-          const int r = wq * 16 + (lane >> 2) + 8 * h, col = 8 * j + 2 * (lane & 3);
-          *reinterpret_cast<uint16_t*>(stg + r * CRT_STG_ROW + col) = (uint16_t)(b ^ 0x8080u);
+          // round 1 (lanes q, q ^ 1): keep the words for lanes with bit 0 = q0, hand over the others
+          const uint32_t r0 = __shfl_xor_sync(0xffffffffu, q0 ? x[0] : x[1], 1);
+          const uint32_t r1 = __shfl_xor_sync(0xffffffffu, q0 ? x[2] : x[3], 1);
+          // words for lane q0 (a) and lane q0 + 2 (b) from the lanes 2 q1 + 0 and 2 q1 + 1
+          const uint32_t a0 = q0 ? r0 : x[0], a1 = q0 ? x[1] : r0;
+          const uint32_t b0 = q0 ? r1 : x[2], b1 = q0 ? x[3] : r1;
+          // round 2 (lanes q, q ^ 2): keep the pair for lane q, hand over the other
+          const uint32_t g0 = __shfl_xor_sync(0xffffffffu, q1 ? a0 : b0, 2);
+          const uint32_t g1 = __shfl_xor_sync(0xffffffffu, q1 ? a1 : b1, 2);
+          const uint32_t k0 = q1 ? b0 : a0, k1 = q1 ? b1 : a1;
+          const uint32_t y0 = q1 ? g0 : k0, y1 = q1 ? g1 : k1, y2 = q1 ? k0 : g0, y3 = q1 ? k1 : g1;   // y[s]: word of lane s
+          // columns 16 c + 4 v .. + 3 of chunk c = 4 i + q: lanes (0, 1) for v = 0, 2 and lanes (2, 3) for v = 1, 3
+          const uint4 v = make_uint4(__byte_perm(y0, y1, 0x5410), __byte_perm(y2, y3, 0x5410),
+                                     __byte_perm(y0, y1, 0x7632), __byte_perm(y2, y3, 0x7632));
+          // three products: 256 columns of one plane; four products: chunks 0-7 real plane, 8-15 imaginary plane
+          const int cc = 4 * i + q;
+          int8_t* dst = KARA ? row_base[h] + cc * 16
+                             : row_base[h] + (i >= 2 ? (long long)p.Np * p.Mp : 0LL) + (cc & 7) * 16;
+          *reinterpret_cast<uint4*>(dst) = v;
         }
-      }
-      wg_bar_sync(1 + c);
-      const long long nrow0 = (long long)w.n0 + c * 64;
-#pragma unroll
-      for (int i = 0; i < 8; i++) {
-        const int q = i * 128 + tid, row = q >> 4, c16 = q & 15;
-        int8_t* dst = KARA ? p.R + ((long long)((w.mod_i * p.nkc + w.kc) * 3 + w.prod) * p.Np + nrow0 + row) * p.Mp + w.m0 + c16 * 16
-                           : p.R + ((long long)((w.mod_i * p.nkc + w.kc) * 2 + (c16 >> 3)) * p.Np + nrow0 + row) * p.Mp + w.m0 + (c16 & 7) * 16;
-        *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(stg + row * CRT_STG_ROW + c16 * 16);
       }
     }
   }
@@ -559,18 +607,23 @@ static EncodeTiledFn get_encode() {
   }
   return fn;
 }
+template <int BK>
 int wg_make_map(CUtensorMap* m, void* ptr, uint64_t rows, uint64_t kbytes) {
+  static_assert(BK == 128 || BK == 64, "SWIZZLE_128B or SWIZZLE_64B");
   EncodeTiledFn enc = get_encode();
   if (!enc) return fail(TNCB_ERR_CUDA, "cuTensorMapEncodeTiled is not available");
   cuuint64_t dims[2] = {kbytes, rows};
   cuuint64_t strides[1] = {kbytes};
-  cuuint32_t box[2] = {(cuuint32_t)WG_BKB, (cuuint32_t)WG_ROWS};
+  cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)WG_ROWS};   // the inner box extent must not exceed the swizzle span
   cuuint32_t estr[2] = {1, 1};
   CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                   BK == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(TNCB_ERR_CUDA, "cuTensorMapEncodeTiled failed: " + std::to_string((int)r));
   return TNCB_OK;
 }
+template int wg_make_map<128>(CUtensorMap*, void*, uint64_t, uint64_t);
+template int wg_make_map<64>(CUtensorMap*, void*, uint64_t, uint64_t);
 
 static inline long long round_up_ll(long long x, long long a) { return (x + a - 1) / a * a; }
 
@@ -634,8 +687,7 @@ int launch_k1_crt(tncb_ctx* ctx, const PairPlan& P, const double2* A, const doub
 
   static bool attr_done_dev[64] = {false};          // cudaFuncSetAttribute is per device
   bool& attr_done = attr_done_dev[ctx->device & 63];
-  const int smem_gemm4 = CrtRing<false>::STAGES * WgStage<false>::BYTES + 2 * CRT_STG_BYTES + 1024;
-  const int smem_gemm3 = CrtRing<true>::STAGES * WgStage<true>::BYTES + 2 * CRT_STG_BYTES + 1024;
+  const int smem_gemm4 = CrtRing<false>::SMEM, smem_gemm3 = CrtRing<true>::SMEM;
   const int smem_res = RES_ROWS * RES_RS * (int)sizeof(double2);
   if (!attr_done) {
     cudaError_t e = cudaFuncSetAttribute(crt_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_gemm4);
@@ -675,7 +727,8 @@ int launch_k1_crt(tncb_ctx* ctx, const PairPlan& P, const double2* A, const doub
     }
     ctx->launches += 2;
     CUtensorMap mapB;
-    if ((rc = wg_make_map(&mapB, pb, (uint64_t)nmod * NPB * Np, (uint64_t)Kp))) { cleanup(); return rc; }
+    if ((rc = kara ? wg_make_map<CrtRing<true>::BK>(&mapB, pb, (uint64_t)nmod * NPB * Np, (uint64_t)Kp)
+                   : wg_make_map<CrtRing<false>::BK>(&mapB, pb, (uint64_t)nmod * NPB * Np, (uint64_t)Kp))) { cleanup(); return rc; }
     for (long long m0 = 0; m0 < P.M; m0 += pm) {
       const long long mcols = std::min(pm, P.M - m0);
       const long long Mp = round_up_ll(mcols, TM);
@@ -689,7 +742,8 @@ int launch_k1_crt(tncb_ctx* ctx, const PairPlan& P, const double2* A, const doub
       }
       ctx->launches += 2;
       CUtensorMap mapA;
-      if ((rc = wg_make_map(&mapA, pa, (uint64_t)nmod * 3 * Mp, (uint64_t)Kp))) { cleanup(); return rc; }
+      if ((rc = kara ? wg_make_map<CrtRing<true>::BK>(&mapA, pa, (uint64_t)nmod * 3 * Mp, (uint64_t)Kp)
+                     : wg_make_map<CrtRing<false>::BK>(&mapA, pa, (uint64_t)nmod * 3 * Mp, (uint64_t)Kp))) { cleanup(); return rc; }
       CrtGemmArgs g;
       g.R = (int8_t*)pr; g.Np = (int)Np; g.Mp = (int)Mp;
       g.tiles_n = (int)(Np / CRT_BT); g.tiles_m = (int)(Mp / TM); g.tile_m = TM;

@@ -35,7 +35,7 @@ namespace tncb {
 
 constexpr int OZ_BT = 128;      // tile rows (n) = tile cols (m)
 constexpr int OZ_BKB = 128;     // K bytes per stage row (one 128-byte swizzle row)
-constexpr int OZ_STAGES = 2;    // 2 x 80 KB
+constexpr int OZ_STAGES = 2;    // 2 x 80 KB (128-byte stages, sm90.h)
 constexpr int OZ_KCHUNK = 8192;                   // int32-safe: 2*(t+1)*K*127^2 < 2^31 for t <= 7
 constexpr int OZ_MAX_S = 8;
 constexpr int kOzExpMin = -1000;                  // as crt.cu's kExpMin: 2^-e stays finite for every row
@@ -159,15 +159,16 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapB, const __grid_constant__
         for (int pp = 0; pp <= t; pp++) {
           const int qq = t - pp;
           for (int kb = kb0; kb < kb1; kb++, it++) {
-            uint8_t* st = wg_produce_begin<OZ_STAGES, false>(smem, full_bar, empty_bar, it);
+            using Stage = WgStage<false, OZ_BKB>;
+            uint8_t* st = wg_produce_begin<OZ_STAGES, false, OZ_BKB>(smem, full_bar, empty_bar, it);
             uint64_t* bar = &full_bar[it % OZ_STAGES];
-            uint8_t* a = st + WgStage<false>::A;
+            uint8_t* a = st + Stage::A;
             const int kx = kb * OZ_BKB;
             wg_tma_2d(&mapB, bar, st, kx, (0 * S + pp) * p.Np + n0);                      // Br_p
-            wg_tma_2d(&mapB, bar, st + WgStage<false>::B1, kx, (1 * S + pp) * p.Np + n0); // Bi_p
+            wg_tma_2d(&mapB, bar, st + Stage::B1, kx, (1 * S + pp) * p.Np + n0);          // Bi_p
             wg_tma_2d(&mapA, bar, a, kx, (0 * S + qq) * p.Mp + m0);                       // nAi_q
-            wg_tma_2d(&mapA, bar, a + WG_TILE, kx, (1 * S + qq) * p.Mp + m0);             // Ar_q
-            wg_tma_2d(&mapA, bar, a + 2 * WG_TILE, kx, (2 * S + qq) * p.Mp + m0);         // Ai_q
+            wg_tma_2d(&mapA, bar, a + Stage::TILE, kx, (1 * S + qq) * p.Mp + m0);         // Ar_q
+            wg_tma_2d(&mapA, bar, a + 2 * Stage::TILE, kx, (2 * S + qq) * p.Mp + m0);     // Ai_q
           }
         }
       }
@@ -175,7 +176,7 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapB, const __grid_constant__
     // ================= consumers: wgmma + epilogue (own 64 Bt rows) =================
     wg_setmaxnreg_consumer();
     const int c = wg - 1, wq = tid >> 5, lane = tid & 31;
-    WgRing<OZ_STAGES, false> ring{smem, full_bar, empty_bar};
+    WgRing<OZ_STAGES, false, OZ_BKB> ring{smem, full_bar, empty_bar};
     long long gn[2];
     bool row_ok[2];
     int en[2];
@@ -251,11 +252,11 @@ int launch_k1_ozaki(tncb_ctx* ctx, const PairPlan& P, const double2* A, const do
   }
   ctx->launches += 4;
   CUtensorMap mapB, mapA;
-  if ((rc = wg_make_map(&mapB, pb, (uint64_t)2 * S * Np, (uint64_t)Kp)) || (rc = wg_make_map(&mapA, pa, (uint64_t)3 * S * Mp, (uint64_t)Kp))) { cleanup(); return rc; }
+  if ((rc = wg_make_map<OZ_BKB>(&mapB, pb, (uint64_t)2 * S * Np, (uint64_t)Kp)) || (rc = wg_make_map<OZ_BKB>(&mapA, pa, (uint64_t)3 * S * Mp, (uint64_t)Kp))) { cleanup(); return rc; }
   OzArgs a;
   a.C = C; a.exp_n = exp_n; a.exp_m = exp_m; a.M = P.M; a.N = P.N; a.Np = (int)Np; a.Mp = (int)Mp;
   a.num_kb = (int)(Kp / OZ_BKB); a.S = S;
-  const int smem_bytes = OZ_STAGES * WgStage<false>::BYTES + 1024;
+  const int smem_bytes = OZ_STAGES * WgStage<false, OZ_BKB>::BYTES + 1024;
   cudaError_t e = cudaFuncSetAttribute(oz_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
   if (e != cudaSuccess) { cleanup(); return fail(TNCB_ERR_CUDA, cudaGetErrorString(e)); }
   const double ops = 2.0 * 4.0 * (S * (S + 1) / 2) * (double)Np * (double)Mp * (double)Kp;

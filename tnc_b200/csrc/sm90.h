@@ -1,10 +1,12 @@
 // Hopper (sm_90a) building blocks of the int8 tensor-core engines (crt.cu, ozaki.cu): mbarrier, TMA, wgmma.
 //
 // Both engines run the same warp-specialised int8 GEMM main loop:
-//   warpgroup 0     TMA producer (one thread; cp.async.bulk.tensor 2D, SWIZZLE_128B, mbarrier complete_tx)
+//   warpgroup 0     TMA producer (one thread; cp.async.bulk.tensor 2D, mbarrier complete_tx)
 //   warpgroups 1-2  consumers: each owns 64 of the CTA's 128 Bt rows and issues wgmma.m64n256k32.s32.s8.s8 from shared
 //                   memory into 128 int32 registers per thread (a 64 x 256 accumulator).
-// A stage holds 128 K bytes (one 128-byte swizzle row) of every operand tile.  Four-product complex form (Br, Bi | -Ai, Ar, Ai):
+// A stage holds BK K bytes of every operand tile: BK = 128 (one 128-byte swizzle row, SWIZZLE_128B) or BK = 64 (SWIZZLE_64B),
+// so that a shallower stage buys a deeper ring in the same shared memory.  The operand planes stay padded to 128 K bytes
+// (WG_BKB); a 128-byte block is 128 / BK stages.  Four-product complex form (Br, Bi | -Ai, Ar, Ai):
 //   stage = Br (128 rows) | Bi (128 rows) | [-Ai ; Ar ; Ai] (384 rows); per 32-byte K step two wgmmas,
 //   Br x [Ar ; Ai]^T and Bi x [-Ai ; Ar]^T, into one accumulator (columns 0-127 real, 128-255 imaginary).
 // Three-product form (one plane per operand): stage = B_p (128 rows) | A_p (256 rows); one wgmma per K step.
@@ -15,15 +17,16 @@
 namespace tncb {
 
 constexpr int WG_ROWS = 128;                 // Bt rows per CTA tile; TMA box rows
-constexpr int WG_BKB = 128;                  // K bytes per stage (one 128-byte swizzle row)
-constexpr int WG_TILE = WG_ROWS * WG_BKB;    // 16 KB: one 128-row operand tile of one stage
+constexpr int WG_BKB = 128;                  // K padding of the operand planes (one 128-byte swizzle row)
 constexpr int WG_THREADS = 384;              // producer warpgroup + two consumer warpgroups
 
-// stage layout (bytes): B0 | B1 (four products only) | A
-template <bool KARA> struct WgStage {
-  static constexpr int B1 = WG_TILE;
-  static constexpr int A = KARA ? WG_TILE : 2 * WG_TILE;
-  static constexpr int BYTES = KARA ? 3 * WG_TILE : 5 * WG_TILE;
+// stage layout (bytes): B0 | B1 (four products only) | A; TILE is one 128-row operand tile of BK K bytes (16 or 8 KB)
+template <bool KARA, int BK> struct WgStage {
+  static_assert(BK == 128 || BK == 64, "a stage is 128 (SWIZZLE_128B) or 64 (SWIZZLE_64B) K bytes deep");
+  static constexpr int TILE = WG_ROWS * BK;
+  static constexpr int B1 = TILE;
+  static constexpr int A = KARA ? TILE : 2 * TILE;
+  static constexpr int BYTES = KARA ? 3 * TILE : 5 * TILE;
 };
 
 __device__ __forceinline__ uint32_t wg_smem(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -50,17 +53,18 @@ __device__ __forceinline__ void wg_tma_2d(const CUtensorMap* map, uint64_t* bar,
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                ::"r"(wg_smem(smem)), "l"(map), "r"(wg_smem(bar)), "r"(c0), "r"(c1) : "memory");
 }
-// named barrier over the 128 threads of one consumer warpgroup (ids 1, 2; 0 is __syncthreads)
-__device__ __forceinline__ void wg_bar_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
-// wgmma shared-memory descriptor of a K-major SWIZZLE_128B tile (1024-byte aligned 8-row groups): LBO unused (1),
-// SBO = 1024 B, layout type 1 (128-byte swizzle).  A K offset inside the swizzle row is added to the start address.
+// wgmma shared-memory descriptor of a K-major tile with BK-byte rows as TMA writes it with SWIZZLE_<BK>B (8-row groups
+// of 8 BK bytes, aligned to that size): LBO unused (1), SBO = 8 BK bytes, layout type 1 (128-byte swizzle) or 2 (64-byte
+// swizzle).  A K offset inside the swizzle row is added to the start address.
+template <int BK>
 __device__ __forceinline__ uint64_t wg_desc(const void* smem) {
+  static_assert(BK == 128 || BK == 64, "SWIZZLE_128B or SWIZZLE_64B");
   uint64_t d = 0;
   d |= (uint64_t)((wg_smem(smem) & 0x3FFFF) >> 4);
   d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 62;
+  d |= (uint64_t)((8 * BK) >> 4) << 32;
+  d |= (uint64_t)(BK == 128 ? 1 : 2) << 62;
   return d;
 }
 
@@ -103,11 +107,13 @@ __device__ __forceinline__ void wg_mma_s8_m64n256k32(uint32_t (&d)[128], uint64_
       : "l"(da), "l"(db), "r"(accumulate));
 }
 
-// Consumer side of the stage ring.  `it` counts stages over the kernel's lifetime (slot it % STAGES, phase (it / STAGES) & 1).
+// Consumer side of the stage ring.  `it` counts stages over the kernel's lifetime (slot it % STAGES, phase (it / STAGES) & 1),
+// so an item whose stage count is not a multiple of STAGES simply leaves the next item starting mid-ring.
 // The stage just issued is released one stage later (wgmma.wait_group 1), so the tensor core never drains between stages;
-// wg_ring_drain releases the last one before the accumulator is read.
-template <int STAGES, bool KARA>
+// drain() releases the last one before the accumulator is read.
+template <int STAGES, bool KARA, int BK>
 struct WgRing {
+  using Stage = WgStage<KARA, BK>;
   uint8_t* smem; uint64_t* full; uint64_t* empty;
   int it = 0, pending = -1;
 
@@ -115,22 +121,22 @@ struct WgRing {
   __device__ __forceinline__ void mma_stage(uint32_t (&acc)[128], int wg, bool& first, bool signal) {
     const int s = it % STAGES;
     wg_mbar_wait(&full[s], (it / STAGES) & 1);
-    const uint8_t* st = smem + s * WgStage<KARA>::BYTES;
-    const uint8_t* b0 = st + wg * 64 * WG_BKB;
-    const uint8_t* a = st + WgStage<KARA>::A;
+    const uint8_t* st = smem + s * Stage::BYTES;
+    const uint8_t* b0 = st + wg * 64 * BK;
+    const uint8_t* a = st + Stage::A;
     wg_fence();
     if (KARA) {
-      const uint64_t d_b = wg_desc(b0), d_a = wg_desc(a);
+      const uint64_t d_b = wg_desc<BK>(b0), d_a = wg_desc<BK>(a);
 #pragma unroll
-      for (int k = 0; k < WG_BKB / 32; k++) {
+      for (int k = 0; k < BK / 32; k++) {
         wg_mma_s8_m64n256k32(acc, d_b + (uint64_t)(k * 2), d_a + (uint64_t)(k * 2), first ? 0u : 1u);   // B_p x A_p
         first = false;
       }
     } else {
-      const uint64_t d_br = wg_desc(b0), d_bi = wg_desc(b0 + WgStage<KARA>::B1);
-      const uint64_t d_x = wg_desc(a + WG_TILE), d_y = wg_desc(a);     // X = [Ar ; Ai], Y = [-Ai ; Ar]
+      const uint64_t d_br = wg_desc<BK>(b0), d_bi = wg_desc<BK>(b0 + Stage::B1);
+      const uint64_t d_x = wg_desc<BK>(a + Stage::TILE), d_y = wg_desc<BK>(a);     // X = [Ar ; Ai], Y = [-Ai ; Ar]
 #pragma unroll
-      for (int k = 0; k < WG_BKB / 32; k++) {
+      for (int k = 0; k < BK / 32; k++) {
         const uint64_t ko = (uint64_t)(k * 2);    // 32 bytes in 16-byte units
         wg_mma_s8_m64n256k32(acc, d_br + ko, d_x + ko, first ? 0u : 1u);
         first = false;
@@ -151,18 +157,18 @@ struct WgRing {
 };
 
 // Producer side: wait until slot it % STAGES is free, arm its barrier with the stage's bytes.  Returns the stage base.
-template <int STAGES, bool KARA>
+template <int STAGES, bool KARA, int BK>
 __device__ __forceinline__ uint8_t* wg_produce_begin(uint8_t* smem, uint64_t* full, uint64_t* empty, int it) {
   const int s = it % STAGES;
   if (it >= STAGES) wg_mbar_wait(&empty[s], ((it / STAGES) - 1) & 1);
-  wg_mbar_expect_tx(&full[s], WgStage<KARA>::BYTES);
-  return smem + s * WgStage<KARA>::BYTES;
+  wg_mbar_expect_tx(&full[s], WgStage<KARA, BK>::BYTES);
+  return smem + s * WgStage<KARA, BK>::BYTES;
 }
 
 __device__ __forceinline__ void wg_setmaxnreg_producer() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
 __device__ __forceinline__ void wg_setmaxnreg_consumer() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
 
-// 2D tensor map over K-major int8 planes [rows][kbytes], box 128 x 128 bytes, 128-byte swizzle
-int wg_make_map(CUtensorMap* m, void* ptr, uint64_t rows, uint64_t kbytes);
+// 2D tensor map over K-major int8 planes [rows][kbytes], box 128 rows x BK bytes, BK-byte swizzle (BK = 128 or 64)
+template <int BK> int wg_make_map(CUtensorMap* m, void* ptr, uint64_t rows, uint64_t kbytes);
 
 }  // namespace tncb

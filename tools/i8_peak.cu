@@ -18,7 +18,7 @@ __global__ void __launch_bounds__(256, 1) i8_peak_kernel(int iters, int* sink) {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy smem writes -> visible to the tensor core
   __syncthreads();
   const int wg = threadIdx.x >> 7;
-  const uint64_t da = wg_desc(smem + wg * 64 * 128), db = wg_desc(smem + 16384);
+  const uint64_t da = wg_desc<128>(smem + wg * 64 * 128), db = wg_desc<128>(smem + 16384);
   uint32_t acc[128];
 #pragma unroll
   for (int i = 0; i < 128; i++) acc[i] = 0u;
