@@ -135,10 +135,13 @@ def test_pairs_k2_streaming_kernel(ctx, built_lib):
 
 
 def test_pairs_k2_large_operands(ctx, built_lib):
-    """K2 with >= 2^16 free elements on the big side (several grid-stride trips per thread): orientations, K = 1..16,
-    NS = 1..16, scattered K legs, odd dims and a ragged last block, against the oracle."""
+    """K2 with >= 2^16 free elements on the big side: orientations, K = 1..16, NS = 1..16, scattered K legs, odd dims and
+    a ragged last block, against the oracle.  launch_k2 caps the grid at 32 blocks of 256 threads per SM, so only the
+    2^23 case (BIG >= 4 * 256 * 32 * SMs) makes every thread take several grid-stride trips."""
+    import torch
     from tnc_b200._lib import u64_array
     rng = np.random.default_rng(43)
+    sm_count = torch.cuda.get_device_properties(0).multi_processor_count
     def cls(a_legs, a_dims, b_legs, b_dims):
         return built_lib.tncb_pair_kernel_class(len(a_legs), u64_array(a_legs), u64_array(a_dims), len(b_legs), u64_array(b_legs), u64_array(b_dims))
     cases = [
@@ -149,12 +152,16 @@ def test_pairs_k2_large_operands(ctx, built_lib):
         ([0, 1, 2, 3], [37, 41, 7, 47], [2, 9], [7, 5]),                              # odd dims: BIG = 37*41*47 = 71299 (ragged block), K = 7, NS = 8 (5 used)
         ([9, 2], [3, 11], [0, 1, 2, 3], [29, 53, 11, 59]),                            # big B, M = 3, K = 11
         (list(range(17)), [2] * 17, [40], [13]),                                      # K = 1: outer product with a 2^17 operand, NS = 16 (13 used)
+        (list(range(24)), [2] * 24, [9], [2]),                                        # BIG = 2^23, K = 2 on a middle leg, NS = 1 (256 MiB)
     ]
     for a_legs, a_dims, b_legs, b_dims in cases:
         assert cls(a_legs, a_dims, b_legs, b_dims) == 2, (a_legs, b_legs)
         ctx.reset_stats()
         check_pair(ctx, rng, a_legs, a_dims, b_legs, b_dims)
         assert ctx.engine_counts()["k2"] == 1
+    big = 2 ** 23
+    blocks = min((big + 255) // 256, 32 * sm_count)
+    assert -(-big // (256 * blocks)) >= 4, (sm_count, blocks)     # grid-stride trips per thread of the last case
 
 
 @pytest.mark.parametrize("mode", ["interleaved", "a_suffix_b_prefix", "a_prefix_b_suffix", "reversed"])
