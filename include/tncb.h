@@ -278,14 +278,25 @@ int tncb_plan_execute(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tn,
  * TNCB_DATA_DEVICE leaves (consumed per call) -> TNCB_ERR_UNSUPPORTED. */
 int tncb_plan_stage(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tn);
 int tncb_plan_run(tncb_ctx* ctx, tncb_plan* plan, tncb_tensor** out, int* n_out, uint64_t* out_legs);
-/* Sliced execution (fixing the value of summed legs splits one contraction into independent contractions whose results
- * add up; the reference's declared future work, book/src/future_work.md:9-11): `plan` is compiled for the sliced
- * structure, the leaf payloads of all n_slices slice networks are materialised and uploaded ONCE, then
- * tncb_plan_run_slices contracts slices first, first + stride, ... with no host work per slice and returns their sum
- * (zeros if the range is empty) -- ranks of a multi-GPU job pass (rank, world) and combine with tncb_comm_allreduce_sum. */
+/* Many networks of the plan's structure: the leaf payloads of all n_slices networks are materialised and uploaded ONCE.
+ * They may be slices (fixing the value of summed legs splits one contraction into independent contractions whose results
+ * add up; the reference's declared future work, book/src/future_work.md:9-11), other bitstrings, other angle sets or any
+ * other payloads.  tncb_plan_run_slices contracts networks first, first + stride, ... with no host work per network and
+ * returns their sum (zeros if the range is empty) -- ranks of a multi-GPU job pass (rank, world) and combine with
+ * tncb_comm_allreduce_sum.  tncb_plan_run_batch returns them one by one instead. */
 int tncb_plan_stage_slices(tncb_ctx* ctx, tncb_plan* plan, size_t n_slices, const tncb_tn* const* slice_tns);
 int tncb_plan_run_slices(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t stride,
                          tncb_tensor** out_sum, int* n_out, uint64_t* out_legs);
+/* Contract the networks first .. first+count-1 staged by tncb_plan_stage_slices, each on its own (NOT summed), and
+ * return them as ONE tensor of rank r+1 and dims [count, d_0 .. d_{r-1}].  *n_out / out_legs describe one instance
+ * (r legs); instance i is the i-th row-major block.  Results are bit-identical to tncb_plan_run_slices(i, n_slices) of
+ * each instance.  The instances are a grid dimension of every kernel: one walk over the schedule per pass, each pass
+ * holding as many copies of the plan's workspace as fit the static-workspace limit (TNCB_PLAN_WS_GB) and the free
+ * device memory.  The plan's staged leaves (tncb_plan_stage) are untouched.  Needs a static plan (else
+ * TNCB_ERR_UNSUPPORTED); count == 0, first + count > n_slices, a result rank of 64, or no staged networks on this
+ * context -> TNCB_ERR_INVALID; not even one workspace copy fits -> TNCB_ERR_OOM. */
+int tncb_plan_run_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t count,
+                        tncb_tensor** out, int* n_out, uint64_t* out_legs);
 /* Schedule facts: #pairs, sum 8MNK, sum 16(MK+KN+MN), peak arena bytes, #kernels. */
 int tncb_plan_info(const tncb_plan* plan, uint64_t* n_pairs, double* flops, double* bytes,
                    uint64_t* peak_bytes, uint64_t* n_kernels);

@@ -106,6 +106,7 @@ SIGNATURES = {
     "tncb_plan_run": (C.c_int, [C.c_void_p, C.c_void_p, vpp, i32p, u64p]),
     "tncb_plan_stage_slices": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.POINTER(TncbTn))]),
     "tncb_plan_run_slices": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, vpp, i32p, u64p]),
+    "tncb_plan_run_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, vpp, i32p, u64p]),
     "tncb_plan_info": (C.c_int, [C.c_void_p, u64p, f64p, f64p, u64p, u64p]),
     "tncb_plan_destroy": (None, [C.c_void_p]),
     "tncb_comm_unique_id": (C.c_int, [C.c_void_p]),

@@ -121,7 +121,11 @@ extern "C" void tncb_plan_release_device_state(struct tncb_plan* plan);
 
 namespace tncb {
 // ---- kernel launchers (kernels.cu) ---------------------------------------------------
-int launch_pair(tncb_ctx* ctx, const PairPlan& p, const double2* A, const double2* B, double2* C);
+// count > 1: the same pair of `count` networks whose operands and result lie `stride` bytes apart (instance i at
+// A + i * stride, ...), as one launch per kernel; every launch decision (tile config, lanes, split-K) is the one a
+// single instance gets, so each instance's result is bit-identical to count = 1
+int launch_pair(tncb_ctx* ctx, const PairPlan& p, const double2* A, const double2* B, double2* C,
+                int count = 1, long long stride = 0);
 int launch_permute(tncb_ctx* ctx, const double2* in, double2* out, int rank,
                    const uint64_t* in_dims, const int* perm);
 int launch_conj(tncb_ctx* ctx, double2* data, uint64_t elems);
@@ -155,7 +159,8 @@ struct K0BatchItem {
 };
 bool k0_batch_eligible(int sm_count, const PairPlan& p);
 int k0_batch_fill(int sm_count, const PairPlan& p, K0BatchItem* item);   // returns the number of 256-thread blocks of the item
-int launch_k0_batch(tncb_ctx* ctx, const K0BatchItem* d_items, const int* d_block_start, int n_items, int total_blocks, char* ws);
+int launch_k0_batch(tncb_ctx* ctx, const K0BatchItem* d_items, const int* d_block_start, int n_items, int total_blocks, char* ws,
+                    int count = 1, long long stride = 0);
 
 int tensor_new(tncb_ctx* ctx, int rank, const uint64_t* dims, tncb_tensor** out);
 

@@ -78,10 +78,19 @@ struct K0Args {
 constexpr int K0_THREADS = 256;
 constexpr int K0_KT = 1024;
 
+// Instance-batched variants (tncb_plan_run_batch): the same body behind a wrapper that moves every pointer by
+// instance * stride bytes, so that one launch contracts the same pair of many networks whose workspaces lie `stride`
+// apart.  The single-instance kernels call the body unchanged.
+__host__ __device__ __forceinline__ const double2* inst_ptr(const double2* p, long long stride) {
+  return reinterpret_cast<const double2*>(reinterpret_cast<const char*>(p) + stride);
+}
+__host__ __device__ __forceinline__ double2* inst_ptr(double2* p, long long stride) {
+  return reinterpret_cast<double2*>(reinterpret_cast<char*>(p) + stride);
+}
+
 template <int G>
-__global__ void __launch_bounds__(K0_THREADS)
-k0_kernel(const double2* __restrict__ A, const double2* __restrict__ B, double2* __restrict__ dst,
-          const __grid_constant__ K0Args p) {
+__device__ __forceinline__ void
+k0_body(const double2* __restrict__ A, const double2* __restrict__ B, double2* __restrict__ dst, const K0Args& p) {
   __shared__ long long s_ka[K0_KT];
   __shared__ long long s_kb[K0_KT];
   const int tid = threadIdx.x;
@@ -123,13 +132,41 @@ k0_kernel(const double2* __restrict__ A, const double2* __restrict__ B, double2*
   if (valid && lane_g == 0) dst[(long long)blockIdx.y * MN + o] = make_double2(cr, ci);
 }
 
-__global__ void reduce_partials_kernel(const double2* __restrict__ part, double2* __restrict__ C,
-                                       long long MN, int ksplit) {
+template <int G>
+__global__ void __launch_bounds__(K0_THREADS)
+k0_kernel(const double2* __restrict__ A, const double2* __restrict__ B, double2* __restrict__ dst,
+          const __grid_constant__ K0Args p) {
+  k0_body<G>(A, B, dst, p);
+}
+
+// blockIdx.z = instance (blockIdx.y is the K range); A, B and dst (C or the plan's split-K scratch) move together
+template <int G>
+__global__ void __launch_bounds__(K0_THREADS)
+k0_inst_kernel(const double2* __restrict__ A, const double2* __restrict__ B, double2* __restrict__ dst,
+               const __grid_constant__ K0Args p, long long stride) {
+  const long long io = (long long)blockIdx.z * stride;
+  k0_body<G>(inst_ptr(A, io), inst_ptr(B, io), inst_ptr(dst, io), p);
+}
+
+__device__ __forceinline__ void reduce_partials_body(const double2* __restrict__ part, double2* __restrict__ C,
+                                                     long long MN, int ksplit) {
   long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (o >= MN) return;
   double cr = 0.0, ci = 0.0;
   for (int s = 0; s < ksplit; s++) { double2 v = part[(long long)s * MN + o]; cr += v.x; ci += v.y; }
   C[o] = make_double2(cr, ci);
+}
+
+__global__ void reduce_partials_kernel(const double2* __restrict__ part, double2* __restrict__ C,
+                                       long long MN, int ksplit) {
+  reduce_partials_body(part, C, MN, ksplit);
+}
+
+// blockIdx.y = instance; the partials and C have their own instance strides
+__global__ void reduce_partials_inst_kernel(const double2* __restrict__ part, double2* __restrict__ C,
+                                            long long MN, int ksplit, long long part_stride, long long c_stride) {
+  reduce_partials_body(inst_ptr(part, (long long)blockIdx.y * part_stride), inst_ptr(C, (long long)blockIdx.y * c_stride),
+                       MN, ksplit);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -200,9 +237,10 @@ struct K1Args {
 // prefetched one chunk ahead into registers and the cp.async gathers of stage kc+STAGES-1 are
 // issued in the middle of chunk kc's DMMA stream, so no table load sits on the critical path
 // (ncu r01: 20 % long_scoreboard on exactly those loads before this change).
-template <int BN, int BM, int WARPS_N, int WARPS_M, int STAGES, bool B_KFAST, bool A_KFAST, int MINB = 1>
-__global__ void __launch_bounds__(WARPS_N* WARPS_M * 32, MINB)
-k1_kernel(const __grid_constant__ K1Args p) {
+// A, B, C: p.A, p.B, p.C, or those of one instance of a batched launch
+template <int BN, int BM, int WARPS_N, int WARPS_M, int STAGES, bool B_KFAST, bool A_KFAST>
+__device__ __forceinline__ void
+k1_body(const K1Args& p, const double2* A, const double2* B, double2* C) {
   constexpr int BK = K1_BK;
   constexpr int NW = WARPS_N * WARPS_M;
   constexpr int NT = NW * 32;
@@ -298,12 +336,12 @@ k1_kernel(const __grid_constant__ K1Args p) {
     for (int q = 0; q < B_KO; q++)
 #pragma unroll
       for (int j = 0; j < B_ROWS; j++)
-        cp_async16(sbase + (unsigned)(b_rslot[j] + b_kslot[q]) * 16u, p.B + (b_off[j] + b_ko[q]), b_ok[j] && b_kok[q]);
+        cp_async16(sbase + (unsigned)(b_rslot[j] + b_kslot[q]) * 16u, B + (b_off[j] + b_ko[q]), b_ok[j] && b_kok[q]);
 #pragma unroll
     for (int q = 0; q < A_KO; q++)
 #pragma unroll
       for (int j = 0; j < A_COLS; j++)
-        cp_async16(sbase + (unsigned)(a_cslot[j] + a_kslot[q]) * 16u, p.A + (a_off[j] + a_ko[q]), a_ok[j] && a_kok[q]);
+        cp_async16(sbase + (unsigned)(a_cslot[j] + a_kslot[q]) * 16u, A + (a_off[j] + a_ko[q]), a_ok[j] && a_kok[q]);
   };
 
   double cr[TI][TJ][2], ci[TI][TJ][2];
@@ -374,11 +412,26 @@ k1_kernel(const __grid_constant__ K1Args p) {
 #pragma unroll
     for (int j = 0; j < TJ; j++) {
       const long long gm = m0 + (wm * TJ + j) * 8 + t2;
-      double2* dst = p.C + (long long)split * p.M * p.N + gn * p.M + gm;
+      double2* dst = C + (long long)split * p.M * p.N + gn * p.M + gm;
       if (gm < p.M) dst[0] = make_double2(cr[i][j][0], ci[i][j][0]);
       if (gm + 1 < p.M) dst[1] = make_double2(cr[i][j][1], ci[i][j][1]);
     }
   }
+}
+
+template <int BN, int BM, int WARPS_N, int WARPS_M, int STAGES, bool B_KFAST, bool A_KFAST, int MINB = 1>
+__global__ void __launch_bounds__(WARPS_N* WARPS_M * 32, MINB)
+k1_kernel(const __grid_constant__ K1Args p) {
+  k1_body<BN, BM, WARPS_N, WARPS_M, STAGES, B_KFAST, A_KFAST>(p, p.A, p.B, p.C);
+}
+
+// blockIdx.y = instance; C is the result or the split-K partials, whose instance stride differs from A's and B's
+template <int BN, int BM, int WARPS_N, int WARPS_M, int STAGES, bool B_KFAST, bool A_KFAST, int MINB = 1>
+__global__ void __launch_bounds__(WARPS_N* WARPS_M * 32, MINB)
+k1_inst_kernel(const __grid_constant__ K1Args p, long long stride, long long c_stride) {
+  const long long z = blockIdx.y;
+  k1_body<BN, BM, WARPS_N, WARPS_M, STAGES, B_KFAST, A_KFAST>(p, inst_ptr(p.A, z * stride), inst_ptr(p.B, z * stride),
+                                                              inst_ptr(p.C, z * c_stride));
 }
 
 // ------------------------------------------------------------------------------------------
@@ -421,8 +474,10 @@ int ensure_partial(tncb_ctx* ctx, size_t elems) {
 }
 
 template <int G>
-static void launch_k0_g(dim3 grid, cudaStream_t st, const double2* A, const double2* B, double2* dst, const K0Args& a) {
-  k0_kernel<G><<<grid, K0_THREADS, 0, st>>>(A, B, dst, a);
+static void launch_k0_g(dim3 grid, cudaStream_t st, const double2* A, const double2* B, double2* dst, const K0Args& a,
+                        long long stride) {
+  if (grid.z == 1) k0_kernel<G><<<grid, K0_THREADS, 0, st>>>(A, B, dst, a);
+  else k0_inst_kernel<G><<<grid, K0_THREADS, 0, st>>>(A, B, dst, a, stride);
 }
 
 // K0 launch geometry: G lanes per output, ksplit K ranges (deterministic two-pass reduction)
@@ -449,7 +504,9 @@ size_t k0_partial_elems(int sm_count, const PairPlan& P) {
   return ksplit > 1 ? (size_t)(P.M * P.N * ksplit) : 0;
 }
 
-static int launch_k0(tncb_ctx* ctx, const PairPlan& P, const double2* A, const double2* B, double2* C) {
+// count > 1: the same pair of `count` instances `stride` bytes apart in one launch (grid.z); their split-K partials then
+// live in each instance's copy of the plan scratch, which moves with the same stride
+static int launch_k0(tncb_ctx* ctx, const PairPlan& P, const double2* A, const double2* B, double2* C, int count, long long stride) {
   K0Args a;
   a.m = P.m; a.n = P.n; a.k = P.k; a.M = P.M; a.N = P.N; a.K = P.K;
   const long long MN = P.M * P.N;
@@ -461,6 +518,7 @@ static int launch_k0(tncb_ctx* ctx, const PairPlan& P, const double2* A, const d
       if ((size_t)(MN * ksplit) > ctx->partial_override_elems) return fail(TNCB_ERR_INVALID, "graph scratch too small");
       dst = ctx->partial_override;
     } else {
+      if (count > 1) return fail(TNCB_ERR_INVALID, "batched K0 split-K needs the plan's scratch");
       int rc = ensure_partial(ctx, (size_t)(MN * ksplit));
       if (rc) return rc;
       dst = ctx->partial;
@@ -469,19 +527,21 @@ static int launch_k0(tncb_ctx* ctx, const PairPlan& P, const double2* A, const d
   const long long per_block = K0_THREADS / G;
   const long long blocks = (MN + per_block - 1) / per_block;
   if (blocks > 0x7fffffffLL) return fail(TNCB_ERR_UNSUPPORTED, "K0 grid too large");
-  dim3 grid((unsigned)blocks, (unsigned)ksplit);
+  dim3 grid((unsigned)blocks, (unsigned)ksplit, (unsigned)count);
   switch (G) {
-    case 1: launch_k0_g<1>(grid, ctx->stream, A, B, dst, a); break;
-    case 2: launch_k0_g<2>(grid, ctx->stream, A, B, dst, a); break;
-    case 4: launch_k0_g<4>(grid, ctx->stream, A, B, dst, a); break;
-    case 8: launch_k0_g<8>(grid, ctx->stream, A, B, dst, a); break;
-    case 16: launch_k0_g<16>(grid, ctx->stream, A, B, dst, a); break;
-    default: launch_k0_g<32>(grid, ctx->stream, A, B, dst, a); break;
+    case 1: launch_k0_g<1>(grid, ctx->stream, A, B, dst, a, stride); break;
+    case 2: launch_k0_g<2>(grid, ctx->stream, A, B, dst, a, stride); break;
+    case 4: launch_k0_g<4>(grid, ctx->stream, A, B, dst, a, stride); break;
+    case 8: launch_k0_g<8>(grid, ctx->stream, A, B, dst, a, stride); break;
+    case 16: launch_k0_g<16>(grid, ctx->stream, A, B, dst, a, stride); break;
+    default: launch_k0_g<32>(grid, ctx->stream, A, B, dst, a, stride); break;
   }
   ctx->launches++;
-  ctx->engine_count[ksplit > 1 ? 1 : 0]++;
+  ctx->engine_count[ksplit > 1 ? 1 : 0] += (uint64_t)count;
   if (ksplit > 1) {
-    reduce_partials_kernel<<<(unsigned)((MN + 255) / 256), 256, 0, ctx->stream>>>(dst, C, MN, (int)ksplit);
+    const unsigned rblocks = (unsigned)((MN + 255) / 256);
+    if (count == 1) reduce_partials_kernel<<<rblocks, 256, 0, ctx->stream>>>(dst, C, MN, (int)ksplit);
+    else reduce_partials_inst_kernel<<<dim3(rblocks, (unsigned)count), 256, 0, ctx->stream>>>(dst, C, MN, (int)ksplit, stride, stride);
     ctx->launches++;
   }
   TNCB_CUDA(cudaGetLastError());
@@ -505,8 +565,8 @@ __device__ __forceinline__ long long decomp_c(long long idx, const CompactLegs& 
   return off;
 }
 
-__global__ void __launch_bounds__(K0_THREADS)
-k0_batch_kernel(const K0BatchItem* __restrict__ items, const int* __restrict__ block_start, int n_items, char* __restrict__ ws) {
+__device__ __forceinline__ void
+k0_batch_body(const K0BatchItem* __restrict__ items, const int* __restrict__ block_start, int n_items, char* __restrict__ ws) {
   int lo = 0, hi = n_items;
   while (hi - lo > 1) {
     const int mid = (lo + hi) >> 1;
@@ -546,6 +606,18 @@ k0_batch_kernel(const K0BatchItem* __restrict__ items, const int* __restrict__ b
   if (valid && lane_g == 0) reinterpret_cast<double2*>(ws + it.offC)[o] = make_double2(cr, ci);
 }
 
+__global__ void __launch_bounds__(K0_THREADS)
+k0_batch_kernel(const K0BatchItem* __restrict__ items, const int* __restrict__ block_start, int n_items, char* __restrict__ ws) {
+  k0_batch_body(items, block_start, n_items, ws);
+}
+
+// blockIdx.y = instance: the item offsets are workspace-relative, so only the workspace base moves
+__global__ void __launch_bounds__(K0_THREADS)
+k0_batch_inst_kernel(const K0BatchItem* __restrict__ items, const int* __restrict__ block_start, int n_items,
+                     char* __restrict__ ws, long long stride) {
+  k0_batch_body(items, block_start, n_items, ws + (long long)blockIdx.y * stride);
+}
+
 static bool compact_ok(const LegList& L) { return L.n <= kBatchGroups; }
 static void compact_fill(const LegList& L, CompactLegs& C) {
   C.n = L.n; C._pad = 0;
@@ -570,32 +642,38 @@ int k0_batch_fill(int sm_count, const PairPlan& P, K0BatchItem* it) {
   return (int)((P.M * P.N + per_block - 1) / per_block);
 }
 
-int launch_k0_batch(tncb_ctx* ctx, const K0BatchItem* d_items, const int* d_block_start, int n_items, int total_blocks, char* ws) {
+int launch_k0_batch(tncb_ctx* ctx, const K0BatchItem* d_items, const int* d_block_start, int n_items, int total_blocks, char* ws,
+                    int count, long long stride) {
   if (n_items <= 0 || total_blocks <= 0) return TNCB_OK;
-  k0_batch_kernel<<<(unsigned)total_blocks, K0_THREADS, 0, ctx->stream>>>(d_items, d_block_start, n_items, ws);
+  if (count == 1) k0_batch_kernel<<<(unsigned)total_blocks, K0_THREADS, 0, ctx->stream>>>(d_items, d_block_start, n_items, ws);
+  else k0_batch_inst_kernel<<<dim3((unsigned)total_blocks, (unsigned)count), K0_THREADS, 0, ctx->stream>>>(d_items, d_block_start, n_items, ws, stride);
   ctx->launches++;
-  ctx->engine_count[0] += (uint64_t)n_items;
+  ctx->engine_count[0] += (uint64_t)n_items * (uint64_t)count;
   TNCB_CUDA(cudaGetLastError());
   return TNCB_OK;
 }
 
+// count > 1: `count` instances in grid.y; A and B move by `stride` bytes per instance, C by `c_stride`
 template <int BN, int BM, int WN, int WM, int ST, bool BKF, bool AKF, int MINB = 1>
-static int launch_k1_cfg(tncb_ctx* ctx, const K1Args& a) {
+static int launch_k1_cfg(tncb_ctx* ctx, const K1Args& a, int count, long long stride, long long c_stride) {
   auto kern = k1_kernel<BN, BM, WN, WM, ST, BKF, AKF, MINB>;
+  auto kern_inst = k1_inst_kernel<BN, BM, WN, WM, ST, BKF, AKF, MINB>;
   const size_t smem = (size_t)ST * (BN * K1_BK + K1_BK * BM) * sizeof(double2);
-  TNCB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if (count == 1) TNCB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  else TNCB_CUDA(cudaFuncSetAttribute(kern_inst, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const long long tiles = (long long)a.tiles_m * a.tiles_n * a.ksplit;
   if (tiles > 0x7fffffffLL) return fail(TNCB_ERR_UNSUPPORTED, "K1 grid too large");
   if (ctx->time_gemm == 1) gemm_timer_begin(ctx);       // (accumulate mode collects the tcgen05 GEMMs only)
-  kern<<<(unsigned)tiles, WN * WM * 32, smem, ctx->stream>>>(a);
-  if (ctx->time_gemm == 1) gemm_timer_end(ctx, 8.0 * (double)a.M * (double)a.N * (double)a.K);
+  if (count == 1) kern<<<(unsigned)tiles, WN * WM * 32, smem, ctx->stream>>>(a);
+  else kern_inst<<<dim3((unsigned)tiles, (unsigned)count), WN * WM * 32, smem, ctx->stream>>>(a, stride, c_stride);
+  if (ctx->time_gemm == 1) gemm_timer_end(ctx, 8.0 * (double)a.M * (double)a.N * (double)a.K * count);
   ctx->launches++;
   TNCB_CUDA(cudaGetLastError());
   return TNCB_OK;
 }
 
 template <int BN, int BM, int WN, int WM, int ST, int MINB = 1>
-static int launch_k1_modes(tncb_ctx* ctx, K1Args& a, bool bkf, bool akf, bool allow_split) {
+static int launch_k1_modes(tncb_ctx* ctx, K1Args& a, bool bkf, bool akf, bool allow_split, int count, long long stride) {
   a.tiles_m = (int)((a.M + BM - 1) / BM);
   a.tiles_n = (int)((a.N + BN - 1) / BN);
   // split-K: few output tiles but a long K would leave most SMs idle (C4: M=2^8, N=2^6, K=2^20
@@ -603,38 +681,53 @@ static int launch_k1_modes(tncb_ctx* ctx, K1Args& a, bool bkf, bool akf, bool al
   // fixed order afterwards (deterministic, no atomics).
   const long long tiles = (long long)a.tiles_m * a.tiles_n;
   const int nk_total = (int)((a.K + K1_BK - 1) / K1_BK);
-  double2* final_c = a.C;
+  const double2* const A0 = a.A; const double2* const B0 = a.B;
+  double2* const final_c = a.C;
   a.ksplit = 1; a.chunks_per_split = nk_total;
   const long long want_ctas = 2LL * ctx->sm_count;
+  const long long MN = a.M * a.N;
+  // split-K is decided per instance, as for one network; the partials of a batch then run in groups of instances
+  // whose partials together stay within the same 1 GiB
+  int group = count;
   if (allow_split && tiles < want_ctas && nk_total >= 16) {
     long long ks = std::min<long long>((want_ctas + tiles - 1) / tiles, nk_total / 8);
-    const long long ws_cap = ((long long)1 << 30) / 16 / std::max(1LL, a.M * a.N); // <= 1 GiB of partials
+    const long long ws_cap = ((long long)1 << 30) / 16 / std::max(1LL, MN); // <= 1 GiB of partials
     ks = std::max(1LL, std::min(ks, ws_cap));
     if (ks > 1) {
       a.chunks_per_split = (int)((nk_total + ks - 1) / ks);
       a.ksplit = (nk_total + a.chunks_per_split - 1) / a.chunks_per_split;
-      int rc = ensure_partial(ctx, (size_t)(a.M * a.N * a.ksplit));
+      group = (int)std::max(1LL, std::min<long long>(count, ws_cap / a.ksplit));
+      int rc = ensure_partial(ctx, (size_t)(MN * a.ksplit * group));
       if (rc) return rc;
       a.C = ctx->partial;
     }
   }
-  int rc;
-  if (bkf && akf) rc = launch_k1_cfg<BN, BM, WN, WM, ST, true, true, MINB>(ctx, a);
-  else if (bkf && !akf) rc = launch_k1_cfg<BN, BM, WN, WM, ST, true, false, MINB>(ctx, a);
-  else if (!bkf && akf) rc = launch_k1_cfg<BN, BM, WN, WM, ST, false, true, MINB>(ctx, a);
-  else rc = launch_k1_cfg<BN, BM, WN, WM, ST, false, false, MINB>(ctx, a);
-  if (rc) return rc;
-  ctx->engine_count[a.ksplit > 1 ? 3 : 2]++;
-  if (a.ksplit > 1) {
-    const long long MN = a.M * a.N;
-    reduce_partials_kernel<<<(unsigned)((MN + 255) / 256), 256, 0, ctx->stream>>>(ctx->partial, final_c, MN, a.ksplit);
-    ctx->launches++;
-    TNCB_CUDA(cudaGetLastError());
+  const long long part_stride = MN * a.ksplit * (long long)sizeof(double2);
+  for (int g0 = 0; g0 < count; g0 += group) {
+    const int n = std::min(group, count - g0);
+    a.A = inst_ptr(A0, g0 * stride); a.B = inst_ptr(B0, g0 * stride);
+    double2* const c = inst_ptr(final_c, g0 * stride);
+    if (a.ksplit == 1) a.C = c;
+    const long long c_stride = a.ksplit > 1 ? part_stride : stride;
+    int rc;
+    if (bkf && akf) rc = launch_k1_cfg<BN, BM, WN, WM, ST, true, true, MINB>(ctx, a, n, stride, c_stride);
+    else if (bkf && !akf) rc = launch_k1_cfg<BN, BM, WN, WM, ST, true, false, MINB>(ctx, a, n, stride, c_stride);
+    else if (!bkf && akf) rc = launch_k1_cfg<BN, BM, WN, WM, ST, false, true, MINB>(ctx, a, n, stride, c_stride);
+    else rc = launch_k1_cfg<BN, BM, WN, WM, ST, false, false, MINB>(ctx, a, n, stride, c_stride);
+    if (rc) return rc;
+    ctx->engine_count[a.ksplit > 1 ? 3 : 2] += (uint64_t)n;
+    if (a.ksplit > 1) {
+      const unsigned rblocks = (unsigned)((MN + 255) / 256);
+      if (n == 1) reduce_partials_kernel<<<rblocks, 256, 0, ctx->stream>>>(ctx->partial, c, MN, a.ksplit);
+      else reduce_partials_inst_kernel<<<dim3(rblocks, (unsigned)n), 256, 0, ctx->stream>>>(ctx->partial, c, MN, a.ksplit, part_stride, stride);
+      ctx->launches++;
+      TNCB_CUDA(cudaGetLastError());
+    }
   }
   return TNCB_OK;
 }
 
-static int launch_k1(tncb_ctx* ctx, const PairPlan& P, const double2* A, const double2* B, double2* C) {
+static int launch_k1(tncb_ctx* ctx, const PairPlan& P, const double2* A, const double2* B, double2* C, int count, long long stride) {
   const size_t tab_elems = (size_t)(P.M + P.N + 2 * P.K);
   int rc = ensure_tab(ctx, tab_elems);
   if (rc) return rc;
@@ -661,8 +754,15 @@ static int launch_k1(tncb_ctx* ctx, const PairPlan& P, const double2* A, const d
     if (ctx->oz_engine == 0) {
       const double mnk = (double)P.M * (double)P.N * (double)P.K;
       if (force || (P.K >= ctx->crt_min_k && mnk >= ctx->crt_min_mnk)) {
+        // compute-bound: a batch runs its instances one after another on the shared offset tables; the first instance
+        // decides the engine for all of them
         int rc = launch_k1_crt(ctx, P, A, B, C, a.offAm, a.offBn, a.offAk, a.offBk);
-        if (rc != TNCB_ERR_OOM && rc != TNCB_ERR_UNSUPPORTED) return rc;   // no room for the residue planes: DMMA engine
+        if (rc != TNCB_ERR_OOM && rc != TNCB_ERR_UNSUPPORTED) {   // else no room for the residue planes: DMMA engine
+          for (int i = 1; i < count && rc == TNCB_OK; i++)
+            rc = launch_k1_crt(ctx, P, inst_ptr(A, i * stride), inst_ptr(B, i * stride), inst_ptr(C, i * stride),
+                               a.offAm, a.offBn, a.offAk, a.offBk);
+          return rc;
+        }
       }
     } else if (P.M >= 256 && P.N >= 256 && P.K >= 256) {
       const long long tiles = ((P.M + 127) / 128) * ((P.N + 127) / 128);
@@ -671,7 +771,14 @@ static int launch_k1(tncb_ctx* ctx, const PairPlan& P, const double2* A, const d
       if (force || (tiles >= ctx->oz_min_tiles && P.K >= ctx->oz_min_k) || (tiles >= 1024 && P.K >= 1024)) {
         int rc = launch_k1_ozaki(ctx, P, A, B, C, ctx->oz_slices, a.offAm, a.offBn, a.offAk, a.offBk);
         if (rc == TNCB_OK) ctx->engine_count[4]++;
-        if (rc != TNCB_ERR_OOM) return rc;   // no room for the digit planes: fall through to the DMMA engine
+        if (rc != TNCB_ERR_OOM) {   // else no room for the digit planes: fall through to the DMMA engine
+          for (int i = 1; i < count && rc == TNCB_OK; i++) {
+            rc = launch_k1_ozaki(ctx, P, inst_ptr(A, i * stride), inst_ptr(B, i * stride), inst_ptr(C, i * stride),
+                                 ctx->oz_slices, a.offAm, a.offBn, a.offAk, a.offBk);
+            if (rc == TNCB_OK) ctx->engine_count[4]++;
+          }
+          return rc;
+        }
       }
     }
   }
@@ -679,10 +786,10 @@ static int launch_k1(tncb_ctx* ctx, const PairPlan& P, const double2* A, const d
   // hide each other's per-chunk barrier/gather bubbles); TNCB_K1_VARIANT=1 selects 128x64 with
   // 4 stages and 1 CTA/SM.  Skinny outputs use a 32-wide tile on the narrow side.
   static const int variant = std::getenv("TNCB_K1_VARIANT") ? atoi(std::getenv("TNCB_K1_VARIANT")) : 0;
-  if (variant == 1) return launch_k1_modes<128, 64, 4, 2, 4, 1>(ctx, a, P.b_kfast, P.a_kfast, true);
-  if (P.N <= 32 && P.M > 32) return launch_k1_modes<32, 64, 1, 2, 2, 2>(ctx, a, P.b_kfast, P.a_kfast, true);
-  if (P.M <= 32 && P.N > 32) return launch_k1_modes<64, 32, 2, 1, 2, 2>(ctx, a, P.b_kfast, P.a_kfast, true);
-  return launch_k1_modes<64, 64, 2, 2, 2, 2>(ctx, a, P.b_kfast, P.a_kfast, true);
+  if (variant == 1) return launch_k1_modes<128, 64, 4, 2, 4, 1>(ctx, a, P.b_kfast, P.a_kfast, true, count, stride);
+  if (P.N <= 32 && P.M > 32) return launch_k1_modes<32, 64, 1, 2, 2, 2>(ctx, a, P.b_kfast, P.a_kfast, true, count, stride);
+  if (P.M <= 32 && P.N > 32) return launch_k1_modes<64, 32, 2, 1, 2, 2>(ctx, a, P.b_kfast, P.a_kfast, true, count, stride);
+  return launch_k1_modes<64, 64, 2, 2, 2, 2>(ctx, a, P.b_kfast, P.a_kfast, true, count, stride);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -713,9 +820,8 @@ __device__ __forceinline__ long long decomp_shift(long long idx, const LegList& 
 }
 
 template <int NS>
-__global__ void __launch_bounds__(256)
-k2_kernel(const double2* __restrict__ Big, const double2* __restrict__ Sml, double2* __restrict__ C,
-          const __grid_constant__ K2Args p) {
+__device__ __forceinline__ void
+k2_body(const double2* __restrict__ Big, const double2* __restrict__ Sml, double2* __restrict__ C, const K2Args& p) {
   __shared__ double2 s_s[16 * 64];     // S[s][k], s < NS, k < K <= 64 ... NS*K <= 256 guaranteed by the planner
   __shared__ long long s_kbig[64];
   const int K = (int)p.K;
@@ -762,7 +868,30 @@ k2_kernel(const double2* __restrict__ Big, const double2* __restrict__ Sml, doub
   }
 }
 
-static int launch_k2(tncb_ctx* ctx, const PairPlan& P, const double2* A, const double2* B, double2* C) {
+template <int NS>
+__global__ void __launch_bounds__(256)
+k2_kernel(const double2* __restrict__ Big, const double2* __restrict__ Sml, double2* __restrict__ C,
+          const __grid_constant__ K2Args p) {
+  k2_body<NS>(Big, Sml, C, p);
+}
+
+// blockIdx.y = instance
+template <int NS>
+__global__ void __launch_bounds__(256)
+k2_inst_kernel(const double2* __restrict__ Big, const double2* __restrict__ Sml, double2* __restrict__ C,
+               const __grid_constant__ K2Args p, long long stride) {
+  const long long io = (long long)blockIdx.y * stride;
+  k2_body<NS>(inst_ptr(Big, io), inst_ptr(Sml, io), inst_ptr(C, io), p);
+}
+
+template <int NS>
+static void launch_k2_ns(tncb_ctx* ctx, int blocks, const double2* Big, const double2* Sml, double2* C, const K2Args& a,
+                         int count, long long stride) {
+  if (count == 1) k2_kernel<NS><<<blocks, 256, 0, ctx->stream>>>(Big, Sml, C, a);
+  else k2_inst_kernel<NS><<<dim3((unsigned)blocks, (unsigned)count), 256, 0, ctx->stream>>>(Big, Sml, C, a, stride);
+}
+
+static int launch_k2(tncb_ctx* ctx, const PairPlan& P, const double2* A, const double2* B, double2* C, int count, long long stride) {
   K2Args a;
   const bool big_a = P.k2_big_is_a;
   a.big = big_a ? P.m : P.n;
@@ -780,24 +909,25 @@ static int launch_k2(tncb_ctx* ctx, const PairPlan& P, const double2* A, const d
   const int blocks = (int)std::min<long long>((a.BIG + 255) / 256, (long long)ctx->sm_count * 32);
   int ns = 1; while (ns < a.SMALL) ns *= 2;
   switch (ns) {
-    case 1: k2_kernel<1><<<blocks, 256, 0, ctx->stream>>>(Big, Sml, C, a); break;
-    case 2: k2_kernel<2><<<blocks, 256, 0, ctx->stream>>>(Big, Sml, C, a); break;
-    case 4: k2_kernel<4><<<blocks, 256, 0, ctx->stream>>>(Big, Sml, C, a); break;
-    case 8: k2_kernel<8><<<blocks, 256, 0, ctx->stream>>>(Big, Sml, C, a); break;
-    default: k2_kernel<16><<<blocks, 256, 0, ctx->stream>>>(Big, Sml, C, a); break;
+    case 1: launch_k2_ns<1>(ctx, blocks, Big, Sml, C, a, count, stride); break;
+    case 2: launch_k2_ns<2>(ctx, blocks, Big, Sml, C, a, count, stride); break;
+    case 4: launch_k2_ns<4>(ctx, blocks, Big, Sml, C, a, count, stride); break;
+    case 8: launch_k2_ns<8>(ctx, blocks, Big, Sml, C, a, count, stride); break;
+    default: launch_k2_ns<16>(ctx, blocks, Big, Sml, C, a, count, stride); break;
   }
   ctx->launches++;
-  ctx->engine_count[5]++;
+  ctx->engine_count[5] += (uint64_t)count;
   TNCB_CUDA(cudaGetLastError());
   return TNCB_OK;
 }
 
-int launch_pair(tncb_ctx* ctx, const PairPlan& P, const double2* A, const double2* B, double2* C) {
+int launch_pair(tncb_ctx* ctx, const PairPlan& P, const double2* A, const double2* B, double2* C, int count, long long stride) {
   if (P.M * P.N == 0) return TNCB_OK;
+  if (count < 1 || count > 65535) return fail(TNCB_ERR_INVALID, "instance count out of range");
   NvtxPairRange nvtx_range(P);
-  if (P.kernel_class == 2) return launch_k2(ctx, P, A, B, C);
-  if (P.kernel_class == 1) return launch_k1(ctx, P, A, B, C);
-  return launch_k0(ctx, P, A, B, C);
+  if (P.kernel_class == 2) return launch_k2(ctx, P, A, B, C, count, stride);
+  if (P.kernel_class == 1) return launch_k1(ctx, P, A, B, C, count, stride);
+  return launch_k0(ctx, P, A, B, C, count, stride);
 }
 
 // ------------------------------------------------------------------------------------------

@@ -353,6 +353,15 @@ struct OffsetAlloc {
   }
 };
 
+// one workspace for all intermediates of a run: at most 0.62 of the device (H100 80 GB: ~46 GiB; leaves room for the
+// int8 engine's 12 GiB of planes and the staged leaves), 46 GiB when the device size is unknown (plan created without a
+// context); TNCB_PLAN_WS_GB overrides.  Read on every call.
+static size_t static_ws_limit(size_t device_bytes) {
+  size_t limit = device_bytes ? (size_t)(0.62 * (double)device_bytes) : (size_t)46 << 30;
+  if (const char* e = std::getenv("TNCB_PLAN_WS_GB")) limit = (size_t)std::max(1, atoi(e)) << 30;
+  return limit;
+}
+
 static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) {
   Schedule& S = P->S;
   P->is_static = !S.steps.empty() && std::getenv("TNCB_NO_STATIC") == nullptr;
@@ -408,12 +417,7 @@ static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) 
     }
   }
   P->ws_bytes = A.top;
-  // one workspace for all intermediates of a run: at most 0.62 of the device (H100 80 GB: ~46 GiB; leaves room for the
-  // int8 engine's 12 GiB of planes and the staged leaves), 46 GiB when the device size is unknown (plan created without a
-  // context); TNCB_PLAN_WS_GB overrides
-  size_t limit = device_bytes ? (size_t)(0.62 * (double)device_bytes) : (size_t)46 << 30;
-  if (const char* e = std::getenv("TNCB_PLAN_WS_GB")) limit = (size_t)std::max(1, atoi(e)) << 30;
-  if (P->ws_bytes > limit) { P->is_static = false; return; }
+  if (P->ws_bytes > static_ws_limit(device_bytes)) { P->is_static = false; return; }
   // ---- batch descriptors ----
   P->item_first.assign(n_levels, 0); P->bs_first.assign(n_levels, 0);
   for (int l = 0; l < n_levels; l++) {
@@ -473,10 +477,10 @@ static int plan_device_state(tncb_ctx* ctx, tncb_plan* P) {
   return TNCB_OK;
 }
 
-// every kernel of the plan on the ctx stream, level by level
-static int enqueue_static(tncb_ctx* ctx, tncb_plan* P) {
+// every kernel of the plan on the ctx stream, level by level, on the workspace `ws`.  count > 1: `count` instances whose
+// workspaces (each laid out like the plan's) lie `stride` bytes apart run in every launch
+static int enqueue_static(tncb_ctx* ctx, tncb_plan* P, char* ws, int count, long long stride) {
   const Schedule& S = P->S;
-  char* ws = (char*)P->ws;
   ctx->partial_override = P->scratch_elems ? (double2*)(ws + P->scratch_off) : nullptr;
   ctx->partial_override_elems = P->scratch_elems;
   int rc = TNCB_OK;
@@ -487,12 +491,12 @@ static int enqueue_static(tncb_ctx* ctx, tncb_plan* P) {
     const int nb = P->level_batched[l];
     if (nb) {
       const int total_blocks = P->block_start[P->bs_first[l] + nb];
-      rc = launch_k0_batch(ctx, d_items + P->item_first[l], d_bs + P->bs_first[l], nb, total_blocks, ws);
+      rc = launch_k0_batch(ctx, d_items + P->item_first[l], d_bs + P->bs_first[l], nb, total_blocks, ws, count, stride);
     }
     for (int q = P->level_begin[l] + nb; q < P->level_begin[l + 1] && !rc; q++) {
       const Step& st = S.steps[q];
       rc = launch_pair(ctx, st.plan, (const double2*)(ws + P->slot_off[st.a]), (const double2*)(ws + P->slot_off[st.b]),
-                       (double2*)(ws + P->slot_off[st.out]));
+                       (double2*)(ws + P->slot_off[st.out]), count, stride);
     }
   }
   ctx->partial_override = nullptr; ctx->partial_override_elems = 0;
@@ -527,7 +531,7 @@ static int execute_static(tncb_ctx* ctx, tncb_plan* P, const tncb_tn* tn, tncb_t
       uint64_t ec_before[8]; for (int i = 0; i < 8; i++) ec_before[i] = ctx->engine_count[i];
       TNCB_CUDA(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
       if (tn) cudaMemcpyAsync(ws + P->leaf_off, P->stage, block_bytes, cudaMemcpyHostToDevice, ctx->stream);
-      rc = enqueue_static(ctx, P);
+      rc = enqueue_static(ctx, P, ws, 1, 0);
       cudaError_t ce = cudaStreamEndCapture(ctx->stream, &graph);
       P->kernels_per_run = ctx->launches - launches_before;
       ctx->launches = launches_before;
@@ -551,7 +555,7 @@ static int execute_static(tncb_ctx* ctx, tncb_plan* P, const tncb_tn* tn, tncb_t
       TNCB_CUDA(cudaEventRecord(P->stage_ev, ctx->stream));
       P->stage_busy = true;
     }
-    if ((rc = enqueue_static(ctx, P))) return rc;
+    if ((rc = enqueue_static(ctx, P, ws, 1, 0))) return rc;
   }
   tncb_tensor* result = nullptr;
   if (S.result_slot >= 0) {
@@ -774,6 +778,81 @@ int tncb_plan_run_slices(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t st
   if (out) *out = sum; else tncb_tensor_free(ctx, sum);
   if (n_out) *n_out = (int)rm.legs.size();
   if (out_legs) for (size_t i = 0; i < rm.legs.size(); i++) out_legs[i] = rm.legs[i];
+  return TNCB_OK;
+}
+
+// Instance-batched execution: the staged networks first .. first+count-1 (slices, bitstrings, angle sets of one
+// structure) are contracted each on its own, with the instance as a grid dimension of every kernel, so that one walk over
+// the schedule does the work of many networks.  A pass of c instances runs on c copies of the plan's workspace, ws_bytes
+// apart in one arena block that lives for this call only; the plan's own workspace and resident leaves stay untouched.
+// Every launch decision is the single-network one, so instance i is bit-identical to tncb_plan_run_slices(i, n_slices).
+int tncb_plan_run_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t count,
+                        tncb_tensor** out, int* n_out, uint64_t* out_legs) {
+  using namespace tncb;
+  if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
+  if (!plan->is_static) return fail(TNCB_ERR_UNSUPPORTED, "batched execution needs a plan with a static layout (no device leaves)");
+  if (!plan->slices_dev || plan->ctx != ctx) return fail(TNCB_ERR_INVALID, "tncb_plan_stage_slices has not been called on this context");
+  if (count == 0 || first > plan->n_slices || count > plan->n_slices - first)
+    return fail(TNCB_ERR_INVALID, "instances [" + std::to_string(first) + ", " + std::to_string(first + count) + ") are not within the " +
+                                  std::to_string(plan->n_slices) + " staged networks");
+  const Schedule& S = plan->S;
+  if (S.result_slot < 0) return fail(TNCB_ERR_INVALID, "plan has no result");
+  const SlotMeta& rm = S.slots[S.result_slot];
+  const int r = (int)rm.dims.size();
+  if (r + 1 > kMaxLegs) return fail(TNCB_ERR_INVALID, "a result of rank 64 leaves no room for the instance dimension");
+  TNCB_CUDA(cudaSetDevice(ctx->device));
+  size_t dev_free = 0, dev_total = 0;
+  TNCB_CUDA(cudaMemGetInfo(&dev_free, &dev_total));
+  int max_pitch = 0;
+  TNCB_CUDA(cudaDeviceGetAttribute(&max_pitch, cudaDevAttrMaxPitch, ctx->device));
+  const size_t ws = plan->ws_bytes;                      // a multiple of 256: every instance base stays aligned
+  size_t c = std::min<size_t>({static_ws_limit(dev_total) / ws, count, (size_t)65535});   // (grid.y / grid.z limit)
+  if (c == 0) return fail(TNCB_ERR_OOM, "the workspace of one instance exceeds the static-workspace limit (TNCB_PLAN_WS_GB)");
+  {
+    // the copies must also leave what the arena keeps in reserve (1 GiB) and the int8 engine's plane budget: an engine
+    // that found no room would fall back to DMMA and change the bits
+    bool int8 = false;
+    for (const Step& st : S.steps) int8 |= st.plan.kernel_class == 1 && ctx->oz_slices > 0;
+    const size_t keep = ((size_t)1 << 30) + (int8 ? ctx->crt_ws_bytes : 0);
+    const size_t room = dev_free + (ctx->arena.reserved - ctx->arena.live);
+    c = std::min(c, room > keep ? (room - keep) / ws : 0);
+    if (c == 0) return fail(TNCB_ERR_OOM, "no room on the device for the workspace of one instance");
+  }
+  std::vector<uint64_t> dims(r + 1);
+  dims[0] = count;
+  for (int i = 0; i < r; i++) dims[i + 1] = rm.dims[i];
+  tncb_tensor* res = nullptr;
+  int rc = tensor_new(ctx, r + 1, dims.data(), &res);
+  if (rc) return rc;
+  void* blk = nullptr;
+  while ((rc = ctx->arena.alloc(c * ws, &blk)) == TNCB_ERR_OOM && c > 1) c = (c + 1) / 2;   // (a fragmented arena)
+  if (rc) { tncb_tensor_free(ctx, res); return rc; }
+  const size_t blk_bytes = c * ws;
+  char* base = (char*)blk;
+  const size_t block_bytes = std::max<size_t>(S.leaf_block_elems, 1) * sizeof(double2);
+  const size_t res_bytes = rm.elems * sizeof(double2);
+  // one strided copy per pass in each direction; a workspace above the device's largest copy pitch (2 GiB) takes one
+  // copy per instance instead
+  const bool strided = ws <= (size_t)max_pitch;
+  auto copy = [&](char* dst, size_t dpitch, const char* src, size_t spitch, size_t width, size_t n) {
+    cudaError_t e = cudaSuccess;
+    if (strided) e = cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, n, cudaMemcpyDeviceToDevice, ctx->stream);
+    else for (size_t i = 0; i < n && e == cudaSuccess; i++)
+      e = cudaMemcpyAsync(dst + i * dpitch, src + i * spitch, width, cudaMemcpyDeviceToDevice, ctx->stream);
+    return e == cudaSuccess ? TNCB_OK : fail(TNCB_ERR_CUDA, std::string("batched copy: ") + cudaGetErrorString(e));
+  };
+  for (size_t done = 0; done < count && !rc; done += c) {
+    const size_t n = std::min(c, count - done);
+    const char* src = (const char*)plan->slices_dev + (first + done) * block_bytes;
+    if ((rc = copy(base + plan->leaf_off, ws, src, block_bytes, block_bytes, n))) break;
+    if ((rc = enqueue_static(ctx, plan, base, (int)n, (long long)ws))) break;
+    if (res_bytes) rc = copy((char*)res->ptr + done * res_bytes, res_bytes, base + plan->slot_off[S.result_slot], ws, res_bytes, n);
+  }
+  ctx->arena.free(blk, blk_bytes);                        // stream-ordered: the next user of the block queues behind this pass
+  if (rc) { tncb_tensor_free(ctx, res); return rc; }
+  if (out) *out = res; else tncb_tensor_free(ctx, res);
+  if (n_out) *n_out = r;
+  if (out_legs) for (int i = 0; i < r; i++) out_legs[i] = rm.legs[i];
   return TNCB_OK;
 }
 

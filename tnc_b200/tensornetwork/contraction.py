@@ -202,11 +202,23 @@ class NetworkPlan:
         return res
 
     def stage_slices(self, slice_tns) -> None:
-        """Materialise + upload the leaf blocks of every slice network once (tncb_plan_stage_slices)."""
+        """Materialise + upload the leaf blocks of many networks of the plan's structure once (tncb_plan_stage_slices):
+        slices, other bitstrings or angle sets."""
         m = _Marshal()
         nodes = [m.tn(t) for t in slice_tns]
         ptrs = (C.POINTER(TncbTn) * len(nodes))(*[C.pointer(n) for n in nodes])
         check(self.ctx._l.tncb_plan_stage_slices(self.ctx.handle, self.handle, len(nodes), ptrs))
+        self.n_staged = len(nodes)
+
+    def run_batch(self, first: int = 0, count: Optional[int] = None):
+        """Contract the staged networks first .. first + count - 1 each on its own, the instances as a grid dimension of
+        every kernel (tncb_plan_run_batch).  count=None: every staged network from `first` on.  Returns (legs of one
+        instance, DeviceTensor of shape (count, *dims)); row i is bit-identical to run_slices(first + i, n_staged)."""
+        if count is None:
+            count = max(0, getattr(self, "n_staged", 0) - int(first))
+        out, n_out, legs = C.c_void_p(), C.c_int(), u64_array([0] * 64)
+        check(self.ctx._l.tncb_plan_run_batch(self.ctx.handle, self.handle, int(first), int(count), C.byref(out), C.byref(n_out), legs))
+        return [legs[i] for i in range(n_out.value)], DeviceTensor.adopt(self.ctx, out)
 
     def run_slices(self, first: int = 0, stride: int = 1) -> Tensor:
         """Sum of the slices first, first + stride, ... on the device, no host work per slice."""
