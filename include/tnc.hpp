@@ -191,6 +191,49 @@ class NetworkPlan {
     tncb_path c_path = m.path(path);
     check(tncb_plan_create(ctx.get(), &c_tn, &c_path, &h_));
   }
+  // A gradient plan (tncb_plan_create_vjp): wrt = leaf indices in depth-first order (children in order), empty = every
+  // leaf with a payload.  stage + run (or execute) contract as a plain plan does; vjp then gives the gradients.
+  struct ForGradients { std::vector<size_t> wrt; };
+  NetworkPlan(Context& ctx, const Tensor& tn, const ContractionPath& path, const ForGradients& g) : ctx_(ctx) {
+    detail::Marshal m;
+    tncb_tn c_tn = m.tn(tn);
+    tncb_path c_path = m.path(path);
+    n_leaves_ = count_leaves(tn);
+    std::vector<uint8_t> mask(n_leaves_ ? n_leaves_ : 1, 0);
+    for (size_t i : g.wrt) {
+      if (i >= n_leaves_) throw Error(TNCB_ERR_INVALID, "wrt: leaf index out of range");
+      mask[i] = 1;
+    }
+    int n_out = 0; uint64_t legs[64];
+    res_dims_.resize(64);
+    check(tncb_network_out_legs(&c_tn, &c_path, &n_out, legs, res_dims_.data()));
+    res_dims_.resize(n_out);
+    check(tncb_plan_create_vjp(ctx.get(), &c_tn, &c_path, g.wrt.empty() ? nullptr : mask.data(), &h_));
+  }
+  // After a forward run: leaf index -> G_l (row-major in the leaf's leg order), G_l[e] = sum_r seed[r] dR[r]/dX_l[e].
+  // seed: row-major over the result's legs; empty = 1 (scalar results only).  One download of the gradient block.
+  std::map<size_t, std::vector<Complex64>> vjp(const std::vector<Complex64>& seed = {}) {
+    tncb_tensor* s = nullptr;
+    if (!seed.empty()) check(tncb_tensor_upload(ctx_.get(), (int)res_dims_.size(), res_dims_.data(), reinterpret_cast<const double*>(seed.data()), &s));
+    tncb_tensor* g = nullptr;
+    const int rc = tncb_plan_vjp(ctx_.get(), h_, s, &g);
+    if (s) tncb_tensor_free(ctx_.get(), s);
+    check(rc);
+    std::vector<Complex64> flat(tncb_tensor_elements(g));
+    const int drc = tncb_tensor_download(ctx_.get(), g, reinterpret_cast<double*>(flat.data()));
+    tncb_tensor_free(ctx_.get(), g);
+    check(drc);
+    std::vector<int64_t> off(n_leaves_ ? n_leaves_ : 1);
+    check(tncb_plan_grad_offsets(h_, off.data()));
+    std::map<size_t, std::vector<Complex64>> out;
+    for (size_t i = 0; i < n_leaves_; i++) {
+      if (off[i] < 0) continue;
+      int64_t end = (int64_t)flat.size();
+      for (size_t j = 0; j < n_leaves_; j++) if (off[j] > off[i] && off[j] < end) end = off[j];
+      out[i].assign(flat.begin() + off[i], flat.begin() + end);
+    }
+    return out;
+  }
   ~NetworkPlan() { tncb_plan_destroy(h_); }
   NetworkPlan(const NetworkPlan&) = delete;
   NetworkPlan& operator=(const NetworkPlan&) = delete;
@@ -219,8 +262,16 @@ class NetworkPlan {
     res.tensordata.device->ctx = ctx_.get(); res.tensordata.device->t = out;
     return res;
   }
+  static size_t count_leaves(const Tensor& t) {
+    if (t.is_leaf()) return 1;
+    size_t n = 0;
+    for (const Tensor& c : t.tensors) n += count_leaves(c);
+    return n;
+  }
   Context& ctx_;
   tncb_plan* h_ = nullptr;
+  size_t n_leaves_ = 0;
+  std::vector<uint64_t> res_dims_;
 };
 
 // tnc::builders (tnc/src/builders/circuit_builder.rs): Permutor (:72-129) and Circuit (:135-335).

@@ -297,9 +297,36 @@ int tncb_plan_run_slices(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t st
  * context -> TNCB_ERR_INVALID; not even one workspace copy fits -> TNCB_ERR_OOM. */
 int tncb_plan_run_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t count,
                         tncb_tensor** out, int* n_out, uint64_t* out_legs);
-/* Schedule facts: #pairs, sum 8MNK, sum 16(MK+KN+MN), peak arena bytes, #kernels. */
+/* Schedule facts: #pairs, sum 8MNK, sum 16(MK+KN+MN), peak arena bytes, #kernels.  For a gradient plan they cover the
+ * whole pass (forward + backward pairs, leaf-gradient gather) and peak_bytes is its static workspace. */
 int tncb_plan_info(const tncb_plan* plan, uint64_t* n_pairs, double* flops, double* bytes,
                    uint64_t* peak_bytes, uint64_t* n_kernels);
+/* ---- gradients with respect to the leaves (reverse mode) ----
+ * For a plan of (tn, path) with result R and a seed S shaped like R, the holomorphic vector-Jacobian product of every
+ * requested leaf X_l:   G_l[e] = sum_r S[r] * dR[r]/dX_l[e]   (plain contraction, no conjugation anywhere).  For a
+ * scalar R and S = 1, G_l is the environment of leaf l: the network contracted without it.  G_l is row-major in the
+ * leaf's OWN leg order (it has the leaf's shape).  The backward pass contracts, for every forward pair C = A.B, the
+ * adjoint of C with B (giving A's adjoint) and with A (giving B's), each of the forward pair's M*N*K volume, on the same
+ * engines; an operand gets its pair only if its subtree holds a requested leaf.  Cost: about two forward passes with
+ * every leaf requested, whatever the number of leaves.
+ * wrt: one flag per leaf (collect order: depth first, children in order); NULL = every leaf that has a payload.
+ * ctx may be NULL (host-only compile: tncb_plan_info / tncb_plan_grad_offsets).  Refused with TNCB_ERR_UNSUPPORTED:
+ * device leaves, networks without pairs, legs joining more than two tensors, and a static workspace (forward operands
+ * kept until the backward pair that reads them + adjoints) above the static-workspace limit (0.62 of the device,
+ * TNCB_PLAN_WS_GB; the message states the bytes needed).  wrt selecting no leaf, or a leaf without a payload ->
+ * TNCB_ERR_INVALID.  Gradient plans always run on their static layout (also under TNCB_TRACE), are never captured into
+ * a CUDA graph and have no pair-by-pair fallback: a workspace that does not fit at run time -> TNCB_ERR_OOM. */
+int tncb_plan_create_vjp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, const uint8_t* wrt, tncb_plan** out);
+/* After tncb_plan_stage + tncb_plan_run (or tncb_plan_execute) of this plan -- which run the forward levels only and
+ * return the result a plain plan returns, bit for bit -- the backward levels + the gather.
+ * seed: device tensor with the result's dims (else TNCB_ERR_SHAPE); NULL only for a rank-0 result (seed 1).
+ * *grads: new rank-1 device tensor holding every requested G_l back to back (tncb_plan_grad_offsets).
+ * TNCB_ERR_INVALID without such a forward run on the currently staged leaves, and for a second call after one (the
+ * backward slots reuse freed forward memory).  tncb_plan_stage_slices / run_slices / run_batch on a gradient plan ->
+ * TNCB_ERR_UNSUPPORTED.  Errors leave the arena as they found it. */
+int tncb_plan_vjp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* seed, tncb_tensor** grads);
+/* Element offset of each leaf's gradient inside *grads, -1 for leaves not requested (n_leaves entries); host only. */
+int tncb_plan_grad_offsets(const tncb_plan* plan, int64_t* offsets);
 void tncb_plan_destroy(tncb_plan* plan);
 
 /* ---- HDF5 tensor files: replaces tnc::io::hdf5 (tnc/src/io/hdf5.rs), which binds libhdf5 through hdf5-metno.

@@ -108,6 +108,9 @@ SIGNATURES = {
     "tncb_plan_run_slices": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, vpp, i32p, u64p]),
     "tncb_plan_run_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, vpp, i32p, u64p]),
     "tncb_plan_info": (C.c_int, [C.c_void_p, u64p, f64p, f64p, u64p, u64p]),
+    "tncb_plan_create_vjp": (C.c_int, [C.c_void_p, C.POINTER(TncbTn), C.POINTER(TncbPath), C.POINTER(C.c_uint8), vpp]),
+    "tncb_plan_vjp": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, vpp]),
+    "tncb_plan_grad_offsets": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
     "tncb_plan_destroy": (None, [C.c_void_p]),
     "tncb_comm_unique_id": (C.c_int, [C.c_void_p]),
     "tncb_comm_init": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p]),

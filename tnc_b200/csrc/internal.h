@@ -162,6 +162,21 @@ int k0_batch_fill(int sm_count, const PairPlan& p, K0BatchItem* item);   // retu
 int launch_k0_batch(tncb_ctx* ctx, const K0BatchItem* d_items, const int* d_block_start, int n_items, int total_blocks, char* ws,
                     int count = 1, long long stride = 0);
 
+// ---- leaf gradients of a gradient plan: every requested leaf adjoint, from its workspace slot (pair output order) into
+// the packed gradient block (the leaf's own leg order), in ONE launch ----
+constexpr int kGradGroups = 8;
+struct GradItem {
+  long long src;                // byte offset of the adjoint slot in the plan workspace
+  long long dst;                // element offset of the leaf's gradient in the output block
+  long long elems;
+  int n, _pad;                  // fused leg groups in the leaf's order, outermost first
+  long long dim[kGradGroups];
+  long long st[kGradGroups];    // element stride of each group in the adjoint slot
+};
+constexpr int kGradThreads = 256;   // outputs per block
+int launch_grad_gather(tncb_ctx* ctx, const GradItem* d_items, const long long* d_block_start, int n_items,
+                       long long total_blocks, const char* ws, double2* out);
+
 int tensor_new(tncb_ctx* ctx, int rank, const uint64_t* dims, tncb_tensor** out);
 
 // TensorData::File leaf (hdf5io.cpp): first member of /tensors, optionally adjointed, checked against the leaf's dims

@@ -1161,4 +1161,43 @@ int launch_conj(tncb_ctx* ctx, double2* data, uint64_t elems) {
   return TNCB_OK;
 }
 
+// ------------------------------------------------------------------------------------------
+// Leaf-gradient gather (tncb_plan_vjp): a circuit network has hundreds of 2x2 / 2x2x2x2 leaves, so one K3 launch per
+// leaf would be pure launch latency.  Every requested leaf adjoint is permuted from its workspace slot (the pair engines'
+// output order) into its place in the packed gradient block (the leaf's own leg order) by ONE launch.  Each block
+// writes kGradThreads consecutive outputs of one item (coalesced writes; the tiny leaves read scattered, but they are
+// a few cache lines each) and finds its item by binary search over the prefix of block counts, as k0_batch_kernel does.
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kGradThreads)
+grad_gather_kernel(const GradItem* __restrict__ items, const long long* __restrict__ block_start, int n_items,
+                   const char* __restrict__ ws, double2* __restrict__ out) {
+  const long long b = blockIdx.x;
+  int lo = 0, hi = n_items;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(block_start + mid) <= b) lo = mid; else hi = mid;
+  }
+  const GradItem& it = items[lo];
+  const long long o = (b - __ldg(block_start + lo)) * kGradThreads + threadIdx.x;
+  if (o >= it.elems) return;
+  long long idx = o, src = 0;
+  for (int g = it.n - 1; g > 0; --g) {
+    const long long d = it.dim[g], q = idx / d;
+    src += (idx - q * d) * it.st[g];
+    idx = q;
+  }
+  if (it.n > 0) src += idx * it.st[0];
+  out[it.dst + o] = reinterpret_cast<const double2*>(ws + it.src)[src];
+}
+
+int launch_grad_gather(tncb_ctx* ctx, const GradItem* d_items, const long long* d_block_start, int n_items,
+                       long long total_blocks, const char* ws, double2* out) {
+  if (n_items <= 0 || total_blocks <= 0) return TNCB_OK;
+  if (total_blocks > 0x7fffffffLL) return fail(TNCB_ERR_UNSUPPORTED, "leaf gradients too large for one gather launch");
+  grad_gather_kernel<<<(unsigned)total_blocks, kGradThreads, 0, ctx->stream>>>(d_items, d_block_start, n_items, ws, out);
+  ctx->launches++;
+  TNCB_CUDA(cudaGetLastError());
+  return TNCB_OK;
+}
+
 } // namespace tncb

@@ -25,7 +25,8 @@ struct SlotMeta {
   int leaf_index = -1;      // >= 0: payload comes from the leaf block / a device handle
 };
 
-struct Step { int a, b, out; PairPlan plan; };
+// bw_level > 0: a backward pair of a gradient plan, on that level of the backward pass (1 = the root's backward)
+struct Step { int a, b, out; PairPlan plan; int bw_level = 0; };
 
 struct Schedule {
   std::vector<SlotMeta> slots;
@@ -325,6 +326,19 @@ struct tncb_plan {
   size_t resident_bytes = 0;
   void* slices_dev = nullptr;        // tncb_plan_stage_slices: n_slices leaf blocks, back to back
   size_t n_slices = 0, slices_bytes = 0;
+  // gradient plans (tncb_plan_create_vjp): the backward pairs follow the forward ones in S.steps and occupy the levels
+  // from n_fwd_levels on; always static, never graphed
+  bool grad = false;
+  int n_fwd_levels = 0;              // levels [0, n_fwd_levels) are the forward pass (all levels of a plain plan)
+  int seed_slot = -1;
+  std::vector<int64_t> grad_offset;  // per leaf (collect order): element offset in the gradient block, -1 = not requested
+  uint64_t grad_elems = 0;
+  std::vector<tncb::GradItem> grad_items;           // leaves the gather kernel permutes
+  std::vector<long long> grad_block_start;          // n_items + 1 prefix entries
+  struct GradPermute { int slot; int64_t dst; std::vector<int> perm; };
+  std::vector<GradPermute> grad_permutes;           // leaves with more fused groups than a GradItem holds: K3
+  void* grad_dev = nullptr; size_t grad_dev_bytes = 0;   // device copy of grad_items + grad_block_start
+  bool fwd_ready = false;            // a forward run left its state in the workspace for one tncb_plan_vjp
 };
 
 namespace tncb {
@@ -364,18 +378,23 @@ static size_t static_ws_limit(size_t device_bytes) {
 
 static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) {
   Schedule& S = P->S;
-  P->is_static = !S.steps.empty() && std::getenv("TNCB_NO_STATIC") == nullptr;
+  P->is_static = !S.steps.empty() && (P->grad || std::getenv("TNCB_NO_STATIC") == nullptr);
   for (int k : S.leaf_kind) if (k == TNCB_DATA_DEVICE) P->is_static = false;   // addresses change per call
   if (!P->is_static) return;
-  // ---- levels: a step's level is 1 + the deepest level among its operands' producers (leaves: 0) ----
+  // ---- levels: a step's level is 1 + the deepest level among its operands' producers (leaves: 0); backward pairs
+  // follow the whole forward pass on their backward level ----
   std::vector<int> slot_level(S.slots.size(), 0), step_level(S.steps.size(), 0);
   int n_levels = 0;
   for (size_t q = 0; q < S.steps.size(); q++) {
     const Step& st = S.steps[q];
+    if (st.bw_level) continue;
     step_level[q] = std::max(slot_level[st.a], slot_level[st.b]) + 1;
     slot_level[st.out] = step_level[q];
     n_levels = std::max(n_levels, step_level[q]);
   }
+  P->n_fwd_levels = n_levels;
+  for (size_t q = 0; q < S.steps.size(); q++)
+    if (S.steps[q].bw_level) { step_level[q] = P->n_fwd_levels + S.steps[q].bw_level; n_levels = std::max(n_levels, step_level[q]); }
   static const bool no_batch = std::getenv("TNCB_NO_BATCH") != nullptr;
   std::vector<size_t> order(S.steps.size());
   for (size_t q = 0; q < order.size(); q++) order[q] = q;
@@ -405,7 +424,16 @@ static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) 
   std::vector<size_t> sz(S.slots.size(), 0);
   for (size_t s2 = 0; s2 < S.slots.size(); s2++)
     if (S.slots[s2].leaf_index >= 0) P->slot_off[s2] = P->leaf_off + S.leaf_offset[S.slots[s2].leaf_index] * sizeof(double2);
+  // a slot is released after the last level that reads it: for a plain plan that is its consumer's level; a gradient
+  // plan keeps each forward operand alive until the backward pair that reads it
+  std::vector<int> last_read(S.slots.size(), -1);
+  for (int l = 0; l < n_levels; l++)
+    for (int q = P->level_begin[l]; q < P->level_begin[l + 1]; q++) last_read[S.steps[q].a] = last_read[S.steps[q].b] = l;
   for (int l = 0; l < n_levels; l++) {
+    if (P->grad && l == P->n_fwd_levels) {         // the seed, written by tncb_plan_vjp before the backward levels
+      sz[P->seed_slot] = std::max<size_t>(S.slots[P->seed_slot].elems * sizeof(double2), 16);
+      P->slot_off[P->seed_slot] = A.alloc(sz[P->seed_slot]);
+    }
     for (int q = P->level_begin[l]; q < P->level_begin[l + 1]; q++) {
       const Step& st = S.steps[q];
       sz[st.out] = std::max<size_t>(S.slots[st.out].elems * sizeof(double2), 16);
@@ -413,7 +441,7 @@ static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) 
     }
     for (int q = P->level_begin[l]; q < P->level_begin[l + 1]; q++) {
       const Step& st = S.steps[q];
-      for (int s2 : {st.a, st.b}) if (sz[s2]) { A.free(P->slot_off[s2], sz[s2]); sz[s2] = 0; }
+      for (int s2 : {st.a, st.b}) if (sz[s2] && last_read[s2] == l) { A.free(P->slot_off[s2], sz[s2]); sz[s2] = 0; }
     }
   }
   P->ws_bytes = A.top;
@@ -436,7 +464,7 @@ static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) 
     }
     P->block_start.push_back(blocks);
   }
-  P->graphable = std::getenv("TNCB_NO_GRAPH") == nullptr && P->ws_bytes <= ((size_t)1 << 30);   // graphs are for small networks
+  P->graphable = !P->grad && std::getenv("TNCB_NO_GRAPH") == nullptr && P->ws_bytes <= ((size_t)1 << 30);   // graphs are for small networks
   for (const Step& st : S.steps) if (st.plan.kernel_class == 1) { P->graphable = false; break; }   // K1/K1' use ctx-owned tables / arena scratch
 }
 
@@ -474,20 +502,27 @@ static int plan_device_state(tncb_ctx* ctx, tncb_plan* P) {
     TNCB_CUDA(cudaMemcpyAsync((char*)P->batch_dev + ib, P->block_start.data(), bb, cudaMemcpyHostToDevice, ctx->stream));
     TNCB_CUDA(cudaStreamSynchronize(ctx->stream));   // (pageable sources)
   }
+  if (!P->grad_dev && !P->grad_items.empty()) {
+    const size_t ib = P->grad_items.size() * sizeof(GradItem), bb = P->grad_block_start.size() * sizeof(long long);
+    if ((rc = ctx->arena.alloc(ib + bb, &P->grad_dev))) return rc;
+    P->grad_dev_bytes = ib + bb;
+    TNCB_CUDA(cudaMemcpyAsync(P->grad_dev, P->grad_items.data(), ib, cudaMemcpyHostToDevice, ctx->stream));
+    TNCB_CUDA(cudaMemcpyAsync((char*)P->grad_dev + ib, P->grad_block_start.data(), bb, cudaMemcpyHostToDevice, ctx->stream));
+    TNCB_CUDA(cudaStreamSynchronize(ctx->stream));
+  }
   return TNCB_OK;
 }
 
-// every kernel of the plan on the ctx stream, level by level, on the workspace `ws`.  count > 1: `count` instances whose
-// workspaces (each laid out like the plan's) lie `stride` bytes apart run in every launch
-static int enqueue_static(tncb_ctx* ctx, tncb_plan* P, char* ws, int count, long long stride) {
+// the kernels of levels [l_begin, l_end) on the ctx stream, level by level, on the workspace `ws`.  count > 1: `count`
+// instances whose workspaces (each laid out like the plan's) lie `stride` bytes apart run in every launch
+static int enqueue_static(tncb_ctx* ctx, tncb_plan* P, char* ws, int count, long long stride, int l_begin, int l_end) {
   const Schedule& S = P->S;
   ctx->partial_override = P->scratch_elems ? (double2*)(ws + P->scratch_off) : nullptr;
   ctx->partial_override_elems = P->scratch_elems;
   int rc = TNCB_OK;
   const K0BatchItem* d_items = (const K0BatchItem*)P->batch_dev;
   const int* d_bs = (const int*)((char*)P->batch_dev + P->items.size() * sizeof(K0BatchItem));
-  const int n_levels = (int)P->level_batched.size();
-  for (int l = 0; l < n_levels && !rc; l++) {
+  for (int l = l_begin; l < l_end && !rc; l++) {
     const int nb = P->level_batched[l];
     if (nb) {
       const int total_blocks = P->block_start[P->bs_first[l] + nb];
@@ -514,6 +549,7 @@ static int execute_static(tncb_ctx* ctx, tncb_plan* P, const tncb_tn* tn, tncb_t
     if ((rc = validate_leaves(S, leaves))) return rc;
   } else if (!P->leaves_resident) return fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this plan");
   if ((rc = plan_device_state(ctx, P))) return rc;
+  P->fwd_ready = false;
   const size_t block_bytes = std::max<size_t>(S.leaf_block_elems * sizeof(double2), 16);
   char* ws = (char*)P->ws;
   const int which = tn ? 0 : 1;
@@ -531,7 +567,7 @@ static int execute_static(tncb_ctx* ctx, tncb_plan* P, const tncb_tn* tn, tncb_t
       uint64_t ec_before[8]; for (int i = 0; i < 8; i++) ec_before[i] = ctx->engine_count[i];
       TNCB_CUDA(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
       if (tn) cudaMemcpyAsync(ws + P->leaf_off, P->stage, block_bytes, cudaMemcpyHostToDevice, ctx->stream);
-      rc = enqueue_static(ctx, P, ws, 1, 0);
+      rc = enqueue_static(ctx, P, ws, 1, 0, 0, P->n_fwd_levels);
       cudaError_t ce = cudaStreamEndCapture(ctx->stream, &graph);
       P->kernels_per_run = ctx->launches - launches_before;
       ctx->launches = launches_before;
@@ -555,8 +591,9 @@ static int execute_static(tncb_ctx* ctx, tncb_plan* P, const tncb_tn* tn, tncb_t
       TNCB_CUDA(cudaEventRecord(P->stage_ev, ctx->stream));
       P->stage_busy = true;
     }
-    if ((rc = enqueue_static(ctx, P, ws, 1, 0))) return rc;
+    if ((rc = enqueue_static(ctx, P, ws, 1, 0, 0, P->n_fwd_levels))) return rc;
   }
+  P->fwd_ready = P->grad;      // the forward operands the backward levels read are in the workspace now
   tncb_tensor* result = nullptr;
   if (S.result_slot >= 0) {
     const SlotMeta& rm = S.slots[S.result_slot];
@@ -567,6 +604,112 @@ static int execute_static(tncb_ctx* ctx, tncb_plan* P, const tncb_tn* tn, tncb_t
   if (n_out) *n_out = S.result_slot >= 0 ? (int)S.slots[S.result_slot].legs.size() : 0;
   if (out_legs && S.result_slot >= 0)
     for (size_t i = 0; i < S.slots[S.result_slot].legs.size(); i++) out_legs[i] = S.slots[S.result_slot].legs[i];
+  return TNCB_OK;
+}
+
+// Appends the backward pairs of a gradient plan to its forward schedule.  For C = contract(A, B) with seed-weighted
+// adjoint C̄, the adjoints are Ā = contract(C̄, B) and B̄ = contract(C̄, A): plain pairwise contractions of the forward
+// pair's M·N·K volume, planned like any other pair.  An operand gets its pair only if its subtree holds a requested
+// leaf.  build() consumes every slot exactly once, so the contraction is a tree, every adjoint is produced exactly once
+// and nothing is accumulated.  leaf_adj[l] = the slot holding leaf l's adjoint (in its pair's output leg order), -1 if
+// not requested.
+static int build_backward(tncb_plan* P, const uint8_t* wrt, std::vector<int>& leaf_adj) {
+  Schedule& S = P->S;
+  const size_t nl = S.n_leaves_total;
+  if (S.steps.empty() || S.result_slot < 0) return fail(TNCB_ERR_UNSUPPORTED, "a gradient plan needs a network with at least one pair");
+  std::vector<int> leaf_slot(nl, -1);
+  for (size_t s = 0; s < S.slots.size(); s++) if (S.slots[s].leaf_index >= 0) leaf_slot[S.slots[s].leaf_index] = (int)s;
+  std::vector<char> want(S.slots.size(), 0);        // the slot's subtree holds a requested leaf
+  bool any = false;
+  for (size_t li = 0; li < nl; li++) {
+    if (wrt ? !wrt[li] : leaf_slot[li] < 0) continue;
+    if (leaf_slot[li] < 0) return fail(TNCB_ERR_INVALID, "leaf " + std::to_string(li) + " has no payload to differentiate");
+    want[leaf_slot[li]] = 1; any = true;
+  }
+  if (!any) return fail(TNCB_ERR_INVALID, "wrt selects no leaf");
+  const size_t n_fwd = S.steps.size();
+  std::vector<int> consumer(S.slots.size(), -1);
+  for (size_t q = 0; q < n_fwd; q++) {
+    const Step& st = S.steps[q];
+    want[st.out] = want[st.a] || want[st.b];
+    consumer[st.a] = consumer[st.b] = (int)q;
+  }
+  {
+    SlotMeta seed;
+    seed.legs = S.slots[S.result_slot].legs; seed.dims = S.slots[S.result_slot].dims; seed.elems = S.slots[S.result_slot].elems;
+    S.slots.push_back(std::move(seed));
+    P->seed_slot = (int)S.slots.size() - 1;
+  }
+  std::vector<int> adj(S.slots.size(), -1), bw_level(n_fwd, 0);
+  adj[S.result_slot] = P->seed_slot;
+  for (size_t q = n_fwd; q-- > 0;) {               // consumers come after their producers: walk the tree from the root
+    const int a = S.steps[q].a, b = S.steps[q].b, out = S.steps[q].out;
+    if (!want[out]) continue;
+    bw_level[q] = out == S.result_slot ? 1 : bw_level[consumer[out]] + 1;
+    for (int x : {a, b}) {
+      if (!want[x]) continue;
+      const int other = x == a ? b : a;
+      Step bs; bs.a = adj[out]; bs.b = other; bs.bw_level = bw_level[q];
+      const SlotMeta& g = S.slots[bs.a];
+      const SlotMeta& o = S.slots[other];
+      int rc = plan_pair((int)g.legs.size(), g.legs.data(), g.dims.data(), (int)o.legs.size(), o.legs.data(), o.dims.data(), bs.plan);
+      if (rc) return rc;
+      std::vector<uint64_t> got = bs.plan.out_legs, exp = S.slots[x].legs;
+      std::sort(got.begin(), got.end()); std::sort(exp.begin(), exp.end());
+      if (got != exp) return fail(TNCB_ERR_UNSUPPORTED, "gradient plans need every leg to join at most two tensors");
+      SlotMeta m; m.legs = bs.plan.out_legs; m.dims = bs.plan.out_dims;
+      for (uint64_t d : m.dims) m.elems *= d;
+      S.slots.push_back(std::move(m));
+      bs.out = (int)S.slots.size() - 1;
+      adj[x] = bs.out;
+      S.flops += bs.plan.flops(); S.bytes += bs.plan.bytes();
+      S.steps.push_back(std::move(bs));
+    }
+  }
+  leaf_adj.assign(nl, -1);
+  P->grad_offset.assign(nl, -1);
+  P->grad_elems = 0;
+  for (size_t li = 0; li < nl; li++)
+    if (leaf_slot[li] >= 0 && want[leaf_slot[li]]) {
+      leaf_adj[li] = adj[leaf_slot[li]];
+      P->grad_offset[li] = (int64_t)P->grad_elems;
+      P->grad_elems += S.slots[leaf_slot[li]].elems;
+    }
+  return TNCB_OK;
+}
+
+// The gather items of the leaf adjoints (after the layout fixed their slots): fused leg groups in the leaf's order with
+// the adjoint slot's strides.  A leaf that needs more groups than a GradItem holds goes through launch_permute (K3).
+static int build_gather(tncb_plan* P, const std::vector<int>& leaf_adj) {
+  const Schedule& S = P->S;
+  long long blocks = 0;
+  for (const SlotMeta& leaf : S.slots) {
+    if (leaf.leaf_index < 0 || leaf_adj[leaf.leaf_index] < 0 || leaf.elems == 0) continue;
+    const int gs = leaf_adj[leaf.leaf_index];
+    const SlotMeta& g = S.slots[gs];
+    const int r = (int)leaf.legs.size();
+    std::vector<long long> gst(r);
+    { long long s = 1; for (int j = r - 1; j >= 0; j--) { gst[j] = s; s *= (long long)g.dims[j]; } }
+    std::vector<int> perm(r);
+    for (int i = 0; i < r; i++) perm[i] = (int)(std::find(g.legs.begin(), g.legs.end(), leaf.legs[i]) - g.legs.begin());
+    GradItem it{};
+    it.src = (long long)P->slot_off[gs]; it.dst = P->grad_offset[leaf.leaf_index]; it.elems = (long long)leaf.elems;
+    bool fits = true;
+    for (int i = 0; i < r && fits; i++) {
+      const long long d = (long long)leaf.dims[i], st = gst[perm[i]];
+      if (d == 1) continue;
+      if (it.n > 0 && it.st[it.n - 1] == st * d) { it.dim[it.n - 1] *= d; it.st[it.n - 1] = st; continue; }
+      if (it.n == kGradGroups) { fits = false; break; }
+      it.dim[it.n] = d; it.st[it.n] = st; it.n++;
+    }
+    if (!fits) { P->grad_permutes.push_back({gs, it.dst, perm}); continue; }
+    for (int k = it.n; k < kGradGroups; k++) { it.dim[k] = 1; it.st[k] = 0; }
+    P->grad_items.push_back(it);
+    P->grad_block_start.push_back(blocks);
+    blocks += (it.elems + kGradThreads - 1) / kGradThreads;
+  }
+  P->grad_block_start.push_back(blocks);
+  if (blocks > 0x7fffffffLL) return fail(TNCB_ERR_UNSUPPORTED, "leaf gradients too large for one gather launch");
   return TNCB_OK;
 }
 
@@ -660,8 +803,89 @@ int tncb_plan_create(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, tn
   return TNCB_OK;
 }
 
+// A gradient plan: the forward schedule, the backward pairs of the `wrt` leaves and the leaf-gradient gather, in one
+// static layout.  There is no pair-by-pair fallback: a layout above the static-workspace limit is refused here.
+int tncb_plan_create_vjp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, const uint8_t* wrt, tncb_plan** out) {
+  if (!tn || !out) return tncb::fail(TNCB_ERR_INVALID, "null argument");
+  {
+    std::vector<const tncb_tn*> lv;
+    tncb::collect_leaf_nodes(tn, lv);
+    for (const tncb_tn* l : lv)
+      if (l->kind == TNCB_DATA_DEVICE) return tncb::fail(TNCB_ERR_UNSUPPORTED, "gradient plans do not take device leaves (they are consumed per call)");
+  }
+  tncb_plan* p = new tncb_plan();
+  p->grad = true;
+  std::vector<int> leaf_adj;
+  int rc = tncb::build_schedule(tn, path, p->S);
+  if (!rc) rc = tncb::build_backward(p, wrt, leaf_adj);
+  if (rc) { delete p; return rc; }
+  size_t dev_free = 0, dev_total = 0;
+  if (ctx) { cudaSetDevice(ctx->device); if (cudaMemGetInfo(&dev_free, &dev_total) != cudaSuccess) { dev_total = 0; cudaGetLastError(); } }
+  tncb::plan_static_layout(p, ctx ? ctx->sm_count : 132, dev_total);
+  if (!p->is_static) {
+    const size_t need = p->ws_bytes, limit = tncb::static_ws_limit(dev_total);
+    delete p;
+    return tncb::fail(TNCB_ERR_UNSUPPORTED, "the gradient workspace needs " + std::to_string(need) + " bytes, above the static-workspace limit of " +
+                                           std::to_string(limit) + " bytes (TNCB_PLAN_WS_GB)");
+  }
+  if ((rc = tncb::build_gather(p, leaf_adj))) { delete p; return rc; }
+  *out = p;
+  return TNCB_OK;
+}
+
+int tncb_plan_grad_offsets(const tncb_plan* plan, int64_t* offsets) {
+  if (!plan || !offsets) return tncb::fail(TNCB_ERR_INVALID, "null argument");
+  if (!plan->grad) return tncb::fail(TNCB_ERR_INVALID, "not a gradient plan (tncb_plan_create_vjp)");
+  for (size_t i = 0; i < plan->grad_offset.size(); i++) offsets[i] = plan->grad_offset[i];
+  return TNCB_OK;
+}
+
+// The backward levels and the leaf-gradient gather of a gradient plan, on the forward state its last run left in the
+// workspace.  The backward slots reuse freed forward memory, so one forward run serves one call.
+int tncb_plan_vjp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* seed, tncb_tensor** grads) {
+  using namespace tncb;
+  if (!ctx || !plan || !grads) return fail(TNCB_ERR_INVALID, "null argument");
+  if (!plan->grad) return fail(TNCB_ERR_INVALID, "not a gradient plan (tncb_plan_create_vjp)");
+  if (plan->ctx != ctx || !plan->fwd_ready)
+    return fail(TNCB_ERR_INVALID, "tncb_plan_vjp needs a forward run (tncb_plan_run / tncb_plan_execute) of the plan on this context "
+                                  "since its leaves were staged or its last tncb_plan_vjp");
+  const Schedule& S = plan->S;
+  const SlotMeta& rm = S.slots[S.result_slot];
+  if (seed) {
+    bool same = seed->rank == (int)rm.dims.size();
+    for (int i = 0; same && i < seed->rank; i++) same = seed->dims[i] == rm.dims[i];
+    if (!same) return fail(TNCB_ERR_SHAPE, "the seed's dims differ from the result's");
+    if (!seed->ptr) return fail(TNCB_ERR_UNCONTRACTED, "the seed tensor has no storage");
+  } else if (!rm.dims.empty()) return fail(TNCB_ERR_INVALID, "a seed is needed for a result of rank " + std::to_string(rm.dims.size()));
+  TNCB_CUDA(cudaSetDevice(ctx->device));
+  const uint64_t n = plan->grad_elems;
+  tncb_tensor* g = nullptr;
+  int rc = tensor_new(ctx, 1, &n, &g);
+  if (rc) return rc;
+  char* ws = (char*)plan->ws;
+  static const double2 one = {1.0, 0.0};
+  cudaError_t ce = seed ? cudaMemcpyAsync(ws + plan->slot_off[plan->seed_slot], seed->ptr, rm.elems * sizeof(double2), cudaMemcpyDeviceToDevice, ctx->stream)
+                        : cudaMemcpyAsync(ws + plan->slot_off[plan->seed_slot], &one, sizeof(double2), cudaMemcpyHostToDevice, ctx->stream);
+  if (ce != cudaSuccess) rc = fail(TNCB_ERR_CUDA, std::string("seed copy: ") + cudaGetErrorString(ce));
+  plan->fwd_ready = false;
+  if (!rc) rc = enqueue_static(ctx, plan, ws, 1, 0, plan->n_fwd_levels, (int)plan->level_batched.size());
+  if (!rc && !plan->grad_items.empty())
+    rc = launch_grad_gather(ctx, (const GradItem*)plan->grad_dev,
+                            (const long long*)((char*)plan->grad_dev + plan->grad_items.size() * sizeof(GradItem)),
+                            (int)plan->grad_items.size(), plan->grad_block_start.back(), ws, g->ptr);
+  for (size_t i = 0; i < plan->grad_permutes.size() && !rc; i++) {
+    const auto& gp = plan->grad_permutes[i];
+    const SlotMeta& sm = S.slots[gp.slot];
+    rc = launch_permute(ctx, (const double2*)(ws + plan->slot_off[gp.slot]), g->ptr + gp.dst, (int)sm.dims.size(), sm.dims.data(), gp.perm.data());
+  }
+  if (rc) { tncb_tensor_free(ctx, g); return rc; }
+  *grads = g;
+  return TNCB_OK;
+}
+
 int tncb_plan_execute(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tn, tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   if (!ctx || !plan || !tn) return tncb::fail(TNCB_ERR_INVALID, "null argument");
+  if (plan->grad) return tncb::execute_static(ctx, plan, tn, out, n_out, out_legs);   // forward levels only, no fallback
   static const bool trace = std::getenv("TNCB_TRACE") != nullptr;   // per-step times come from the pair-by-pair executor
   if (plan->is_static && !trace && (plan->ctx == nullptr || plan->ctx == ctx)) {
     int rc = tncb::execute_static(ctx, plan, tn, out, n_out, out_legs);
@@ -687,10 +911,11 @@ int tncb_plan_stage(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tn) {
   const size_t bytes = std::max<size_t>(S.leaf_block_elems * sizeof(double2), 16);
   std::vector<std::complex<double>> host(std::max<size_t>(S.leaf_block_elems, 1));
   if (plan->is_static && (rc = tncb::plan_device_state(ctx, plan))) {
-    if (rc != TNCB_ERR_OOM || plan->ws) return rc;
+    if (rc != TNCB_ERR_OOM || plan->ws || plan->grad) return rc;
     plan->is_static = false;    // the static workspace does not fit: resident leaf block + pair-by-pair executor
   }
   if (plan->is_static) {      // the leaf block lives inside the plan workspace
+    plan->fwd_ready = false;
     TNCB_CUDA(cudaStreamSynchronize(ctx->stream));
     if ((rc = tncb::stage_leaves(S, leaves, (std::complex<double>*)plan->stage))) return rc;
     TNCB_CUDA(cudaMemcpyAsync((char*)plan->ws + plan->leaf_off, plan->stage, bytes, cudaMemcpyHostToDevice, ctx->stream));
@@ -713,7 +938,7 @@ int tncb_plan_run(tncb_ctx* ctx, tncb_plan* plan, tncb_tensor** out, int* n_out,
   if (!ctx || !plan) return tncb::fail(TNCB_ERR_INVALID, "null argument");
   static const bool trace = std::getenv("TNCB_TRACE") != nullptr;
   if (plan->is_static && plan->leaves_resident && plan->ctx == ctx) {
-    if (!trace) return tncb::execute_static(ctx, plan, nullptr, out, n_out, out_legs);
+    if (!trace || plan->grad) return tncb::execute_static(ctx, plan, nullptr, out, n_out, out_legs);
     return tncb::execute(ctx, plan->S, nullptr, out, n_out, out_legs, (const double2*)((char*)plan->ws + plan->leaf_off));
   }
   if (!plan->resident || plan->ctx != ctx) return tncb::fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this context");
@@ -726,6 +951,7 @@ int tncb_plan_run(tncb_ctx* ctx, tncb_plan* plan, tncb_tensor** out, int* n_out,
 // block (KBs), the plan's kernels (batched / graph as usual), one accumulation kernel.
 int tncb_plan_stage_slices(tncb_ctx* ctx, tncb_plan* plan, size_t n_slices, const tncb_tn* const* slice_tns) {
   if (!ctx || !plan || !slice_tns || n_slices == 0) return tncb::fail(TNCB_ERR_INVALID, "null argument");
+  if (plan->grad) return tncb::fail(TNCB_ERR_UNSUPPORTED, "gradient plans run one staged network at a time");
   if (!plan->is_static) return tncb::fail(TNCB_ERR_UNSUPPORTED, "sliced execution needs a plan with a static layout (no device leaves)");
   const tncb::Schedule& S = plan->S;
   TNCB_CUDA(cudaSetDevice(ctx->device));
@@ -752,6 +978,7 @@ int tncb_plan_stage_slices(tncb_ctx* ctx, tncb_plan* plan, size_t n_slices, cons
 
 int tncb_plan_run_slices(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t stride, tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   if (!ctx || !plan || stride == 0) return tncb::fail(TNCB_ERR_INVALID, "bad argument");
+  if (plan->grad) return tncb::fail(TNCB_ERR_UNSUPPORTED, "gradient plans run one staged network at a time");
   if (!plan->slices_dev || plan->ctx != ctx) return tncb::fail(TNCB_ERR_INVALID, "tncb_plan_stage_slices has not been called on this context");
   const tncb::Schedule& S = plan->S;
   if (S.result_slot < 0) return tncb::fail(TNCB_ERR_INVALID, "plan has no result");
@@ -790,6 +1017,7 @@ int tncb_plan_run_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
                         tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   using namespace tncb;
   if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
+  if (plan->grad) return fail(TNCB_ERR_UNSUPPORTED, "gradient plans run one staged network at a time");
   if (!plan->is_static) return fail(TNCB_ERR_UNSUPPORTED, "batched execution needs a plan with a static layout (no device leaves)");
   if (!plan->slices_dev || plan->ctx != ctx) return fail(TNCB_ERR_INVALID, "tncb_plan_stage_slices has not been called on this context");
   if (count == 0 || first > plan->n_slices || count > plan->n_slices - first)
@@ -845,7 +1073,7 @@ int tncb_plan_run_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
     const size_t n = std::min(c, count - done);
     const char* src = (const char*)plan->slices_dev + (first + done) * block_bytes;
     if ((rc = copy(base + plan->leaf_off, ws, src, block_bytes, block_bytes, n))) break;
-    if ((rc = enqueue_static(ctx, plan, base, (int)n, (long long)ws))) break;
+    if ((rc = enqueue_static(ctx, plan, base, (int)n, (long long)ws, 0, (int)plan->level_batched.size()))) break;
     if (res_bytes) rc = copy((char*)res->ptr + done * res_bytes, res_bytes, base + plan->slot_off[S.result_slot], ws, res_bytes, n);
   }
   ctx->arena.free(blk, blk_bytes);                        // stream-ordered: the next user of the block queues behind this pass
@@ -880,7 +1108,8 @@ int tncb_plan_info(const tncb_plan* plan, uint64_t* n_pairs, double* flops, doub
   if (n_pairs) *n_pairs = S.steps.size();
   if (flops) *flops = S.flops;
   if (bytes) *bytes = S.bytes;
-  if (peak_bytes) { // replay the liveness: leaves + live intermediates
+  if (peak_bytes && plan->grad) *peak_bytes = plan->ws_bytes;   // the whole pass lives in its static workspace
+  else if (peak_bytes) { // replay the liveness: leaves + live intermediates
     size_t live = S.leaf_block_elems * 16, peak = live;
     std::vector<size_t> sz(S.slots.size(), 0);
     for (const tncb::Step& st : S.steps) {
@@ -894,7 +1123,8 @@ int tncb_plan_info(const tncb_plan* plan, uint64_t* n_pairs, double* flops, doub
     uint64_t k = 0;
     for (const tncb::Step& st : S.steps) k += st.plan.kernel_class == 1 ? 2 : 1;  // (K1: table build + GEMM)
     for (int nb : plan->level_batched) if (nb) k -= (uint64_t)(nb - 1);            // a batch is one launch
-    *n_kernels = k;
+    if (!plan->grad_items.empty()) k++;                                            // the leaf-gradient gather
+    *n_kernels = k + 2 * plan->grad_permutes.size();                               // (K3: tables + transpose)
   }
   return TNCB_OK;
 }
@@ -908,6 +1138,8 @@ void tncb_plan_release_device_state(tncb_plan* plan) {
   cudaStreamSynchronize(ctx->stream);
   for (int i = 0; i < 2; i++) if (plan->exec[i]) { cudaGraphExecDestroy(plan->exec[i]); plan->exec[i] = nullptr; }
   if (plan->batch_dev) { ctx->arena.free(plan->batch_dev, plan->batch_bytes); plan->batch_dev = nullptr; }
+  if (plan->grad_dev) { ctx->arena.free(plan->grad_dev, plan->grad_dev_bytes); plan->grad_dev = nullptr; }
+  plan->fwd_ready = false;
   if (plan->slices_dev) { ctx->arena.free(plan->slices_dev, plan->slices_bytes); plan->slices_dev = nullptr; plan->n_slices = 0; }
   plan->leaves_resident = false;
   if (plan->ws) { ctx->arena.free(plan->ws, plan->ws_bytes); plan->ws = nullptr; }

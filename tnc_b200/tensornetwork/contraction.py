@@ -167,6 +167,14 @@ def contract_tensor_network(tn: Tensor, contract_path: ContractionPath, ctx: Opt
     return res
 
 
+def leaves(tn: Tensor) -> List[Tensor]:
+    """The leaves of `tn` depth first, children in order: the leaf order that gradient plans' `wrt` and their gradients
+    are indexed by."""
+    if not tn.tensors:
+        return [tn]
+    return [leaf for child in tn.tensors for leaf in leaves(child)]
+
+
 class NetworkPlan:
     """Compile once / execute many (tncb_plan_*): same structure, new payloads."""
 
@@ -177,6 +185,58 @@ class NetworkPlan:
         h = C.c_void_p()
         check(self.ctx._l.tncb_plan_create(self.ctx.handle, C.byref(c_tn), C.byref(c_path), C.byref(h)))
         self.handle = h
+
+    @classmethod
+    def for_gradients(cls, tn: Tensor, contract_path: ContractionPath, wrt=None, ctx: Optional[Context] = None) -> "NetworkPlan":
+        """A gradient plan (tncb_plan_create_vjp): `stage` + `run` (or `execute`) contract the network as a plain plan
+        does, then `vjp` returns the gradient of the result with respect to the leaves `wrt` (indices into
+        `leaves(tn)`; None = every leaf with a payload) in one backward pass."""
+        self = cls.__new__(cls)
+        self.handle = None
+        self.ctx = ctx or default_context()
+        shapes = [tuple(int(d) for d in leaf.bond_dims) for leaf in leaves(tn)]
+        mask = None
+        if wrt is not None:
+            mask = (C.c_uint8 * max(len(shapes), 1))()
+            for i in wrt:
+                if not 0 <= int(i) < len(shapes):
+                    raise IndexError(f"leaf index {i} out of range ({len(shapes)} leaves)")
+                mask[int(i)] = 1
+        m = _Marshal()
+        c_tn, c_path = m.tn(tn), m.path(contract_path)
+        h = C.c_void_p()
+        check(self.ctx._l.tncb_plan_create_vjp(self.ctx.handle, C.byref(c_tn), C.byref(c_path), mask, C.byref(h)))
+        self.handle = h
+        self.leaf_shapes = shapes
+        return self
+
+    def grad_offsets(self) -> List[int]:
+        """Element offset of every leaf's gradient in the block `vjp` downloads, -1 for leaves not requested."""
+        offs = (C.c_int64 * max(len(self.leaf_shapes), 1))()
+        check(self.ctx._l.tncb_plan_grad_offsets(self.handle, offs))
+        return [offs[i] for i in range(len(self.leaf_shapes))]
+
+    def vjp(self, seed=None) -> dict:
+        """After a forward `run`/`execute` of a gradient plan: {leaf index: G} for every requested leaf, G shaped like
+        the leaf with G[e] = sum_r seed[r] dR[r]/dX[e] (no conjugation).  seed: array or DeviceTensor with the result's
+        shape; None for a scalar result (seed 1).  One device-to-host copy of the whole gradient block."""
+        tmp = None
+        if seed is not None and not isinstance(seed, DeviceTensor):
+            seed = tmp = DeviceTensor.from_numpy(self.ctx, np.asarray(seed, dtype=np.complex128))
+        out = C.c_void_p()
+        try:
+            check(self.ctx._l.tncb_plan_vjp(self.ctx.handle, self.handle, seed.handle if seed is not None else None, C.byref(out)))
+        finally:
+            if tmp is not None:
+                tmp.free()
+        block = DeviceTensor.adopt(self.ctx, out)
+        flat = block.to_numpy()
+        block.free()
+        grads = {}
+        for i, (off, shape) in enumerate(zip(self.grad_offsets(), self.leaf_shapes)):
+            if off >= 0:
+                grads[i] = flat[off:off + int(np.prod(shape, dtype=np.int64))].reshape(shape)
+        return grads
 
     def info(self) -> dict:
         n, k = C.c_uint64(), C.c_uint64()
