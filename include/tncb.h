@@ -325,8 +325,40 @@ int tncb_plan_create_vjp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path
  * backward slots reuse freed forward memory).  tncb_plan_stage_slices / run_slices / run_batch on a gradient plan ->
  * TNCB_ERR_UNSUPPORTED.  Errors leave the arena as they found it. */
 int tncb_plan_vjp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* seed, tncb_tensor** grads);
-/* Element offset of each leaf's gradient inside *grads, -1 for leaves not requested (n_leaves entries); host only. */
+/* Element offset of each leaf's gradient inside *grads, -1 for leaves not requested (n_leaves entries); host only.
+ * For a sliced gradient plan the offsets pack the FULL leaves' shapes. */
 int tncb_plan_grad_offsets(const tncb_plan* plan, int64_t* offsets);
+/* ---- sliced gradients: networks whose gradient workspace does not fit unsliced ----
+ * Fixing the sliced legs splits R into slices, R = sum_q R_q, so dR/dX_l = sum_q dR_q/dX_l; a slice leaf is a
+ * fixed-index sub-block of the full leaf, so its adjoint adds into that sub-block of the full gradient.
+ * tn is the FULL network and `path` the path every slice uses (slicing removes legs, not leaves).  The slice structure
+ * (every leaf without the sliced legs; a leaf may become rank 0) is compiled exactly as tncb_plan_create_vjp compiles the
+ * host-sliced slice network: the same pairs, backward schedule, static layout and refusals; tncb_plan_info covers one
+ * slice's pass (with its leaf extraction and gradient accumulation launches) and peak_bytes is the per-slice workspace.
+ * Slice q is the row-major mixed-radix digit vector of q over sliced_legs in the order given, last leg fastest.  wrt
+ * indexes the full network's leaves (collect order).  ctx may be NULL (host-only compile).  A sliced leg that does not
+ * occur, occurs once (an open leg), has dimension 0 or is listed twice, and a slice count above 2^64 - 1 ->
+ * TNCB_ERR_INVALID; a leaf carrying more than 8 sliced legs, or needing more than 8 leg groups to address its slices ->
+ * TNCB_ERR_UNSUPPORTED.
+ * Use: tncb_plan_stage(ctx, plan, full tn) validates against the full structure and uploads the full leaf block once
+ * into a plan-owned block outside the workspace (re-staging replaces it); tncb_plan_run_slices(ctx, plan, first,
+ * stride, ...) runs the forward levels of slices first, first+stride, ... and returns their sum, bit-identical to a
+ * plain plan of the host-sliced networks staged with tncb_plan_stage_slices; tncb_plan_vjp_sliced adds the backward.
+ * tncb_plan_run / tncb_plan_execute / tncb_plan_vjp / tncb_plan_stage_slices / tncb_plan_run_batch on such a plan ->
+ * TNCB_ERR_UNSUPPORTED. */
+int tncb_plan_create_vjp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, size_t n_sliced,
+                                const uint64_t* sliced_legs, const uint8_t* wrt, tncb_plan** out);
+/* Per slice q = first, first+stride, ...: extract q's sub-blocks of the leaves that carry a sliced leg (one launch),
+ * forward levels, seed copy, backward levels, accumulate every requested leaf adjoint into q's sub-block of its
+ * full-shape gradient (one launch).  No host work per slice; slices run in stream order, so results repeat bit for bit.
+ * seed: device tensor with the result's dims, NULL only for a rank-0 result (seed 1); the same seed for every slice.
+ * *value: new tensor, the sum of the slices' results, bit-identical to tncb_plan_run_slices(first, stride).
+ * *grads: new rank-1 tensor, every requested full-shape G_l back to back (tncb_plan_grad_offsets).  An empty range
+ * (more ranks than slices) gives zeros for both; partial ranges add up, so ranks of a multi-GPU job pass (rank, world)
+ * and run tncb_comm_allreduce_sum on both tensors.  Not staged on this context / not a sliced gradient plan / stride 0
+ * -> TNCB_ERR_INVALID; seed errors as tncb_plan_vjp.  Errors leave the arena as they found it. */
+int tncb_plan_vjp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t stride, const tncb_tensor* seed,
+                         tncb_tensor** value, tncb_tensor** grads);
 void tncb_plan_destroy(tncb_plan* plan);
 
 /* ---- HDF5 tensor files: replaces tnc::io::hdf5 (tnc/src/io/hdf5.rs), which binds libhdf5 through hdf5-metno.

@@ -5,7 +5,8 @@
     (amp.abs() ** 2).backward()                     # u3.grad, u7.grad
 
 Gate angles differentiate through ordinary torch code that builds the gate matrices; the library needs no
-angle-derivative table.  One backward pass gives the gradient of every input, at about two forward passes of cost."""
+angle-derivative table.  One backward pass gives the gradient of every input, at about two forward passes of cost.
+With `sliced_legs`, a network whose gradient workspace does not fit unsliced runs slice by slice (SlicedPlan.for_gradients)."""
 from __future__ import annotations
 
 from typing import Optional, Sequence
@@ -15,6 +16,7 @@ import torch
 
 from . import Context, default_context
 from .contractionpath import ContractionPath
+from .contractionpath.slicing import SlicedPlan
 from .tensornetwork import NetworkPlan, Tensor, leaves
 from .tensornetwork.tensordata import TensorData
 
@@ -44,17 +46,24 @@ class _NetworkFn(torch.autograd.Function):
     def backward(ctx, grad_out):
         xs = ctx.saved_tensors           # raises on a second backward through a graph that was not retained
         runner = ctx.runner
-        if runner._token != ctx.token:   # another forward (or an earlier backward) used the plan's state since
-            ctx.token = runner._forward(xs)
-        runner._token = None             # the backward levels overwrite the forward state
-        g = runner.plan.vjp(np.conj(grad_out.detach().to(torch.complex128).cpu().numpy()))
+        seed = np.conj(grad_out.detach().to(torch.complex128).cpu().numpy())
+        if runner.sliced:                # vjp_sliced re-runs every slice's forward: it only needs these inputs staged
+            if runner._token != ctx.token:
+                ctx.token = runner._stage(xs)
+            g = runner.plan.vjp(seed)[1]
+        else:
+            if runner._token != ctx.token:   # another forward (or an earlier backward) used the plan's state since
+                ctx.token = runner._forward(xs)
+            runner._token = None             # the backward levels overwrite the forward state
+            g = runner.plan.vjp(seed)
         return (None,) + tuple(torch.from_numpy(np.conj(g[i])).to(x.device) for i, x in zip(runner.wrt, xs))
 
 
 class NetworkFunction:
     """The callable network_function returns: inputs -> contracted result, differentiable in every input."""
 
-    def __init__(self, tn: Tensor, path: ContractionPath, wrt: Sequence[int], ctx: Optional[Context] = None):
+    def __init__(self, tn: Tensor, path: ContractionPath, wrt: Sequence[int], ctx: Optional[Context] = None,
+                 sliced_legs: Sequence[int] = ()):
         self.wrt = [int(i) for i in wrt]
         lv = leaves(tn)
         for i in self.wrt:
@@ -62,22 +71,31 @@ class NetworkFunction:
                 raise ValueError(f"leaf {i} is not a Matrix leaf of the network (wrt must name Matrix leaves)")
         self.shapes = [tuple(int(d) for d in lv[i].bond_dims) for i in self.wrt]
         self.tn, self.path = tn, path
-        self.plan = NetworkPlan.for_gradients(tn, path, self.wrt, ctx=ctx or default_context())
+        self.sliced = len(sliced_legs) > 0
+        if self.sliced:
+            self.plan = SlicedPlan.for_gradients(tn, path, sliced_legs, self.wrt, ctx=ctx or default_context())
+        else:
+            self.plan = NetworkPlan.for_gradients(tn, path, self.wrt, ctx=ctx or default_context())
         self._token, self._count, self._result = None, 0, None
 
-    def _forward(self, xs):
-        """stage the inputs as the wrt leaves' payloads (through the host) and run the forward levels"""
+    def _stage(self, xs):
+        """stage the inputs as the wrt leaves' payloads (through the host)"""
         pay = {}
         for i, shape, x in zip(self.wrt, self.shapes, xs):
             if tuple(x.shape) != shape:
                 raise ValueError(f"input for leaf {i} has shape {tuple(x.shape)}, the leaf {shape}")
             pay[i] = np.ascontiguousarray(x.detach().to(torch.complex128).cpu().numpy())
         self.plan.stage(_with_payloads(self.tn, pay, [0]))
-        res = self.plan.run()
-        self._result = torch.from_numpy(np.asarray(res.to_numpy()).copy())
         self._count += 1
         self._token = self._count
         return self._token
+
+    def _forward(self, xs):
+        """stage the inputs and run the forward levels (every slice's, summed, on a sliced plan)"""
+        token = self._stage(xs)
+        res = self.plan.run()
+        self._result = torch.from_numpy(np.asarray(res.to_numpy()).copy())
+        return token
 
     def __call__(self, *xs: torch.Tensor) -> torch.Tensor:
         if len(xs) != len(self.wrt):
@@ -85,7 +103,8 @@ class NetworkFunction:
         return _NetworkFn.apply(self, *xs)
 
 
-def network_function(tn: Tensor, path: ContractionPath, wrt: Sequence[int], ctx: Optional[Context] = None) -> NetworkFunction:
+def network_function(tn: Tensor, path: ContractionPath, wrt: Sequence[int], ctx: Optional[Context] = None,
+                     sliced_legs: Sequence[int] = ()) -> NetworkFunction:
     """A torch.autograd.Function over the network `tn` contracted along `path`: the returned callable takes one torch
     complex128 tensor per leaf index in `wrt` (indices into leaves(tn); each must be a Matrix leaf) and returns the
     contracted result as a torch tensor.  Its backward is conj(vjp(conj(grad_out))) of the gradient plan, torch's
@@ -94,5 +113,11 @@ def network_function(tn: Tensor, path: ContractionPath, wrt: Sequence[int], ctx:
     Forward = stage + run: the inputs are copied to the host and staged the way NetworkPlan.stage stages any payload
     (no device-side staging of torch tensors).  A backward needs the plan's forward state: when another call of the
     same function ran in between, or a retained graph is differentiated again, the backward re-runs the forward from
-    the saved inputs first.  A second backward through a graph that was not retained raises torch's error."""
-    return NetworkFunction(tn, path, wrt, ctx)
+    the saved inputs first.  A second backward through a graph that was not retained raises torch's error.
+
+    sliced_legs: legs of `tn` to slice (e.g. from contractionpath.slicing.find_slices), for networks whose gradient
+    workspace does not fit unsliced.  Forward = stage + the forward levels of every slice, summed on the device;
+    backward = SlicedPlan.vjp with the seed.  No workspace holds all slices' forward state, so the backward runs every
+    slice's forward again before its backward levels: about 4 forward passes in all, against about 3 unsliced.  The
+    backward needs only the staged inputs, so it re-stages (without a forward) when another call ran in between."""
+    return NetworkFunction(tn, path, wrt, ctx, sliced_legs)

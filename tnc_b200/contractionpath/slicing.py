@@ -165,6 +165,89 @@ class SlicedPlan:
         self.plan = NetworkPlan(nets[0], path, ctx=self.ctx)
         self.plan.stage_slices(nets)
 
+    @classmethod
+    def for_gradients(cls, tn: Tensor, path: ContractionPath, legs: Sequence[int], wrt=None, ctx=None) -> "SlicedPlan":
+        """A sliced gradient plan (tncb_plan_create_vjp_sliced): compiled for the FULL network `tn` and the legs to slice;
+        `stage(tn)` uploads the full leaves once, `run` sums the slices' results and `vjp` also returns every requested
+        leaf's gradient in the full leaf's shape, each slice extracted and accumulated on the device.  wrt: indices into
+        `leaves(tn)`; None = every leaf with a payload.  Slice q is the row-major digit vector of q over `legs`, last leg
+        fastest (the order of `slice_assignments`)."""
+        import ctypes as C
+        from .. import default_context
+        from .._lib import check, u64_array
+        from ..tensornetwork.contraction import NetworkPlan, _Marshal, leaves
+        self = cls.__new__(cls)
+        self.ctx = ctx or default_context()
+        self.sn = None
+        lv = leaves(tn)
+        shapes = [tuple(int(d) for d in leaf.bond_dims) for leaf in lv]
+        mask = None
+        if wrt is not None:
+            mask = (C.c_uint8 * max(len(shapes), 1))()
+            for i in wrt:
+                if not 0 <= int(i) < len(shapes):
+                    raise IndexError(f"leaf index {i} out of range ({len(shapes)} leaves)")
+                mask[int(i)] = 1
+        legs = [int(l) for l in legs]
+        m = _Marshal()
+        c_tn, c_path = m.tn(tn), m.path(path)
+        c_legs = u64_array(legs or [0])
+        h = C.c_void_p()
+        check(self.ctx._l.tncb_plan_create_vjp_sliced(self.ctx.handle, C.byref(c_tn), C.byref(c_path), len(legs), c_legs, mask, C.byref(h)))
+        plan = NetworkPlan.__new__(NetworkPlan)
+        plan.ctx, plan.handle, plan.leaf_shapes = self.ctx, h, shapes
+        self.plan = plan
+        self._legs = None
+        dim = {l: int(d) for t in lv for l, d in zip(t.legs, t.bond_dims)}
+        self.n_slices = int(np.prod([dim[l] for l in legs], dtype=object)) if legs else 1
+        return self
+
+    def stage(self, tn: Tensor) -> None:
+        """Upload the full network's leaves once (a sliced gradient plan); re-staging replaces them."""
+        self.plan.stage(tn)
+
+    def grad_offsets(self) -> List[int]:
+        return self.plan.grad_offsets()
+
+    def info(self) -> dict:
+        """One slice's pass: pairs, flops, bytes, peak_bytes (the per-slice workspace), kernels."""
+        return self.plan.info()
+
+    def vjp(self, seed=None, rank: int = 0, world: int = 1, allreduce: bool = True):
+        """(value, {leaf index: G}) summed over the slices rank, rank + world, ...: value is bit-identical to `run`, G has
+        the full leaf's shape with G[e] = sum_r seed[r] dR[r]/dX[e] (no conjugation).  seed: array or DeviceTensor with
+        the result's shape, None for a scalar result.  With world > 1 and allreduce, both are summed over the ranks."""
+        import ctypes as C
+        from .. import DeviceTensor
+        from .._lib import check
+        from ..tensornetwork.tensordata import TensorData
+        ctx = self.ctx
+        tmp = None
+        if seed is not None and not isinstance(seed, DeviceTensor):
+            seed = tmp = DeviceTensor.from_numpy(ctx, np.asarray(seed, dtype=np.complex128))
+        val, out = C.c_void_p(), C.c_void_p()
+        try:
+            check(ctx._l.tncb_plan_vjp_sliced(ctx.handle, self.plan.handle, int(rank), int(world),
+                                              seed.handle if seed is not None else None, C.byref(val), C.byref(out)))
+        finally:
+            if tmp is not None:
+                tmp.free()
+        value, block = DeviceTensor.adopt(ctx, val), DeviceTensor.adopt(ctx, out)
+        if world > 1 and allreduce:
+            check(ctx._l.tncb_comm_allreduce_sum(ctx.handle, value.handle))
+            check(ctx._l.tncb_comm_allreduce_sum(ctx.handle, block.handle))
+        flat = block.to_numpy()
+        block.free()
+        grads = {}
+        for i, (off, shape) in enumerate(zip(self.plan.grad_offsets(), self.plan.leaf_shapes)):
+            if off >= 0:
+                grads[i] = flat[off:off + int(np.prod(shape, dtype=np.int64))].reshape(shape)
+        if self._legs is None:        # the result's leg order: an empty slice range returns it without running a kernel
+            self._legs = list(self.plan.run_slices(self.n_slices, 1).legs)
+        res = Tensor(self._legs, value.shape)
+        res.set_tensor_data(TensorData.Matrix(value))
+        return res, grads
+
     def run(self, rank: int = 0, world: int = 1, allreduce: bool = True) -> Tensor:
         from .._lib import check
         total = self.plan.run_slices(rank, world)

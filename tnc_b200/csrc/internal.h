@@ -177,6 +177,28 @@ constexpr int kGradThreads = 256;   // outputs per block
 int launch_grad_gather(tncb_ctx* ctx, const GradItem* d_items, const long long* d_block_start, int n_items,
                        long long total_blocks, const char* ws, double2* out);
 
+// ---- sliced gradient plans: slice q's sub-block of every full leaf <-> the slice leaf in the workspace, in ONE launch
+// per direction.  Element o of the slice leaf (row-major in its kept legs, the full leaf's order) decomposes over the
+// fused groups; the slot side reads / writes sum_g i_g * st[g], the full side base(q) + sum_g i_g * fst[g] with
+// base(q) = sum_k ((q / sdiv[k]) % sdim[k]) * sst[k] over the leaf's sliced legs ----
+constexpr int kSliceGroups = 8, kSliceLegs = 8;
+struct SliceItem {
+  long long slot;               // byte offset in the plan workspace (or in the plan's permute scratch, from_scratch)
+  long long full;               // element offset of the full leaf in the full leaf block / the full gradient block
+  long long elems;              // elements of the slice leaf
+  int n, ns;                    // fused leg groups (outermost first); sliced legs of this leaf
+  int from_scratch, _pad;
+  long long dim[kSliceGroups];
+  long long st[kSliceGroups];   // element stride of each group on the slot side
+  long long fst[kSliceGroups];  // element stride of each group in the full leaf
+  unsigned long long sdiv[kSliceLegs], sdim[kSliceLegs];   // digit k of slice q: (q / sdiv[k]) % sdim[k]
+  long long sst[kSliceLegs];    // element stride of that sliced leg in the full leaf
+};
+int launch_slice_extract(tncb_ctx* ctx, const SliceItem* d_items, const long long* d_block_start, int n_items,
+                         long long total_blocks, const double2* full, char* ws, unsigned long long q);
+int launch_grad_accumulate(tncb_ctx* ctx, const SliceItem* d_items, const long long* d_block_start, int n_items,
+                           long long total_blocks, const char* ws, const double2* scratch, double2* grad, unsigned long long q);
+
 int tensor_new(tncb_ctx* ctx, int rank, const uint64_t* dims, tncb_tensor** out);
 
 // TensorData::File leaf (hdf5io.cpp): first member of /tensors, optionally adjointed, checked against the leaf's dims

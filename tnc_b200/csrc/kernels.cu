@@ -1200,4 +1200,85 @@ int launch_grad_gather(tncb_ctx* ctx, const GradItem* d_items, const long long* 
   return TNCB_OK;
 }
 
+// ------------------------------------------------------------------------------------------
+// Sliced gradient plans (tncb_plan_vjp_sliced / tncb_plan_run_slices): per slice q, slice_extract_kernel copies q's
+// sub-block of every full leaf that carries a sliced leg into that leaf's place in the workspace, and
+// grad_accumulate_kernel adds every requested leaf adjoint into q's sub-block of its full-shape gradient.  One launch
+// each for hundreds of tiny leaves: a block serves kGradThreads consecutive elements of one item, found by binary search
+// over the block-count prefix (as grad_gather_kernel does).  q's base offset comes from q itself, so a slice needs no
+// host work.  Within one slice every full-gradient element gets at most one contribution: plain +=, no atomics.
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ int slice_item_of(const long long* __restrict__ block_start, int n_items, long long b) {
+  int lo = 0, hi = n_items;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(block_start + mid) <= b) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+// element o of the item: its slot-side and full-side element offsets for slice q
+__device__ __forceinline__ void slice_offsets(const SliceItem& it, long long o, unsigned long long q, long long* s, long long* f) {
+  long long fo = 0;
+  for (int k = 0; k < it.ns; k++) fo += (long long)((q / it.sdiv[k]) % it.sdim[k]) * it.sst[k];
+  long long so = 0, idx = o;
+  for (int g = it.n - 1; g > 0; --g) {
+    const long long d = it.dim[g], r = idx / d, i = idx - r * d;
+    so += i * it.st[g]; fo += i * it.fst[g];
+    idx = r;
+  }
+  if (it.n > 0) { so += idx * it.st[0]; fo += idx * it.fst[0]; }
+  *s = so; *f = fo;
+}
+
+__global__ void __launch_bounds__(kGradThreads)
+slice_extract_kernel(const SliceItem* __restrict__ items, const long long* __restrict__ block_start, int n_items,
+                     const double2* __restrict__ full, char* __restrict__ ws, unsigned long long q) {
+  const long long b = blockIdx.x;
+  const int i = slice_item_of(block_start, n_items, b);
+  const SliceItem& it = items[i];
+  const long long o = (b - __ldg(block_start + i)) * kGradThreads + threadIdx.x;
+  if (o >= it.elems) return;
+  long long s, f;
+  slice_offsets(it, o, q, &s, &f);
+  reinterpret_cast<double2*>(ws + it.slot)[s] = full[it.full + f];
+}
+
+__global__ void __launch_bounds__(kGradThreads)
+grad_accumulate_kernel(const SliceItem* __restrict__ items, const long long* __restrict__ block_start, int n_items,
+                       const char* __restrict__ ws, const double2* __restrict__ scratch, double2* __restrict__ grad,
+                       unsigned long long q) {
+  const long long b = blockIdx.x;
+  const int i = slice_item_of(block_start, n_items, b);
+  const SliceItem& it = items[i];
+  const long long o = (b - __ldg(block_start + i)) * kGradThreads + threadIdx.x;
+  if (o >= it.elems) return;
+  long long s, f;
+  slice_offsets(it, o, q, &s, &f);
+  const double2 v = it.from_scratch ? scratch[it.slot + s] : reinterpret_cast<const double2*>(ws + it.slot)[s];
+  double2 g = grad[it.full + f];
+  g.x += v.x; g.y += v.y;
+  grad[it.full + f] = g;
+}
+
+int launch_slice_extract(tncb_ctx* ctx, const SliceItem* d_items, const long long* d_block_start, int n_items,
+                         long long total_blocks, const double2* full, char* ws, unsigned long long q) {
+  if (n_items <= 0 || total_blocks <= 0) return TNCB_OK;
+  if (total_blocks > 0x7fffffffLL) return fail(TNCB_ERR_UNSUPPORTED, "slice leaves too large for one extract launch");
+  slice_extract_kernel<<<(unsigned)total_blocks, kGradThreads, 0, ctx->stream>>>(d_items, d_block_start, n_items, full, ws, q);
+  ctx->launches++;
+  TNCB_CUDA(cudaGetLastError());
+  return TNCB_OK;
+}
+
+int launch_grad_accumulate(tncb_ctx* ctx, const SliceItem* d_items, const long long* d_block_start, int n_items,
+                           long long total_blocks, const char* ws, const double2* scratch, double2* grad, unsigned long long q) {
+  if (n_items <= 0 || total_blocks <= 0) return TNCB_OK;
+  if (total_blocks > 0x7fffffffLL) return fail(TNCB_ERR_UNSUPPORTED, "leaf gradients too large for one accumulate launch");
+  grad_accumulate_kernel<<<(unsigned)total_blocks, kGradThreads, 0, ctx->stream>>>(d_items, d_block_start, n_items, ws, scratch, grad, q);
+  ctx->launches++;
+  TNCB_CUDA(cudaGetLastError());
+  return TNCB_OK;
+}
+
 } // namespace tncb

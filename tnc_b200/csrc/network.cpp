@@ -14,6 +14,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <memory>
 
 namespace tncb {
 
@@ -339,6 +340,18 @@ struct tncb_plan {
   std::vector<GradPermute> grad_permutes;           // leaves with more fused groups than a GradItem holds: K3
   void* grad_dev = nullptr; size_t grad_dev_bytes = 0;   // device copy of grad_items + grad_block_start
   bool fwd_ready = false;            // a forward run left its state in the workspace for one tncb_plan_vjp
+  // sliced gradient plans (tncb_plan_create_vjp_sliced): S is the structure of one slice, `full` holds the full
+  // network's leaves; tncb_plan_stage uploads the full leaf block once and every slice is extracted from it on the device
+  bool sliced = false;
+  uint64_t n_sl = 1;                                // slices: the product of the sliced legs' dims
+  tncb::Schedule full;                              // leaves only: kinds, dims, offsets in the full leaf block
+  std::vector<tncb::SliceItem> sl_items, const_items, acc_items;   // extract (leaves with / without a sliced leg), accumulate
+  std::vector<long long> sl_bs, const_bs, acc_bs;   // their block-count prefixes (n_items + 1 entries each)
+  size_t acc_scratch_elems = 0;                     // permute scratch of the leaves that take K3 before the accumulate
+  void* sl_dev = nullptr; size_t sl_dev_bytes = 0;  // device copy of the items + prefixes, the seed 1, the permute scratch
+  size_t sl_off[7] = {};                            // byte offsets inside sl_dev: 3 item arrays, 3 prefixes, seed 1 (+ scratch)
+  void* full_dev = nullptr; size_t full_bytes = 0;  // the staged full leaf block (outside the workspace)
+  bool full_staged = false;
 };
 
 namespace tncb {
@@ -509,6 +522,27 @@ static int plan_device_state(tncb_ctx* ctx, tncb_plan* P) {
     TNCB_CUDA(cudaMemcpyAsync(P->grad_dev, P->grad_items.data(), ib, cudaMemcpyHostToDevice, ctx->stream));
     TNCB_CUDA(cudaMemcpyAsync((char*)P->grad_dev + ib, P->grad_block_start.data(), bb, cudaMemcpyHostToDevice, ctx->stream));
     TNCB_CUDA(cudaStreamSynchronize(ctx->stream));
+  }
+  if (P->sliced && !P->sl_dev) {
+    auto up16 = [](size_t b) { return (b + 15) / 16 * 16; };
+    const std::vector<SliceItem>* iv[3] = {&P->sl_items, &P->const_items, &P->acc_items};
+    const std::vector<long long>* bv[3] = {&P->sl_bs, &P->const_bs, &P->acc_bs};
+    size_t off = 0;
+    for (int i = 0; i < 3; i++) { P->sl_off[i] = off; off = up16(off + iv[i]->size() * sizeof(SliceItem)); }
+    for (int i = 0; i < 3; i++) { P->sl_off[3 + i] = off; off = up16(off + bv[i]->size() * sizeof(long long)); }
+    P->sl_off[6] = off; off += sizeof(double2);
+    std::vector<char> host(off, 0);
+    for (int i = 0; i < 3; i++) {
+      if (!iv[i]->empty()) std::memcpy(host.data() + P->sl_off[i], iv[i]->data(), iv[i]->size() * sizeof(SliceItem));
+      if (!bv[i]->empty()) std::memcpy(host.data() + P->sl_off[3 + i], bv[i]->data(), bv[i]->size() * sizeof(long long));
+    }
+    const double2 one = {1.0, 0.0};
+    std::memcpy(host.data() + P->sl_off[6], &one, sizeof(one));
+    const size_t bytes = off + P->acc_scratch_elems * sizeof(double2);
+    if ((rc = ctx->arena.alloc(bytes, &P->sl_dev))) return rc;
+    P->sl_dev_bytes = bytes;
+    TNCB_CUDA(cudaMemcpyAsync(P->sl_dev, host.data(), off, cudaMemcpyHostToDevice, ctx->stream));
+    TNCB_CUDA(cudaStreamSynchronize(ctx->stream));   // (pageable source)
   }
   return TNCB_OK;
 }
@@ -713,6 +747,178 @@ static int build_gather(tncb_plan* P, const std::vector<int>& leaf_adj) {
   return TNCB_OK;
 }
 
+// ---- sliced gradient plans ----
+// `tn` with the sliced legs dropped from every leaf: the structure every slice shares.  A leaf may lose all its legs.
+// Payload leaves become MATRIX stand-ins (the schedule reads no payload, and a gate's table would not match its sliced
+// dims); the full leaves are validated and staged through the plan's `full` schedule instead.
+struct SliceTree { std::vector<std::unique_ptr<tncb_tn[]>> nodes; std::vector<std::unique_ptr<uint64_t[]>> arrs; };
+static void slice_tree(const tncb_tn* src, tncb_tn* dst, const std::vector<uint64_t>& sl, SliceTree& keep) {
+  static const double stand_in[2] = {0.0, 0.0};
+  *dst = *src;
+  if (src->n_children) {
+    keep.nodes.emplace_back(new tncb_tn[src->n_children]);
+    tncb_tn* ch = keep.nodes.back().get();
+    for (size_t i = 0; i < src->n_children; i++) slice_tree(&src->children[i], &ch[i], sl, keep);
+    dst->children = ch;
+    return;
+  }
+  if (src->kind == TNCB_DATA_UNCONTRACTED) return;
+  if (src->rank > 0 && src->rank <= kMaxLegs && src->legs && src->dims) {
+    keep.arrs.emplace_back(new uint64_t[2 * src->rank]);
+    uint64_t* a = keep.arrs.back().get();
+    int r = 0;
+    for (int i = 0; i < src->rank; i++)
+      if (std::find(sl.begin(), sl.end(), src->legs[i]) == sl.end()) { a[r] = src->legs[i]; a[src->rank + r] = src->dims[i]; r++; }
+    dst->rank = r; dst->legs = a; dst->dims = a + src->rank;
+  }
+  dst->kind = TNCB_DATA_MATRIX; dst->host_re_im = stand_in;
+  dst->gate_name = nullptr; dst->gate_angles = nullptr; dst->n_gate_angles = 0; dst->gate_adjoint = 0;
+  dst->device = nullptr; dst->file_path = nullptr; dst->file_adjoint = 0;
+}
+
+// fuses neighbouring groups that are contiguous on both sides; false if more than kSliceGroups remain
+static bool fuse_slice_groups(SliceItem& it, const std::vector<long long>& d, const std::vector<long long>& st, const std::vector<long long>& fst) {
+  it.n = 0;
+  for (size_t i = 0; i < d.size(); i++) {
+    if (d[i] == 1) continue;
+    if (it.n > 0 && it.st[it.n - 1] == st[i] * d[i] && it.fst[it.n - 1] == fst[i] * d[i]) {
+      it.dim[it.n - 1] *= d[i]; it.st[it.n - 1] = st[i]; it.fst[it.n - 1] = fst[i]; continue;
+    }
+    if (it.n == kSliceGroups) return false;
+    it.dim[it.n] = d[i]; it.st[it.n] = st[i]; it.fst[it.n] = fst[i]; it.n++;
+  }
+  for (int k = it.n; k < kSliceGroups; k++) { it.dim[k] = 1; it.st[k] = 0; it.fst[k] = 0; }
+  return true;
+}
+
+static void push_item(std::vector<SliceItem>& items, std::vector<long long>& bs, const SliceItem& it) {
+  if (bs.empty()) bs.push_back(0);
+  items.push_back(it);
+  bs.push_back(bs.back() + (it.elems + kGradThreads - 1) / kGradThreads);
+}
+
+// The full leaves (P->full), the gradient offsets in full-leaf shapes, the extract items (after the layout fixed the leaf
+// slots) and the accumulate items of the leaf adjoints.  An accumulate item whose adjoint order needs more groups than an
+// item holds reads a K3-permuted copy of the adjoint (slice-leaf order) from the plan's permute scratch instead.
+static int build_slice_items(tncb_plan* P, const std::vector<const tncb_tn*>& lv, const std::vector<uint64_t>& sl,
+                             const std::vector<uint64_t>& sdim, const std::vector<int>& leaf_adj) {
+  const Schedule& S = P->S;
+  Schedule& F = P->full;
+  const size_t nl = S.n_leaves_total;
+  std::vector<int> sslot(nl, -1), fslot(nl, -1);
+  for (size_t s = 0; s < S.slots.size(); s++) if (S.slots[s].leaf_index >= 0) sslot[S.slots[s].leaf_index] = (int)s;
+  F.n_leaves_total = nl;
+  F.leaf_offset.assign(nl, 0);
+  F.leaf_kind.assign(nl, TNCB_DATA_UNCONTRACTED);
+  for (size_t li = 0; li < nl; li++) {             // collect order, as build() adds them
+    if (sslot[li] < 0) continue;
+    int rc = add_leaf(lv[li], F, li, &fslot[li]);
+    if (rc) return rc;
+  }
+  const size_t ns = sl.size();
+  std::vector<unsigned long long> div(ns);
+  { unsigned long long d = 1; for (size_t k = ns; k-- > 0;) { div[k] = d; d *= sdim[k]; } }   // last leg fastest
+  P->grad_offset.assign(nl, -1);
+  P->grad_elems = 0;
+  for (size_t li = 0; li < nl; li++)
+    if (leaf_adj[li] >= 0) { P->grad_offset[li] = (int64_t)P->grad_elems; P->grad_elems += F.slots[fslot[li]].elems; }
+  size_t scratch = 0;
+  for (size_t li = 0; li < nl; li++) {
+    if (sslot[li] < 0) continue;
+    const SlotMeta& sm = S.slots[sslot[li]];
+    const SlotMeta& fm = F.slots[fslot[li]];
+    if (sm.elems == 0) continue;
+    const int fr = (int)fm.legs.size();
+    std::vector<long long> fstr(fr);
+    { long long s = 1; for (int j = fr - 1; j >= 0; j--) { fstr[j] = s; s *= (long long)fm.dims[j]; } }
+    SliceItem it{};
+    std::vector<long long> d, fst;                  // the kept legs, in the leaf's order = the slice leaf's legs
+    for (int j = 0; j < fr; j++) {
+      const size_t k = std::find(sl.begin(), sl.end(), fm.legs[j]) - sl.begin();
+      if (k == ns) { d.push_back((long long)fm.dims[j]); fst.push_back(fstr[j]); continue; }
+      if (it.ns == kSliceLegs) return fail(TNCB_ERR_UNSUPPORTED, "leaf " + std::to_string(li) + " carries more than " + std::to_string(kSliceLegs) + " sliced legs");
+      it.sdiv[it.ns] = div[k]; it.sdim[it.ns] = sdim[k]; it.sst[it.ns] = fstr[j]; it.ns++;
+    }
+    std::vector<long long> rm(d.size());
+    { long long s = 1; for (size_t j = d.size(); j-- > 0;) { rm[j] = s; s *= d[j]; } }
+    it.elems = (long long)sm.elems;
+    // extract: full leaf block -> the leaf's slot in the workspace (row-major slice leaf)
+    SliceItem ex = it;
+    ex.slot = (long long)P->slot_off[sslot[li]]; ex.full = (long long)F.leaf_offset[li];
+    if (!fuse_slice_groups(ex, d, rm, fst))
+      return fail(TNCB_ERR_UNSUPPORTED, "leaf " + std::to_string(li) + " needs more than " + std::to_string(kSliceGroups) + " leg groups to address its slices");
+    if (ex.ns) push_item(P->sl_items, P->sl_bs, ex); else push_item(P->const_items, P->const_bs, ex);
+    if (leaf_adj[li] < 0) continue;
+    // accumulate: the adjoint slot (pair output order) -> q's sub-block of the full-shape gradient
+    const int gs = leaf_adj[li];
+    const SlotMeta& g = S.slots[gs];
+    std::vector<long long> gst(g.legs.size());
+    { long long s = 1; for (size_t j = g.legs.size(); j-- > 0;) { gst[j] = s; s *= (long long)g.dims[j]; } }
+    std::vector<int> perm(sm.legs.size());
+    std::vector<long long> ast(sm.legs.size());
+    for (size_t i = 0; i < sm.legs.size(); i++) {
+      perm[i] = (int)(std::find(g.legs.begin(), g.legs.end(), sm.legs[i]) - g.legs.begin());
+      ast[i] = gst[perm[i]];
+    }
+    SliceItem ac = it;
+    ac.full = (long long)P->grad_offset[li];
+    ac.slot = (long long)P->slot_off[gs];
+    if (!fuse_slice_groups(ac, d, ast, fst)) {       // many groups: K3 into the scratch, then the same kernel
+      ac.from_scratch = 1; ac.slot = (long long)scratch;
+      fuse_slice_groups(ac, d, rm, fst);            // (the extract item fitted with the same groups)
+      P->grad_permutes.push_back({gs, (int64_t)scratch, perm});
+      scratch += sm.elems;
+    }
+    push_item(P->acc_items, P->acc_bs, ac);
+  }
+  P->acc_scratch_elems = scratch;
+  for (const auto* bs : {&P->sl_bs, &P->const_bs, &P->acc_bs})
+    if (!bs->empty() && bs->back() > 0x7fffffffLL) return fail(TNCB_ERR_UNSUPPORTED, "slice leaves too large for one launch");
+  return TNCB_OK;
+}
+
+// Per slice q of [first, n_sl) step stride: extract, forward levels, value accumulation and, with `grad`, the seed copy,
+// backward levels, K3 of the many-group adjoints and the accumulation into the full-shape gradient (zeroed here).  The
+// leaves without a sliced leg are the same in every slice: they are copied once per call (the leaf block is never
+// released by the layout, so they stay in place across slices).
+static int run_sliced(tncb_ctx* ctx, tncb_plan* P, size_t first, size_t stride, const double2* seed, double2* value, double2* grad) {
+  const Schedule& S = P->S;
+  char* ws = (char*)P->ws;
+  char* dev = (char*)P->sl_dev;
+  const SlotMeta& rm = S.slots[S.result_slot];
+  const size_t vbytes = std::max<size_t>(rm.elems, 1) * sizeof(double2);
+  auto items = [&](int i) { return (const SliceItem*)(dev + P->sl_off[i]); };
+  auto bs = [&](int i) { return (const long long*)(dev + P->sl_off[3 + i]); };
+  double2* scratch = (double2*)(dev + P->sl_off[6] + sizeof(double2));
+  const double2* full = (const double2*)P->full_dev;
+  P->fwd_ready = false;
+  if (grad) TNCB_CUDA(cudaMemsetAsync(grad, 0, std::max<uint64_t>(P->grad_elems, 1) * sizeof(double2), ctx->stream));
+  if (first >= P->n_sl) {                          // more ranks than slices
+    TNCB_CUDA(cudaMemsetAsync(value, 0, vbytes, ctx->stream));
+    return TNCB_OK;
+  }
+  int rc = launch_slice_extract(ctx, items(1), bs(1), (int)P->const_items.size(), P->const_items.empty() ? 0 : P->const_bs.back(), full, ws, 0);
+  for (size_t q = first; q < P->n_sl && !rc; q += stride) {
+    if (!P->sl_items.empty() && (rc = launch_slice_extract(ctx, items(0), bs(0), (int)P->sl_items.size(), P->sl_bs.back(), full, ws, q))) break;
+    if ((rc = enqueue_static(ctx, P, ws, 1, 0, 0, P->n_fwd_levels))) break;
+    const double2* r = (const double2*)(ws + P->slot_off[S.result_slot]);
+    if (q == first) TNCB_CUDA(cudaMemcpyAsync(value, r, rm.elems * sizeof(double2), cudaMemcpyDeviceToDevice, ctx->stream));
+    else if ((rc = launch_add(ctx, value, r, rm.elems))) break;
+    if (!grad) continue;
+    TNCB_CUDA(cudaMemcpyAsync(ws + P->slot_off[P->seed_slot], seed ? seed : (const double2*)(dev + P->sl_off[6]),
+                              rm.elems * sizeof(double2), cudaMemcpyDeviceToDevice, ctx->stream));
+    if ((rc = enqueue_static(ctx, P, ws, 1, 0, P->n_fwd_levels, (int)P->level_batched.size()))) break;
+    for (size_t i = 0; i < P->grad_permutes.size() && !rc; i++) {
+      const auto& gp = P->grad_permutes[i];
+      const SlotMeta& sm = S.slots[gp.slot];
+      rc = launch_permute(ctx, (const double2*)(ws + P->slot_off[gp.slot]), scratch + gp.dst, (int)sm.dims.size(), sm.dims.data(), gp.perm.data());
+    }
+    if (!rc && !P->acc_items.empty())
+      rc = launch_grad_accumulate(ctx, items(2), bs(2), (int)P->acc_items.size(), P->acc_bs.back(), ws, scratch, grad, q);
+  }
+  return rc;
+}
+
 } // namespace tncb
 
 extern "C" {
@@ -833,6 +1039,59 @@ int tncb_plan_create_vjp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path
   return TNCB_OK;
 }
 
+// A sliced gradient plan: the gradient plan of one slice's structure (compiled exactly as tncb_plan_create_vjp compiles
+// the host-sliced slice network), plus the extract / accumulate items that move slice q's sub-blocks between the full
+// leaves and the workspace.
+int tncb_plan_create_vjp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, size_t n_sliced,
+                                const uint64_t* sliced_legs, const uint8_t* wrt, tncb_plan** out) {
+  using namespace tncb;
+  if (!tn || !out || (n_sliced && !sliced_legs)) return fail(TNCB_ERR_INVALID, "null argument");
+  std::vector<const tncb_tn*> lv;
+  collect_leaf_nodes(tn, lv);
+  for (const tncb_tn* l : lv)
+    if (l->kind == TNCB_DATA_DEVICE) return fail(TNCB_ERR_UNSUPPORTED, "gradient plans do not take device leaves (they are consumed per call)");
+  std::vector<uint64_t> sl(sliced_legs, sliced_legs + n_sliced), sdim(n_sliced, 0);
+  uint64_t n_sl = 1;
+  bool overflow = false;
+  for (size_t k = 0; k < n_sliced; k++) {
+    const std::string name = "sliced leg " + std::to_string(sl[k]);
+    if (std::find(sl.begin(), sl.begin() + k, sl[k]) != sl.begin() + k) return fail(TNCB_ERR_INVALID, name + " is listed twice");
+    int count = 0;
+    for (const tncb_tn* l : lv)
+      if (l->rank > 0 && l->rank <= kMaxLegs && l->legs && l->dims)
+        for (int i = 0; i < l->rank; i++)
+          if (l->legs[i] == sl[k]) { count++; sdim[k] = l->dims[i]; }
+    if (count == 0) return fail(TNCB_ERR_INVALID, name + " does not occur in the network");
+    if (count == 1) return fail(TNCB_ERR_INVALID, name + " occurs once: it is an open leg of the result");
+    if (sdim[k] == 0) return fail(TNCB_ERR_INVALID, name + " has dimension 0");
+    if (n_sl > UINT64_MAX / sdim[k]) overflow = true;
+    else n_sl *= sdim[k];
+  }
+  if (overflow) return fail(TNCB_ERR_INVALID, "the slice count overflows 64 bits");
+  SliceTree keep;
+  tncb_tn st;
+  slice_tree(tn, &st, sl, keep);
+  tncb_plan* p = new tncb_plan();
+  p->grad = p->sliced = true;
+  p->n_sl = n_sl;
+  std::vector<int> leaf_adj;
+  int rc = build_schedule(&st, path, p->S);
+  if (!rc) rc = build_backward(p, wrt, leaf_adj);
+  if (rc) { delete p; return rc; }
+  size_t dev_free = 0, dev_total = 0;
+  if (ctx) { cudaSetDevice(ctx->device); if (cudaMemGetInfo(&dev_free, &dev_total) != cudaSuccess) { dev_total = 0; cudaGetLastError(); } }
+  plan_static_layout(p, ctx ? ctx->sm_count : 132, dev_total);
+  if (!p->is_static) {
+    const size_t need = p->ws_bytes, limit = static_ws_limit(dev_total);
+    delete p;
+    return fail(TNCB_ERR_UNSUPPORTED, "the gradient workspace of one slice needs " + std::to_string(need) + " bytes, above the static-workspace limit of " +
+                                      std::to_string(limit) + " bytes (TNCB_PLAN_WS_GB)");
+  }
+  if ((rc = build_slice_items(p, lv, sl, sdim, leaf_adj))) { delete p; return rc; }
+  *out = p;
+  return TNCB_OK;
+}
+
 int tncb_plan_grad_offsets(const tncb_plan* plan, int64_t* offsets) {
   if (!plan || !offsets) return tncb::fail(TNCB_ERR_INVALID, "null argument");
   if (!plan->grad) return tncb::fail(TNCB_ERR_INVALID, "not a gradient plan (tncb_plan_create_vjp)");
@@ -845,6 +1104,7 @@ int tncb_plan_grad_offsets(const tncb_plan* plan, int64_t* offsets) {
 int tncb_plan_vjp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* seed, tncb_tensor** grads) {
   using namespace tncb;
   if (!ctx || !plan || !grads) return fail(TNCB_ERR_INVALID, "null argument");
+  if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_vjp_sliced");
   if (!plan->grad) return fail(TNCB_ERR_INVALID, "not a gradient plan (tncb_plan_create_vjp)");
   if (plan->ctx != ctx || !plan->fwd_ready)
     return fail(TNCB_ERR_INVALID, "tncb_plan_vjp needs a forward run (tncb_plan_run / tncb_plan_execute) of the plan on this context "
@@ -883,8 +1143,40 @@ int tncb_plan_vjp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* seed, tncb_
   return TNCB_OK;
 }
 
+// Per slice first, first+stride, ...: extract, forward levels, seed copy, backward levels, accumulate into the
+// full-shape gradients.  No host work per slice; the slices are stream-ordered, so the sums repeat bit for bit.
+int tncb_plan_vjp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t stride, const tncb_tensor* seed,
+                         tncb_tensor** value, tncb_tensor** grads) {
+  using namespace tncb;
+  if (!ctx || !plan || !value || !grads || stride == 0) return fail(TNCB_ERR_INVALID, "bad argument");
+  if (!plan->sliced) return fail(TNCB_ERR_INVALID, "not a sliced gradient plan (tncb_plan_create_vjp_sliced)");
+  if (plan->ctx != ctx || !plan->full_staged) return fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this context");
+  const Schedule& S = plan->S;
+  const SlotMeta& rm = S.slots[S.result_slot];
+  if (seed) {
+    bool same = seed->rank == (int)rm.dims.size();
+    for (int i = 0; same && i < seed->rank; i++) same = seed->dims[i] == rm.dims[i];
+    if (!same) return fail(TNCB_ERR_SHAPE, "the seed's dims differ from the result's");
+    if (!seed->ptr) return fail(TNCB_ERR_UNCONTRACTED, "the seed tensor has no storage");
+  } else if (!rm.dims.empty()) return fail(TNCB_ERR_INVALID, "a seed is needed for a result of rank " + std::to_string(rm.dims.size()));
+  TNCB_CUDA(cudaSetDevice(ctx->device));
+  tncb_tensor *v = nullptr, *g = nullptr;
+  const uint64_t n = plan->grad_elems;
+  int rc = tensor_new(ctx, (int)rm.dims.size(), rm.dims.data(), &v);
+  if (!rc) rc = tensor_new(ctx, 1, &n, &g);
+  if (!rc) rc = run_sliced(ctx, plan, first, stride, seed ? seed->ptr : nullptr, v->ptr, g->ptr);
+  if (rc) {
+    if (v) tncb_tensor_free(ctx, v);
+    if (g) tncb_tensor_free(ctx, g);
+    return rc;
+  }
+  *value = v; *grads = g;
+  return TNCB_OK;
+}
+
 int tncb_plan_execute(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tn, tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   if (!ctx || !plan || !tn) return tncb::fail(TNCB_ERR_INVALID, "null argument");
+  if (plan->sliced) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_run_slices / tncb_plan_vjp_sliced");
   if (plan->grad) return tncb::execute_static(ctx, plan, tn, out, n_out, out_legs);   // forward levels only, no fallback
   static const bool trace = std::getenv("TNCB_TRACE") != nullptr;   // per-step times come from the pair-by-pair executor
   if (plan->is_static && !trace && (plan->ctx == nullptr || plan->ctx == ctx)) {
@@ -906,6 +1198,23 @@ int tncb_plan_stage(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tn) {
   TNCB_CUDA(cudaSetDevice(ctx->device));
   std::vector<const tncb_tn*> leaves;
   tncb::collect_leaf_nodes(tn, leaves);
+  if (plan->sliced) {         // the FULL leaves, once, into a plan-owned block outside the workspace
+    const tncb::Schedule& F = plan->full;
+    int rc = tncb::validate_leaves(F, leaves);
+    if (rc) return rc;
+    std::vector<std::complex<double>> host(std::max<size_t>(F.leaf_block_elems, 1));
+    if ((rc = tncb::stage_leaves(F, leaves, host.data()))) return rc;
+    if ((rc = tncb::plan_device_state(ctx, plan))) return rc;
+    if (!plan->full_dev) {
+      if ((rc = ctx->arena.alloc(host.size() * sizeof(double2), &plan->full_dev))) return rc;
+      plan->full_bytes = host.size() * sizeof(double2);
+    }
+    plan->full_staged = false;
+    TNCB_CUDA(cudaMemcpyAsync(plan->full_dev, host.data(), plan->full_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    TNCB_CUDA(cudaStreamSynchronize(ctx->stream));   // `host` dies with this frame
+    plan->full_staged = true;
+    return TNCB_OK;
+  }
   int rc = tncb::validate_leaves(S, leaves);
   if (rc) return rc;
   const size_t bytes = std::max<size_t>(S.leaf_block_elems * sizeof(double2), 16);
@@ -936,6 +1245,7 @@ int tncb_plan_stage(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tn) {
 
 int tncb_plan_run(tncb_ctx* ctx, tncb_plan* plan, tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   if (!ctx || !plan) return tncb::fail(TNCB_ERR_INVALID, "null argument");
+  if (plan->sliced) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_run_slices / tncb_plan_vjp_sliced");
   static const bool trace = std::getenv("TNCB_TRACE") != nullptr;
   if (plan->is_static && plan->leaves_resident && plan->ctx == ctx) {
     if (!trace || plan->grad) return tncb::execute_static(ctx, plan, nullptr, out, n_out, out_legs);
@@ -951,6 +1261,7 @@ int tncb_plan_run(tncb_ctx* ctx, tncb_plan* plan, tncb_tensor** out, int* n_out,
 // block (KBs), the plan's kernels (batched / graph as usual), one accumulation kernel.
 int tncb_plan_stage_slices(tncb_ctx* ctx, tncb_plan* plan, size_t n_slices, const tncb_tn* const* slice_tns) {
   if (!ctx || !plan || !slice_tns || n_slices == 0) return tncb::fail(TNCB_ERR_INVALID, "null argument");
+  if (plan->sliced) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan stages its full network once (tncb_plan_stage)");
   if (plan->grad) return tncb::fail(TNCB_ERR_UNSUPPORTED, "gradient plans run one staged network at a time");
   if (!plan->is_static) return tncb::fail(TNCB_ERR_UNSUPPORTED, "sliced execution needs a plan with a static layout (no device leaves)");
   const tncb::Schedule& S = plan->S;
@@ -978,6 +1289,19 @@ int tncb_plan_stage_slices(tncb_ctx* ctx, tncb_plan* plan, size_t n_slices, cons
 
 int tncb_plan_run_slices(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t stride, tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   if (!ctx || !plan || stride == 0) return tncb::fail(TNCB_ERR_INVALID, "bad argument");
+  if (plan->sliced) {         // forward levels only, slices extracted on the device from the staged full leaves
+    if (plan->ctx != ctx || !plan->full_staged) return tncb::fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this context");
+    const tncb::SlotMeta& rm = plan->S.slots[plan->S.result_slot];
+    TNCB_CUDA(cudaSetDevice(ctx->device));
+    tncb_tensor* sum = nullptr;
+    int rc = tncb::tensor_new(ctx, (int)rm.dims.size(), rm.dims.data(), &sum);
+    if (!rc) rc = tncb::run_sliced(ctx, plan, first, stride, nullptr, sum->ptr, nullptr);
+    if (rc) { if (sum) tncb_tensor_free(ctx, sum); return rc; }
+    if (out) *out = sum; else tncb_tensor_free(ctx, sum);
+    if (n_out) *n_out = (int)rm.legs.size();
+    if (out_legs) for (size_t i = 0; i < rm.legs.size(); i++) out_legs[i] = rm.legs[i];
+    return TNCB_OK;
+  }
   if (plan->grad) return tncb::fail(TNCB_ERR_UNSUPPORTED, "gradient plans run one staged network at a time");
   if (!plan->slices_dev || plan->ctx != ctx) return tncb::fail(TNCB_ERR_INVALID, "tncb_plan_stage_slices has not been called on this context");
   const tncb::Schedule& S = plan->S;
@@ -1017,6 +1341,7 @@ int tncb_plan_run_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
                         tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   using namespace tncb;
   if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
+  if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_run_slices / tncb_plan_vjp_sliced");
   if (plan->grad) return fail(TNCB_ERR_UNSUPPORTED, "gradient plans run one staged network at a time");
   if (!plan->is_static) return fail(TNCB_ERR_UNSUPPORTED, "batched execution needs a plan with a static layout (no device leaves)");
   if (!plan->slices_dev || plan->ctx != ctx) return fail(TNCB_ERR_INVALID, "tncb_plan_stage_slices has not been called on this context");
@@ -1124,6 +1449,8 @@ int tncb_plan_info(const tncb_plan* plan, uint64_t* n_pairs, double* flops, doub
     for (const tncb::Step& st : S.steps) k += st.plan.kernel_class == 1 ? 2 : 1;  // (K1: table build + GEMM)
     for (int nb : plan->level_batched) if (nb) k -= (uint64_t)(nb - 1);            // a batch is one launch
     if (!plan->grad_items.empty()) k++;                                            // the leaf-gradient gather
+    if (!plan->acc_items.empty()) k++;                                             // a slice's gradient accumulation
+    if (!plan->sl_items.empty()) k++;                                              // a slice's leaf extraction
     *n_kernels = k + 2 * plan->grad_permutes.size();                               // (K3: tables + transpose)
   }
   return TNCB_OK;
@@ -1139,6 +1466,9 @@ void tncb_plan_release_device_state(tncb_plan* plan) {
   for (int i = 0; i < 2; i++) if (plan->exec[i]) { cudaGraphExecDestroy(plan->exec[i]); plan->exec[i] = nullptr; }
   if (plan->batch_dev) { ctx->arena.free(plan->batch_dev, plan->batch_bytes); plan->batch_dev = nullptr; }
   if (plan->grad_dev) { ctx->arena.free(plan->grad_dev, plan->grad_dev_bytes); plan->grad_dev = nullptr; }
+  if (plan->sl_dev) { ctx->arena.free(plan->sl_dev, plan->sl_dev_bytes); plan->sl_dev = nullptr; }
+  if (plan->full_dev) { ctx->arena.free(plan->full_dev, plan->full_bytes); plan->full_dev = nullptr; }
+  plan->full_staged = false;
   plan->fwd_ready = false;
   if (plan->slices_dev) { ctx->arena.free(plan->slices_dev, plan->slices_bytes); plan->slices_dev = nullptr; plan->n_slices = 0; }
   plan->leaves_resident = false;
