@@ -323,7 +323,8 @@ int tncb_plan_create_vjp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path
  * *grads: new rank-1 device tensor holding every requested G_l back to back (tncb_plan_grad_offsets).
  * TNCB_ERR_INVALID without such a forward run on the currently staged leaves, and for a second call after one (the
  * backward slots reuse freed forward memory).  tncb_plan_stage_slices / run_slices / run_batch on a gradient plan ->
- * TNCB_ERR_UNSUPPORTED.  Errors leave the arena as they found it. */
+ * TNCB_ERR_UNSUPPORTED; many networks of its structure go through tncb_plan_stage_batch / tncb_plan_vjp_batch.  Errors
+ * leave the arena as they found it. */
 int tncb_plan_vjp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* seed, tncb_tensor** grads);
 /* Element offset of each leaf's gradient inside *grads, -1 for leaves not requested (n_leaves entries); host only.
  * For a sliced gradient plan the offsets pack the FULL leaves' shapes. */
@@ -359,6 +360,31 @@ int tncb_plan_create_vjp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_pat
  * -> TNCB_ERR_INVALID; seed errors as tncb_plan_vjp.  Errors leave the arena as they found it. */
 int tncb_plan_vjp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t stride, const tncb_tensor* seed,
                          tncb_tensor** value, tncb_tensor** grads);
+/* ---- batched gradients: many networks of one gradient plan's structure (sampled bitstrings, angle sets, input states)
+ * Stage n networks of a (non-sliced) gradient plan's structure for tncb_plan_vjp_batch: every leaf validated and
+ * materialised, one H2D; the structure-validation errors are those of tncb_plan_stage_slices.  The plan's own staged
+ * leaves (tncb_plan_stage) and forward state are untouched.  Not a gradient plan -> TNCB_ERR_INVALID (plain plans use
+ * tncb_plan_stage_slices); a sliced gradient plan -> TNCB_ERR_UNSUPPORTED.  tncb_plan_stage_slices / run_slices /
+ * run_batch stay TNCB_ERR_UNSUPPORTED on gradient plans. */
+int tncb_plan_stage_batch(tncb_ctx* ctx, tncb_plan* plan, size_t n, const tncb_tn* const* tns);
+/* Instances first .. first+count-1, each contracted forward and backward on its own with the instance as a grid
+ * dimension of every kernel, in passes of as many workspace copies as fit (as tncb_plan_run_batch; a gradient workspace
+ * is about twice a forward one).  Each output may be NULL (not produced); at least one must be non-NULL.
+ *   seeds:      [count, result dims..] device tensor; NULL only for a rank-0 result (seed 1 for every instance) or
+ *               when no gradient is requested
+ *   *values:    new [count, result dims..]; row i bit-identical to stage(net_i) + run
+ *   *grad_rows: new [count, grad_elems]; row i bit-identical to stage(net_i) + run + tncb_plan_vjp(seed_i), leaves at
+ *               tncb_plan_grad_offsets inside each row
+ *   *grad_sum:  new [grad_elems]; the left fold 0 + row_0 + row_1 + ... in instance order, bit for bit
+ * grad_rows == grad_sum == NULL: forward levels only.  The plan's workspace, staged leaves and forward state are left
+ * alone, so stage + run + tncb_plan_vjp_batch + tncb_plan_vjp works.  Ranks of a multi-GPU job may split [first, count)
+ * and combine their grad_sum with tncb_comm_allreduce_sum.
+ * Not a gradient plan, nothing staged by tncb_plan_stage_batch on this context, count == 0, a range past the staged
+ * networks, every output NULL, NULL seeds for a non-scalar result with gradients requested, a result of rank 64 ->
+ * TNCB_ERR_INVALID; a sliced gradient plan -> TNCB_ERR_UNSUPPORTED; seed dims other than [count, result dims] ->
+ * TNCB_ERR_SHAPE; not even one workspace copy fits -> TNCB_ERR_OOM.  Errors leave the arena as they found it. */
+int tncb_plan_vjp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t count, const tncb_tensor* seeds,
+                        tncb_tensor** values, tncb_tensor** grad_rows, tncb_tensor** grad_sum);
 void tncb_plan_destroy(tncb_plan* plan);
 
 /* ---- HDF5 tensor files: replaces tnc::io::hdf5 (tnc/src/io/hdf5.rs), which binds libhdf5 through hdf5-metno.

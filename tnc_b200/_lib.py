@@ -114,6 +114,8 @@ SIGNATURES = {
     "tncb_plan_create_vjp_sliced": (C.c_int, [C.c_void_p, C.POINTER(TncbTn), C.POINTER(TncbPath), C.c_size_t, u64p,
                                               C.POINTER(C.c_uint8), vpp]),
     "tncb_plan_vjp_sliced": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, vpp, vpp]),
+    "tncb_plan_stage_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.POINTER(TncbTn))]),
+    "tncb_plan_vjp_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, vpp, vpp, vpp]),
     "tncb_plan_destroy": (None, [C.c_void_p]),
     "tncb_comm_unique_id": (C.c_int, [C.c_void_p]),
     "tncb_comm_init": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p]),

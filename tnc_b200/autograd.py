@@ -6,7 +6,9 @@
 
 Gate angles differentiate through ordinary torch code that builds the gate matrices; the library needs no
 angle-derivative table.  One backward pass gives the gradient of every input, at about two forward passes of cost.
-With `sliced_legs`, a network whose gradient workspace does not fit unsliced runs slice by slice (SlicedPlan.for_gradients)."""
+With `sliced_legs`, a network whose gradient workspace does not fit unsliced runs slice by slice (SlicedPlan.for_gradients).
+With `batched`, B networks that differ in some leaves (bitstrings, input states) run in one batched pass
+(NetworkPlan.vjp_batch) and the result gets a leading dimension B."""
 from __future__ import annotations
 
 from typing import Optional, Sequence
@@ -47,6 +49,10 @@ class _NetworkFn(torch.autograd.Function):
         xs = ctx.saved_tensors           # raises on a second backward through a graph that was not retained
         runner = ctx.runner
         seed = np.conj(grad_out.detach().to(torch.complex128).cpu().numpy())
+        if runner.batched:               # vjp_batch runs forward and backward of every instance: it only needs them staged
+            if runner._token != ctx.token:
+                ctx.token = runner._stage_batch(xs)
+            return (None,) + runner._batch_grads(seed, xs)
         if runner.sliced:                # vjp_sliced re-runs every slice's forward: it only needs these inputs staged
             if runner._token != ctx.token:
                 ctx.token = runner._stage(xs)
@@ -63,13 +69,23 @@ class NetworkFunction:
     """The callable network_function returns: inputs -> contracted result, differentiable in every input."""
 
     def __init__(self, tn: Tensor, path: ContractionPath, wrt: Sequence[int], ctx: Optional[Context] = None,
-                 sliced_legs: Sequence[int] = ()):
+                 sliced_legs: Sequence[int] = (), batched: Sequence[int] = ()):
         self.wrt = [int(i) for i in wrt]
         lv = leaves(tn)
         for i in self.wrt:
             if not 0 <= i < len(lv) or lv[i].tensordata.kind != "matrix":
                 raise ValueError(f"leaf {i} is not a Matrix leaf of the network (wrt must name Matrix leaves)")
-        self.shapes = [tuple(int(d) for d in lv[i].bond_dims) for i in self.wrt]
+        self.batched = [int(i) for i in batched]
+        for i in self.batched:
+            if not 0 <= i < len(lv) or lv[i].tensordata.kind != "matrix":
+                raise ValueError(f"leaf {i} is not a Matrix leaf of the network (batched must name Matrix leaves)")
+        if len(set(self.batched)) != len(self.batched):
+            raise ValueError("batched names a leaf twice")
+        if self.batched and len(sliced_legs) > 0:
+            raise ValueError("batched inputs and sliced_legs cannot be combined")
+        # the inputs: one per wrt leaf, then one per batched leaf that is not in wrt
+        self.inputs = self.wrt + [i for i in self.batched if i not in self.wrt]
+        self.shapes = [tuple(int(d) for d in lv[i].bond_dims) for i in self.inputs]
         self.tn, self.path = tn, path
         self.sliced = len(sliced_legs) > 0
         if self.sliced:
@@ -90,21 +106,73 @@ class NetworkFunction:
         self._token = self._count
         return self._token
 
+    def _batch_size(self, xs) -> int:
+        """the common leading dimension B of the batched inputs; every input's shape checked"""
+        b = None
+        for i, shape, x in zip(self.inputs, self.shapes, xs):
+            want = shape
+            if i in self.batched:
+                if x.dim() < 1:
+                    raise ValueError(f"batched input for leaf {i} needs a leading batch dimension")
+                if b is None:
+                    b = int(x.shape[0])
+                elif int(x.shape[0]) != b:
+                    raise ValueError(f"batched input for leaf {i} has {int(x.shape[0])} instances, an earlier one {b}")
+                want = (b,) + shape
+            if tuple(x.shape) != want:
+                raise ValueError(f"input for leaf {i} has shape {tuple(x.shape)}, expected {want}")
+        if b == 0:
+            raise ValueError("batched inputs hold no instance")
+        return b
+
+    def _stage_batch(self, xs):
+        """stage B networks: batched leaves take their row b, the others the same payload in every instance"""
+        b = self._batch_size(xs)
+        arrs = [np.ascontiguousarray(x.detach().to(torch.complex128).cpu().numpy()) for x in xs]
+        nets = []
+        for k in range(b):
+            pay = {i: (a[k] if i in self.batched else a) for i, a in zip(self.inputs, arrs)}
+            nets.append(_with_payloads(self.tn, pay, [0]))
+        self.plan.stage_batch(nets)
+        self._count += 1
+        self._token = self._count
+        return self._token
+
+    def _batch_grads(self, seed, xs):
+        """conj of the rows (batched leaves in wrt) or of the sum (shared leaves in wrt); None for the other inputs"""
+        want_rows = any(i in self.batched for i in self.wrt)
+        want_sum = any(i not in self.batched for i in self.wrt)
+        _, _, rows, total = self.plan.vjp_batch(0, None, seeds=seed, rows=want_rows, sum=want_sum, values=False)
+        grads = []
+        for i, x in zip(self.inputs, xs):
+            if i not in self.wrt:
+                grads.append(None)
+            else:
+                g = rows[i] if i in self.batched else total[i]
+                grads.append(torch.from_numpy(np.conj(g)).to(x.device))
+        return tuple(grads)
+
     def _forward(self, xs):
-        """stage the inputs and run the forward levels (every slice's, summed, on a sliced plan)"""
+        """stage the inputs and run the forward levels (every slice's, summed, on a sliced plan; every instance's, one
+        per row, with batched inputs)"""
+        if self.batched:
+            token = self._stage_batch(xs)
+            _, vals, _, _ = self.plan.vjp_batch(0, None, rows=False, sum=False, values=True)
+            self._result = torch.from_numpy(np.asarray(vals).copy())
+            return token
         token = self._stage(xs)
         res = self.plan.run()
         self._result = torch.from_numpy(np.asarray(res.to_numpy()).copy())
         return token
 
     def __call__(self, *xs: torch.Tensor) -> torch.Tensor:
-        if len(xs) != len(self.wrt):
-            raise TypeError(f"expected {len(self.wrt)} inputs, got {len(xs)}")
+        if len(xs) != len(self.inputs):
+            raise TypeError(f"expected {len(self.inputs)} inputs, got {len(xs)}")
         return _NetworkFn.apply(self, *xs)
 
 
 def network_function(tn: Tensor, path: ContractionPath, wrt: Sequence[int], ctx: Optional[Context] = None,
-                     sliced_legs: Sequence[int] = ()) -> NetworkFunction:
+                     sliced_legs: Sequence[int] = (), batched: Sequence[int] = ()) -> NetworkFunction:
     """A torch.autograd.Function over the network `tn` contracted along `path`: the returned callable takes one torch
     complex128 tensor per leaf index in `wrt` (indices into leaves(tn); each must be a Matrix leaf) and returns the
     contracted result as a torch tensor.  Its backward is conj(vjp(conj(grad_out))) of the gradient plan, torch's
@@ -119,5 +187,14 @@ def network_function(tn: Tensor, path: ContractionPath, wrt: Sequence[int], ctx:
     workspace does not fit unsliced.  Forward = stage + the forward levels of every slice, summed on the device;
     backward = SlicedPlan.vjp with the seed.  No workspace holds all slices' forward state, so the backward runs every
     slice's forward again before its backward levels: about 4 forward passes in all, against about 3 unsliced.  The
-    backward needs only the staged inputs, so it re-stages (without a forward) when another call ran in between."""
-    return NetworkFunction(tn, path, wrt, ctx, sliced_legs)
+    backward needs only the staged inputs, so it re-stages (without a forward) when another call ran in between.
+
+    batched: Matrix leaves whose payload differs per instance, e.g. bitstring projectors or per-sample input states; they
+    may include leaves not in `wrt`.  The callable then takes one tensor per `wrt` leaf followed by one per batched leaf
+    not in `wrt`, in the order given; a batched leaf's tensor is [B, *leaf shape] with one B for all of them, the others
+    are [*leaf shape] and shared by every instance.  It returns [B, *result].  Forward = stage_batch + the forward pass
+    of every instance (NetworkPlan.vjp_batch, values only); backward = vjp_batch with seeds conj(grad_out), a forward
+    plus backward pass of every instance: per-instance gradient rows for batched inputs in `wrt`, their sum over the
+    instances for shared ones.  About 4 forward passes per forward + backward in all, against about 3 for one
+    unbatched network; the instances share every launch.  Not combinable with sliced_legs."""
+    return NetworkFunction(tn, path, wrt, ctx, sliced_legs, batched)

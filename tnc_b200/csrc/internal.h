@@ -176,6 +176,11 @@ struct GradItem {
 constexpr int kGradThreads = 256;   // outputs per block
 int launch_grad_gather(tncb_ctx* ctx, const GradItem* d_items, const long long* d_block_start, int n_items,
                        long long total_blocks, const char* ws, double2* out);
+// n instances' workspaces `stride` bytes apart: instance i's gradients into rows + i * row_elems (rows != nullptr) and/or
+// added to sum in instance order (sum != nullptr); one launch for the pass
+int launch_grad_gather_batch(tncb_ctx* ctx, const GradItem* d_items, const long long* d_block_start, int n_items,
+                             long long total_blocks, const char* ws, long long stride, int n, double2* rows,
+                             long long row_elems, double2* sum);
 
 // ---- sliced gradient plans: slice q's sub-block of every full leaf <-> the slice leaf in the workspace, in ONE launch
 // per direction.  Element o of the slice leaf (row-major in its kept legs, the full leaf's order) decomposes over the

@@ -1200,6 +1200,54 @@ int launch_grad_gather(tncb_ctx* ctx, const GradItem* d_items, const long long* 
   return TNCB_OK;
 }
 
+// The same gather for a pass of n instances whose workspaces lie `stride` bytes apart (tncb_plan_vjp_batch).  A thread
+// computes its source offset once and walks the instances in order: instance i's adjoint element goes to row i of `rows`
+// (row_elems apart) and/or is added to `sum`.  Every element of `sum` is read once, gets the n values added one after
+// another in instance order and is written once, so passes in stream order make `sum` the left fold of the rows bit for
+// bit, with no atomics.
+__global__ void __launch_bounds__(kGradThreads)
+grad_gather_batch_kernel(const GradItem* __restrict__ items, const long long* __restrict__ block_start, int n_items,
+                         const char* __restrict__ ws, long long stride, int n, double2* __restrict__ rows,
+                         long long row_elems, double2* __restrict__ sum) {
+  const long long b = blockIdx.x;
+  int lo = 0, hi = n_items;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(block_start + mid) <= b) lo = mid; else hi = mid;
+  }
+  const GradItem& it = items[lo];
+  const long long o = (b - __ldg(block_start + lo)) * kGradThreads + threadIdx.x;
+  if (o >= it.elems) return;
+  long long idx = o, src = 0;
+  for (int g = it.n - 1; g > 0; --g) {
+    const long long d = it.dim[g], q = idx / d;
+    src += (idx - q * d) * it.st[g];
+    idx = q;
+  }
+  if (it.n > 0) src += idx * it.st[0];
+  const char* p = ws + it.src + src * (long long)sizeof(double2);
+  const long long dst = it.dst + o;
+  double2 acc = sum ? sum[dst] : make_double2(0.0, 0.0);
+  for (int i = 0; i < n; i++, p += stride) {
+    const double2 v = *reinterpret_cast<const double2*>(p);
+    if (rows) rows[i * row_elems + dst] = v;
+    acc.x += v.x; acc.y += v.y;
+  }
+  if (sum) sum[dst] = acc;
+}
+
+int launch_grad_gather_batch(tncb_ctx* ctx, const GradItem* d_items, const long long* d_block_start, int n_items,
+                             long long total_blocks, const char* ws, long long stride, int n, double2* rows,
+                             long long row_elems, double2* sum) {
+  if (n_items <= 0 || total_blocks <= 0 || n <= 0 || (!rows && !sum)) return TNCB_OK;
+  if (total_blocks > 0x7fffffffLL) return fail(TNCB_ERR_UNSUPPORTED, "leaf gradients too large for one gather launch");
+  grad_gather_batch_kernel<<<(unsigned)total_blocks, kGradThreads, 0, ctx->stream>>>(d_items, d_block_start, n_items, ws, stride, n,
+                                                                                      rows, row_elems, sum);
+  ctx->launches++;
+  TNCB_CUDA(cudaGetLastError());
+  return TNCB_OK;
+}
+
 // ------------------------------------------------------------------------------------------
 // Sliced gradient plans (tncb_plan_vjp_sliced / tncb_plan_run_slices): per slice q, slice_extract_kernel copies q's
 // sub-block of every full leaf that carries a sliced leg into that leaf's place in the workspace, and

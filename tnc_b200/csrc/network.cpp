@@ -499,14 +499,15 @@ static int stage_leaves(const Schedule& S, const std::vector<const tncb_tn*>& le
   return TNCB_OK;
 }
 
-// workspace, pinned staging and the device copy of the batch descriptors (once per plan and context)
-static int plan_device_state(tncb_ctx* ctx, tncb_plan* P) {
+// workspace, pinned staging and the device copy of the batch descriptors (once per plan and context).  workspace =
+// false: the descriptors only (a gradient plan's batched pass runs on workspace copies of its own)
+static int plan_device_state(tncb_ctx* ctx, tncb_plan* P, bool workspace = true) {
   if (P->ctx && P->ctx != ctx) return fail(TNCB_ERR_INVALID, "plan belongs to another context");
   if (!P->ctx) { P->ctx = ctx; ctx->plans.push_back(P); }
   int rc;
-  if (!P->ws && (rc = ctx->arena.alloc(P->ws_bytes, &P->ws))) return rc;
+  if (workspace && !P->ws && (rc = ctx->arena.alloc(P->ws_bytes, &P->ws))) return rc;
   const size_t block_bytes = std::max<size_t>(P->S.leaf_block_elems * sizeof(double2), 16);
-  if (!P->stage) TNCB_CUDA(cudaMallocHost(&P->stage, block_bytes));
+  if (workspace && !P->stage) TNCB_CUDA(cudaMallocHost(&P->stage, block_bytes));
   if (!P->batch_dev && !P->items.empty()) {
     const size_t ib = P->items.size() * sizeof(K0BatchItem), bb = P->block_start.size() * sizeof(int);
     P->batch_bytes = ib + bb;
@@ -919,6 +920,86 @@ static int run_sliced(tncb_ctx* ctx, tncb_plan* P, size_t first, size_t stride, 
   return rc;
 }
 
+// ---- many networks of one structure (tncb_plan_stage_slices / tncb_plan_stage_batch, tncb_plan_run_batch /
+// tncb_plan_vjp_batch) ----
+// Validates and materialises the leaves of n networks of the plan's structure, then uploads them in one H2D copy into
+// slices_dev: n leaf blocks back to back.  workspace = false: the plan's own workspace is not needed (gradient plans).
+static int stage_networks(tncb_ctx* ctx, tncb_plan* P, size_t n, const tncb_tn* const* tns, bool workspace) {
+  const Schedule& S = P->S;
+  TNCB_CUDA(cudaSetDevice(ctx->device));
+  int rc;
+  if ((rc = plan_device_state(ctx, P, workspace))) return rc;
+  const size_t block = std::max<size_t>(S.leaf_block_elems, 1);
+  std::vector<std::complex<double>> host(block * n);
+  for (size_t q = 0; q < n; q++) {
+    if (!tns[q]) return fail(TNCB_ERR_INVALID, "slice network is null");
+    std::vector<const tncb_tn*> leaves;
+    collect_leaf_nodes(tns[q], leaves);
+    if ((rc = validate_leaves(S, leaves))) return rc;
+    if ((rc = stage_leaves(S, leaves, host.data() + q * block))) return rc;
+  }
+  TNCB_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (P->slices_dev) { ctx->arena.free(P->slices_dev, P->slices_bytes); P->slices_dev = nullptr; }
+  P->slices_bytes = host.size() * sizeof(double2);
+  if ((rc = ctx->arena.alloc(P->slices_bytes, &P->slices_dev))) return rc;
+  TNCB_CUDA(cudaMemcpyAsync(P->slices_dev, host.data(), P->slices_bytes, cudaMemcpyHostToDevice, ctx->stream));
+  TNCB_CUDA(cudaStreamSynchronize(ctx->stream));
+  P->n_slices = n;
+  return TNCB_OK;
+}
+
+// A batched pass runs c instances on c copies of the plan's workspace, ws_bytes apart (a multiple of 256: every instance
+// base stays aligned) in one arena block that lives for one call.
+struct BatchBlock {
+  size_t ws = 0, c = 0;         // bytes per copy, copies per pass
+  bool strided = true;          // the copies fit the device's largest copy pitch (2 GiB): one 2D copy per pass
+  void* blk = nullptr;
+};
+
+// c = min(count, static-workspace limit / ws, 65535 (grid.y / grid.z limit), what the device can give): the copies must
+// also leave what the arena keeps in reserve (1 GiB) and the int8 engine's plane budget, because an engine that found
+// no room would fall back to DMMA and change the bits.
+static int batch_size(tncb_ctx* ctx, const tncb_plan* P, size_t count, BatchBlock* B) {
+  size_t dev_free = 0, dev_total = 0;
+  TNCB_CUDA(cudaMemGetInfo(&dev_free, &dev_total));
+  int max_pitch = 0;
+  TNCB_CUDA(cudaDeviceGetAttribute(&max_pitch, cudaDevAttrMaxPitch, ctx->device));
+  B->ws = P->ws_bytes;
+  B->strided = B->ws <= (size_t)max_pitch;
+  B->c = std::min<size_t>({static_ws_limit(dev_total) / B->ws, count, (size_t)65535});
+  if (B->c == 0) return fail(TNCB_ERR_OOM, "the workspace of one instance exceeds the static-workspace limit (TNCB_PLAN_WS_GB)");
+  bool int8 = false;
+  for (const Step& st : P->S.steps) int8 |= st.plan.kernel_class == 1 && ctx->oz_slices > 0;
+  const size_t keep = ((size_t)1 << 30) + (int8 ? ctx->crt_ws_bytes : 0);
+  const size_t room = dev_free + (ctx->arena.reserved - ctx->arena.live);
+  B->c = std::min(B->c, room > keep ? (room - keep) / B->ws : 0);
+  if (B->c == 0) return fail(TNCB_ERR_OOM, "no room on the device for the workspace of one instance");
+  return TNCB_OK;
+}
+
+// the block of c copies; c halves until it fits (a fragmented arena)
+static int batch_alloc(tncb_ctx* ctx, BatchBlock* B) {
+  int rc;
+  while ((rc = ctx->arena.alloc(B->c * B->ws, &B->blk)) == TNCB_ERR_OOM && B->c > 1) B->c = (B->c + 1) / 2;
+  return rc;
+}
+
+static void batch_free(tncb_ctx* ctx, BatchBlock* B) {
+  if (B->blk) ctx->arena.free(B->blk, B->c * B->ws);   // stream-ordered: the next user of the block queues behind the pass
+  B->blk = nullptr;
+}
+
+// n rows of `width` bytes, pitches dpitch / spitch, device to device: one strided copy, or one copy per row above the
+// largest copy pitch
+static int batch_copy(tncb_ctx* ctx, const BatchBlock& B, char* dst, size_t dpitch, const char* src, size_t spitch,
+                      size_t width, size_t n) {
+  cudaError_t e = cudaSuccess;
+  if (B.strided) e = cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, n, cudaMemcpyDeviceToDevice, ctx->stream);
+  else for (size_t i = 0; i < n && e == cudaSuccess; i++)
+    e = cudaMemcpyAsync(dst + i * dpitch, src + i * spitch, width, cudaMemcpyDeviceToDevice, ctx->stream);
+  return e == cudaSuccess ? TNCB_OK : fail(TNCB_ERR_CUDA, std::string("batched copy: ") + cudaGetErrorString(e));
+}
+
 } // namespace tncb
 
 extern "C" {
@@ -1264,27 +1345,7 @@ int tncb_plan_stage_slices(tncb_ctx* ctx, tncb_plan* plan, size_t n_slices, cons
   if (plan->sliced) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan stages its full network once (tncb_plan_stage)");
   if (plan->grad) return tncb::fail(TNCB_ERR_UNSUPPORTED, "gradient plans run one staged network at a time");
   if (!plan->is_static) return tncb::fail(TNCB_ERR_UNSUPPORTED, "sliced execution needs a plan with a static layout (no device leaves)");
-  const tncb::Schedule& S = plan->S;
-  TNCB_CUDA(cudaSetDevice(ctx->device));
-  int rc;
-  if ((rc = tncb::plan_device_state(ctx, plan))) return rc;
-  const size_t block = std::max<size_t>(S.leaf_block_elems, 1);
-  std::vector<std::complex<double>> host(block * n_slices);
-  for (size_t q = 0; q < n_slices; q++) {
-    if (!slice_tns[q]) return tncb::fail(TNCB_ERR_INVALID, "slice network is null");
-    std::vector<const tncb_tn*> leaves;
-    tncb::collect_leaf_nodes(slice_tns[q], leaves);
-    if ((rc = tncb::validate_leaves(S, leaves))) return rc;
-    if ((rc = tncb::stage_leaves(S, leaves, host.data() + q * block))) return rc;
-  }
-  TNCB_CUDA(cudaStreamSynchronize(ctx->stream));
-  if (plan->slices_dev) { ctx->arena.free(plan->slices_dev, plan->slices_bytes); plan->slices_dev = nullptr; }
-  plan->slices_bytes = host.size() * sizeof(double2);
-  if ((rc = ctx->arena.alloc(plan->slices_bytes, &plan->slices_dev))) return rc;
-  TNCB_CUDA(cudaMemcpyAsync(plan->slices_dev, host.data(), plan->slices_bytes, cudaMemcpyHostToDevice, ctx->stream));
-  TNCB_CUDA(cudaStreamSynchronize(ctx->stream));
-  plan->n_slices = n_slices;
-  return TNCB_OK;
+  return tncb::stage_networks(ctx, plan, n_slices, slice_tns, true);
 }
 
 int tncb_plan_run_slices(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t stride, tncb_tensor** out, int* n_out, uint64_t* out_legs) {
@@ -1354,58 +1415,151 @@ int tncb_plan_run_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
   const int r = (int)rm.dims.size();
   if (r + 1 > kMaxLegs) return fail(TNCB_ERR_INVALID, "a result of rank 64 leaves no room for the instance dimension");
   TNCB_CUDA(cudaSetDevice(ctx->device));
-  size_t dev_free = 0, dev_total = 0;
-  TNCB_CUDA(cudaMemGetInfo(&dev_free, &dev_total));
-  int max_pitch = 0;
-  TNCB_CUDA(cudaDeviceGetAttribute(&max_pitch, cudaDevAttrMaxPitch, ctx->device));
-  const size_t ws = plan->ws_bytes;                      // a multiple of 256: every instance base stays aligned
-  size_t c = std::min<size_t>({static_ws_limit(dev_total) / ws, count, (size_t)65535});   // (grid.y / grid.z limit)
-  if (c == 0) return fail(TNCB_ERR_OOM, "the workspace of one instance exceeds the static-workspace limit (TNCB_PLAN_WS_GB)");
-  {
-    // the copies must also leave what the arena keeps in reserve (1 GiB) and the int8 engine's plane budget: an engine
-    // that found no room would fall back to DMMA and change the bits
-    bool int8 = false;
-    for (const Step& st : S.steps) int8 |= st.plan.kernel_class == 1 && ctx->oz_slices > 0;
-    const size_t keep = ((size_t)1 << 30) + (int8 ? ctx->crt_ws_bytes : 0);
-    const size_t room = dev_free + (ctx->arena.reserved - ctx->arena.live);
-    c = std::min(c, room > keep ? (room - keep) / ws : 0);
-    if (c == 0) return fail(TNCB_ERR_OOM, "no room on the device for the workspace of one instance");
-  }
+  BatchBlock B;
+  int rc = batch_size(ctx, plan, count, &B);
+  if (rc) return rc;
   std::vector<uint64_t> dims(r + 1);
   dims[0] = count;
   for (int i = 0; i < r; i++) dims[i + 1] = rm.dims[i];
   tncb_tensor* res = nullptr;
-  int rc = tensor_new(ctx, r + 1, dims.data(), &res);
-  if (rc) return rc;
-  void* blk = nullptr;
-  while ((rc = ctx->arena.alloc(c * ws, &blk)) == TNCB_ERR_OOM && c > 1) c = (c + 1) / 2;   // (a fragmented arena)
-  if (rc) { tncb_tensor_free(ctx, res); return rc; }
-  const size_t blk_bytes = c * ws;
-  char* base = (char*)blk;
+  if ((rc = tensor_new(ctx, r + 1, dims.data(), &res))) return rc;
+  if ((rc = batch_alloc(ctx, &B))) { tncb_tensor_free(ctx, res); return rc; }
+  const size_t ws = B.ws, c = B.c;
+  char* base = (char*)B.blk;
   const size_t block_bytes = std::max<size_t>(S.leaf_block_elems, 1) * sizeof(double2);
   const size_t res_bytes = rm.elems * sizeof(double2);
-  // one strided copy per pass in each direction; a workspace above the device's largest copy pitch (2 GiB) takes one
-  // copy per instance instead
-  const bool strided = ws <= (size_t)max_pitch;
-  auto copy = [&](char* dst, size_t dpitch, const char* src, size_t spitch, size_t width, size_t n) {
-    cudaError_t e = cudaSuccess;
-    if (strided) e = cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, n, cudaMemcpyDeviceToDevice, ctx->stream);
-    else for (size_t i = 0; i < n && e == cudaSuccess; i++)
-      e = cudaMemcpyAsync(dst + i * dpitch, src + i * spitch, width, cudaMemcpyDeviceToDevice, ctx->stream);
-    return e == cudaSuccess ? TNCB_OK : fail(TNCB_ERR_CUDA, std::string("batched copy: ") + cudaGetErrorString(e));
-  };
   for (size_t done = 0; done < count && !rc; done += c) {
     const size_t n = std::min(c, count - done);
     const char* src = (const char*)plan->slices_dev + (first + done) * block_bytes;
-    if ((rc = copy(base + plan->leaf_off, ws, src, block_bytes, block_bytes, n))) break;
+    if ((rc = batch_copy(ctx, B, base + plan->leaf_off, ws, src, block_bytes, block_bytes, n))) break;
     if ((rc = enqueue_static(ctx, plan, base, (int)n, (long long)ws, 0, (int)plan->level_batched.size()))) break;
-    if (res_bytes) rc = copy((char*)res->ptr + done * res_bytes, res_bytes, base + plan->slot_off[S.result_slot], ws, res_bytes, n);
+    if (res_bytes) rc = batch_copy(ctx, B, (char*)res->ptr + done * res_bytes, res_bytes, base + plan->slot_off[S.result_slot], ws, res_bytes, n);
   }
-  ctx->arena.free(blk, blk_bytes);                        // stream-ordered: the next user of the block queues behind this pass
+  batch_free(ctx, &B);
   if (rc) { tncb_tensor_free(ctx, res); return rc; }
   if (out) *out = res; else tncb_tensor_free(ctx, res);
   if (n_out) *n_out = r;
   if (out_legs) for (int i = 0; i < r; i++) out_legs[i] = rm.legs[i];
+  return TNCB_OK;
+}
+
+// Instances of a gradient plan's structure for tncb_plan_vjp_batch: staged like tncb_plan_stage_slices stages them, but
+// without the plan's own workspace, which a batched pass does not use.
+int tncb_plan_stage_batch(tncb_ctx* ctx, tncb_plan* plan, size_t n, const tncb_tn* const* tns) {
+  using namespace tncb;
+  if (!ctx || !plan || !tns || n == 0) return fail(TNCB_ERR_INVALID, "null argument");
+  if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan has no batched gradients");
+  if (!plan->grad) return fail(TNCB_ERR_INVALID, "not a gradient plan (plain plans stage many networks with tncb_plan_stage_slices)");
+  return stage_networks(ctx, plan, n, tns, false);
+}
+
+// Instance-batched reverse mode.  Per pass of c instances on c workspace copies: leaf blocks in, forward levels, values
+// out, seeds in, backward levels, one gather launch that writes gradient rows and/or folds them into the sum.  Every
+// launch decision is the single-network one, so each instance is bit-identical to stage + run + tncb_plan_vjp; passes
+// run in stream order, so the sum is the left fold of the rows in instance order.
+int tncb_plan_vjp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t count, const tncb_tensor* seeds,
+                        tncb_tensor** values, tncb_tensor** grad_rows, tncb_tensor** grad_sum) {
+  using namespace tncb;
+  if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
+  if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan has no batched gradients");
+  if (!plan->grad) return fail(TNCB_ERR_INVALID, "not a gradient plan (tncb_plan_create_vjp)");
+  if (!plan->slices_dev || plan->ctx != ctx) return fail(TNCB_ERR_INVALID, "tncb_plan_stage_batch has not been called on this context");
+  if (count == 0 || first > plan->n_slices || count > plan->n_slices - first)
+    return fail(TNCB_ERR_INVALID, "instances [" + std::to_string(first) + ", " + std::to_string(first + count) + ") are not within the " +
+                                  std::to_string(plan->n_slices) + " staged networks");
+  if (!values && !grad_rows && !grad_sum) return fail(TNCB_ERR_INVALID, "no output requested");
+  const Schedule& S = plan->S;
+  const SlotMeta& rm = S.slots[S.result_slot];
+  const int r = (int)rm.dims.size();
+  if (r + 1 > kMaxLegs) return fail(TNCB_ERR_INVALID, "a result of rank 64 leaves no room for the instance dimension");
+  const bool grad = grad_rows || grad_sum;
+  if (seeds) {
+    bool same = seeds->rank == r + 1 && seeds->dims[0] == count;
+    for (int i = 0; same && i < r; i++) same = seeds->dims[i + 1] == rm.dims[i];
+    if (!same) return fail(TNCB_ERR_SHAPE, "the seeds' dims differ from [count, result dims]");
+    if (!seeds->ptr) return fail(TNCB_ERR_UNCONTRACTED, "the seed tensor has no storage");
+  } else if (grad && r > 0) return fail(TNCB_ERR_INVALID, "seeds are needed for a result of rank " + std::to_string(r));
+  TNCB_CUDA(cudaSetDevice(ctx->device));
+  BatchBlock B;
+  int rc = batch_size(ctx, plan, count, &B);
+  if (rc) return rc;
+  tncb_tensor *v = nullptr, *gr = nullptr, *gs = nullptr;
+  void* aux = nullptr;                 // the seed 1 of every copy (scalar result, NULL seeds), the K3 scratch of the sum
+  size_t aux_bytes = 0;
+  auto cleanup = [&]() {
+    batch_free(ctx, &B);
+    if (aux) ctx->arena.free(aux, aux_bytes);
+    for (tncb_tensor* t : {v, gr, gs}) if (t) tncb_tensor_free(ctx, t);
+  };
+  const uint64_t ge = plan->grad_elems;
+  if (values) {
+    std::vector<uint64_t> dims(r + 1);
+    dims[0] = count;
+    for (int i = 0; i < r; i++) dims[i + 1] = rm.dims[i];
+    rc = tensor_new(ctx, r + 1, dims.data(), &v);
+  }
+  if (!rc && grad_rows) { const uint64_t dims[2] = {count, ge}; rc = tensor_new(ctx, 2, dims, &gr); }
+  if (!rc && grad_sum) rc = tensor_new(ctx, 1, &ge, &gs);
+  if (!rc) rc = batch_alloc(ctx, &B);
+  const size_t ws = B.ws, c = B.c;
+  const size_t ones = grad && !seeds ? c : 0;
+  size_t scratch = 0;
+  if (grad_sum) for (const auto& gp : plan->grad_permutes) scratch = std::max<size_t>(scratch, S.slots[gp.slot].elems);
+  if (!rc && (ones || scratch)) {
+    aux_bytes = (ones + scratch) * sizeof(double2);
+    rc = ctx->arena.alloc(aux_bytes, &aux);
+    if (!rc && ones) {
+      const std::vector<double2> one(ones, double2{1.0, 0.0});
+      cudaError_t e = cudaMemcpyAsync(aux, one.data(), ones * sizeof(double2), cudaMemcpyHostToDevice, ctx->stream);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);      // `one` dies with this scope
+      if (e != cudaSuccess) rc = fail(TNCB_ERR_CUDA, std::string("seed copy: ") + cudaGetErrorString(e));
+    }
+  }
+  if (!rc && gs) {
+    cudaError_t e = cudaMemsetAsync(gs->ptr, 0, std::max<uint64_t>(ge, 1) * sizeof(double2), ctx->stream);
+    if (e != cudaSuccess) rc = fail(TNCB_ERR_CUDA, std::string("gradient sum: ") + cudaGetErrorString(e));
+  }
+  if (rc) { cleanup(); return rc; }
+  char* base = (char*)B.blk;
+  const double2* d_one = (const double2*)aux;
+  double2* d_scratch = (double2*)aux + ones;
+  const size_t block_bytes = std::max<size_t>(S.leaf_block_elems, 1) * sizeof(double2);
+  const size_t res_bytes = rm.elems * sizeof(double2);
+  const int n_levels = (int)plan->level_batched.size();
+  const GradItem* d_items = (const GradItem*)plan->grad_dev;
+  const long long* d_bs = (const long long*)((char*)plan->grad_dev + plan->grad_items.size() * sizeof(GradItem));
+  for (size_t done = 0; done < count && !rc; done += c) {
+    const size_t n = std::min(c, count - done);
+    const char* src = (const char*)plan->slices_dev + (first + done) * block_bytes;
+    if ((rc = batch_copy(ctx, B, base + plan->leaf_off, ws, src, block_bytes, block_bytes, n))) break;
+    if ((rc = enqueue_static(ctx, plan, base, (int)n, (long long)ws, 0, plan->n_fwd_levels))) break;
+    if (v && res_bytes &&
+        (rc = batch_copy(ctx, B, (char*)v->ptr + done * res_bytes, res_bytes, base + plan->slot_off[S.result_slot], ws, res_bytes, n))) break;
+    if (!grad) continue;
+    char* seed_dst = base + plan->slot_off[plan->seed_slot];
+    if (seeds) { if (res_bytes && (rc = batch_copy(ctx, B, seed_dst, ws, (const char*)seeds->ptr + done * res_bytes, res_bytes, res_bytes, n))) break; }
+    else if ((rc = batch_copy(ctx, B, seed_dst, ws, (const char*)d_one, sizeof(double2), sizeof(double2), n))) break;
+    if ((rc = enqueue_static(ctx, plan, base, (int)n, (long long)ws, plan->n_fwd_levels, n_levels))) break;
+    if (!plan->grad_items.empty() &&
+        (rc = launch_grad_gather_batch(ctx, d_items, d_bs, (int)plan->grad_items.size(), plan->grad_block_start.back(), base,
+                                       (long long)ws, (int)n, gr ? gr->ptr + done * ge : nullptr, (long long)ge, gs ? gs->ptr : nullptr))) break;
+    // leaves with more fused groups than a GradItem holds: K3 per instance, in instance order
+    for (size_t i = 0; i < n && !rc; i++)
+      for (size_t k = 0; k < plan->grad_permutes.size() && !rc; k++) {
+        const auto& gp = plan->grad_permutes[k];
+        const SlotMeta& sm = S.slots[gp.slot];
+        const double2* adj = (const double2*)(base + i * ws + plan->slot_off[gp.slot]);
+        if (gr) rc = launch_permute(ctx, adj, gr->ptr + (done + i) * ge + gp.dst, (int)sm.dims.size(), sm.dims.data(), gp.perm.data());
+        if (!rc && gs) rc = launch_permute(ctx, adj, d_scratch, (int)sm.dims.size(), sm.dims.data(), gp.perm.data());
+        if (!rc && gs) rc = launch_add(ctx, gs->ptr + gp.dst, d_scratch, sm.elems);
+      }
+  }
+  if (rc) { cleanup(); return rc; }
+  batch_free(ctx, &B);
+  if (aux) ctx->arena.free(aux, aux_bytes);
+  if (values) *values = v;
+  if (grad_rows) *grad_rows = gr;
+  if (grad_sum) *grad_sum = gs;
   return TNCB_OK;
 }
 

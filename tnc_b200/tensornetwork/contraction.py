@@ -208,6 +208,10 @@ class NetworkPlan:
         check(self.ctx._l.tncb_plan_create_vjp(self.ctx.handle, C.byref(c_tn), C.byref(c_path), mask, C.byref(h)))
         self.handle = h
         self.leaf_shapes = shapes
+        n_out, legs, dims = C.c_int(), u64_array([0] * 64), u64_array([0] * 64)
+        check(self.ctx._l.tncb_network_out_legs(C.byref(c_tn), C.byref(c_path), C.byref(n_out), legs, dims))
+        self.result_legs = [legs[i] for i in range(n_out.value)]
+        self.result_dims = tuple(int(dims[i]) for i in range(n_out.value))
         return self
 
     def grad_offsets(self) -> List[int]:
@@ -237,6 +241,58 @@ class NetworkPlan:
             if off >= 0:
                 grads[i] = flat[off:off + int(np.prod(shape, dtype=np.int64))].reshape(shape)
         return grads
+
+    def stage_batch(self, nets) -> None:
+        """Materialise + upload the leaves of many networks of a gradient plan's structure once (tncb_plan_stage_batch):
+        bitstrings, angle sets or input states for `vjp_batch`.  The plan's own staged leaves stay as they are."""
+        m = _Marshal()
+        nodes = [m.tn(t) for t in nets]
+        ptrs = (C.POINTER(TncbTn) * max(len(nodes), 1))(*[C.pointer(n) for n in nodes])
+        check(self.ctx._l.tncb_plan_stage_batch(self.ctx.handle, self.handle, len(nodes), ptrs))
+        self.n_staged = len(nodes)
+
+    def vjp_batch(self, first: int = 0, count: Optional[int] = None, seeds=None, rows: bool = True, sum: bool = False,
+                  values: bool = True):
+        """Forward and backward of the staged networks first .. first + count - 1, each on its own, the instances as a
+        grid dimension of every kernel (tncb_plan_vjp_batch).  count=None: every staged network from `first` on.
+        seeds: [count, *result dims] array or DeviceTensor; None for a scalar result (seed 1) or without gradients.
+        Returns (legs of one instance, values [count, *dims] or None, {leaf: [count, *leaf shape]} or None,
+        {leaf: leaf-shaped sum over the instances} or None).  Row i equals stage(net_i) + run + vjp(seed_i) bit for bit;
+        the sum is the left fold of the rows in instance order, also bit for bit."""
+        if count is None:
+            count = max(0, getattr(self, "n_staged", 0) - int(first))
+        tmp = None
+        if seeds is not None and not isinstance(seeds, DeviceTensor):
+            seeds = tmp = DeviceTensor.from_numpy(self.ctx, np.asarray(seeds, dtype=np.complex128))
+        outs = [C.c_void_p() if want else None for want in (values, rows, sum)]
+        try:
+            check(self.ctx._l.tncb_plan_vjp_batch(self.ctx.handle, self.handle, int(first), int(count),
+                                                  seeds.handle if seeds is not None else None,
+                                                  *[C.byref(o) if o is not None else None for o in outs]))
+        finally:
+            if tmp is not None:
+                tmp.free()
+        host = []
+        for o in outs:
+            if o is None:
+                host.append(None)
+                continue
+            dt = DeviceTensor.adopt(self.ctx, o)
+            host.append(dt.to_numpy())
+            dt.free()
+        vals, row_block, sum_block = host
+        offs = self.grad_offsets()
+
+        def unpack(block, lead):
+            if block is None:
+                return None
+            out = {}
+            for i, (off, shape) in enumerate(zip(offs, self.leaf_shapes)):
+                if off >= 0:
+                    size = int(np.prod(shape, dtype=np.int64))
+                    out[i] = block[..., off:off + size].reshape(lead + tuple(shape))
+            return out
+        return (list(self.result_legs), vals, unpack(row_block, (int(count),)), unpack(sum_block, ()))
 
     def info(self) -> dict:
         n, k = C.c_uint64(), C.c_uint64()
