@@ -385,6 +385,32 @@ int tncb_plan_stage_batch(tncb_ctx* ctx, tncb_plan* plan, size_t n, const tncb_t
  * TNCB_ERR_SHAPE; not even one workspace copy fits -> TNCB_ERR_OOM.  Errors leave the arena as they found it. */
 int tncb_plan_vjp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t count, const tncb_tensor* seeds,
                         tncb_tensor** values, tncb_tensor** grad_rows, tncb_tensor** grad_sum);
+/* ---- leaf payloads from device memory (e.g. torch CUDA tensors): no host round trip ----
+ * A source is row-major complex128 (re, im) in the leaf's own leg order, 16-byte aligned, in device (or managed) memory of
+ * the ctx's device.  The library copies it (one launch of leaf_stage_kernel on the ctx stream, asynchronous); the caller
+ * orders its writes before the call and keeps the memory alive until the ctx stream has passed the call.
+ * Validation is complete before any copy, and a failure leaves every staged state untouched: a leaf index out of range,
+ * listed twice or naming a leaf without a payload, a null / misaligned source, one that is not device memory of the ctx's
+ * device, or whose bytes run past the end of the allocation that holds it (cuMemGetAddressRange) -> TNCB_ERR_INVALID;
+ * plans with TNCB_DATA_DEVICE leaves -> TNCB_ERR_UNSUPPORTED.
+ *
+ * Overwrite the payloads of leaves leaf_index[0..n) of a STAGED plan with device memory: src[k] points to the leaf's
+ * elements.  The payloads go where the next run reads them: a static plan's leaf block (also replayed by its graph), a
+ * non-static plan's resident block, a sliced gradient plan's full leaf block (leaf indices and shapes of the full
+ * network).  A gradient plan then needs a new forward run before tncb_plan_vjp.  They stay in place across runs,
+ * tncb_plan_vjp and tncb_plan_vjp_sliced, as staged leaves do.  Not staged on this ctx (tncb_plan_stage) ->
+ * TNCB_ERR_INVALID. */
+int tncb_plan_set_leaves(tncb_ctx* ctx, tncb_plan* plan, size_t n, const uint64_t* leaf_index, const void* const* src);
+/* Stage n_instances networks of the plan's structure: every leaf from the host template `tmpl` (validated as
+ * tncb_plan_stage validates a network; materialised and uploaded ONCE, whatever n_instances is), except leaves
+ * leaf_index[0..n), whose instance i reads src[k] + i * instance_stride[k] elements (stride 0 = the same device payload
+ * in every instance; a non-zero stride below the leaf's element count -> TNCB_ERR_INVALID).  Plain plans: replaces
+ * tncb_plan_stage_slices (feeds run_slices / run_batch; needs a static plan, else TNCB_ERR_UNSUPPORTED).  Gradient plans:
+ * replaces tncb_plan_stage_batch (feeds vjp_batch; the plan's own workspace is not allocated).  Staged instances are
+ * bit-identical to the host-staged networks with the same payloads.  n_instances == 0 -> TNCB_ERR_INVALID; a sliced
+ * gradient plan -> TNCB_ERR_UNSUPPORTED (it uses tncb_plan_set_leaves). */
+int tncb_plan_stage_instances(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tmpl, size_t n_instances,
+                              size_t n, const uint64_t* leaf_index, const void* const* src, const uint64_t* instance_stride);
 void tncb_plan_destroy(tncb_plan* plan);
 
 /* ---- HDF5 tensor files: replaces tnc::io::hdf5 (tnc/src/io/hdf5.rs), which binds libhdf5 through hdf5-metno.

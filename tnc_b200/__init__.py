@@ -163,6 +163,44 @@ class DeviceTensor:
     def device_ptr(self) -> int:
         return int(self.ctx._l.tncb_tensor_device_ptr(self.handle) or 0)
 
+    def _torch_view(self):
+        """float64 [elements, 2] torch view of the device memory (no copy; valid while this tensor lives)"""
+        import torch
+        elems = int(np.prod(self.shape, dtype=np.int64))
+        return torch.as_tensor(_CudaArray(self.device_ptr(), elems), device=torch.device("cuda", self.ctx.device))
+
+    def to_torch(self):
+        """A torch complex128 tensor on the context's device with this tensor's shape: a device-to-device copy on the
+        context stream, after the library's work there; torch's current stream waits for it."""
+        import torch
+        if self.handle is None:
+            raise TncbError(-3, "Cannot convert uncontracted tensor to data")
+        cur, ext = torch_streams(self.ctx)
+        out = torch.empty(self.shape, dtype=torch.complex128, device=cur.device)
+        if out.numel():
+            ext.wait_stream(cur)                 # out's block may still be read or written by earlier torch work
+            with torch.cuda.stream(ext):
+                torch.view_as_real(out).view(-1, 2).copy_(self._torch_view())
+            cur.wait_stream(ext)
+        return out
+
+    @classmethod
+    def from_torch(cls, ctx: Context, t) -> "DeviceTensor":
+        """A library tensor holding a copy of the torch CUDA tensor `t` (on the context's device; cast to complex128 on
+        the device).  The copy runs on the context stream after torch's current stream, and torch's current stream then
+        waits for it, so `t`'s memory is not handed to later work before the copy has read it."""
+        import torch
+        check_cuda_tensor(ctx, t, "the tensor")
+        src = t.detach().to(torch.complex128).contiguous()
+        out = cls.empty(ctx, tuple(src.shape))
+        if src.numel():
+            cur, ext = torch_streams(ctx)
+            ext.wait_stream(cur)
+            with torch.cuda.stream(ext):
+                out._torch_view().copy_(torch.view_as_real(src).reshape(-1, 2))
+            cur.wait_stream(ext)
+        return out
+
     def release(self):
         """Give up ownership (the C side consumed the handle)."""
         h, self.handle = self.handle, None
@@ -178,6 +216,31 @@ class DeviceTensor:
             self.free()
         except Exception:
             pass
+
+
+class _CudaArray:
+    """__cuda_array_interface__ of `elems` complex128 at device address `ptr`, as float64 [elems, 2]"""
+
+    def __init__(self, ptr: int, elems: int):
+        self.__cuda_array_interface__ = {"shape": (elems, 2), "typestr": "<f8", "data": (ptr, False), "version": 3,
+                                         "strides": None}
+
+
+def torch_streams(ctx: Context):
+    """(torch's current stream, the context stream as a torch stream) on the context's device"""
+    import torch
+    dev = torch.device("cuda", ctx.device)
+    return torch.cuda.current_stream(dev), torch.cuda.ExternalStream(ctx.stream, device=dev)
+
+
+def check_cuda_tensor(ctx: Context, t, what: str) -> None:
+    """ValueError unless `t` is a torch tensor on the context's CUDA device"""
+    import torch
+    if not isinstance(t, torch.Tensor) or not t.is_cuda:
+        raise ValueError(f"{what} must be a torch CUDA tensor, got {type(t).__name__}"
+                         + (f" on {t.device}" if isinstance(t, torch.Tensor) else ""))
+    if t.device.index != ctx.device:
+        raise ValueError(f"{what} is on {t.device}, the context on cuda:{ctx.device}")
 
 
 def tcgen05_bound(k: int, rel: float = 0.0, n_moduli: int = 0) -> dict:

@@ -116,6 +116,8 @@ SIGNATURES = {
     "tncb_plan_vjp_sliced": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, vpp, vpp]),
     "tncb_plan_stage_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.POINTER(TncbTn))]),
     "tncb_plan_vjp_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, vpp, vpp, vpp]),
+    "tncb_plan_set_leaves": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, u64p, vpp]),
+    "tncb_plan_stage_instances": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(TncbTn), C.c_size_t, C.c_size_t, u64p, vpp, u64p]),
     "tncb_plan_destroy": (None, [C.c_void_p]),
     "tncb_comm_unique_id": (C.c_int, [C.c_void_p]),
     "tncb_comm_init": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p]),

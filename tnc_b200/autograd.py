@@ -8,7 +8,8 @@ Gate angles differentiate through ordinary torch code that builds the gate matri
 angle-derivative table.  One backward pass gives the gradient of every input, at about two forward passes of cost.
 With `sliced_legs`, a network whose gradient workspace does not fit unsliced runs slice by slice (SlicedPlan.for_gradients).
 With `batched`, B networks that differ in some leaves (bitstrings, input states) run in one batched pass
-(NetworkPlan.vjp_batch) and the result gets a leading dimension B."""
+(NetworkPlan.vjp_batch) and the result gets a leading dimension B.  With `on_device=True`, CUDA inputs are copied into the
+staged plan on the device and the result and gradients come back as CUDA tensors."""
 from __future__ import annotations
 
 from typing import Optional, Sequence
@@ -16,10 +17,10 @@ from typing import Optional, Sequence
 import numpy as np
 import torch
 
-from . import Context, default_context
+from . import Context, DeviceTensor, check_cuda_tensor, default_context
 from .contractionpath import ContractionPath
 from .contractionpath.slicing import SlicedPlan
-from .tensornetwork import NetworkPlan, Tensor, leaves
+from .tensornetwork import NetworkPlan, PreparedNetwork, Tensor, leaves
 from .tensornetwork.tensordata import TensorData
 
 
@@ -40,7 +41,7 @@ class _NetworkFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, runner, *xs):
         ctx.runner = runner
-        ctx.token = runner._forward(xs)
+        ctx.token = runner._forward_device(xs) if runner.on_device else runner._forward(xs)
         ctx.save_for_backward(*xs)
         return runner._result
 
@@ -48,6 +49,8 @@ class _NetworkFn(torch.autograd.Function):
     def backward(ctx, grad_out):
         xs = ctx.saved_tensors           # raises on a second backward through a graph that was not retained
         runner = ctx.runner
+        if runner.on_device:
+            return (None,) + runner._backward_device(ctx, grad_out, xs)
         seed = np.conj(grad_out.detach().to(torch.complex128).cpu().numpy())
         if runner.batched:               # vjp_batch runs forward and backward of every instance: it only needs them staged
             if runner._token != ctx.token:
@@ -69,7 +72,7 @@ class NetworkFunction:
     """The callable network_function returns: inputs -> contracted result, differentiable in every input."""
 
     def __init__(self, tn: Tensor, path: ContractionPath, wrt: Sequence[int], ctx: Optional[Context] = None,
-                 sliced_legs: Sequence[int] = (), batched: Sequence[int] = ()):
+                 sliced_legs: Sequence[int] = (), batched: Sequence[int] = (), on_device: bool = False):
         self.wrt = [int(i) for i in wrt]
         lv = leaves(tn)
         for i in self.wrt:
@@ -93,6 +96,105 @@ class NetworkFunction:
         else:
             self.plan = NetworkPlan.for_gradients(tn, path, self.wrt, ctx=ctx or default_context())
         self._token, self._count, self._result = None, 0, None
+        self.on_device = bool(on_device)
+        self._staged = False             # on_device: the template network is staged (unbatched and sliced)
+        self._template = None            # on_device, batched: the network marshalled once
+        self._offsets = None
+
+    # ---- on_device: inputs, results and gradients stay on the GPU ----
+    def _check_device(self, xs):
+        for i, x in zip(self.inputs, xs):
+            check_cuda_tensor(self.plan.ctx, x, f"input for leaf {i}")
+
+    def _set_device(self, xs):
+        """the inputs as the wrt leaves' payloads, copied on the device into the staged network (staged once, from the
+        network's own payloads, on first use)"""
+        self._check_device(xs)
+        for i, shape, x in zip(self.wrt, self.shapes, xs):
+            if tuple(x.shape) != shape:
+                raise ValueError(f"input for leaf {i} has shape {tuple(x.shape)}, the leaf {shape}")
+        if not self._staged:
+            self.plan.stage(self.tn)
+            self._staged = True
+        self.plan.set_leaves(dict(zip(self.wrt, xs)))
+        self._count += 1
+        self._token = self._count
+        return self._token
+
+    def _stage_instances(self, xs):
+        """B instances staged from device memory: batched inputs row by row, the others shared"""
+        self._check_device(xs)
+        b = self._batch_size(xs)
+        if self._template is None:
+            self._template = PreparedNetwork(self.tn)
+        self.plan.stage_instances(self._template, dict(zip(self.inputs, xs)), b)
+        self._count += 1
+        self._token = self._count
+        return self._token
+
+    def _split(self, block, lead=()):
+        """{wrt leaf: its slice of a [..., grad_elems] torch gradient block, shaped lead + leaf shape}"""
+        if self._offsets is None:
+            self._offsets = self.plan.grad_offsets()
+        out = {}
+        for i, shape in zip(self.wrt, self.shapes):
+            off = self._offsets[i]
+            out[i] = block[..., off:off + int(np.prod(shape, dtype=np.int64))].reshape(tuple(lead) + shape)
+        return out
+
+    def _forward_device(self, xs):
+        if self.batched:
+            token = self._stage_instances(xs)
+            vals = self.plan.vjp_batch_blocks(0, None, rows=False, sum=False, values=True)[0]
+        else:
+            token = self._set_device(xs)
+            vals = self.plan.run().tensordata.matrix
+        self._result = vals.to_torch()
+        vals.free()
+        return token
+
+    def _backward_device(self, fctx, grad_out, xs):
+        seed = DeviceTensor.from_torch(self.plan.ctx, torch.conj_physical(grad_out.detach().to(torch.complex128)))
+        try:
+            if self.batched:
+                if self._token != fctx.token:
+                    fctx.token = self._stage_instances(xs)
+                return self._batch_grads_device(seed, xs)
+            if self.sliced:
+                if self._token != fctx.token:
+                    fctx.token = self._set_device(xs)
+                value, block = self.plan.vjp_blocks(seed)
+                value.free()
+            else:
+                if self._token != fctx.token:
+                    fctx.token = self._forward_device(xs)
+                self._token = None
+                block = self.plan.vjp_block(seed)
+            flat = torch.conj_physical(block.to_torch())
+            block.free()
+        finally:
+            seed.free()
+        g = self._split(flat)
+        return tuple(g[i] for i in self.wrt)
+
+    def _batch_grads_device(self, seed, xs):
+        want_rows = any(i in self.batched for i in self.wrt)
+        want_sum = any(i not in self.batched for i in self.wrt)
+        _, rows, total = self.plan.vjp_batch_blocks(0, None, seeds=seed, rows=want_rows, sum=want_sum, values=False)
+        blocks = []
+        for dt in (rows, total):
+            blocks.append(None if dt is None else torch.conj_physical(dt.to_torch()))
+            if dt is not None:
+                dt.free()
+        rows_g = self._split(blocks[0], (self.plan.n_staged,)) if want_rows else {}
+        sum_g = self._split(blocks[1]) if want_sum else {}
+        grads = []
+        for i in self.inputs:
+            if i not in self.wrt:
+                grads.append(None)
+            else:
+                grads.append(rows_g[i] if i in self.batched else sum_g[i])
+        return tuple(grads)
 
     def _stage(self, xs):
         """stage the inputs as the wrt leaves' payloads (through the host)"""
@@ -172,14 +274,14 @@ class NetworkFunction:
 
 
 def network_function(tn: Tensor, path: ContractionPath, wrt: Sequence[int], ctx: Optional[Context] = None,
-                     sliced_legs: Sequence[int] = (), batched: Sequence[int] = ()) -> NetworkFunction:
+                     sliced_legs: Sequence[int] = (), batched: Sequence[int] = (), on_device: bool = False) -> NetworkFunction:
     """A torch.autograd.Function over the network `tn` contracted along `path`: the returned callable takes one torch
     complex128 tensor per leaf index in `wrt` (indices into leaves(tn); each must be a Matrix leaf) and returns the
     contracted result as a torch tensor.  Its backward is conj(vjp(conj(grad_out))) of the gradient plan, torch's
     convention for complex inputs.
 
     Forward = stage + run: the inputs are copied to the host and staged the way NetworkPlan.stage stages any payload
-    (no device-side staging of torch tensors).  A backward needs the plan's forward state: when another call of the
+    (with on_device=False, the default; see below).  A backward needs the plan's forward state: when another call of the
     same function ran in between, or a retained graph is differentiated again, the backward re-runs the forward from
     the saved inputs first.  A second backward through a graph that was not retained raises torch's error.
 
@@ -196,5 +298,11 @@ def network_function(tn: Tensor, path: ContractionPath, wrt: Sequence[int], ctx:
     of every instance (NetworkPlan.vjp_batch, values only); backward = vjp_batch with seeds conj(grad_out), a forward
     plus backward pass of every instance: per-instance gradient rows for batched inputs in `wrt`, their sum over the
     instances for shared ones.  About 4 forward passes per forward + backward in all, against about 3 for one
-    unbatched network; the instances share every launch.  Not combinable with sliced_legs."""
-    return NetworkFunction(tn, path, wrt, ctx, sliced_legs, batched)
+    unbatched network; the instances share every launch.  Not combinable with sliced_legs.
+
+    on_device=True: the inputs must be torch CUDA tensors on the context's device (else ValueError), and the result and
+    the gradients are CUDA tensors there; no payload, result or gradient goes through the host.  The first call stages
+    `tn` itself; every call then copies the inputs into the staged network on the device (NetworkPlan.set_leaves, or
+    NetworkPlan.stage_instances of the network marshalled once with `batched`), ordered against torch's current stream
+    both ways.  Values and gradients equal those of on_device=False bit for bit."""
+    return NetworkFunction(tn, path, wrt, ctx, sliced_legs, batched, on_device)

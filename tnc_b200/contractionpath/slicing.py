@@ -217,10 +217,25 @@ class SlicedPlan:
         """(value, {leaf index: G}) summed over the slices rank, rank + world, ...: value is bit-identical to `run`, G has
         the full leaf's shape with G[e] = sum_r seed[r] dR[r]/dX[e] (no conjugation).  seed: array or DeviceTensor with
         the result's shape, None for a scalar result.  With world > 1 and allreduce, both are summed over the ranks."""
+        from ..tensornetwork.tensordata import TensorData
+        value, block = self.vjp_blocks(seed, rank, world, allreduce)
+        flat = block.to_numpy()
+        block.free()
+        grads = {}
+        for i, (off, shape) in enumerate(zip(self.plan.grad_offsets(), self.plan.leaf_shapes)):
+            if off >= 0:
+                grads[i] = flat[off:off + int(np.prod(shape, dtype=np.int64))].reshape(shape)
+        if self._legs is None:        # the result's leg order: an empty slice range returns it without running a kernel
+            self._legs = list(self.plan.run_slices(self.n_slices, 1).legs)
+        res = Tensor(self._legs, value.shape)
+        res.set_tensor_data(TensorData.Matrix(value))
+        return res, grads
+
+    def vjp_blocks(self, seed=None, rank: int = 0, world: int = 1, allreduce: bool = True):
+        """`vjp` left on the device: (value, rank-1 gradient block at grad_offsets()) as DeviceTensors"""
         import ctypes as C
         from .. import DeviceTensor
         from .._lib import check
-        from ..tensornetwork.tensordata import TensorData
         ctx = self.ctx
         tmp = None
         if seed is not None and not isinstance(seed, DeviceTensor):
@@ -236,17 +251,15 @@ class SlicedPlan:
         if world > 1 and allreduce:
             check(ctx._l.tncb_comm_allreduce_sum(ctx.handle, value.handle))
             check(ctx._l.tncb_comm_allreduce_sum(ctx.handle, block.handle))
-        flat = block.to_numpy()
-        block.free()
-        grads = {}
-        for i, (off, shape) in enumerate(zip(self.plan.grad_offsets(), self.plan.leaf_shapes)):
-            if off >= 0:
-                grads[i] = flat[off:off + int(np.prod(shape, dtype=np.int64))].reshape(shape)
-        if self._legs is None:        # the result's leg order: an empty slice range returns it without running a kernel
-            self._legs = list(self.plan.run_slices(self.n_slices, 1).legs)
-        res = Tensor(self._legs, value.shape)
-        res.set_tensor_data(TensorData.Matrix(value))
-        return res, grads
+        return value, block
+
+    def set_leaves(self, payloads: dict) -> None:
+        """New payloads for leaves of the staged FULL network straight from device memory ({leaf index: torch CUDA tensor
+        shaped like the full leaf}, see NetworkPlan.set_leaves); the next run / vjp slices them on the device.  Sliced
+        gradient plans only (SlicedPlan.for_gradients)."""
+        if self.sn is not None:
+            raise TypeError("set_leaves needs a sliced gradient plan (SlicedPlan.for_gradients); this plan stages every slice on the host")
+        self.plan.set_leaves(payloads)
 
     def run(self, rank: int = 0, world: int = 1, allreduce: bool = True) -> Tensor:
         from .._lib import check

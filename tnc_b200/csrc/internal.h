@@ -204,6 +204,25 @@ int launch_slice_extract(tncb_ctx* ctx, const SliceItem* d_items, const long lon
 int launch_grad_accumulate(tncb_ctx* ctx, const SliceItem* d_items, const long long* d_block_start, int n_items,
                            long long total_blocks, const char* ws, const double2* scratch, double2* grad, unsigned long long q);
 
+// ---- device staging of leaf payloads (tncb_plan_set_leaves / tncb_plan_stage_instances): copies from arbitrary device
+// addresses into leaf blocks, n instances per launch.  Items never overlap; the table travels as a kernel parameter ----
+constexpr int kStageThreads = 256;  // elements per block
+constexpr int kStageItems = 512;    // items per launch (table + prefix: 20.5 KB of the 32 KB parameter space)
+struct LeafStageItem {
+  const double2* src;           // instance i reads src + i * src_stride
+  unsigned long long src_stride; // elements between instances, 0 = the same payload for every instance
+  long long dst;                // element offset in the leaf block
+  long long elems;
+};
+struct LeafStageBatch {
+  int n, _pad;
+  long long block_start[kStageItems + 1];   // block-count prefix
+  LeafStageItem items[kStageItems];
+};
+// instance i's leaf block at dst + i * block_elems; any number of items and instances (several launches if needed)
+int launch_leaf_stage(tncb_ctx* ctx, const LeafStageItem* items, size_t n_items, double2* dst, long long block_elems,
+                      size_t n_instances);
+
 int tensor_new(tncb_ctx* ctx, int rank, const uint64_t* dims, tncb_tensor** out);
 
 // TensorData::File leaf (hdf5io.cpp): first member of /tensors, optionally adjointed, checked against the leaf's dims

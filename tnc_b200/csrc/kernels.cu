@@ -1329,4 +1329,54 @@ int launch_grad_accumulate(tncb_ctx* ctx, const SliceItem* d_items, const long l
   return TNCB_OK;
 }
 
+// ------------------------------------------------------------------------------------------
+// Device staging of leaf payloads (tncb_plan_set_leaves / tncb_plan_stage_instances): every leaf that takes a device
+// payload, and the runs of template leaves between them, copied into the leaf blocks of n instances by ONE launch, the
+// instance a grid dimension.  A block copies kStageThreads consecutive elements of one item, found by binary search over
+// the block-count prefix (as grad_gather_kernel does); one 16-byte load and store per element.  The item table is a
+// __grid_constant__ parameter: read in place, no host-to-device copy and nothing to keep alive after the launch.
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kStageThreads)
+leaf_stage_kernel(const __grid_constant__ LeafStageBatch batch, double2* __restrict__ dst, long long block_elems,
+                  unsigned long long inst0) {
+  const long long b = blockIdx.x;
+  int lo = 0, hi = batch.n;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (batch.block_start[mid] <= b) lo = mid; else hi = mid;
+  }
+  const LeafStageItem& it = batch.items[lo];
+  const long long o = (b - batch.block_start[lo]) * kStageThreads + threadIdx.x;
+  if (o >= it.elems) return;
+  const unsigned long long inst = inst0 + blockIdx.y;
+  dst[(long long)inst * block_elems + it.dst + o] = __ldg(it.src + inst * it.src_stride + o);
+}
+
+int launch_leaf_stage(tncb_ctx* ctx, const LeafStageItem* items, size_t n_items, double2* dst, long long block_elems,
+                      size_t n_instances) {
+  static thread_local LeafStageBatch batch;     // 20.5 KB, kept off the host stack; the launch copies it
+  for (size_t i = 0; i < n_items;) {
+    batch.n = 0;
+    batch.block_start[0] = 0;
+    for (; i < n_items && batch.n < kStageItems; i++) {
+      if (items[i].elems <= 0) continue;
+      const long long nb = (items[i].elems + kStageThreads - 1) / kStageThreads;
+      if (batch.n > 0 && batch.block_start[batch.n] + nb > 0x7fffffffLL) break;   // grid.x limit: next launch
+      if (nb > 0x7fffffffLL) return fail(TNCB_ERR_UNSUPPORTED, "a leaf too large for one staging launch");
+      batch.items[batch.n] = items[i];
+      batch.block_start[batch.n + 1] = batch.block_start[batch.n] + nb;
+      batch.n++;
+    }
+    const long long blocks = batch.block_start[batch.n];
+    if (blocks == 0) continue;
+    for (size_t f = 0; f < n_instances; f += 65535) {    // grid.y limit
+      const unsigned ny = (unsigned)std::min<size_t>(65535, n_instances - f);
+      leaf_stage_kernel<<<dim3((unsigned)blocks, ny), kStageThreads, 0, ctx->stream>>>(batch, dst, block_elems, f);
+      ctx->launches++;
+      TNCB_CUDA(cudaGetLastError());
+    }
+  }
+  return TNCB_OK;
+}
+
 } // namespace tncb

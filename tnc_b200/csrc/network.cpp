@@ -8,6 +8,7 @@
 // on the context stream without host round trips.  Arena memory of consumed operands is
 // recycled in stream order.
 #include "internal.h"
+#include <cuda.h>
 #include <algorithm>
 #include <complex>
 #include <cstdio>
@@ -352,6 +353,11 @@ struct tncb_plan {
   size_t sl_off[7] = {};                            // byte offsets inside sl_dev: 3 item arrays, 3 prefixes, seed 1 (+ scratch)
   void* full_dev = nullptr; size_t full_bytes = 0;  // the staged full leaf block (outside the workspace)
   bool full_staged = false;
+  // tncb_plan_stage_instances: the template's leaves that take no device payload, packed, in plan-owned pinned memory
+  // (re-used once tmpl_ev says its last upload ran) and on the device
+  void* tmpl_host = nullptr; void* tmpl_dev = nullptr; size_t tmpl_bytes = 0;
+  cudaEvent_t tmpl_ev = nullptr;
+  bool tmpl_busy = false;
 };
 
 namespace tncb {
@@ -481,20 +487,26 @@ static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) 
   for (const Step& st : S.steps) if (st.plan.kernel_class == 1) { P->graphable = false; break; }   // K1/K1' use ctx-owned tables / arena scratch
 }
 
+// the payload of one leaf into `dst`
+static int stage_leaf(const tncb_tn* lf, std::complex<double>* dst) {
+  if (lf->kind == TNCB_DATA_GATE) {
+    int cnt = gate_matrix(lf->gate_name, lf->gate_angles, lf->n_gate_angles, lf->gate_adjoint != 0, dst);
+    if (cnt < 0) return cnt;
+  } else if (lf->kind == TNCB_DATA_MATRIX) {
+    uint64_t e = 1; for (int i = 0; i < lf->rank; i++) e *= lf->dims[i];
+    std::memcpy(dst, lf->host_re_im, e * sizeof(double2));
+  } else if (lf->kind == TNCB_DATA_FILE) {      // into_data for TensorData::File (tensordata.rs:43-49)
+    int rc = h5::load_file_leaf(lf->file_path, lf->file_adjoint != 0, lf->rank, lf->dims, (double*)dst);
+    if (rc) return rc;
+  }
+  return TNCB_OK;
+}
+
 static int stage_leaves(const Schedule& S, const std::vector<const tncb_tn*>& leaves, std::complex<double>* stage) {
   for (size_t li = 0; li < leaves.size(); li++) {
-    const tncb_tn* lf = leaves[li];
-    if (S.leaf_kind[li] != lf->kind) return fail(TNCB_ERR_INVALID, "network payload kinds do not match the plan");
-    if (lf->kind == TNCB_DATA_GATE) {
-      int cnt = gate_matrix(lf->gate_name, lf->gate_angles, lf->n_gate_angles, lf->gate_adjoint != 0, stage + S.leaf_offset[li]);
-      if (cnt < 0) return cnt;
-    } else if (lf->kind == TNCB_DATA_MATRIX) {
-      uint64_t e = 1; for (int i = 0; i < lf->rank; i++) e *= lf->dims[i];
-      std::memcpy(stage + S.leaf_offset[li], lf->host_re_im, e * sizeof(double2));
-    } else if (lf->kind == TNCB_DATA_FILE) {      // into_data for TensorData::File (tensordata.rs:43-49)
-      int rc = h5::load_file_leaf(lf->file_path, lf->file_adjoint != 0, lf->rank, lf->dims, (double*)(stage + S.leaf_offset[li]));
-      if (rc) return rc;
-    }
+    if (S.leaf_kind[li] != leaves[li]->kind) return fail(TNCB_ERR_INVALID, "network payload kinds do not match the plan");
+    int rc = stage_leaf(leaves[li], stage + S.leaf_offset[li]);
+    if (rc) return rc;
   }
   return TNCB_OK;
 }
@@ -998,6 +1010,66 @@ static int batch_copy(tncb_ctx* ctx, const BatchBlock& B, char* dst, size_t dpit
   else for (size_t i = 0; i < n && e == cudaSuccess; i++)
     e = cudaMemcpyAsync(dst + i * dpitch, src + i * spitch, width, cudaMemcpyDeviceToDevice, ctx->stream);
   return e == cudaSuccess ? TNCB_OK : fail(TNCB_ERR_CUDA, std::string("batched copy: ") + cudaGetErrorString(e));
+}
+
+// ---- leaf payloads from device memory (tncb_plan_set_leaves / tncb_plan_stage_instances) ----
+// cuMemGetAddressRange, resolved through the runtime as crt.cu resolves cuTensorMapEncodeTiled: the allocation that holds
+// a device address, so that a source range running past its end is refused before anything is launched
+typedef CUresult (*MemRangeFn)(CUdeviceptr*, size_t*, CUdeviceptr);
+static MemRangeFn get_mem_range() {
+  static const MemRangeFn fn = [] {
+    cudaDriverEntryPointQueryResult q;
+    void* p = nullptr;
+    if (cudaGetDriverEntryPoint("cuMemGetAddressRange", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
+      return (MemRangeFn)p;
+    cudaGetLastError();
+    return (MemRangeFn) nullptr;
+  }();
+  return fn;
+}
+
+// The stage items of the leaves leaf_index[0..n) of S, leaf k read from src[k] + i * stride[k] elements for instance
+// i < n_inst (stride == NULL: one instance).  Everything a launch could trip over is checked here, on the host, before
+// any copy: the leaf (in range, listed once, with a payload), the stride, and the source (non-null, 16-byte aligned,
+// device or managed memory of the ctx's device, every byte it reads inside one allocation).
+static int device_items(const tncb_ctx* ctx, const Schedule& S, size_t n_inst, size_t n, const uint64_t* leaf_index,
+                        const void* const* src, const uint64_t* stride, std::vector<LeafStageItem>& items) {
+  std::vector<long long> elems(S.n_leaves_total, -1);   // payload elements per leaf, -1 = no payload
+  for (const SlotMeta& m : S.slots) if (m.leaf_index >= 0) elems[m.leaf_index] = (long long)m.elems;
+  std::vector<char> seen(elems.size(), 0);
+  items.clear();
+  for (size_t k = 0; k < n; k++) {
+    const uint64_t li = leaf_index[k];
+    const std::string name = "leaf " + std::to_string(li);
+    if (li >= elems.size()) return fail(TNCB_ERR_INVALID, name + " is out of range (" + std::to_string(elems.size()) + " leaves)");
+    if (seen[li]) return fail(TNCB_ERR_INVALID, name + " is listed twice");
+    seen[li] = 1;
+    if (elems[li] < 0) return fail(TNCB_ERR_INVALID, name + " has no payload");
+    const unsigned long long e = (unsigned long long)elems[li], st = stride ? stride[k] : 0;
+    if (st != 0 && st < e)
+      return fail(TNCB_ERR_INVALID, name + ": instance stride " + std::to_string(st) + " is below its " + std::to_string(e) + " elements");
+    const void* p = src[k];
+    if (!p) return fail(TNCB_ERR_INVALID, name + ": the source is null");
+    if ((uintptr_t)p % 16) return fail(TNCB_ERR_INVALID, name + ": the source is not 16-byte aligned");
+    cudaPointerAttributes a{};
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return fail(TNCB_ERR_INVALID, name + ": the source is not device memory"); }
+    if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) return fail(TNCB_ERR_INVALID, name + ": the source is not device memory");
+    if (a.device != ctx->device)
+      return fail(TNCB_ERR_INVALID, name + ": the source is on device " + std::to_string(a.device) + ", the context on device " + std::to_string(ctx->device));
+    unsigned long long span = 0, bytes = 0;        // [p, p + ((n_inst - 1) * stride + elems) * 16)
+    if (__builtin_mul_overflow((unsigned long long)(n_inst - 1), st, &span) || __builtin_add_overflow(span, e, &span) ||
+        __builtin_mul_overflow(span, 16ull, &bytes))
+      return fail(TNCB_ERR_INVALID, name + ": the source range overflows 64 bits");
+    const MemRangeFn range = get_mem_range();
+    if (!range) return fail(TNCB_ERR_CUDA, "cuMemGetAddressRange is not available");
+    CUdeviceptr base = 0;
+    size_t size = 0;
+    if (range(&base, &size, (CUdeviceptr)p) != CUDA_SUCCESS) return fail(TNCB_ERR_INVALID, name + ": no device allocation holds the source");
+    if ((unsigned long long)((CUdeviceptr)p - base) + bytes > size)
+      return fail(TNCB_ERR_INVALID, name + ": the source's " + std::to_string(bytes) + " bytes run past the end of its allocation");
+    items.push_back({(const double2*)p, st, (long long)S.leaf_offset[li], (long long)e});
+  }
+  return TNCB_OK;
 }
 
 } // namespace tncb
@@ -1563,6 +1635,108 @@ int tncb_plan_vjp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
   return TNCB_OK;
 }
 
+// New payloads for some leaves of the staged network, straight from device memory: one launch on the ctx stream into the
+// leaf block the next run reads (a static plan's workspace block, which its graph replays also read; a non-static plan's
+// resident block; a sliced gradient plan's full block).  The static layout never releases its leaf block, so the new
+// payloads stay in place across runs and tncb_plan_vjp, as staged leaves do.
+int tncb_plan_set_leaves(tncb_ctx* ctx, tncb_plan* plan, size_t n, const uint64_t* leaf_index, const void* const* src) {
+  using namespace tncb;
+  if (!ctx || !plan || (n && (!leaf_index || !src))) return fail(TNCB_ERR_INVALID, "null argument");
+  for (int k : plan->S.leaf_kind)
+    if (k == TNCB_DATA_DEVICE) return fail(TNCB_ERR_UNSUPPORTED, "plans with device leaves cannot be staged (they are consumed per call)");
+  const Schedule* S = &plan->S;
+  double2* block = nullptr;
+  if (plan->ctx == ctx) {
+    if (plan->sliced) { if (plan->full_staged) { S = &plan->full; block = (double2*)plan->full_dev; } }
+    else if (plan->is_static) { if (plan->leaves_resident) block = (double2*)((char*)plan->ws + plan->leaf_off); }
+    else block = (double2*)plan->resident;
+  }
+  if (!block) return fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this plan and context");
+  TNCB_CUDA(cudaSetDevice(ctx->device));
+  std::vector<LeafStageItem> items;
+  int rc = device_items(ctx, *S, 1, n, leaf_index, src, nullptr, items);
+  if (rc || n == 0) return rc;
+  plan->fwd_ready = false;     // a gradient plan's forward state belongs to the old payloads
+  return launch_leaf_stage(ctx, items.data(), items.size(), block, 0, 1);
+}
+
+// n_instances networks of the plan's structure, for tncb_plan_run_slices / run_batch (plain plans) or
+// tncb_plan_vjp_batch (gradient plans).  The host work is O(leaves) whatever n_instances is: the template's other leaves
+// are materialised once, packed into plan-owned pinned memory, uploaded in one copy; then one launch per 65535 instances
+// (and per kStageItems items) fills every instance's leaf block, the device payloads in place, the template's runs
+// between them with stride 0.  No host synchronisation once the arguments are validated.
+int tncb_plan_stage_instances(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tmpl, size_t n_instances, size_t n,
+                              const uint64_t* leaf_index, const void* const* src, const uint64_t* instance_stride) {
+  using namespace tncb;
+  if (!ctx || !plan || !tmpl || (n && (!leaf_index || !src || !instance_stride))) return fail(TNCB_ERR_INVALID, "null argument");
+  if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan takes device payloads through tncb_plan_set_leaves");
+  const Schedule& S = plan->S;
+  for (int k : S.leaf_kind)
+    if (k == TNCB_DATA_DEVICE) return fail(TNCB_ERR_UNSUPPORTED, "plans with device leaves cannot be staged (they are consumed per call)");
+  if (!plan->grad && !plan->is_static) return fail(TNCB_ERR_UNSUPPORTED, "many networks need a plan with a static layout");
+  if (plan->ctx && plan->ctx != ctx) return fail(TNCB_ERR_INVALID, "plan belongs to another context");
+  if (n_instances == 0) return fail(TNCB_ERR_INVALID, "n_instances is 0");
+  TNCB_CUDA(cudaSetDevice(ctx->device));
+  std::vector<const tncb_tn*> leaves;
+  collect_leaf_nodes(tmpl, leaves);
+  int rc = validate_leaves(S, leaves);
+  if (rc) return rc;
+  std::vector<LeafStageItem> items;
+  if ((rc = device_items(ctx, S, n_instances, n, leaf_index, src, instance_stride, items))) return rc;
+  const size_t block = std::max<size_t>(S.leaf_block_elems, 1);
+  size_t bytes = 0;
+  if (__builtin_mul_overflow(n_instances, block * sizeof(double2), &bytes)) return fail(TNCB_ERR_OOM, "the instances' leaf blocks overflow 64 bits");
+  // the runs of the leaf block between the device payloads come from the template: run r covers block elements
+  // [start, start + len) and sits at `packed` in the packed template
+  struct Run { long long start, len, packed; };
+  std::vector<Run> runs;
+  std::sort(items.begin(), items.end(), [](const LeafStageItem& x, const LeafStageItem& y) { return x.dst < y.dst; });
+  {
+    long long pos = 0, packed = 0;
+    auto gap = [&](long long end) { if (end > pos) { runs.push_back({pos, end - pos, packed}); packed += end - pos; } };
+    for (const LeafStageItem& it : items) { gap(it.dst); pos = std::max(pos, it.dst + it.elems); }
+    gap((long long)block);
+  }
+  if ((rc = plan_device_state(ctx, plan, !plan->grad))) return rc;
+  if (!plan->tmpl_host) {
+    plan->tmpl_bytes = block * sizeof(double2);
+    TNCB_CUDA(cudaMallocHost(&plan->tmpl_host, plan->tmpl_bytes));
+    if ((rc = ctx->arena.alloc(plan->tmpl_bytes, &plan->tmpl_dev))) { cudaFreeHost(plan->tmpl_host); plan->tmpl_host = nullptr; return rc; }
+    TNCB_CUDA(cudaEventCreateWithFlags(&plan->tmpl_ev, cudaEventDisableTiming));
+  } else if (plan->tmpl_busy) {
+    TNCB_CUDA(cudaEventSynchronize(plan->tmpl_ev));   // the previous call's upload out of tmpl_host has run
+    plan->tmpl_busy = false;
+  }
+  std::vector<char> device_leaf(leaves.size(), 0);
+  for (size_t k = 0; k < n; k++) device_leaf[leaf_index[k]] = 1;
+  std::complex<double>* host = (std::complex<double>*)plan->tmpl_host;
+  for (size_t li = 0; li < leaves.size(); li++) {
+    if (device_leaf[li] || S.leaf_kind[li] == TNCB_DATA_UNCONTRACTED) continue;
+    const long long off = (long long)S.leaf_offset[li];
+    const Run& r = *(std::upper_bound(runs.begin(), runs.end(), off, [](long long o, const Run& x) { return o < x.start; }) - 1);
+    if ((rc = stage_leaf(leaves[li], host + r.packed + (off - r.start)))) return rc;
+  }
+  void* blk = nullptr;
+  if ((rc = ctx->arena.alloc(bytes, &blk))) return rc;
+  const long long packed = runs.empty() ? 0 : runs.back().packed + runs.back().len;
+  if (packed) {
+    cudaError_t e = cudaMemcpyAsync(plan->tmpl_dev, plan->tmpl_host, packed * sizeof(double2), cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaEventRecord(plan->tmpl_ev, ctx->stream);
+    if (e != cudaSuccess) { ctx->arena.free(blk, bytes); return fail(TNCB_ERR_CUDA, std::string("template upload: ") + cudaGetErrorString(e)); }
+    plan->tmpl_busy = true;
+  }
+  for (const Run& r : runs) items.push_back({(const double2*)plan->tmpl_dev + r.packed, 0, r.start, r.len});
+  if ((rc = launch_leaf_stage(ctx, items.data(), items.size(), (double2*)blk, (long long)block, n_instances))) {
+    ctx->arena.free(blk, bytes);
+    return rc;
+  }
+  if (plan->slices_dev) ctx->arena.free(plan->slices_dev, plan->slices_bytes);   // stream-ordered
+  plan->slices_dev = blk;
+  plan->slices_bytes = bytes;
+  plan->n_slices = n_instances;
+  return TNCB_OK;
+}
+
 // Legs and bond dimensions of contract_tensor_network(tn, path) from metadata alone (no GPU work): what a receiver of the
 // fan-in needs to know about a raw buffer it is about to get (communication.rs:221-226; the reference ships the legs inside
 // the serialised tensor instead).
@@ -1630,6 +1804,9 @@ void tncb_plan_release_device_state(tncb_plan* plan) {
   if (plan->stage) { cudaFreeHost(plan->stage); plan->stage = nullptr; }
   if (plan->stage_ev) { cudaEventDestroy(plan->stage_ev); plan->stage_ev = nullptr; plan->stage_busy = false; }
   if (plan->resident) { ctx->arena.free(plan->resident, plan->resident_bytes); plan->resident = nullptr; }
+  if (plan->tmpl_dev) { ctx->arena.free(plan->tmpl_dev, plan->tmpl_bytes); plan->tmpl_dev = nullptr; }
+  if (plan->tmpl_host) { cudaFreeHost(plan->tmpl_host); plan->tmpl_host = nullptr; }
+  if (plan->tmpl_ev) { cudaEventDestroy(plan->tmpl_ev); plan->tmpl_ev = nullptr; plan->tmpl_busy = false; }
   for (size_t i = 0; i < ctx->plans.size(); i++)
     if (ctx->plans[i] == plan) { ctx->plans.erase(ctx->plans.begin() + i); break; }
   plan->ctx = nullptr;

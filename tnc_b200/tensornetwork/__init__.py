@@ -1,5 +1,5 @@
 from .tensor import Tensor
 from .tensordata import TensorData
-from .contraction import contract_tensor_network, leaves, NetworkPlan
+from .contraction import contract_tensor_network, leaves, NetworkPlan, PreparedNetwork
 
-__all__ = ["Tensor", "TensorData", "contract_tensor_network", "leaves", "NetworkPlan"]
+__all__ = ["Tensor", "TensorData", "contract_tensor_network", "leaves", "NetworkPlan", "PreparedNetwork"]

@@ -175,6 +175,61 @@ def leaves(tn: Tensor) -> List[Tensor]:
     return [leaf for child in tn.tensors for leaf in leaves(child)]
 
 
+class PreparedNetwork:
+    """A network marshalled once for the C ABI: the host template NetworkPlan.stage_instances can take call after call
+    without walking the tree again.  The network's payloads are read by every call, so it must outlive its use."""
+
+    def __init__(self, tn: Tensor):
+        self._m = _Marshal()
+        self.node = self._m.tn(tn)
+
+
+def _device_sources(ctx: Context, shapes, payloads: dict, count: Optional[int] = None):
+    """{leaf index: torch CUDA tensor} as (leaf indices, device addresses, instance strides in elements, the complex128
+    tensors read).  count=None: one payload shaped like its leaf.  Else per instance, [count, *leaf shape] (its rows may
+    lie further apart than a row's size: the stride is the tensor's own), or shared, [*leaf shape] (stride 0)."""
+    import torch
+    from .. import check_cuda_tensor
+    idx, ptrs, strides, keep = [], [], [], []
+    for leaf, x in payloads.items():
+        leaf = int(leaf)
+        if not 0 <= leaf < len(shapes):
+            raise IndexError(f"leaf index {leaf} out of range ({len(shapes)} leaves)")
+        check_cuda_tensor(ctx, x, f"the payload of leaf {leaf}")
+        shape = tuple(shapes[leaf])
+        elems = int(np.prod(shape, dtype=np.int64))
+        if tuple(x.shape) == shape:
+            src, stride = x.detach().to(torch.complex128).contiguous(), 0
+        elif count is not None and tuple(x.shape) == (int(count),) + shape:
+            src = x.detach().to(torch.complex128)
+            if count > 1 and src[0].is_contiguous() and src.stride(0) >= elems:
+                stride = src.stride(0)
+            else:
+                src, stride = src.contiguous(), elems
+        else:
+            want = f"{shape}" if count is None else f"{(int(count),) + shape} or {shape}"
+            raise ValueError(f"the payload of leaf {leaf} has shape {tuple(x.shape)}, expected {want}")
+        idx.append(leaf)
+        ptrs.append(src.data_ptr())
+        strides.append(stride)
+        keep.append(src)
+    return idx, ptrs, strides, keep
+
+
+def _call_after_torch(ctx: Context, keep, call) -> None:
+    """`call()` (a library call that reads the torch tensors `keep` on the context stream) ordered after torch's current
+    stream; torch's current stream then waits for the context stream, so the caching allocator cannot hand `keep`'s
+    memory to later work before the library has read it (record_stream would tie the tensors to a stream that dies with
+    the context)"""
+    from .. import torch_streams
+    cur, ext = torch_streams(ctx)
+    ext.wait_stream(cur)
+    try:
+        check(call())
+    finally:
+        cur.wait_stream(ext)
+
+
 class NetworkPlan:
     """Compile once / execute many (tncb_plan_*): same structure, new payloads."""
 
@@ -185,6 +240,7 @@ class NetworkPlan:
         h = C.c_void_p()
         check(self.ctx._l.tncb_plan_create(self.ctx.handle, C.byref(c_tn), C.byref(c_path), C.byref(h)))
         self.handle = h
+        self.leaf_shapes = [tuple(int(d) for d in leaf.bond_dims) for leaf in leaves(tn)]
 
     @classmethod
     def for_gradients(cls, tn: Tensor, contract_path: ContractionPath, wrt=None, ctx: Optional[Context] = None) -> "NetworkPlan":
@@ -224,6 +280,17 @@ class NetworkPlan:
         """After a forward `run`/`execute` of a gradient plan: {leaf index: G} for every requested leaf, G shaped like
         the leaf with G[e] = sum_r seed[r] dR[r]/dX[e] (no conjugation).  seed: array or DeviceTensor with the result's
         shape; None for a scalar result (seed 1).  One device-to-host copy of the whole gradient block."""
+        block = self.vjp_block(seed)
+        flat = block.to_numpy()
+        block.free()
+        grads = {}
+        for i, (off, shape) in enumerate(zip(self.grad_offsets(), self.leaf_shapes)):
+            if off >= 0:
+                grads[i] = flat[off:off + int(np.prod(shape, dtype=np.int64))].reshape(shape)
+        return grads
+
+    def vjp_block(self, seed=None) -> DeviceTensor:
+        """`vjp` left on the device: the rank-1 block of every requested leaf's G at grad_offsets()"""
         tmp = None
         if seed is not None and not isinstance(seed, DeviceTensor):
             seed = tmp = DeviceTensor.from_numpy(self.ctx, np.asarray(seed, dtype=np.complex128))
@@ -233,14 +300,30 @@ class NetworkPlan:
         finally:
             if tmp is not None:
                 tmp.free()
-        block = DeviceTensor.adopt(self.ctx, out)
-        flat = block.to_numpy()
-        block.free()
-        grads = {}
-        for i, (off, shape) in enumerate(zip(self.grad_offsets(), self.leaf_shapes)):
-            if off >= 0:
-                grads[i] = flat[off:off + int(np.prod(shape, dtype=np.int64))].reshape(shape)
-        return grads
+        return DeviceTensor.adopt(self.ctx, out)
+
+    def set_leaves(self, payloads: dict) -> None:
+        """New payloads for leaves of the staged network straight from device memory (tncb_plan_set_leaves): {leaf index
+        (into leaves(tn)): torch CUDA tensor shaped like the leaf}, on the context's device, cast to complex128 there.
+        One copy kernel on the context stream, after torch's current stream; the next run / vjp reads them.  A gradient
+        plan needs a new run before vjp."""
+        idx, ptrs, _, keep = _device_sources(self.ctx, self.leaf_shapes, payloads)
+        c_ptrs = (C.c_void_p * max(len(ptrs), 1))(*ptrs)
+        _call_after_torch(self.ctx, keep, lambda: self.ctx._l.tncb_plan_set_leaves(
+            self.ctx.handle, self.handle, len(idx), u64_array(idx), c_ptrs))
+
+    def stage_instances(self, template, payloads: dict, count: int) -> None:
+        """Stage `count` networks of the plan's structure from device memory (tncb_plan_stage_instances): every leaf from
+        `template` (a Tensor of the plan's structure, or a PreparedNetwork of one), except the leaves in `payloads`,
+        {leaf index: torch CUDA tensor}, [count, *leaf shape] for a payload per instance or [*leaf shape] for one shared
+        by all.  The host work does not grow with count.  Plain plans: feeds run_slices / run_batch, as stage_slices does;
+        gradient plans: feeds vjp_batch, as stage_batch does."""
+        tmpl = template if isinstance(template, PreparedNetwork) else PreparedNetwork(template)
+        idx, ptrs, strides, keep = _device_sources(self.ctx, self.leaf_shapes, payloads, int(count))
+        c_ptrs = (C.c_void_p * max(len(ptrs), 1))(*ptrs)
+        _call_after_torch(self.ctx, keep, lambda: self.ctx._l.tncb_plan_stage_instances(
+            self.ctx.handle, self.handle, C.byref(tmpl.node), int(count), len(idx), u64_array(idx), c_ptrs, u64_array(strides)))
+        self.n_staged = int(count)
 
     def stage_batch(self, nets) -> None:
         """Materialise + upload the leaves of many networks of a gradient plan's structure once (tncb_plan_stage_batch):
@@ -261,23 +344,11 @@ class NetworkPlan:
         the sum is the left fold of the rows in instance order, also bit for bit."""
         if count is None:
             count = max(0, getattr(self, "n_staged", 0) - int(first))
-        tmp = None
-        if seeds is not None and not isinstance(seeds, DeviceTensor):
-            seeds = tmp = DeviceTensor.from_numpy(self.ctx, np.asarray(seeds, dtype=np.complex128))
-        outs = [C.c_void_p() if want else None for want in (values, rows, sum)]
-        try:
-            check(self.ctx._l.tncb_plan_vjp_batch(self.ctx.handle, self.handle, int(first), int(count),
-                                                  seeds.handle if seeds is not None else None,
-                                                  *[C.byref(o) if o is not None else None for o in outs]))
-        finally:
-            if tmp is not None:
-                tmp.free()
         host = []
-        for o in outs:
-            if o is None:
+        for dt in self.vjp_batch_blocks(first, count, seeds, rows, sum, values):
+            if dt is None:
                 host.append(None)
                 continue
-            dt = DeviceTensor.adopt(self.ctx, o)
             host.append(dt.to_numpy())
             dt.free()
         vals, row_block, sum_block = host
@@ -293,6 +364,25 @@ class NetworkPlan:
                     out[i] = block[..., off:off + size].reshape(lead + tuple(shape))
             return out
         return (list(self.result_legs), vals, unpack(row_block, (int(count),)), unpack(sum_block, ()))
+
+    def vjp_batch_blocks(self, first: int = 0, count: Optional[int] = None, seeds=None, rows: bool = True,
+                         sum: bool = False, values: bool = True):
+        """`vjp_batch` left on the device: [values [count, *dims], rows [count, grad_elems], sum [grad_elems]] as
+        DeviceTensors, None where not requested"""
+        if count is None:
+            count = max(0, getattr(self, "n_staged", 0) - int(first))
+        tmp = None
+        if seeds is not None and not isinstance(seeds, DeviceTensor):
+            seeds = tmp = DeviceTensor.from_numpy(self.ctx, np.asarray(seeds, dtype=np.complex128))
+        outs = [C.c_void_p() if want else None for want in (values, rows, sum)]
+        try:
+            check(self.ctx._l.tncb_plan_vjp_batch(self.ctx.handle, self.handle, int(first), int(count),
+                                                  seeds.handle if seeds is not None else None,
+                                                  *[C.byref(o) if o is not None else None for o in outs]))
+        finally:
+            if tmp is not None:
+                tmp.free()
+        return [None if o is None else DeviceTensor.adopt(self.ctx, o) for o in outs]
 
     def info(self) -> dict:
         n, k = C.c_uint64(), C.c_uint64()
