@@ -234,6 +234,51 @@ class NetworkPlan {
     }
     return out;
   }
+  // A tangent plan (tncb_plan_create_jvp): wrt as for ForGradients.  stage, then jvp gives the result and its
+  // directional derivative along tangents of those leaves.
+  struct ForTangents { std::vector<size_t> wrt; };
+  NetworkPlan(Context& ctx, const Tensor& tn, const ContractionPath& path, const ForTangents& t) : ctx_(ctx) {
+    detail::Marshal m;
+    tncb_tn c_tn = m.tn(tn);
+    tncb_path c_path = m.path(path);
+    n_leaves_ = count_leaves(tn);
+    leaf_elems(tn, leaf_elems_);
+    std::vector<uint8_t> mask(n_leaves_ ? n_leaves_ : 1, 0);
+    for (size_t i : t.wrt) {
+      if (i >= n_leaves_) throw Error(TNCB_ERR_INVALID, "wrt: leaf index out of range");
+      mask[i] = 1;
+    }
+    check(tncb_plan_create_jvp(ctx.get(), &c_tn, &c_path, t.wrt.empty() ? nullptr : mask.data(), &h_));
+  }
+  // After stage: {value R, tangent Ṙ}, both row-major over the result's legs, Ṙ[r] = sum_l sum_e dR[r]/dX_l[e] Ẋ_l[e].
+  // tangents: leaf index -> Ẋ_l (row-major in the leaf's leg order); requested leaves left out have zero tangent.
+  std::pair<std::vector<Complex64>, std::vector<Complex64>> jvp(const std::map<size_t, std::vector<Complex64>>& tangents) {
+    std::vector<int64_t> off(n_leaves_ ? n_leaves_ : 1);
+    check(tncb_plan_grad_offsets(h_, off.data()));
+    uint64_t elems = 0;
+    for (size_t i = 0; i < n_leaves_; i++) if (off[i] >= 0) elems += leaf_elems_[i];
+    std::vector<Complex64> block(elems);
+    for (const auto& [i, x] : tangents) {
+      if (i >= n_leaves_ || off[i] < 0) throw Error(TNCB_ERR_INVALID, "jvp: tangent for a leaf the plan does not request");
+      if (x.size() != leaf_elems_[i]) throw Error(TNCB_ERR_SHAPE, "jvp: tangent size differs from the leaf's");
+      std::copy(x.begin(), x.end(), block.begin() + off[i]);
+    }
+    tncb_tensor* tb = nullptr;
+    check(tncb_tensor_upload(ctx_.get(), 1, &elems, reinterpret_cast<const double*>(block.data()), &tb));
+    tncb_tensor *v = nullptr, *t = nullptr;
+    const int rc = tncb_plan_jvp(ctx_.get(), h_, tb, &v, &t);
+    tncb_tensor_free(ctx_.get(), tb);
+    check(rc);
+    std::pair<std::vector<Complex64>, std::vector<Complex64>> out;
+    out.first.resize(tncb_tensor_elements(v));
+    out.second.resize(tncb_tensor_elements(t));
+    int drc = tncb_tensor_download(ctx_.get(), v, reinterpret_cast<double*>(out.first.data()));
+    if (!drc) drc = tncb_tensor_download(ctx_.get(), t, reinterpret_cast<double*>(out.second.data()));
+    tncb_tensor_free(ctx_.get(), v);
+    tncb_tensor_free(ctx_.get(), t);
+    check(drc);
+    return out;
+  }
   ~NetworkPlan() { tncb_plan_destroy(h_); }
   NetworkPlan(const NetworkPlan&) = delete;
   NetworkPlan& operator=(const NetworkPlan&) = delete;
@@ -268,10 +313,20 @@ class NetworkPlan {
     for (const Tensor& c : t.tensors) n += count_leaves(c);
     return n;
   }
+  static void leaf_elems(const Tensor& t, std::vector<uint64_t>& out) {
+    if (t.is_leaf()) {
+      uint64_t e = 1;
+      for (uint64_t d : t.bond_dims) e *= d;
+      out.push_back(e);
+      return;
+    }
+    for (const Tensor& c : t.tensors) leaf_elems(c, out);
+  }
   Context& ctx_;
   tncb_plan* h_ = nullptr;
   size_t n_leaves_ = 0;
   std::vector<uint64_t> res_dims_;
+  std::vector<uint64_t> leaf_elems_;                 // tangent plans: elements of every leaf, collect order
 };
 
 // tnc::builders (tnc/src/builders/circuit_builder.rs): Permutor (:72-129) and Circuit (:135-335).

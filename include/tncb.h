@@ -327,7 +327,8 @@ int tncb_plan_create_vjp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path
  * leave the arena as they found it. */
 int tncb_plan_vjp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* seed, tncb_tensor** grads);
 /* Element offset of each leaf's gradient inside *grads, -1 for leaves not requested (n_leaves entries); host only.
- * For a sliced gradient plan the offsets pack the FULL leaves' shapes. */
+ * For a sliced gradient plan the offsets pack the FULL leaves' shapes; for a tangent plan they place each requested
+ * leaf's tangent in a tangent row (tncb_plan_jvp). */
 int tncb_plan_grad_offsets(const tncb_plan* plan, int64_t* offsets);
 /* ---- sliced gradients: networks whose gradient workspace does not fit unsliced ----
  * Fixing the sliced legs splits R into slices, R = sum_q R_q, so dR/dX_l = sum_q dR_q/dX_l; a slice leaf is a
@@ -363,8 +364,8 @@ int tncb_plan_vjp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t st
 /* ---- batched gradients: many networks of one gradient plan's structure (sampled bitstrings, angle sets, input states)
  * Stage n networks of a (non-sliced) gradient plan's structure for tncb_plan_vjp_batch: every leaf validated and
  * materialised, one H2D; the structure-validation errors are those of tncb_plan_stage_slices.  The plan's own staged
- * leaves (tncb_plan_stage) and forward state are untouched.  Not a gradient plan -> TNCB_ERR_INVALID (plain plans use
- * tncb_plan_stage_slices); a sliced gradient plan -> TNCB_ERR_UNSUPPORTED.  tncb_plan_stage_slices / run_slices /
+ * leaves (tncb_plan_stage) and forward state are untouched.  Tangent plans take it as well (for tncb_plan_jvp_batch).
+ * Not a gradient or tangent plan -> TNCB_ERR_INVALID (plain plans use tncb_plan_stage_slices); a sliced gradient plan -> TNCB_ERR_UNSUPPORTED.  tncb_plan_stage_slices / run_slices /
  * run_batch stay TNCB_ERR_UNSUPPORTED on gradient plans. */
 int tncb_plan_stage_batch(tncb_ctx* ctx, tncb_plan* plan, size_t n, const tncb_tn* const* tns);
 /* Instances first .. first+count-1, each contracted forward and backward on its own with the instance as a grid
@@ -406,11 +407,49 @@ int tncb_plan_set_leaves(tncb_ctx* ctx, tncb_plan* plan, size_t n, const uint64_
  * leaf_index[0..n), whose instance i reads src[k] + i * instance_stride[k] elements (stride 0 = the same device payload
  * in every instance; a non-zero stride below the leaf's element count -> TNCB_ERR_INVALID).  Plain plans: replaces
  * tncb_plan_stage_slices (feeds run_slices / run_batch; needs a static plan, else TNCB_ERR_UNSUPPORTED).  Gradient plans:
- * replaces tncb_plan_stage_batch (feeds vjp_batch; the plan's own workspace is not allocated).  Staged instances are
+ * replaces tncb_plan_stage_batch (feeds vjp_batch; the plan's own workspace is not allocated); tangent plans likewise
+ * (feeds jvp_batch).  Staged instances are
  * bit-identical to the host-staged networks with the same payloads.  n_instances == 0 -> TNCB_ERR_INVALID; a sliced
  * gradient plan -> TNCB_ERR_UNSUPPORTED (it uses tncb_plan_set_leaves). */
 int tncb_plan_stage_instances(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tmpl, size_t n_instances,
                               size_t n, const uint64_t* leaf_index, const void* const* src, const uint64_t* instance_stride);
+/* ---- directional derivatives with respect to the leaves (forward mode) ----
+ * For a plan of (tn, path) with result R and tangents Ẋ_l of the requested leaves, the holomorphic Jacobian-vector product
+ *   Ṙ[r] = sum_l sum_e dR[r]/dX_l[e] * Ẋ_l[e]      (plain contraction, no conjugation anywhere)
+ * the transpose of tncb_plan_vjp: sum_r S[r] Ṙ[r] = sum_l sum_e G_l[e] Ẋ_l[e] with G = vjp(S).  Leaves not requested have
+ * zero tangent.  The tangents are one packed rank-1 block: every requested leaf's Ẋ_l row-major in the leaf's OWN leg
+ * order at tncb_plan_grad_offsets, the layout tncb_plan_vjp returns, so a gradient block and a tangent block are
+ * interchangeable.  For every forward pair C = A.B with a requested leaf below it, the tangent pass contracts Ȧ with B
+ * and/or A with Ḃ, each with the forward pair's legs and GEMM view on the same engines, on the forward pair's own tree
+ * level, and adds the two when both exist (one launch per level).  Cost: about three forward passes with every leaf
+ * requested, in ONE walk over the forward levels.
+ * wrt: one flag per leaf (collect order); NULL = every leaf that has a payload.  ctx may be NULL (host-only compile:
+ * tncb_plan_info, which then covers forward pairs, tangent pairs and sums, and tncb_plan_grad_offsets).  Refused with
+ * TNCB_ERR_UNSUPPORTED: device leaves, networks without pairs, and a static workspace above the static-workspace limit
+ * (TNCB_PLAN_WS_GB; the message states the bytes needed).  wrt selecting no leaf, or a leaf without a payload ->
+ * TNCB_ERR_INVALID.  Tangent plans always run on their static layout, are never captured into a CUDA graph and have no
+ * pair-by-pair fallback.  tncb_plan_run / execute / run_slices / run_batch / stage_slices / vjp / vjp_sliced /
+ * vjp_batch on a tangent plan -> TNCB_ERR_UNSUPPORTED. */
+int tncb_plan_create_jvp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, const uint8_t* wrt, tncb_plan** out);
+/* One forward-mode pass on the leaves staged by tncb_plan_stage (and overwritten by tncb_plan_set_leaves).
+ * tangents: [tangent_elems] device tensor (tangent_elems = the sum of the requested leaves' sizes).
+ * *value: new tensor with the result's dims, bit-identical to a plain plan's tncb_plan_run on the same leaves.
+ * *tangent_out: new tensor with the result's dims, Ṙ.  Either may be NULL, not both.  Each call is self-contained and
+ * repeats bit for bit.  Not a tangent plan, not staged on this context, both outputs NULL, NULL tangents ->
+ * TNCB_ERR_INVALID; tangent dims other than [tangent_elems] -> TNCB_ERR_SHAPE.  Errors leave the arena as they found it. */
+int tncb_plan_jvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, tncb_tensor** value, tncb_tensor** tangent_out);
+/* Instances first .. first+count-1 staged by tncb_plan_stage_batch or tncb_plan_stage_instances, each with its own
+ * tangent row, in passes of as many workspace copies as fit (as tncb_plan_run_batch).
+ *   tangents:      [count, tangent_elems] device tensor, row i for instance first + i
+ *   *values:       new [count, result dims..]; row i bit-identical to tncb_plan_jvp of instance i
+ *   *tangent_rows: new [count, result dims..]; row i bit-identical to tncb_plan_jvp of instance i with tangent row i
+ * Either output may be NULL, not both.  Many directions of one network: stage count instances of it with
+ * tncb_plan_stage_instances (every device source at stride 0, or the host template alone) and pass one tangent row per
+ * direction.  Not a tangent plan, nothing staged on this context, count == 0, a range past the staged networks, both
+ * outputs NULL, NULL tangents, a result of rank 64 -> TNCB_ERR_INVALID; tangent dims other than [count, tangent_elems]
+ * -> TNCB_ERR_SHAPE; not even one workspace copy fits -> TNCB_ERR_OOM.  Errors leave the arena as they found it. */
+int tncb_plan_jvp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t count, const tncb_tensor* tangents,
+                        tncb_tensor** values, tncb_tensor** tangent_rows);
 void tncb_plan_destroy(tncb_plan* plan);
 
 /* ---- HDF5 tensor files: replaces tnc::io::hdf5 (tnc/src/io/hdf5.rs), which binds libhdf5 through hdf5-metno.

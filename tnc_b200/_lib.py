@@ -118,6 +118,9 @@ SIGNATURES = {
     "tncb_plan_vjp_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, vpp, vpp, vpp]),
     "tncb_plan_set_leaves": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, u64p, vpp]),
     "tncb_plan_stage_instances": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(TncbTn), C.c_size_t, C.c_size_t, u64p, vpp, u64p]),
+    "tncb_plan_create_jvp": (C.c_int, [C.c_void_p, C.POINTER(TncbTn), C.POINTER(TncbPath), C.POINTER(C.c_uint8), vpp]),
+    "tncb_plan_jvp": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, vpp, vpp]),
+    "tncb_plan_jvp_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, vpp, vpp]),
     "tncb_plan_destroy": (None, [C.c_void_p]),
     "tncb_comm_unique_id": (C.c_int, [C.c_void_p]),
     "tncb_comm_init": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p]),

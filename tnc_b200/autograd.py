@@ -38,12 +38,27 @@ def _with_payloads(tn: Tensor, payloads: dict, counter: list) -> Tensor:
 
 
 class _NetworkFn(torch.autograd.Function):
+    # forward / setup_context (rather than forward(ctx, ...)) so that torch.func transforms (torch.func.jvp) accept it
     @staticmethod
-    def forward(ctx, runner, *xs):
-        ctx.runner = runner
-        ctx.token = runner._forward_device(xs) if runner.on_device else runner._forward(xs)
-        ctx.save_for_backward(*xs)
+    def forward(runner, *xs):
+        runner._forward_device(xs) if runner.on_device else runner._forward(xs)
         return runner._result
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        runner, xs = inputs[0], inputs[1:]
+        ctx.runner = runner
+        ctx.token = runner._token        # the staging the forward just did
+        ctx.save_for_backward(*xs)
+        ctx.save_for_forward(*xs)
+        ctx.out_meta = (tuple(output.shape), output.device)
+
+    @staticmethod
+    def jvp(ctx, _runner_tangent, *tangents):
+        # torch.func.jvp calls this inside its transform, where reading a tensor's storage (numpy, the library's
+        # device copies) is refused; the work here is outside torch's tracing anyway
+        with torch._C._DisableFuncTorch():
+            return ctx.runner._jvp(ctx.saved_tensors, tangents, ctx.out_meta)
 
     @staticmethod
     def backward(ctx, grad_out):
@@ -100,6 +115,10 @@ class NetworkFunction:
         self._staged = False             # on_device: the template network is staged (unbatched and sliced)
         self._template = None            # on_device, batched: the network marshalled once
         self._offsets = None
+        self._ctx = ctx or default_context()
+        self._sliced_legs = tuple(sliced_legs)
+        self._tplan = None               # the tangent plan, compiled on the first forward-mode call
+        self._tstaged = False            # on_device, unbatched: the tangent plan has `tn` staged
 
     # ---- on_device: inputs, results and gradients stay on the GPU ----
     def _check_device(self, xs):
@@ -267,6 +286,60 @@ class NetworkFunction:
         self._result = torch.from_numpy(np.asarray(res.to_numpy()).copy())
         return token
 
+    # ---- forward mode (torch.autograd.forward_ad, torch.func.jvp): a tangent plan, compiled on first use ----
+    def _jvp(self, xs, tangents, out_meta):
+        """Ṙ for the tangents of the inputs (None = zero; tangents of inputs not in wrt are ignored, as backward gives
+        them no gradient): the tangent plan staged with the inputs, then NetworkPlan.jvp / jvp_batch"""
+        if self.sliced:
+            raise NotImplementedError("forward-mode AD (jvp) is not supported with sliced_legs: tangent plans are not sliced")
+        shape, device = out_meta
+        tans = {i: t for i, t in zip(self.inputs, tangents) if t is not None and i in self.wrt}
+        if not tans:
+            return torch.zeros(shape, dtype=torch.complex128, device=device)
+        if self._tplan is None:
+            self._tplan = NetworkPlan.for_tangents(self.tn, self.path, self.wrt, ctx=self._ctx)
+        plan = self._tplan
+        if self.on_device:
+            self._check_device(xs)
+            for i, t in tans.items():
+                check_cuda_tensor(plan.ctx, t, f"tangent for leaf {i}")
+            if self.batched:
+                if self._template is None:
+                    self._template = PreparedNetwork(self.tn)
+                plan.stage_instances(self._template, dict(zip(self.inputs, xs)), self._batch_size(xs))
+                _, rows = plan.jvp_batch_blocks(0, None, tans, values=False)
+                out = rows.to_torch()
+                rows.free()
+                return out
+            for i, shape_i, x in zip(self.wrt, self.shapes, xs):
+                if tuple(x.shape) != shape_i:
+                    raise ValueError(f"input for leaf {i} has shape {tuple(x.shape)}, the leaf {shape_i}")
+            if not self._tstaged:
+                plan.stage(self.tn)
+                self._tstaged = True
+            plan.set_leaves(dict(zip(self.wrt, xs)))
+            val, tan = plan.jvp_block(tans)
+            val.free()
+            out = tan.to_torch()
+            tan.free()
+            return out
+        host = {i: np.ascontiguousarray(t.detach().to(torch.complex128).resolve_conj().cpu().numpy()) for i, t in tans.items()}
+        if self.batched:
+            b = self._batch_size(xs)
+            arrs = [np.ascontiguousarray(x.detach().to(torch.complex128).resolve_conj().cpu().numpy()) for x in xs]
+            plan.stage_batch([_with_payloads(self.tn, {i: (a[k] if i in self.batched else a) for i, a in zip(self.inputs, arrs)}, [0])
+                              for k in range(b)])
+            _, _, rows = plan.jvp_batch(0, None, host, values=False)
+            return torch.from_numpy(rows).to(device)
+        pay = {}
+        for i, shape_i, x in zip(self.wrt, self.shapes, xs):
+            if tuple(x.shape) != shape_i:
+                raise ValueError(f"input for leaf {i} has shape {tuple(x.shape)}, the leaf {shape_i}")
+            pay[i] = np.ascontiguousarray(x.detach().to(torch.complex128).resolve_conj().cpu().numpy())
+        plan.stage(_with_payloads(self.tn, pay, [0]))
+        _, tan = plan.jvp(host)
+        return torch.from_numpy(tan).to(device)
+
     def __call__(self, *xs: torch.Tensor) -> torch.Tensor:
         if len(xs) != len(self.inputs):
             raise TypeError(f"expected {len(self.inputs)} inputs, got {len(xs)}")
@@ -299,6 +372,13 @@ def network_function(tn: Tensor, path: ContractionPath, wrt: Sequence[int], ctx:
     plus backward pass of every instance: per-instance gradient rows for batched inputs in `wrt`, their sum over the
     instances for shared ones.  About 4 forward passes per forward + backward in all, against about 3 for one
     unbatched network; the instances share every launch.  Not combinable with sliced_legs.
+
+    Forward mode: torch.autograd.forward_ad dual inputs and torch.func.jvp(f, inputs, tangents) give Ṙ = sum over the
+    inputs of dR/dx · ẋ (the plain directional derivative, torch's forward-mode convention for holomorphic functions), from
+    a tangent plan (NetworkPlan.for_tangents) compiled on the first forward-mode call.  With `batched`, tangents of
+    batched inputs are [B, *leaf shape], those of shared inputs [*leaf shape] and the same for every instance; the
+    instances run in one NetworkPlan.jvp_batch pass.  Tangents of inputs not in `wrt` are ignored, as their gradients are
+    None.  sliced_legs with forward mode raises NotImplementedError.
 
     on_device=True: the inputs must be torch CUDA tensors on the context's device (else ValueError), and the result and
     the gradients are CUDA tensors there; no payload, result or gradient goes through the host.  The first call stages

@@ -223,6 +223,13 @@ struct LeafStageBatch {
 int launch_leaf_stage(tncb_ctx* ctx, const LeafStageItem* items, size_t n_items, double2* dst, long long block_elems,
                       size_t n_instances);
 
+// ---- tangent sums of a tangent plan: every two-sided forward step of one level, out = t1 + t2, in ONE launch; count
+// instances whose workspaces lie `stride` bytes apart (the instance a grid dimension) ----
+constexpr int kSumThreads = 256;    // elements per block
+struct TangentSumItem { long long t1, t2, out, elems; };   // byte offsets in the plan workspace; elements
+int launch_tangent_sum(tncb_ctx* ctx, const TangentSumItem* d_items, const long long* d_block_start, int n_items,
+                       long long total_blocks, char* ws, int count, long long stride);
+
 int tensor_new(tncb_ctx* ctx, int rank, const uint64_t* dims, tncb_tensor** out);
 
 // TensorData::File leaf (hdf5io.cpp): first member of /tensors, optionally adjointed, checked against the leaf's dims

@@ -1379,4 +1379,41 @@ int launch_leaf_stage(tncb_ctx* ctx, const LeafStageItem* items, size_t n_items,
   return TNCB_OK;
 }
 
+// ------------------------------------------------------------------------------------------
+// Tangent sums (tncb_plan_jvp / tncb_plan_jvp_batch): a forward step whose operands both carry a tangent has two tangent
+// pairs, and its output's tangent is their sum.  Every such sum of one tree level is ONE launch: a block adds
+// kSumThreads consecutive elements of one item, found by binary search over the block-count prefix (as
+// grad_gather_kernel does), with one 16-byte load per operand and one 16-byte store per element; blockIdx.y is the
+// instance, its workspace `stride` bytes further on.  Always t1 + t2, so results repeat bit for bit.
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kSumThreads)
+tangent_sum_kernel(const TangentSumItem* __restrict__ items, const long long* __restrict__ block_start, int n_items,
+                   char* __restrict__ ws, long long stride) {
+  const long long b = blockIdx.x;
+  int lo = 0, hi = n_items;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(block_start + mid) <= b) lo = mid; else hi = mid;
+  }
+  const TangentSumItem& it = items[lo];
+  const long long o = (b - __ldg(block_start + lo)) * kSumThreads + threadIdx.x;
+  if (o >= it.elems) return;
+  char* base = ws + (long long)blockIdx.y * stride;
+  const double2 x = reinterpret_cast<const double2*>(base + it.t1)[o];
+  const double2 y = reinterpret_cast<const double2*>(base + it.t2)[o];
+  reinterpret_cast<double2*>(base + it.out)[o] = make_double2(x.x + y.x, x.y + y.y);
+}
+
+int launch_tangent_sum(tncb_ctx* ctx, const TangentSumItem* d_items, const long long* d_block_start, int n_items,
+                       long long total_blocks, char* ws, int count, long long stride) {
+  if (n_items <= 0 || total_blocks <= 0 || count <= 0) return TNCB_OK;
+  if (total_blocks > 0x7fffffffLL) return fail(TNCB_ERR_UNSUPPORTED, "tangent sums too large for one launch");
+  if (count > 65535) return fail(TNCB_ERR_INVALID, "more than 65535 instances in one tangent-sum launch");
+  tangent_sum_kernel<<<dim3((unsigned)total_blocks, (unsigned)count), kSumThreads, 0, ctx->stream>>>(d_items, d_block_start, n_items,
+                                                                                                    ws, stride);
+  ctx->launches++;
+  TNCB_CUDA(cudaGetLastError());
+  return TNCB_OK;
+}
+
 } // namespace tncb

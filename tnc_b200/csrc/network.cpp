@@ -358,6 +358,19 @@ struct tncb_plan {
   void* tmpl_host = nullptr; void* tmpl_dev = nullptr; size_t tmpl_bytes = 0;
   cudaEvent_t tmpl_ev = nullptr;
   bool tmpl_busy = false;
+  // tangent plans (tncb_plan_create_jvp): the tangent pairs follow the forward ones in S.steps, each on its forward
+  // step's level; grad_offset / grad_elems give the packing of the leaf tangents.  Always static, never graphed.
+  bool tangent = false;
+  int tan_result = -1;                              // the slot of the result's tangent
+  struct TanLeaf { int slot; int64_t off; };        // a requested leaf's tangent slot and its offset in a tangent row
+  std::vector<TanLeaf> tan_leaves;
+  struct TanSum { int t1, t2; };                    // a two-sided step: t1 += t2 (t1 becomes the output's tangent)
+  std::vector<TanSum> tan_sums;
+  std::vector<tncb::TangentSumItem> sum_items;      // the sums of all levels, level by level
+  std::vector<long long> sum_bs;                    // per level with sums: n + 1 block-count prefix entries
+  std::vector<int> sum_first, sum_count;            // per level: first index into sum_items, number of sums
+  std::vector<size_t> sum_bs_first;                 // per level: first index into sum_bs
+  void* sum_dev = nullptr; size_t sum_dev_bytes = 0;  // device copy of sum_items + sum_bs
 };
 
 namespace tncb {
@@ -397,11 +410,12 @@ static size_t static_ws_limit(size_t device_bytes) {
 
 static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) {
   Schedule& S = P->S;
-  P->is_static = !S.steps.empty() && (P->grad || std::getenv("TNCB_NO_STATIC") == nullptr);
+  P->is_static = !S.steps.empty() && (P->grad || P->tangent || std::getenv("TNCB_NO_STATIC") == nullptr);
   for (int k : S.leaf_kind) if (k == TNCB_DATA_DEVICE) P->is_static = false;   // addresses change per call
   if (!P->is_static) return;
   // ---- levels: a step's level is 1 + the deepest level among its operands' producers (leaves: 0); backward pairs
-  // follow the whole forward pass on their backward level ----
+  // follow the whole forward pass on their backward level.  A tangent pair reads a tangent of its forward step's operand
+  // (on that operand's level) and the other forward operand, so it lands on its forward step's level ----
   std::vector<int> slot_level(S.slots.size(), 0), step_level(S.steps.size(), 0);
   int n_levels = 0;
   for (size_t q = 0; q < S.steps.size(); q++) {
@@ -448,6 +462,17 @@ static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) 
   std::vector<int> last_read(S.slots.size(), -1);
   for (int l = 0; l < n_levels; l++)
     for (int q = P->level_begin[l]; q < P->level_begin[l + 1]; q++) last_read[S.steps[q].a] = last_read[S.steps[q].b] = l;
+  // a tangent plan: the sums run after their level's pairs and release the second tangent pair's output; the leaf
+  // tangents are written before the first level
+  std::vector<int> sum_level(P->tan_sums.size());
+  for (size_t k = 0; k < P->tan_sums.size(); k++) {
+    sum_level[k] = slot_level[P->tan_sums[k].t1] - 1;
+    last_read[P->tan_sums[k].t2] = sum_level[k];
+  }
+  for (const auto& tl : P->tan_leaves) {
+    sz[tl.slot] = std::max<size_t>(S.slots[tl.slot].elems * sizeof(double2), 16);
+    P->slot_off[tl.slot] = A.alloc(sz[tl.slot]);
+  }
   for (int l = 0; l < n_levels; l++) {
     if (P->grad && l == P->n_fwd_levels) {         // the seed, written by tncb_plan_vjp before the backward levels
       sz[P->seed_slot] = std::max<size_t>(S.slots[P->seed_slot].elems * sizeof(double2), 16);
@@ -461,6 +486,10 @@ static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) 
     for (int q = P->level_begin[l]; q < P->level_begin[l + 1]; q++) {
       const Step& st = S.steps[q];
       for (int s2 : {st.a, st.b}) if (sz[s2] && last_read[s2] == l) { A.free(P->slot_off[s2], sz[s2]); sz[s2] = 0; }
+    }
+    for (size_t k = 0; k < P->tan_sums.size(); k++) {
+      const int t2 = P->tan_sums[k].t2;
+      if (sum_level[k] == l && sz[t2]) { A.free(P->slot_off[t2], sz[t2]); sz[t2] = 0; }
     }
   }
   P->ws_bytes = A.top;
@@ -483,7 +512,24 @@ static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) 
     }
     P->block_start.push_back(blocks);
   }
-  P->graphable = !P->grad && std::getenv("TNCB_NO_GRAPH") == nullptr && P->ws_bytes <= ((size_t)1 << 30);   // graphs are for small networks
+  if (P->tangent) {
+    P->sum_first.assign(n_levels, 0); P->sum_count.assign(n_levels, 0); P->sum_bs_first.assign(n_levels, 0);
+    for (int l = 0; l < n_levels; l++) {
+      P->sum_first[l] = (int)P->sum_items.size(); P->sum_bs_first[l] = P->sum_bs.size();
+      long long blocks = 0;
+      for (size_t k = 0; k < P->tan_sums.size(); k++) {
+        if (sum_level[k] != l) continue;
+        const auto& ts = P->tan_sums[k];
+        const long long e = (long long)S.slots[ts.t1].elems;
+        P->sum_items.push_back({(long long)P->slot_off[ts.t1], (long long)P->slot_off[ts.t2], (long long)P->slot_off[ts.t1], e});
+        P->sum_bs.push_back(blocks);
+        blocks += (e + kSumThreads - 1) / kSumThreads;
+      }
+      P->sum_count[l] = (int)P->sum_items.size() - P->sum_first[l];
+      if (P->sum_count[l]) P->sum_bs.push_back(blocks);
+    }
+  }
+  P->graphable = !P->grad && !P->tangent && std::getenv("TNCB_NO_GRAPH") == nullptr && P->ws_bytes <= ((size_t)1 << 30);   // graphs are for small networks
   for (const Step& st : S.steps) if (st.plan.kernel_class == 1) { P->graphable = false; break; }   // K1/K1' use ctx-owned tables / arena scratch
 }
 
@@ -536,6 +582,14 @@ static int plan_device_state(tncb_ctx* ctx, tncb_plan* P, bool workspace = true)
     TNCB_CUDA(cudaMemcpyAsync((char*)P->grad_dev + ib, P->grad_block_start.data(), bb, cudaMemcpyHostToDevice, ctx->stream));
     TNCB_CUDA(cudaStreamSynchronize(ctx->stream));
   }
+  if (!P->sum_dev && !P->sum_items.empty()) {
+    const size_t ib = P->sum_items.size() * sizeof(TangentSumItem), bb = P->sum_bs.size() * sizeof(long long);
+    if ((rc = ctx->arena.alloc(ib + bb, &P->sum_dev))) return rc;
+    P->sum_dev_bytes = ib + bb;
+    TNCB_CUDA(cudaMemcpyAsync(P->sum_dev, P->sum_items.data(), ib, cudaMemcpyHostToDevice, ctx->stream));
+    TNCB_CUDA(cudaMemcpyAsync((char*)P->sum_dev + ib, P->sum_bs.data(), bb, cudaMemcpyHostToDevice, ctx->stream));
+    TNCB_CUDA(cudaStreamSynchronize(ctx->stream));
+  }
   if (P->sliced && !P->sl_dev) {
     auto up16 = [](size_t b) { return (b + 15) / 16 * 16; };
     const std::vector<SliceItem>* iv[3] = {&P->sl_items, &P->const_items, &P->acc_items};
@@ -579,6 +633,13 @@ static int enqueue_static(tncb_ctx* ctx, tncb_plan* P, char* ws, int count, long
       const Step& st = S.steps[q];
       rc = launch_pair(ctx, st.plan, (const double2*)(ws + P->slot_off[st.a]), (const double2*)(ws + P->slot_off[st.b]),
                        (double2*)(ws + P->slot_off[st.out]), count, stride);
+    }
+    if (!rc && P->tangent && P->sum_count[l]) {    // a tangent plan: the level's tangent sums, after its pairs
+      const TangentSumItem* d_sum = (const TangentSumItem*)P->sum_dev;
+      const long long* d_sbs = (const long long*)((char*)P->sum_dev + P->sum_items.size() * sizeof(TangentSumItem));
+      const int ns = P->sum_count[l];
+      rc = launch_tangent_sum(ctx, d_sum + P->sum_first[l], d_sbs + P->sum_bs_first[l], ns, P->sum_bs[P->sum_bs_first[l] + ns],
+                              ws, count, stride);
     }
   }
   ctx->partial_override = nullptr; ctx->partial_override_elems = 0;
@@ -757,6 +818,63 @@ static int build_gather(tncb_plan* P, const std::vector<int>& leaf_adj) {
   }
   P->grad_block_start.push_back(blocks);
   if (blocks > 0x7fffffffLL) return fail(TNCB_ERR_UNSUPPORTED, "leaf gradients too large for one gather launch");
+  return TNCB_OK;
+}
+
+// Appends the tangent pairs of a tangent plan to its forward schedule.  For C = contract(A, B) the tangent is
+// Ċ = contract(Ȧ, B) + contract(A, Ḃ); each term has the forward pair's legs, shapes and GEMM view, so it takes the
+// forward step's PairPlan unchanged.  A slot has a tangent only if its subtree holds a requested leaf; a step with one
+// such operand gets one tangent pair, a step with two gets two and a sum (t1 += t2, always in that order).  The requested
+// leaves' tangents get slots of their own (written from the caller's tangent row before the first level), packed in a
+// row at grad_offset like a gradient plan's gradients.
+static int build_tangent(tncb_plan* P, const uint8_t* wrt) {
+  Schedule& S = P->S;
+  const size_t nl = S.n_leaves_total;
+  if (S.steps.empty() || S.result_slot < 0) return fail(TNCB_ERR_UNSUPPORTED, "a tangent plan needs a network with at least one pair");
+  std::vector<int> leaf_slot(nl, -1);
+  for (size_t s = 0; s < S.slots.size(); s++) if (S.slots[s].leaf_index >= 0) leaf_slot[S.slots[s].leaf_index] = (int)s;
+  const size_t n_slots = S.slots.size();
+  std::vector<int> tan(n_slots, -1);                // the tangent slot of a forward slot, -1 = zero tangent
+  P->grad_offset.assign(nl, -1);
+  P->grad_elems = 0;
+  bool any = false;
+  for (size_t li = 0; li < nl; li++) {
+    if (wrt ? !wrt[li] : leaf_slot[li] < 0) continue;
+    if (leaf_slot[li] < 0) return fail(TNCB_ERR_INVALID, "leaf " + std::to_string(li) + " has no payload to differentiate");
+    any = true;
+  }
+  if (!any) return fail(TNCB_ERR_INVALID, "wrt selects no leaf");
+  for (size_t li = 0; li < nl; li++) {
+    if (leaf_slot[li] < 0 || (wrt && !wrt[li])) continue;
+    SlotMeta m;
+    const SlotMeta& leaf = S.slots[leaf_slot[li]];
+    m.legs = leaf.legs; m.dims = leaf.dims; m.elems = leaf.elems;
+    S.slots.push_back(std::move(m));
+    tan[leaf_slot[li]] = (int)S.slots.size() - 1;
+    P->grad_offset[li] = (int64_t)P->grad_elems;
+    P->tan_leaves.push_back({tan[leaf_slot[li]], (int64_t)P->grad_elems});
+    P->grad_elems += S.slots[tan[leaf_slot[li]]].elems;
+  }
+  const size_t n_fwd = S.steps.size();
+  for (size_t q = 0; q < n_fwd; q++) {             // producers come before their consumers
+    const int a = S.steps[q].a, b = S.steps[q].b, out = S.steps[q].out;
+    int first = -1;
+    for (int x : {a, b}) {
+      if (tan[x] < 0) continue;
+      Step ts; ts.a = x == a ? tan[a] : a; ts.b = x == b ? tan[b] : b;
+      ts.plan = S.steps[q].plan;
+      SlotMeta m; m.legs = S.slots[out].legs; m.dims = S.slots[out].dims; m.elems = S.slots[out].elems;
+      S.slots.push_back(std::move(m));
+      ts.out = (int)S.slots.size() - 1;
+      S.flops += ts.plan.flops(); S.bytes += ts.plan.bytes();
+      S.steps.push_back(std::move(ts));
+      if (first < 0) first = S.steps.back().out;
+      else P->tan_sums.push_back({first, S.steps.back().out});
+    }
+    tan[out] = first;
+  }
+  P->tan_result = tan[S.result_slot];
+  if (P->tan_result < 0) return fail(TNCB_ERR_INVALID, "no requested leaf reaches the result");
   return TNCB_OK;
 }
 
@@ -1247,7 +1365,7 @@ int tncb_plan_create_vjp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_pat
 
 int tncb_plan_grad_offsets(const tncb_plan* plan, int64_t* offsets) {
   if (!plan || !offsets) return tncb::fail(TNCB_ERR_INVALID, "null argument");
-  if (!plan->grad) return tncb::fail(TNCB_ERR_INVALID, "not a gradient plan (tncb_plan_create_vjp)");
+  if (!plan->grad && !plan->tangent) return tncb::fail(TNCB_ERR_INVALID, "not a gradient or tangent plan (tncb_plan_create_vjp / _jvp)");
   for (size_t i = 0; i < plan->grad_offset.size(); i++) offsets[i] = plan->grad_offset[i];
   return TNCB_OK;
 }
@@ -1258,6 +1376,7 @@ int tncb_plan_vjp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* seed, tncb_
   using namespace tncb;
   if (!ctx || !plan || !grads) return fail(TNCB_ERR_INVALID, "null argument");
   if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_vjp_sliced");
+  if (plan->tangent) return fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp");
   if (!plan->grad) return fail(TNCB_ERR_INVALID, "not a gradient plan (tncb_plan_create_vjp)");
   if (plan->ctx != ctx || !plan->fwd_ready)
     return fail(TNCB_ERR_INVALID, "tncb_plan_vjp needs a forward run (tncb_plan_run / tncb_plan_execute) of the plan on this context "
@@ -1302,6 +1421,7 @@ int tncb_plan_vjp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t st
                          tncb_tensor** value, tncb_tensor** grads) {
   using namespace tncb;
   if (!ctx || !plan || !value || !grads || stride == 0) return fail(TNCB_ERR_INVALID, "bad argument");
+  if (plan->tangent) return fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp");
   if (!plan->sliced) return fail(TNCB_ERR_INVALID, "not a sliced gradient plan (tncb_plan_create_vjp_sliced)");
   if (plan->ctx != ctx || !plan->full_staged) return fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this context");
   const Schedule& S = plan->S;
@@ -1330,6 +1450,7 @@ int tncb_plan_vjp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t st
 int tncb_plan_execute(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tn, tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   if (!ctx || !plan || !tn) return tncb::fail(TNCB_ERR_INVALID, "null argument");
   if (plan->sliced) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_run_slices / tncb_plan_vjp_sliced");
+  if (plan->tangent) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp");
   if (plan->grad) return tncb::execute_static(ctx, plan, tn, out, n_out, out_legs);   // forward levels only, no fallback
   static const bool trace = std::getenv("TNCB_TRACE") != nullptr;   // per-step times come from the pair-by-pair executor
   if (plan->is_static && !trace && (plan->ctx == nullptr || plan->ctx == ctx)) {
@@ -1373,7 +1494,7 @@ int tncb_plan_stage(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tn) {
   const size_t bytes = std::max<size_t>(S.leaf_block_elems * sizeof(double2), 16);
   std::vector<std::complex<double>> host(std::max<size_t>(S.leaf_block_elems, 1));
   if (plan->is_static && (rc = tncb::plan_device_state(ctx, plan))) {
-    if (rc != TNCB_ERR_OOM || plan->ws || plan->grad) return rc;
+    if (rc != TNCB_ERR_OOM || plan->ws || plan->grad || plan->tangent) return rc;
     plan->is_static = false;    // the static workspace does not fit: resident leaf block + pair-by-pair executor
   }
   if (plan->is_static) {      // the leaf block lives inside the plan workspace
@@ -1399,6 +1520,7 @@ int tncb_plan_stage(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tn) {
 int tncb_plan_run(tncb_ctx* ctx, tncb_plan* plan, tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   if (!ctx || !plan) return tncb::fail(TNCB_ERR_INVALID, "null argument");
   if (plan->sliced) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_run_slices / tncb_plan_vjp_sliced");
+  if (plan->tangent) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp");
   static const bool trace = std::getenv("TNCB_TRACE") != nullptr;
   if (plan->is_static && plan->leaves_resident && plan->ctx == ctx) {
     if (!trace || plan->grad) return tncb::execute_static(ctx, plan, nullptr, out, n_out, out_legs);
@@ -1416,12 +1538,14 @@ int tncb_plan_stage_slices(tncb_ctx* ctx, tncb_plan* plan, size_t n_slices, cons
   if (!ctx || !plan || !slice_tns || n_slices == 0) return tncb::fail(TNCB_ERR_INVALID, "null argument");
   if (plan->sliced) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan stages its full network once (tncb_plan_stage)");
   if (plan->grad) return tncb::fail(TNCB_ERR_UNSUPPORTED, "gradient plans run one staged network at a time");
+  if (plan->tangent) return tncb::fail(TNCB_ERR_UNSUPPORTED, "tangent plans stage many networks with tncb_plan_stage_batch");
   if (!plan->is_static) return tncb::fail(TNCB_ERR_UNSUPPORTED, "sliced execution needs a plan with a static layout (no device leaves)");
   return tncb::stage_networks(ctx, plan, n_slices, slice_tns, true);
 }
 
 int tncb_plan_run_slices(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t stride, tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   if (!ctx || !plan || stride == 0) return tncb::fail(TNCB_ERR_INVALID, "bad argument");
+  if (plan->tangent) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp / tncb_plan_jvp_batch");
   if (plan->sliced) {         // forward levels only, slices extracted on the device from the staged full leaves
     if (plan->ctx != ctx || !plan->full_staged) return tncb::fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this context");
     const tncb::SlotMeta& rm = plan->S.slots[plan->S.result_slot];
@@ -1476,6 +1600,7 @@ int tncb_plan_run_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
   if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
   if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_run_slices / tncb_plan_vjp_sliced");
   if (plan->grad) return fail(TNCB_ERR_UNSUPPORTED, "gradient plans run one staged network at a time");
+  if (plan->tangent) return fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp_batch");
   if (!plan->is_static) return fail(TNCB_ERR_UNSUPPORTED, "batched execution needs a plan with a static layout (no device leaves)");
   if (!plan->slices_dev || plan->ctx != ctx) return fail(TNCB_ERR_INVALID, "tncb_plan_stage_slices has not been called on this context");
   if (count == 0 || first > plan->n_slices || count > plan->n_slices - first)
@@ -1521,7 +1646,8 @@ int tncb_plan_stage_batch(tncb_ctx* ctx, tncb_plan* plan, size_t n, const tncb_t
   using namespace tncb;
   if (!ctx || !plan || !tns || n == 0) return fail(TNCB_ERR_INVALID, "null argument");
   if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan has no batched gradients");
-  if (!plan->grad) return fail(TNCB_ERR_INVALID, "not a gradient plan (plain plans stage many networks with tncb_plan_stage_slices)");
+  if (!plan->grad && !plan->tangent)
+    return fail(TNCB_ERR_INVALID, "not a gradient or tangent plan (plain plans stage many networks with tncb_plan_stage_slices)");
   return stage_networks(ctx, plan, n, tns, false);
 }
 
@@ -1534,6 +1660,7 @@ int tncb_plan_vjp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
   using namespace tncb;
   if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
   if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan has no batched gradients");
+  if (plan->tangent) return fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp_batch");
   if (!plan->grad) return fail(TNCB_ERR_INVALID, "not a gradient plan (tncb_plan_create_vjp)");
   if (!plan->slices_dev || plan->ctx != ctx) return fail(TNCB_ERR_INVALID, "tncb_plan_stage_batch has not been called on this context");
   if (count == 0 || first > plan->n_slices || count > plan->n_slices - first)
@@ -1635,6 +1762,151 @@ int tncb_plan_vjp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
   return TNCB_OK;
 }
 
+// A tangent plan: the forward schedule and the tangent pairs of the `wrt` leaves, on the forward levels of one static
+// layout.  There is no pair-by-pair fallback: a layout above the static-workspace limit is refused here.
+int tncb_plan_create_jvp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, const uint8_t* wrt, tncb_plan** out) {
+  using namespace tncb;
+  if (!tn || !out) return fail(TNCB_ERR_INVALID, "null argument");
+  {
+    std::vector<const tncb_tn*> lv;
+    collect_leaf_nodes(tn, lv);
+    for (const tncb_tn* l : lv)
+      if (l->kind == TNCB_DATA_DEVICE) return fail(TNCB_ERR_UNSUPPORTED, "tangent plans do not take device leaves (they are consumed per call)");
+  }
+  tncb_plan* p = new tncb_plan();
+  p->tangent = true;
+  int rc = build_schedule(tn, path, p->S);
+  if (!rc) rc = build_tangent(p, wrt);
+  if (rc) { delete p; return rc; }
+  size_t dev_free = 0, dev_total = 0;
+  if (ctx) { cudaSetDevice(ctx->device); if (cudaMemGetInfo(&dev_free, &dev_total) != cudaSuccess) { dev_total = 0; cudaGetLastError(); } }
+  plan_static_layout(p, ctx ? ctx->sm_count : 132, dev_total);
+  if (!p->is_static) {
+    const size_t need = p->ws_bytes, limit = static_ws_limit(dev_total);
+    delete p;
+    return fail(TNCB_ERR_UNSUPPORTED, "the tangent workspace needs " + std::to_string(need) + " bytes, above the static-workspace limit of " +
+                                      std::to_string(limit) + " bytes (TNCB_PLAN_WS_GB)");
+  }
+  *out = p;
+  return TNCB_OK;
+}
+
+namespace tncb {
+// the checks tncb_plan_jvp and tncb_plan_jvp_batch share: a tangent plan, an output, tangents shaped `want` with storage
+static int jvp_args(const tncb_plan* plan, const tncb_tensor* tangents, bool any_out, const std::vector<uint64_t>& want) {
+  if (!plan->tangent) return fail(TNCB_ERR_INVALID, "not a tangent plan (tncb_plan_create_jvp)");
+  if (!any_out) return fail(TNCB_ERR_INVALID, "no output requested");
+  if (!tangents) return fail(TNCB_ERR_INVALID, "tangents are needed");
+  bool same = tangents->rank == (int)want.size();
+  for (size_t i = 0; same && i < want.size(); i++) same = tangents->dims[i] == want[i];
+  if (!same) {
+    std::string w;
+    for (uint64_t d : want) w += (w.empty() ? "" : ", ") + std::to_string(d);
+    return fail(TNCB_ERR_SHAPE, "the tangents' dims differ from [" + w + "]");
+  }
+  if (!tangents->ptr) return fail(TNCB_ERR_UNCONTRACTED, "the tangent tensor has no storage");
+  return TNCB_OK;
+}
+
+// the leaf tangents of n instances (rows of `row_elems` elements from `tangents` on) into the workspaces at `ws`,
+// `stride` bytes apart: one leaf_stage_kernel launch, the instance a grid dimension
+static int stage_tangents(tncb_ctx* ctx, const tncb_plan* P, const double2* tangents, unsigned long long row_elems,
+                          char* ws, long long stride, size_t n) {
+  std::vector<LeafStageItem> items;
+  for (const auto& tl : P->tan_leaves)
+    items.push_back({tangents + tl.off, n > 1 ? row_elems : 0, (long long)(P->slot_off[tl.slot] / sizeof(double2)),
+                     (long long)P->S.slots[tl.slot].elems});
+  return launch_leaf_stage(ctx, items.data(), items.size(), (double2*)ws, stride / (long long)sizeof(double2), n);
+}
+} // namespace tncb
+
+// One forward-mode pass on the staged leaves: leaf tangents in, every level (forward pairs, tangent pairs, sums), the
+// result and its tangent out.  Nothing is kept between calls, so a call can be repeated and gives the same bits.
+int tncb_plan_jvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, tncb_tensor** value, tncb_tensor** tangent_out) {
+  using namespace tncb;
+  if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
+  int rc = jvp_args(plan, tangents, value || tangent_out, {plan->grad_elems});
+  if (rc) return rc;
+  if (plan->ctx != ctx || !plan->leaves_resident) return fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this plan and context");
+  TNCB_CUDA(cudaSetDevice(ctx->device));
+  const Schedule& S = plan->S;
+  const SlotMeta& rm = S.slots[S.result_slot];
+  tncb_tensor *v = nullptr, *t = nullptr;
+  if (value) rc = tensor_new(ctx, (int)rm.dims.size(), rm.dims.data(), &v);
+  if (!rc && tangent_out) rc = tensor_new(ctx, (int)rm.dims.size(), rm.dims.data(), &t);
+  char* ws = (char*)plan->ws;
+  if (!rc) rc = stage_tangents(ctx, plan, tangents->ptr, plan->grad_elems, ws, 0, 1);
+  if (!rc) rc = enqueue_static(ctx, plan, ws, 1, 0, 0, (int)plan->level_batched.size());
+  const size_t res_bytes = rm.elems * sizeof(double2);
+  for (auto [dst, slot] : {std::pair<tncb_tensor*, int>{v, S.result_slot}, {t, plan->tan_result}}) {
+    if (rc || !dst || !res_bytes) continue;
+    cudaError_t e = cudaMemcpyAsync(dst->ptr, ws + plan->slot_off[slot], res_bytes, cudaMemcpyDeviceToDevice, ctx->stream);
+    if (e != cudaSuccess) rc = fail(TNCB_ERR_CUDA, std::string("result copy: ") + cudaGetErrorString(e));
+  }
+  if (rc) {
+    for (tncb_tensor* x : {v, t}) if (x) tncb_tensor_free(ctx, x);
+    return rc;
+  }
+  if (value) *value = v;
+  if (tangent_out) *tangent_out = t;
+  return TNCB_OK;
+}
+
+// Instance-batched forward mode over the networks staged by tncb_plan_stage_batch / tncb_plan_stage_instances.  Per pass
+// of c instances on c workspace copies: leaf blocks in, leaf tangents in (row i of `tangents` for instance i), every
+// level, values and tangents out.  Every launch decision is the single-network one, so row i is bit-identical to
+// tncb_plan_jvp of instance i with tangent row i.
+int tncb_plan_jvp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t count, const tncb_tensor* tangents,
+                        tncb_tensor** values, tncb_tensor** tangent_rows) {
+  using namespace tncb;
+  if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
+  if (!plan->tangent) return fail(TNCB_ERR_INVALID, "not a tangent plan (tncb_plan_create_jvp)");
+  if (!plan->slices_dev || plan->ctx != ctx)
+    return fail(TNCB_ERR_INVALID, "tncb_plan_stage_batch / tncb_plan_stage_instances has not been called on this context");
+  if (count == 0 || first > plan->n_slices || count > plan->n_slices - first)
+    return fail(TNCB_ERR_INVALID, "instances [" + std::to_string(first) + ", " + std::to_string(first + count) + ") are not within the " +
+                                  std::to_string(plan->n_slices) + " staged networks");
+  const Schedule& S = plan->S;
+  const SlotMeta& rm = S.slots[S.result_slot];
+  const int r = (int)rm.dims.size();
+  if (r + 1 > kMaxLegs) return fail(TNCB_ERR_INVALID, "a result of rank 64 leaves no room for the instance dimension");
+  int rc = jvp_args(plan, tangents, values || tangent_rows, {(uint64_t)count, plan->grad_elems});
+  if (rc) return rc;
+  TNCB_CUDA(cudaSetDevice(ctx->device));
+  BatchBlock B;
+  if ((rc = batch_size(ctx, plan, count, &B))) return rc;
+  std::vector<uint64_t> dims(r + 1);
+  dims[0] = count;
+  for (int i = 0; i < r; i++) dims[i + 1] = rm.dims[i];
+  tncb_tensor *v = nullptr, *t = nullptr;
+  if (values) rc = tensor_new(ctx, r + 1, dims.data(), &v);
+  if (!rc && tangent_rows) rc = tensor_new(ctx, r + 1, dims.data(), &t);
+  if (!rc) rc = batch_alloc(ctx, &B);
+  const size_t ws = B.ws, c = B.c;
+  char* base = (char*)B.blk;
+  const size_t block_bytes = std::max<size_t>(S.leaf_block_elems, 1) * sizeof(double2);
+  const size_t res_bytes = rm.elems * sizeof(double2);
+  const uint64_t te = plan->grad_elems;
+  for (size_t done = 0; done < count && !rc; done += c) {
+    const size_t n = std::min(c, count - done);
+    const char* src = (const char*)plan->slices_dev + (first + done) * block_bytes;
+    if ((rc = batch_copy(ctx, B, base + plan->leaf_off, ws, src, block_bytes, block_bytes, n))) break;
+    if ((rc = stage_tangents(ctx, plan, tangents->ptr + done * te, te, base, (long long)ws, n))) break;
+    if ((rc = enqueue_static(ctx, plan, base, (int)n, (long long)ws, 0, (int)plan->level_batched.size()))) break;
+    if (!res_bytes) continue;
+    if (v && (rc = batch_copy(ctx, B, (char*)v->ptr + done * res_bytes, res_bytes, base + plan->slot_off[S.result_slot], ws, res_bytes, n))) break;
+    if (t && (rc = batch_copy(ctx, B, (char*)t->ptr + done * res_bytes, res_bytes, base + plan->slot_off[plan->tan_result], ws, res_bytes, n))) break;
+  }
+  batch_free(ctx, &B);
+  if (rc) {
+    for (tncb_tensor* x : {v, t}) if (x) tncb_tensor_free(ctx, x);
+    return rc;
+  }
+  if (values) *values = v;
+  if (tangent_rows) *tangent_rows = t;
+  return TNCB_OK;
+}
+
 // New payloads for some leaves of the staged network, straight from device memory: one launch on the ctx stream into the
 // leaf block the next run reads (a static plan's workspace block, which its graph replays also read; a non-static plan's
 // resident block; a sliced gradient plan's full block).  The static layout never releases its leaf block, so the new
@@ -1697,7 +1969,7 @@ int tncb_plan_stage_instances(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tmp
     for (const LeafStageItem& it : items) { gap(it.dst); pos = std::max(pos, it.dst + it.elems); }
     gap((long long)block);
   }
-  if ((rc = plan_device_state(ctx, plan, !plan->grad))) return rc;
+  if ((rc = plan_device_state(ctx, plan, !plan->grad && !plan->tangent))) return rc;
   if (!plan->tmpl_host) {
     plan->tmpl_bytes = block * sizeof(double2);
     TNCB_CUDA(cudaMallocHost(&plan->tmpl_host, plan->tmpl_bytes));
@@ -1761,7 +2033,7 @@ int tncb_plan_info(const tncb_plan* plan, uint64_t* n_pairs, double* flops, doub
   if (n_pairs) *n_pairs = S.steps.size();
   if (flops) *flops = S.flops;
   if (bytes) *bytes = S.bytes;
-  if (peak_bytes && plan->grad) *peak_bytes = plan->ws_bytes;   // the whole pass lives in its static workspace
+  if (peak_bytes && (plan->grad || plan->tangent)) *peak_bytes = plan->ws_bytes;   // the whole pass lives in its static workspace
   else if (peak_bytes) { // replay the liveness: leaves + live intermediates
     size_t live = S.leaf_block_elems * 16, peak = live;
     std::vector<size_t> sz(S.slots.size(), 0);
@@ -1779,6 +2051,8 @@ int tncb_plan_info(const tncb_plan* plan, uint64_t* n_pairs, double* flops, doub
     if (!plan->grad_items.empty()) k++;                                            // the leaf-gradient gather
     if (!plan->acc_items.empty()) k++;                                             // a slice's gradient accumulation
     if (!plan->sl_items.empty()) k++;                                              // a slice's leaf extraction
+    k += (plan->tan_leaves.size() + tncb::kStageItems - 1) / tncb::kStageItems;    // the leaf tangents' staging
+    for (int ns : plan->sum_count) if (ns) k++;                                    // a level's tangent sums
     *n_kernels = k + 2 * plan->grad_permutes.size();                               // (K3: tables + transpose)
   }
   return TNCB_OK;
@@ -1794,6 +2068,7 @@ void tncb_plan_release_device_state(tncb_plan* plan) {
   for (int i = 0; i < 2; i++) if (plan->exec[i]) { cudaGraphExecDestroy(plan->exec[i]); plan->exec[i] = nullptr; }
   if (plan->batch_dev) { ctx->arena.free(plan->batch_dev, plan->batch_bytes); plan->batch_dev = nullptr; }
   if (plan->grad_dev) { ctx->arena.free(plan->grad_dev, plan->grad_dev_bytes); plan->grad_dev = nullptr; }
+  if (plan->sum_dev) { ctx->arena.free(plan->sum_dev, plan->sum_dev_bytes); plan->sum_dev = nullptr; }
   if (plan->sl_dev) { ctx->arena.free(plan->sl_dev, plan->sl_dev_bytes); plan->sl_dev = nullptr; }
   if (plan->full_dev) { ctx->arena.free(plan->full_dev, plan->full_bytes); plan->full_dev = nullptr; }
   plan->full_staged = false;

@@ -247,6 +247,18 @@ class NetworkPlan:
         """A gradient plan (tncb_plan_create_vjp): `stage` + `run` (or `execute`) contract the network as a plain plan
         does, then `vjp` returns the gradient of the result with respect to the leaves `wrt` (indices into
         `leaves(tn)`; None = every leaf with a payload) in one backward pass."""
+        return cls._derivative_plan("tncb_plan_create_vjp", tn, contract_path, wrt, ctx)
+
+    @classmethod
+    def for_tangents(cls, tn: Tensor, contract_path: ContractionPath, wrt=None, ctx: Optional[Context] = None) -> "NetworkPlan":
+        """A tangent plan (tncb_plan_create_jvp): after `stage`, `jvp` returns the result and its directional derivative
+        along tangents of the leaves `wrt` (indices into `leaves(tn)`; None = every leaf with a payload) in one pass over
+        the forward levels.  `stage_batch` / `stage_instances` + `jvp_batch` do the same for many networks, or for
+        many directions of one network."""
+        return cls._derivative_plan("tncb_plan_create_jvp", tn, contract_path, wrt, ctx)
+
+    @classmethod
+    def _derivative_plan(cls, create: str, tn: Tensor, contract_path: ContractionPath, wrt, ctx) -> "NetworkPlan":
         self = cls.__new__(cls)
         self.handle = None
         self.ctx = ctx or default_context()
@@ -261,7 +273,7 @@ class NetworkPlan:
         m = _Marshal()
         c_tn, c_path = m.tn(tn), m.path(contract_path)
         h = C.c_void_p()
-        check(self.ctx._l.tncb_plan_create_vjp(self.ctx.handle, C.byref(c_tn), C.byref(c_path), mask, C.byref(h)))
+        check(getattr(self.ctx._l, create)(self.ctx.handle, C.byref(c_tn), C.byref(c_path), mask, C.byref(h)))
         self.handle = h
         self.leaf_shapes = shapes
         n_out, legs, dims = C.c_int(), u64_array([0] * 64), u64_array([0] * 64)
@@ -301,6 +313,95 @@ class NetworkPlan:
             if tmp is not None:
                 tmp.free()
         return DeviceTensor.adopt(self.ctx, out)
+
+    def _tangent_block(self, tangents: dict, count: Optional[int] = None) -> DeviceTensor:
+        """{leaf index: tangent} packed at grad_offsets() into a [tangent_elems] (count=None) or [count, tangent_elems]
+        block on the device; leaves left out have zero tangent.  A tangent is shaped like its leaf (with count: shared by
+        every instance) or, with count, [count, *leaf shape].  Any torch CUDA tensor among them: packed by torch on the
+        context's device (host arrays are uploaded first), nothing goes through the host; else packed on the host, one
+        upload."""
+        offs = self.grad_offsets()
+        sizes = [int(np.prod(s, dtype=np.int64)) for s in self.leaf_shapes]
+        elems = sum(sz for off, sz in zip(offs, sizes) if off >= 0)
+        lead = () if count is None else (int(count),)
+        on_device = any(type(x).__module__.split(".")[0] == "torch" for x in tangents.values())
+        if on_device:
+            import torch
+            from .. import check_cuda_tensor
+            block = torch.zeros(lead + (elems,), dtype=torch.complex128, device=torch.device("cuda", self.ctx.device))
+        else:
+            block = np.zeros(lead + (elems,), dtype=np.complex128)
+        for leaf, x in tangents.items():
+            leaf = int(leaf)
+            if not 0 <= leaf < len(offs):
+                raise IndexError(f"leaf index {leaf} out of range ({len(offs)} leaves)")
+            if offs[leaf] < 0:
+                raise ValueError(f"leaf {leaf} is not requested by this tangent plan")
+            shape = tuple(self.leaf_shapes[leaf])
+            if on_device:
+                if isinstance(x, torch.Tensor):
+                    check_cuda_tensor(self.ctx, x, f"the tangent of leaf {leaf}")
+                    x = x.detach().to(torch.complex128)
+                else:
+                    x = torch.as_tensor(np.asarray(x, dtype=np.complex128), device=block.device)
+            else:
+                x = np.asarray(x, dtype=np.complex128)
+            got = tuple(x.shape)
+            if got != shape and (count is None or got != lead + shape):
+                want = f"{shape}" if count is None else f"{lead + shape} or {shape}"
+                raise ValueError(f"the tangent of leaf {leaf} has shape {got}, expected {want}")
+            block[..., offs[leaf]:offs[leaf] + sizes[leaf]] = x.reshape(lead + (sizes[leaf],) if got != shape else (sizes[leaf],))
+        return DeviceTensor.from_torch(self.ctx, block) if on_device else DeviceTensor.from_numpy(self.ctx, block)
+
+    def jvp_block(self, tangents: dict):
+        """One forward-mode pass on the staged leaves (tncb_plan_jvp), left on the device: (value, tangent) DeviceTensors
+        with the result's shape.  tangents: {leaf index: array or torch CUDA tensor shaped like the leaf}; requested
+        leaves left out have zero tangent.  The value equals a plain plan's run bit for bit; a call repeats bit for bit."""
+        block = self._tangent_block(tangents)
+        val, tan = C.c_void_p(), C.c_void_p()
+        try:
+            check(self.ctx._l.tncb_plan_jvp(self.ctx.handle, self.handle, block.handle, C.byref(val), C.byref(tan)))
+        finally:
+            block.free()
+        return DeviceTensor.adopt(self.ctx, val), DeviceTensor.adopt(self.ctx, tan)
+
+    def jvp(self, tangents: dict):
+        """`jvp_block` with the derivative downloaded: (value Tensor on the device with the result's legs, tangent
+        ndarray), tangent[r] = sum_l sum_e dR[r]/dX_l[e] tangents[l][e] (no conjugation)."""
+        val, tan = self.jvp_block(tangents)
+        res = Tensor(list(self.result_legs), val.shape)
+        res.set_tensor_data(TensorData.Matrix(val))
+        out = tan.to_numpy()
+        tan.free()
+        return res, out
+
+    def jvp_batch_blocks(self, first: int = 0, count: Optional[int] = None, tangents: Optional[dict] = None,
+                         values: bool = True):
+        """`jvp_batch` left on the device: [values [count, *dims] or None, tangents [count, *dims]] as DeviceTensors"""
+        if count is None:
+            count = max(0, getattr(self, "n_staged", 0) - int(first))
+        block = self._tangent_block(tangents or {}, int(count))
+        outs = [C.c_void_p() if values else None, C.c_void_p()]
+        try:
+            check(self.ctx._l.tncb_plan_jvp_batch(self.ctx.handle, self.handle, int(first), int(count), block.handle,
+                                                  *[C.byref(o) if o is not None else None for o in outs]))
+        finally:
+            block.free()
+        return [None if o is None else DeviceTensor.adopt(self.ctx, o) for o in outs]
+
+    def jvp_batch(self, first: int = 0, count: Optional[int] = None, tangents: Optional[dict] = None, values: bool = True):
+        """Forward mode over the staged networks first .. first + count - 1 (stage_batch / stage_instances), each with
+        its own tangents, the instances a grid dimension of every kernel (tncb_plan_jvp_batch).  tangents: {leaf index:
+        [count, *leaf shape] (a row per instance) or [*leaf shape] (the same for every instance)}.  Returns (legs of one
+        instance, values [count, *dims] or None, tangents [count, *dims]); row i equals jvp of instance i with its
+        tangent rows, bit for bit.  Many directions of one network: stage_instances of it with count copies, one
+        tangent row per direction."""
+        host = []
+        for dt in self.jvp_batch_blocks(first, count, tangents, values):
+            host.append(None if dt is None else dt.to_numpy())
+            if dt is not None:
+                dt.free()
+        return list(self.result_legs), host[0], host[1]
 
     def set_leaves(self, payloads: dict) -> None:
         """New payloads for leaves of the staged network straight from device memory (tncb_plan_set_leaves): {leaf index
