@@ -279,6 +279,74 @@ class NetworkPlan {
     check(drc);
     return out;
   }
+  // A Hessian-vector plan (tncb_plan_create_hvp): wrt as for ForGradients.  stage, then hvp gives R, Ṙ, the gradients G
+  // and their forward derivative Ġ in one pass.
+  struct ForHvp { std::vector<size_t> wrt; };
+  NetworkPlan(Context& ctx, const Tensor& tn, const ContractionPath& path, const ForHvp& h) : ctx_(ctx) {
+    detail::Marshal m;
+    tncb_tn c_tn = m.tn(tn);
+    tncb_path c_path = m.path(path);
+    n_leaves_ = count_leaves(tn);
+    leaf_elems(tn, leaf_elems_);
+    std::vector<uint8_t> mask(n_leaves_ ? n_leaves_ : 1, 0);
+    for (size_t i : h.wrt) {
+      if (i >= n_leaves_) throw Error(TNCB_ERR_INVALID, "wrt: leaf index out of range");
+      mask[i] = 1;
+    }
+    int n_out = 0; uint64_t legs[64];
+    res_dims_.resize(64);
+    check(tncb_network_out_legs(&c_tn, &c_path, &n_out, legs, res_dims_.data()));
+    res_dims_.resize(n_out);
+    check(tncb_plan_create_hvp(ctx.get(), &c_tn, &c_path, h.wrt.empty() ? nullptr : mask.data(), &h_));
+  }
+  // value R and tangent Ṙ row-major over the result's legs; grads G_l and grad_tangents Ġ_l per requested leaf,
+  // row-major in the leaf's leg order
+  struct Hvp {
+    std::vector<Complex64> value, tangent;
+    std::map<size_t, std::vector<Complex64>> grads, grad_tangents;
+  };
+  // After stage: one forward-over-reverse pass.  tangents: leaf index -> Ẋ_l (requested leaves left out: zero);
+  // seed: row-major over the result's legs, empty = 1 (scalar results only); seed_tangent: Ṡ, empty = zero.
+  Hvp hvp(const std::map<size_t, std::vector<Complex64>>& tangents, const std::vector<Complex64>& seed = {},
+          const std::vector<Complex64>& seed_tangent = {}) {
+    std::vector<int64_t> off(n_leaves_ ? n_leaves_ : 1);
+    check(tncb_plan_grad_offsets(h_, off.data()));
+    uint64_t elems = 0;
+    for (size_t i = 0; i < n_leaves_; i++) if (off[i] >= 0) elems += leaf_elems_[i];
+    std::vector<Complex64> block(elems);
+    for (const auto& [i, x] : tangents) {
+      if (i >= n_leaves_ || off[i] < 0) throw Error(TNCB_ERR_INVALID, "hvp: tangent for a leaf the plan does not request");
+      if (x.size() != leaf_elems_[i]) throw Error(TNCB_ERR_SHAPE, "hvp: tangent size differs from the leaf's");
+      std::copy(x.begin(), x.end(), block.begin() + off[i]);
+    }
+    tncb_tensor* in[3] = {nullptr, nullptr, nullptr};        // tangents, seed, seed tangent
+    int rc = tncb_tensor_upload(ctx_.get(), 1, &elems, reinterpret_cast<const double*>(block.data()), &in[0]);
+    if (!rc && !seed.empty())
+      rc = tncb_tensor_upload(ctx_.get(), (int)res_dims_.size(), res_dims_.data(), reinterpret_cast<const double*>(seed.data()), &in[1]);
+    if (!rc && !seed_tangent.empty())
+      rc = tncb_tensor_upload(ctx_.get(), (int)res_dims_.size(), res_dims_.data(), reinterpret_cast<const double*>(seed_tangent.data()), &in[2]);
+    tncb_tensor* out[4] = {nullptr, nullptr, nullptr, nullptr};   // R, Ṙ, G, Ġ
+    if (!rc) rc = tncb_plan_hvp(ctx_.get(), h_, in[0], in[1], in[2], &out[0], &out[1], &out[2], &out[3]);
+    for (tncb_tensor* x : in) if (x) tncb_tensor_free(ctx_.get(), x);
+    check(rc);
+    std::vector<Complex64> host[4];
+    int drc = 0;
+    for (int k = 0; k < 4; k++) {
+      host[k].resize(tncb_tensor_elements(out[k]));
+      if (!drc) drc = tncb_tensor_download(ctx_.get(), out[k], reinterpret_cast<double*>(host[k].data()));
+      tncb_tensor_free(ctx_.get(), out[k]);
+    }
+    check(drc);
+    Hvp res;
+    res.value = std::move(host[0]);
+    res.tangent = std::move(host[1]);
+    for (size_t i = 0; i < n_leaves_; i++) {
+      if (off[i] < 0) continue;
+      res.grads[i].assign(host[2].begin() + off[i], host[2].begin() + off[i] + leaf_elems_[i]);
+      res.grad_tangents[i].assign(host[3].begin() + off[i], host[3].begin() + off[i] + leaf_elems_[i]);
+    }
+    return res;
+  }
   ~NetworkPlan() { tncb_plan_destroy(h_); }
   NetworkPlan(const NetworkPlan&) = delete;
   NetworkPlan& operator=(const NetworkPlan&) = delete;

@@ -450,6 +450,38 @@ int tncb_plan_jvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, t
  * -> TNCB_ERR_SHAPE; not even one workspace copy fits -> TNCB_ERR_OOM.  Errors leave the arena as they found it. */
 int tncb_plan_jvp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t count, const tncb_tensor* tangents,
                         tncb_tensor** values, tncb_tensor** tangent_rows);
+/* ---- Hessian-vector products (forward over reverse) ----
+ * For a plan of (tn, path) with result R, seed S, leaf tangents Ẋ_l of the requested leaves and a seed tangent Ṡ, one
+ * pass gives (holomorphic, no conjugation anywhere)
+ *   R;   Ṙ = sum_l sum_e dR/dX_l[e] Ẋ_l[e]                                   (as tncb_plan_jvp)
+ *   G_l  = sum_r S[r] dR[r]/dX_l                                             (as tncb_plan_vjp)
+ *   Ġ_l  = sum_r Ṡ[r] dR[r]/dX_l + sum_r S[r] sum_m sum_e' d²R[r]/dX_l dX_m[e'] Ẋ_m[e']
+ * the forward derivative of G in the direction (Ẋ, Ṡ).  Second derivatives are symmetric, so the vjp of (X, S) -> G
+ * with cotangent W is (Ġ with Ẋ = W and Ṡ = 0, Ṙ with Ẋ = W): one call serves double backward and forward-over-reverse.
+ * Every leaf occurs once, so R is multilinear and the diagonal blocks (l = m) of the Hessian are zero.  The plan holds
+ * the forward pairs, the tangent pairs of tncb_plan_create_jvp, the backward pairs of tncb_plan_create_vjp and, for
+ * every backward pair x̄ = C̄.O, its tangent dx̄ = dC̄.O + C̄.dO: pairs with the backward pair's legs and GEMM view on
+ * the same engines and backward level, summed in that order when both exist.  Cost: about nine forward passes with
+ * every leaf requested, in one walk over the levels.  Arguments and refusals as tncb_plan_create_jvp (the message of
+ * a workspace above the limit states the bytes needed); ctx may be NULL (host-only compile: tncb_plan_info and
+ * tncb_plan_grad_offsets).  Always static, never graphed, no pair-by-pair fallback.  Every other plan entry point but
+ * tncb_plan_stage / set_leaves / info / grad_offsets -> TNCB_ERR_UNSUPPORTED on a Hessian-vector plan. */
+int tncb_plan_create_hvp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, const uint8_t* wrt, tncb_plan** out);
+/* One forward-over-reverse pass on the leaves staged by tncb_plan_stage (and overwritten by tncb_plan_set_leaves).
+ * tangents:     [tangent_elems] device tensor at tncb_plan_grad_offsets (the gradient block's layout)
+ * seed:         the result's dims; NULL only for a rank-0 result (seed 1)
+ * seed_tangent: the result's dims; NULL = zero
+ * *value, *tangent_out: new tensors with the result's dims, R (bit-identical to a plain plan's tncb_plan_run) and Ṙ
+ *   (bit-identical to tncb_plan_jvp with the same tangents)
+ * *grads, *grad_tangents: new [tangent_elems] tensors at tncb_plan_grad_offsets, G (bit-identical to tncb_plan_vjp(seed)
+ *   of a gradient plan after a run) and Ġ
+ * Each output may be NULL, not all four.  Each call is self-contained and repeats bit for bit.  Not a Hessian-vector
+ * plan, not staged on this context, no output, NULL tangents, a NULL seed for a result of rank > 0 ->
+ * TNCB_ERR_INVALID; tangent, seed or seed-tangent dims that do not match -> TNCB_ERR_SHAPE.  Errors leave the arena as
+ * they found it. */
+int tncb_plan_hvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, const tncb_tensor* seed,
+                  const tncb_tensor* seed_tangent, tncb_tensor** value, tncb_tensor** tangent_out, tncb_tensor** grads,
+                  tncb_tensor** grad_tangents);
 void tncb_plan_destroy(tncb_plan* plan);
 
 /* ---- HDF5 tensor files: replaces tnc::io::hdf5 (tnc/src/io/hdf5.rs), which binds libhdf5 through hdf5-metno.

@@ -121,6 +121,8 @@ SIGNATURES = {
     "tncb_plan_create_jvp": (C.c_int, [C.c_void_p, C.POINTER(TncbTn), C.POINTER(TncbPath), C.POINTER(C.c_uint8), vpp]),
     "tncb_plan_jvp": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, vpp, vpp]),
     "tncb_plan_jvp_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, vpp, vpp]),
+    "tncb_plan_create_hvp": (C.c_int, [C.c_void_p, C.POINTER(TncbTn), C.POINTER(TncbPath), C.POINTER(C.c_uint8), vpp]),
+    "tncb_plan_hvp": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, vpp, vpp, vpp, vpp]),
     "tncb_plan_destroy": (None, [C.c_void_p]),
     "tncb_comm_unique_id": (C.c_int, [C.c_void_p]),
     "tncb_comm_init": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p]),

@@ -9,7 +9,12 @@ angle-derivative table.  One backward pass gives the gradient of every input, at
 With `sliced_legs`, a network whose gradient workspace does not fit unsliced runs slice by slice (SlicedPlan.for_gradients).
 With `batched`, B networks that differ in some leaves (bitstrings, input states) run in one batched pass
 (NetworkPlan.vjp_batch) and the result gets a leading dimension B.  With `on_device=True`, CUDA inputs are copied into the
-staged plan on the device and the result and gradients come back as CUDA tensors."""
+staged plan on the device and the result and gradients come back as CUDA tensors.
+
+Forward mode (torch.autograd.forward_ad, torch.func.jvp) runs on a tangent plan (NetworkPlan.for_tangents).  Without
+`batched` or `sliced_legs`, the backward is itself differentiable: `grad(..., create_graph=True)` followed by another
+`grad`, torch.autograd.functional.hvp / hessian and torch.func.jvp of torch.func.grad get the second-order terms that
+pass through the network from Hessian-vector products of a forward-over-reverse plan (NetworkPlan.for_hvp)."""
 from __future__ import annotations
 
 from typing import Optional, Sequence
@@ -64,6 +69,14 @@ class _NetworkFn(torch.autograd.Function):
     def backward(ctx, grad_out):
         xs = ctx.saved_tensors           # raises on a second backward through a graph that was not retained
         runner = ctx.runner
+        if not runner.batched and not runner.sliced:
+            # G through a differentiable Function of (seed, xs), so that create_graph=True keeps the second-order terms
+            g = _GradFn.apply(runner, ctx, torch.conj_physical(grad_out), *xs)
+            return (None,) + tuple(torch.conj_physical(x) for x in g)
+        if torch.is_grad_enabled():      # create_graph=True: the gradients would have no graph back to the inputs
+            what = "batched inputs" if runner.batched else "sliced_legs"
+            raise NotImplementedError(f"second-order derivatives (create_graph=True) are not supported with {what}: "
+                                      "Hessian-vector plans are neither batched nor sliced")
         if runner.on_device:
             return (None,) + runner._backward_device(ctx, grad_out, xs)
         seed = np.conj(grad_out.detach().to(torch.complex128).cpu().numpy())
@@ -71,16 +84,74 @@ class _NetworkFn(torch.autograd.Function):
             if runner._token != ctx.token:
                 ctx.token = runner._stage_batch(xs)
             return (None,) + runner._batch_grads(seed, xs)
-        if runner.sliced:                # vjp_sliced re-runs every slice's forward: it only needs these inputs staged
-            if runner._token != ctx.token:
-                ctx.token = runner._stage(xs)
-            g = runner.plan.vjp(seed)[1]
-        else:
-            if runner._token != ctx.token:   # another forward (or an earlier backward) used the plan's state since
-                ctx.token = runner._forward(xs)
-            runner._token = None             # the backward levels overwrite the forward state
-            g = runner.plan.vjp(seed)
+        # sliced: vjp_sliced re-runs every slice's forward, it only needs these inputs staged
+        if runner._token != ctx.token:
+            ctx.token = runner._stage(xs)
+        g = runner.plan.vjp(seed)[1]
         return (None,) + tuple(torch.from_numpy(np.conj(g[i])).to(x.device) for i, x in zip(runner.wrt, xs))
+
+
+class _GradFn(torch.autograd.Function):
+    """(seed, *xs) -> G of an unbatched, unsliced network_function: G_i = sum_r seed[r] dR[r]/dx_i, holomorphic in the
+    seed and the inputs (no conjugation).  forward is the gradient plan's run + vjp.  Second derivatives are symmetric,
+    so the vjp of this map with cotangent W is (Ṙ, Ġ) of a Hessian-vector pass with leaf tangents W and no seed tangent
+    (_HessFn, itself differentiable in W), and its jvp is Ġ: one NetworkPlan.hvp_blocks call each (torch's
+    conjugations for a holomorphic map around them)."""
+
+    @staticmethod
+    def forward(runner, fctx, seed, *xs):
+        return runner._grads(fctx, seed, xs)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        runner, seed, xs = inputs[0], inputs[2], inputs[3:]
+        ctx.runner = runner
+        ctx.save_for_backward(seed, *xs)
+        ctx.save_for_forward(seed, *xs)
+
+    @staticmethod
+    def backward(ctx, *w):
+        seed, *xs = ctx.saved_tensors
+        us = [torch.zeros_like(x) if t is None else torch.conj_physical(t) for x, t in zip(xs, w)]
+        rdot, *gdot = _HessFn.apply(ctx.runner, seed, *xs, *us)
+        return (None, None, torch.conj_physical(rdot)) + tuple(torch.conj_physical(g) for g in gdot)
+
+    @staticmethod
+    def jvp(ctx, _runner_tangent, _fctx_tangent, seed_tangent, *tangents):
+        seed, *xs = ctx.saved_tensors
+        runner = ctx.runner
+        with torch._C._DisableFuncTorch():   # (see _NetworkFn.jvp)
+            tans = {i: t for i, t in zip(runner.wrt, tangents) if t is not None}
+            _, gdot = runner._hvp(xs, seed, tans, seed_tangent, want_rdot=False)
+        return gdot
+
+
+class _HessFn(torch.autograd.Function):
+    """(seed, xs, us) -> (Ṙ, Ġ_i) of a Hessian-vector pass with leaf tangents us and no seed tangent: the holomorphic
+    vjp of _GradFn, linear in us.  Its own vjp with respect to us, which torch.autograd.functional.hvp needs (it
+    differentiates a backward with respect to its cotangent), is its transpose: Ġ of one pass with leaf tangents from
+    the cotangent of Ġ and the seed tangent from the cotangent of Ṙ.  No gradient flows to the seed and the inputs
+    through it: derivatives of third order are not computed."""
+
+    @staticmethod
+    def forward(runner, seed, *xs_us):
+        n = len(xs_us) // 2
+        rdot, gdot = runner._hvp(xs_us[:n], seed, dict(zip(runner.wrt, xs_us[n:])), None, want_rdot=True)
+        return (rdot,) + gdot
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        ctx.runner = inputs[0]
+        ctx.save_for_backward(*inputs[1:len(inputs) - (len(inputs) - 2) // 2])
+
+    @staticmethod
+    def backward(ctx, a, *b):
+        seed, *xs = ctx.saved_tensors
+        runner = ctx.runner
+        with torch._C._DisableFuncTorch():   # (see _NetworkFn.jvp)
+            tans = {i: torch.conj_physical(t) for i, t in zip(runner.wrt, b) if t is not None}
+            _, gdot = runner._hvp(xs, seed, tans, None if a is None else torch.conj_physical(a), want_rdot=False)
+        return (None, None) + (None,) * len(xs) + tuple(torch.conj_physical(g) for g in gdot)
 
 
 class NetworkFunction:
@@ -119,6 +190,8 @@ class NetworkFunction:
         self._sliced_legs = tuple(sliced_legs)
         self._tplan = None               # the tangent plan, compiled on the first forward-mode call
         self._tstaged = False            # on_device, unbatched: the tangent plan has `tn` staged
+        self._hplan = None               # the Hessian-vector plan, compiled on the first second-order call
+        self._hstaged = False            # on_device: the Hessian-vector plan has `tn` staged
 
     # ---- on_device: inputs, results and gradients stay on the GPU ----
     def _check_device(self, xs):
@@ -173,28 +246,92 @@ class NetworkFunction:
         return token
 
     def _backward_device(self, fctx, grad_out, xs):
+        """the gradients of batched or sliced inputs (torch's convention, conj of the holomorphic vjp)"""
         seed = DeviceTensor.from_torch(self.plan.ctx, torch.conj_physical(grad_out.detach().to(torch.complex128)))
         try:
             if self.batched:
                 if self._token != fctx.token:
                     fctx.token = self._stage_instances(xs)
                 return self._batch_grads_device(seed, xs)
-            if self.sliced:
-                if self._token != fctx.token:
-                    fctx.token = self._set_device(xs)
-                value, block = self.plan.vjp_blocks(seed)
-                value.free()
-            else:
-                if self._token != fctx.token:
-                    fctx.token = self._forward_device(xs)
-                self._token = None
-                block = self.plan.vjp_block(seed)
+            if self._token != fctx.token:
+                fctx.token = self._set_device(xs)
+            value, block = self.plan.vjp_blocks(seed)
+            value.free()
             flat = torch.conj_physical(block.to_torch())
             block.free()
         finally:
             seed.free()
         g = self._split(flat)
         return tuple(g[i] for i in self.wrt)
+
+    def _grads(self, fctx, seed, xs):
+        """G_i = sum_r seed[r] dR[r]/dx_i (holomorphic, no conjugation) of the unbatched, unsliced plan, one per wrt input:
+        the forward of the _NetworkFn call `fctx` (re-run when another call used the plan's state since), then vjp"""
+        seed = seed.detach().to(torch.complex128)
+        if self.on_device:
+            s = DeviceTensor.from_torch(self.plan.ctx, seed)
+            try:
+                if self._token != fctx.token:
+                    fctx.token = self._forward_device(xs)
+                self._token = None
+                block = self.plan.vjp_block(s)
+                flat = block.to_torch()
+                block.free()
+            finally:
+                s.free()
+            g = self._split(flat)
+            return tuple(g[i] for i in self.wrt)
+        if self._token != fctx.token:    # another forward (or an earlier backward) used the plan's state since
+            fctx.token = self._forward(xs)
+        self._token = None               # the backward levels overwrite the forward state
+        g = self.plan.vjp(seed.cpu().numpy())
+        return tuple(torch.from_numpy(g[i]).to(x.device) for i, x in zip(self.wrt, xs))
+
+    # ---- second order (create_graph=True, torch.autograd.functional.hvp / hessian, torch.func.jvp of torch.func.grad):
+    # a Hessian-vector plan, compiled on the first second-order call ----
+    def _hvp(self, xs, seed, tangents: dict, seed_tangent, want_rdot: bool):
+        """(Ṙ or None, (Ġ_i per wrt input)) of one NetworkPlan.hvp_blocks pass on the inputs xs with seed `seed`, leaf
+        tangents {wrt leaf: tensor} (left out: zero) and seed tangent `seed_tangent` (None: zero); no conjugation"""
+        if self._hplan is None:
+            self._hplan = NetworkPlan.for_hvp(self.tn, self.path, self.wrt, ctx=self._ctx)
+        plan = self._hplan
+        for i, shape, x in zip(self.wrt, self.shapes, xs):
+            if tuple(x.shape) != shape:
+                raise ValueError(f"input for leaf {i} has shape {tuple(x.shape)}, the leaf {shape}")
+        outputs = (False, want_rdot, False, True)
+
+        def phys(t):
+            return t.detach().to(torch.complex128).resolve_conj()
+        if self.on_device:
+            self._check_device(xs)
+            for i, t in tangents.items():
+                check_cuda_tensor(plan.ctx, t, f"tangent for leaf {i}")
+            if not self._hstaged:
+                plan.stage(self.tn)
+                self._hstaged = True
+            plan.set_leaves(dict(zip(self.wrt, xs)))
+            _, rdot, _, gdot = plan.hvp_blocks({i: phys(t) for i, t in tangents.items()}, phys(seed),
+                                               None if seed_tangent is None else phys(seed_tangent), outputs)
+            out = []
+            for dt in (rdot, gdot):
+                out.append(None if dt is None else dt.to_torch())
+                if dt is not None:
+                    dt.free()
+            g = self._split(out[1])
+            return out[0], tuple(g[i] for i in self.wrt)
+
+        def host(t):                     # (np.ascontiguousarray would make a rank-0 seed rank 1)
+            return phys(t).contiguous().cpu().numpy()
+        plan.stage(_with_payloads(self.tn, {i: host(x) for i, x in zip(self.wrt, xs)}, [0]))
+        _, rdot, _, gdot = plan.hvp_blocks({i: host(t) for i, t in tangents.items()}, host(seed),
+                                           None if seed_tangent is None else host(seed_tangent), outputs)
+        out = []
+        for dt in (rdot, gdot):
+            out.append(None if dt is None else torch.from_numpy(dt.to_numpy()).to(seed.device))
+            if dt is not None:
+                dt.free()
+        g = self._split(out[1])
+        return out[0], tuple(g[i].to(x.device) for i, x in zip(self.wrt, xs))
 
     def _batch_grads_device(self, seed, xs):
         want_rows = any(i in self.batched for i in self.wrt)
@@ -379,6 +516,15 @@ def network_function(tn: Tensor, path: ContractionPath, wrt: Sequence[int], ctx:
     batched inputs are [B, *leaf shape], those of shared inputs [*leaf shape] and the same for every instance; the
     instances run in one NetworkPlan.jvp_batch pass.  Tangents of inputs not in `wrt` are ignored, as their gradients are
     None.  sliced_legs with forward mode raises NotImplementedError.
+
+    Second order (unbatched and unsliced, on_device False or True): the backward computes G = vjp(conj(grad_out)) through
+    a holomorphic autograd.Function of (conj(grad_out), inputs), so with create_graph=True the gradients have a graph
+    back to the inputs and to grad_out.  Differentiating them again (a second torch.autograd.grad,
+    torch.autograd.functional.hvp / hessian, torch.func.jvp of torch.func.grad) makes one Hessian-vector pass per
+    call (NetworkPlan.hvp_blocks) on a plan compiled on the first second-order call; it costs about nine forward passes
+    with every input requested.  First-order gradients keep their bits with and without create_graph.  With `batched`
+    or `sliced_legs`, a backward with create_graph=True raises NotImplementedError rather than return gradients
+    without a graph.  torch.func.hessian / jacrev / jacfwd need a vmap rule the function does not have.
 
     on_device=True: the inputs must be torch CUDA tensors on the context's device (else ValueError), and the result and
     the gradients are CUDA tensors there; no payload, result or gradient goes through the host.  The first call stages

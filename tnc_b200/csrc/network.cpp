@@ -371,6 +371,15 @@ struct tncb_plan {
   std::vector<int> sum_first, sum_count;            // per level: first index into sum_items, number of sums
   std::vector<size_t> sum_bs_first;                 // per level: first index into sum_bs
   void* sum_dev = nullptr; size_t sum_dev_bytes = 0;  // device copy of sum_items + sum_bs
+  // Hessian-vector plans (tncb_plan_create_hvp) are gradient and tangent plans at once: S.steps holds the forward,
+  // tangent, backward and backward-tangent pairs; tan_sums holds the sums of both tangent passes.  grad_* gathers the
+  // leaf adjoints (G), dgrad_* their tangents (Ġ), both at grad_offset.
+  bool hvp = false;
+  int seed_tan_slot = -1;                           // Ṡ, written (or zeroed) by tncb_plan_hvp before the backward levels
+  std::vector<tncb::GradItem> dgrad_items;
+  std::vector<long long> dgrad_block_start;
+  std::vector<GradPermute> dgrad_permutes;
+  void* dgrad_dev = nullptr; size_t dgrad_dev_bytes = 0;   // device copy of dgrad_items + dgrad_block_start
 };
 
 namespace tncb {
@@ -408,6 +417,9 @@ static size_t static_ws_limit(size_t device_bytes) {
   return limit;
 }
 
+// what every plan entry point but tncb_plan_stage / set_leaves / hvp / info / grad_offsets answers a Hessian-vector plan
+static int hvp_refused() { return fail(TNCB_ERR_UNSUPPORTED, "a Hessian-vector plan runs through tncb_plan_hvp"); }
+
 static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) {
   Schedule& S = P->S;
   P->is_static = !S.steps.empty() && (P->grad || P->tangent || std::getenv("TNCB_NO_STATIC") == nullptr);
@@ -415,7 +427,8 @@ static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) 
   if (!P->is_static) return;
   // ---- levels: a step's level is 1 + the deepest level among its operands' producers (leaves: 0); backward pairs
   // follow the whole forward pass on their backward level.  A tangent pair reads a tangent of its forward step's operand
-  // (on that operand's level) and the other forward operand, so it lands on its forward step's level ----
+  // (on that operand's level) and the other forward operand, so it lands on its forward step's level; a backward-tangent
+  // pair carries its backward pair's bw_level ----
   std::vector<int> slot_level(S.slots.size(), 0), step_level(S.steps.size(), 0);
   int n_levels = 0;
   for (size_t q = 0; q < S.steps.size(); q++) {
@@ -427,7 +440,11 @@ static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) 
   }
   P->n_fwd_levels = n_levels;
   for (size_t q = 0; q < S.steps.size(); q++)
-    if (S.steps[q].bw_level) { step_level[q] = P->n_fwd_levels + S.steps[q].bw_level; n_levels = std::max(n_levels, step_level[q]); }
+    if (S.steps[q].bw_level) {
+      step_level[q] = P->n_fwd_levels + S.steps[q].bw_level;
+      slot_level[S.steps[q].out] = step_level[q];
+      n_levels = std::max(n_levels, step_level[q]);
+    }
   static const bool no_batch = std::getenv("TNCB_NO_BATCH") != nullptr;
   std::vector<size_t> order(S.steps.size());
   for (size_t q = 0; q < order.size(); q++) order[q] = q;
@@ -462,8 +479,8 @@ static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) 
   std::vector<int> last_read(S.slots.size(), -1);
   for (int l = 0; l < n_levels; l++)
     for (int q = P->level_begin[l]; q < P->level_begin[l + 1]; q++) last_read[S.steps[q].a] = last_read[S.steps[q].b] = l;
-  // a tangent plan: the sums run after their level's pairs and release the second tangent pair's output; the leaf
-  // tangents are written before the first level
+  // a tangent plan: the sums run after the pairs of the level that produced t1 and release the second tangent pair's
+  // output; the leaf tangents are written before the first level
   std::vector<int> sum_level(P->tan_sums.size());
   for (size_t k = 0; k < P->tan_sums.size(); k++) {
     sum_level[k] = slot_level[P->tan_sums[k].t1] - 1;
@@ -477,6 +494,10 @@ static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) 
     if (P->grad && l == P->n_fwd_levels) {         // the seed, written by tncb_plan_vjp before the backward levels
       sz[P->seed_slot] = std::max<size_t>(S.slots[P->seed_slot].elems * sizeof(double2), 16);
       P->slot_off[P->seed_slot] = A.alloc(sz[P->seed_slot]);
+      if (P->seed_tan_slot >= 0) {                 // a Hessian-vector plan's seed tangent, written with the seed
+        sz[P->seed_tan_slot] = sz[P->seed_slot];
+        P->slot_off[P->seed_tan_slot] = A.alloc(sz[P->seed_tan_slot]);
+      }
     }
     for (int q = P->level_begin[l]; q < P->level_begin[l + 1]; q++) {
       const Step& st = S.steps[q];
@@ -580,6 +601,14 @@ static int plan_device_state(tncb_ctx* ctx, tncb_plan* P, bool workspace = true)
     P->grad_dev_bytes = ib + bb;
     TNCB_CUDA(cudaMemcpyAsync(P->grad_dev, P->grad_items.data(), ib, cudaMemcpyHostToDevice, ctx->stream));
     TNCB_CUDA(cudaMemcpyAsync((char*)P->grad_dev + ib, P->grad_block_start.data(), bb, cudaMemcpyHostToDevice, ctx->stream));
+    TNCB_CUDA(cudaStreamSynchronize(ctx->stream));
+  }
+  if (!P->dgrad_dev && !P->dgrad_items.empty()) {
+    const size_t ib = P->dgrad_items.size() * sizeof(GradItem), bb = P->dgrad_block_start.size() * sizeof(long long);
+    if ((rc = ctx->arena.alloc(ib + bb, &P->dgrad_dev))) return rc;
+    P->dgrad_dev_bytes = ib + bb;
+    TNCB_CUDA(cudaMemcpyAsync(P->dgrad_dev, P->dgrad_items.data(), ib, cudaMemcpyHostToDevice, ctx->stream));
+    TNCB_CUDA(cudaMemcpyAsync((char*)P->dgrad_dev + ib, P->dgrad_block_start.data(), bb, cudaMemcpyHostToDevice, ctx->stream));
     TNCB_CUDA(cudaStreamSynchronize(ctx->stream));
   }
   if (!P->sum_dev && !P->sum_items.empty()) {
@@ -720,8 +749,8 @@ static int execute_static(tncb_ctx* ctx, tncb_plan* P, const tncb_tn* tn, tncb_t
 // pair's M·N·K volume, planned like any other pair.  An operand gets its pair only if its subtree holds a requested
 // leaf.  build() consumes every slot exactly once, so the contraction is a tree, every adjoint is produced exactly once
 // and nothing is accumulated.  leaf_adj[l] = the slot holding leaf l's adjoint (in its pair's output leg order), -1 if
-// not requested.
-static int build_backward(tncb_plan* P, const uint8_t* wrt, std::vector<int>& leaf_adj) {
+// not requested.  The forward steps are S.steps[0, n_fwd): a Hessian-vector plan has appended its tangent pairs after them.
+static int build_backward(tncb_plan* P, const uint8_t* wrt, std::vector<int>& leaf_adj, size_t n_fwd) {
   Schedule& S = P->S;
   const size_t nl = S.n_leaves_total;
   if (S.steps.empty() || S.result_slot < 0) return fail(TNCB_ERR_UNSUPPORTED, "a gradient plan needs a network with at least one pair");
@@ -735,7 +764,6 @@ static int build_backward(tncb_plan* P, const uint8_t* wrt, std::vector<int>& le
     want[leaf_slot[li]] = 1; any = true;
   }
   if (!any) return fail(TNCB_ERR_INVALID, "wrt selects no leaf");
-  const size_t n_fwd = S.steps.size();
   std::vector<int> consumer(S.slots.size(), -1);
   for (size_t q = 0; q < n_fwd; q++) {
     const Step& st = S.steps[q];
@@ -788,7 +816,9 @@ static int build_backward(tncb_plan* P, const uint8_t* wrt, std::vector<int>& le
 
 // The gather items of the leaf adjoints (after the layout fixed their slots): fused leg groups in the leaf's order with
 // the adjoint slot's strides.  A leaf that needs more groups than a GradItem holds goes through launch_permute (K3).
-static int build_gather(tncb_plan* P, const std::vector<int>& leaf_adj) {
+// items / block_start / permutes: the plan's grad_* set, or a Hessian-vector plan's dgrad_* set for the adjoints' tangents.
+static int build_gather(tncb_plan* P, const std::vector<int>& leaf_adj, std::vector<GradItem>& items,
+                        std::vector<long long>& block_start, std::vector<tncb_plan::GradPermute>& permutes) {
   const Schedule& S = P->S;
   long long blocks = 0;
   for (const SlotMeta& leaf : S.slots) {
@@ -810,13 +840,13 @@ static int build_gather(tncb_plan* P, const std::vector<int>& leaf_adj) {
       if (it.n == kGradGroups) { fits = false; break; }
       it.dim[it.n] = d; it.st[it.n] = st; it.n++;
     }
-    if (!fits) { P->grad_permutes.push_back({gs, it.dst, perm}); continue; }
+    if (!fits) { permutes.push_back({gs, it.dst, perm}); continue; }
     for (int k = it.n; k < kGradGroups; k++) { it.dim[k] = 1; it.st[k] = 0; }
-    P->grad_items.push_back(it);
-    P->grad_block_start.push_back(blocks);
+    items.push_back(it);
+    block_start.push_back(blocks);
     blocks += (it.elems + kGradThreads - 1) / kGradThreads;
   }
-  P->grad_block_start.push_back(blocks);
+  block_start.push_back(blocks);
   if (blocks > 0x7fffffffLL) return fail(TNCB_ERR_UNSUPPORTED, "leaf gradients too large for one gather launch");
   return TNCB_OK;
 }
@@ -826,8 +856,9 @@ static int build_gather(tncb_plan* P, const std::vector<int>& leaf_adj) {
 // forward step's PairPlan unchanged.  A slot has a tangent only if its subtree holds a requested leaf; a step with one
 // such operand gets one tangent pair, a step with two gets two and a sum (t1 += t2, always in that order).  The requested
 // leaves' tangents get slots of their own (written from the caller's tangent row before the first level), packed in a
-// row at grad_offset like a gradient plan's gradients.
-static int build_tangent(tncb_plan* P, const uint8_t* wrt) {
+// row at grad_offset like a gradient plan's gradients.  tan_of (optional): the tangent slot of every forward slot, -1 =
+// zero tangent.
+static int build_tangent(tncb_plan* P, const uint8_t* wrt, std::vector<int>* tan_of = nullptr) {
   Schedule& S = P->S;
   const size_t nl = S.n_leaves_total;
   if (S.steps.empty() || S.result_slot < 0) return fail(TNCB_ERR_UNSUPPORTED, "a tangent plan needs a network with at least one pair");
@@ -875,6 +906,50 @@ static int build_tangent(tncb_plan* P, const uint8_t* wrt) {
   }
   P->tan_result = tan[S.result_slot];
   if (P->tan_result < 0) return fail(TNCB_ERR_INVALID, "no requested leaf reaches the result");
+  if (tan_of) tan_of->swap(tan);
+  return TNCB_OK;
+}
+
+// Appends the backward-tangent pairs of a Hessian-vector plan: the forward derivative of every backward pair
+// x̄ = contract(C̄, O) (S.steps[b0, end), appended by build_backward) in the direction of the leaf tangents and the seed
+// tangent, dx̄ = contract(dC̄, O) + contract(C̄, dO).  Each term has the backward pair's legs and GEMM view, so it takes
+// the backward pair's PairPlan and bw_level; with both terms a sum follows (first term += second term, in that order).
+// The seed tangent always has a slot, so every adjoint gets a tangent.  tan: the forward slots' tangents
+// (build_tangent); leaf_dadj[l] = the slot holding the tangent of leaf l's adjoint, -1 if not requested.
+static int build_backward_tangent(tncb_plan* P, size_t b0, const std::vector<int>& tan, const std::vector<int>& leaf_adj,
+                                  std::vector<int>& leaf_dadj) {
+  Schedule& S = P->S;
+  {
+    const SlotMeta& seed = S.slots[P->seed_slot];
+    SlotMeta m; m.legs = seed.legs; m.dims = seed.dims; m.elems = seed.elems;
+    S.slots.push_back(std::move(m));
+    P->seed_tan_slot = (int)S.slots.size() - 1;
+  }
+  std::vector<int> dadj(S.slots.size(), -1);        // the tangent slot of an adjoint slot
+  dadj[P->seed_slot] = P->seed_tan_slot;
+  const size_t b1 = S.steps.size();
+  for (size_t q = b0; q < b1; q++) {               // a consumer's adjoint is produced before its operands' adjoints
+    const Step bs = S.steps[q];                    // (a copy: push_back below may move the steps)
+    int first = -1;
+    for (int side = 0; side < 2; side++) {
+      const int a = side == 0 ? dadj[bs.a] : bs.a;
+      const int b = side == 0 ? bs.b : (bs.b < (int)tan.size() ? tan[bs.b] : -1);
+      if (a < 0 || b < 0) continue;
+      Step ts; ts.a = a; ts.b = b; ts.plan = bs.plan; ts.bw_level = bs.bw_level;
+      const SlotMeta& o = S.slots[bs.out];
+      SlotMeta m; m.legs = o.legs; m.dims = o.dims; m.elems = o.elems;
+      S.slots.push_back(std::move(m));
+      ts.out = (int)S.slots.size() - 1;
+      S.flops += ts.plan.flops(); S.bytes += ts.plan.bytes();
+      S.steps.push_back(std::move(ts));
+      if (first < 0) first = S.steps.back().out;
+      else P->tan_sums.push_back({first, S.steps.back().out});
+    }
+    dadj[bs.out] = first;
+  }
+  leaf_dadj.assign(leaf_adj.size(), -1);
+  for (size_t li = 0; li < leaf_adj.size(); li++)
+    if (leaf_adj[li] >= 0) leaf_dadj[li] = dadj[leaf_adj[li]];
   return TNCB_OK;
 }
 
@@ -1294,7 +1369,7 @@ int tncb_plan_create_vjp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path
   p->grad = true;
   std::vector<int> leaf_adj;
   int rc = tncb::build_schedule(tn, path, p->S);
-  if (!rc) rc = tncb::build_backward(p, wrt, leaf_adj);
+  if (!rc) rc = tncb::build_backward(p, wrt, leaf_adj, p->S.steps.size());
   if (rc) { delete p; return rc; }
   size_t dev_free = 0, dev_total = 0;
   if (ctx) { cudaSetDevice(ctx->device); if (cudaMemGetInfo(&dev_free, &dev_total) != cudaSuccess) { dev_total = 0; cudaGetLastError(); } }
@@ -1305,7 +1380,7 @@ int tncb_plan_create_vjp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path
     return tncb::fail(TNCB_ERR_UNSUPPORTED, "the gradient workspace needs " + std::to_string(need) + " bytes, above the static-workspace limit of " +
                                            std::to_string(limit) + " bytes (TNCB_PLAN_WS_GB)");
   }
-  if ((rc = tncb::build_gather(p, leaf_adj))) { delete p; return rc; }
+  if ((rc = tncb::build_gather(p, leaf_adj, p->grad_items, p->grad_block_start, p->grad_permutes))) { delete p; return rc; }
   *out = p;
   return TNCB_OK;
 }
@@ -1347,7 +1422,7 @@ int tncb_plan_create_vjp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_pat
   p->n_sl = n_sl;
   std::vector<int> leaf_adj;
   int rc = build_schedule(&st, path, p->S);
-  if (!rc) rc = build_backward(p, wrt, leaf_adj);
+  if (!rc) rc = build_backward(p, wrt, leaf_adj, p->S.steps.size());
   if (rc) { delete p; return rc; }
   size_t dev_free = 0, dev_total = 0;
   if (ctx) { cudaSetDevice(ctx->device); if (cudaMemGetInfo(&dev_free, &dev_total) != cudaSuccess) { dev_total = 0; cudaGetLastError(); } }
@@ -1376,6 +1451,7 @@ int tncb_plan_vjp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* seed, tncb_
   using namespace tncb;
   if (!ctx || !plan || !grads) return fail(TNCB_ERR_INVALID, "null argument");
   if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_vjp_sliced");
+  if (plan->hvp) return hvp_refused();
   if (plan->tangent) return fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp");
   if (!plan->grad) return fail(TNCB_ERR_INVALID, "not a gradient plan (tncb_plan_create_vjp)");
   if (plan->ctx != ctx || !plan->fwd_ready)
@@ -1421,6 +1497,7 @@ int tncb_plan_vjp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t st
                          tncb_tensor** value, tncb_tensor** grads) {
   using namespace tncb;
   if (!ctx || !plan || !value || !grads || stride == 0) return fail(TNCB_ERR_INVALID, "bad argument");
+  if (plan->hvp) return hvp_refused();
   if (plan->tangent) return fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp");
   if (!plan->sliced) return fail(TNCB_ERR_INVALID, "not a sliced gradient plan (tncb_plan_create_vjp_sliced)");
   if (plan->ctx != ctx || !plan->full_staged) return fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this context");
@@ -1450,6 +1527,7 @@ int tncb_plan_vjp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t st
 int tncb_plan_execute(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tn, tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   if (!ctx || !plan || !tn) return tncb::fail(TNCB_ERR_INVALID, "null argument");
   if (plan->sliced) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_run_slices / tncb_plan_vjp_sliced");
+  if (plan->hvp) return tncb::hvp_refused();
   if (plan->tangent) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp");
   if (plan->grad) return tncb::execute_static(ctx, plan, tn, out, n_out, out_legs);   // forward levels only, no fallback
   static const bool trace = std::getenv("TNCB_TRACE") != nullptr;   // per-step times come from the pair-by-pair executor
@@ -1520,6 +1598,7 @@ int tncb_plan_stage(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tn) {
 int tncb_plan_run(tncb_ctx* ctx, tncb_plan* plan, tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   if (!ctx || !plan) return tncb::fail(TNCB_ERR_INVALID, "null argument");
   if (plan->sliced) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_run_slices / tncb_plan_vjp_sliced");
+  if (plan->hvp) return tncb::hvp_refused();
   if (plan->tangent) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp");
   static const bool trace = std::getenv("TNCB_TRACE") != nullptr;
   if (plan->is_static && plan->leaves_resident && plan->ctx == ctx) {
@@ -1537,6 +1616,7 @@ int tncb_plan_run(tncb_ctx* ctx, tncb_plan* plan, tncb_tensor** out, int* n_out,
 int tncb_plan_stage_slices(tncb_ctx* ctx, tncb_plan* plan, size_t n_slices, const tncb_tn* const* slice_tns) {
   if (!ctx || !plan || !slice_tns || n_slices == 0) return tncb::fail(TNCB_ERR_INVALID, "null argument");
   if (plan->sliced) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan stages its full network once (tncb_plan_stage)");
+  if (plan->hvp) return tncb::hvp_refused();
   if (plan->grad) return tncb::fail(TNCB_ERR_UNSUPPORTED, "gradient plans run one staged network at a time");
   if (plan->tangent) return tncb::fail(TNCB_ERR_UNSUPPORTED, "tangent plans stage many networks with tncb_plan_stage_batch");
   if (!plan->is_static) return tncb::fail(TNCB_ERR_UNSUPPORTED, "sliced execution needs a plan with a static layout (no device leaves)");
@@ -1545,6 +1625,7 @@ int tncb_plan_stage_slices(tncb_ctx* ctx, tncb_plan* plan, size_t n_slices, cons
 
 int tncb_plan_run_slices(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t stride, tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   if (!ctx || !plan || stride == 0) return tncb::fail(TNCB_ERR_INVALID, "bad argument");
+  if (plan->hvp) return tncb::hvp_refused();
   if (plan->tangent) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp / tncb_plan_jvp_batch");
   if (plan->sliced) {         // forward levels only, slices extracted on the device from the staged full leaves
     if (plan->ctx != ctx || !plan->full_staged) return tncb::fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this context");
@@ -1599,6 +1680,7 @@ int tncb_plan_run_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
   using namespace tncb;
   if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
   if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_run_slices / tncb_plan_vjp_sliced");
+  if (plan->hvp) return hvp_refused();
   if (plan->grad) return fail(TNCB_ERR_UNSUPPORTED, "gradient plans run one staged network at a time");
   if (plan->tangent) return fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp_batch");
   if (!plan->is_static) return fail(TNCB_ERR_UNSUPPORTED, "batched execution needs a plan with a static layout (no device leaves)");
@@ -1646,6 +1728,7 @@ int tncb_plan_stage_batch(tncb_ctx* ctx, tncb_plan* plan, size_t n, const tncb_t
   using namespace tncb;
   if (!ctx || !plan || !tns || n == 0) return fail(TNCB_ERR_INVALID, "null argument");
   if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan has no batched gradients");
+  if (plan->hvp) return hvp_refused();
   if (!plan->grad && !plan->tangent)
     return fail(TNCB_ERR_INVALID, "not a gradient or tangent plan (plain plans stage many networks with tncb_plan_stage_slices)");
   return stage_networks(ctx, plan, n, tns, false);
@@ -1660,6 +1743,7 @@ int tncb_plan_vjp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
   using namespace tncb;
   if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
   if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan has no batched gradients");
+  if (plan->hvp) return hvp_refused();
   if (plan->tangent) return fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp_batch");
   if (!plan->grad) return fail(TNCB_ERR_INVALID, "not a gradient plan (tncb_plan_create_vjp)");
   if (!plan->slices_dev || plan->ctx != ctx) return fail(TNCB_ERR_INVALID, "tncb_plan_stage_batch has not been called on this context");
@@ -1825,6 +1909,7 @@ static int stage_tangents(tncb_ctx* ctx, const tncb_plan* P, const double2* tang
 int tncb_plan_jvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, tncb_tensor** value, tncb_tensor** tangent_out) {
   using namespace tncb;
   if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
+  if (plan->hvp) return hvp_refused();
   int rc = jvp_args(plan, tangents, value || tangent_out, {plan->grad_elems});
   if (rc) return rc;
   if (plan->ctx != ctx || !plan->leaves_resident) return fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this plan and context");
@@ -1860,6 +1945,7 @@ int tncb_plan_jvp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
                         tncb_tensor** values, tncb_tensor** tangent_rows) {
   using namespace tncb;
   if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
+  if (plan->hvp) return hvp_refused();
   if (!plan->tangent) return fail(TNCB_ERR_INVALID, "not a tangent plan (tncb_plan_create_jvp)");
   if (!plan->slices_dev || plan->ctx != ctx)
     return fail(TNCB_ERR_INVALID, "tncb_plan_stage_batch / tncb_plan_stage_instances has not been called on this context");
@@ -1907,6 +1993,128 @@ int tncb_plan_jvp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
   return TNCB_OK;
 }
 
+// A Hessian-vector plan: the forward schedule, the tangent pairs (build_tangent), the backward pairs (build_backward) and
+// the backward-tangent pairs of the `wrt` leaves, plus the gathers of G and Ġ, in one static layout.  There is no
+// pair-by-pair fallback: a layout above the static-workspace limit is refused here.
+int tncb_plan_create_hvp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, const uint8_t* wrt, tncb_plan** out) {
+  using namespace tncb;
+  if (!tn || !out) return fail(TNCB_ERR_INVALID, "null argument");
+  {
+    std::vector<const tncb_tn*> lv;
+    collect_leaf_nodes(tn, lv);
+    for (const tncb_tn* l : lv)
+      if (l->kind == TNCB_DATA_DEVICE) return fail(TNCB_ERR_UNSUPPORTED, "Hessian-vector plans do not take device leaves (they are consumed per call)");
+  }
+  tncb_plan* p = new tncb_plan();
+  p->hvp = p->grad = p->tangent = true;
+  std::vector<int> tan, leaf_adj, leaf_dadj;
+  int rc = build_schedule(tn, path, p->S);
+  size_t n_fwd = 0, b0 = 0;
+  if (!rc) { n_fwd = p->S.steps.size(); rc = build_tangent(p, wrt, &tan); }
+  if (!rc) { b0 = p->S.steps.size(); rc = build_backward(p, wrt, leaf_adj, n_fwd); }
+  if (!rc) rc = build_backward_tangent(p, b0, tan, leaf_adj, leaf_dadj);
+  if (rc) { delete p; return rc; }
+  size_t dev_free = 0, dev_total = 0;
+  if (ctx) { cudaSetDevice(ctx->device); if (cudaMemGetInfo(&dev_free, &dev_total) != cudaSuccess) { dev_total = 0; cudaGetLastError(); } }
+  plan_static_layout(p, ctx ? ctx->sm_count : 132, dev_total);
+  if (!p->is_static) {
+    const size_t need = p->ws_bytes, limit = static_ws_limit(dev_total);
+    delete p;
+    return fail(TNCB_ERR_UNSUPPORTED, "the Hessian-vector workspace needs " + std::to_string(need) + " bytes, above the static-workspace limit of " +
+                                      std::to_string(limit) + " bytes (TNCB_PLAN_WS_GB)");
+  }
+  if ((rc = build_gather(p, leaf_adj, p->grad_items, p->grad_block_start, p->grad_permutes)) ||
+      (rc = build_gather(p, leaf_dadj, p->dgrad_items, p->dgrad_block_start, p->dgrad_permutes))) { delete p; return rc; }
+  *out = p;
+  return TNCB_OK;
+}
+
+namespace tncb {
+// a seed or seed tangent: the result's dims, with storage
+static int seed_args(const SlotMeta& rm, const tncb_tensor* t, const char* what) {
+  bool same = t->rank == (int)rm.dims.size();
+  for (int i = 0; same && i < t->rank; i++) same = t->dims[i] == rm.dims[i];
+  if (!same) return fail(TNCB_ERR_SHAPE, std::string("the ") + what + "'s dims differ from the result's");
+  if (!t->ptr) return fail(TNCB_ERR_UNCONTRACTED, std::string("the ") + what + " tensor has no storage");
+  return TNCB_OK;
+}
+
+// one gather set (grad_* or dgrad_*) from the workspace into the packed block `out`: one grad_gather_kernel launch, K3
+// for the leaves with more fused groups than a GradItem holds
+static int gather_set(tncb_ctx* ctx, const tncb_plan* P, const std::vector<GradItem>& items, const std::vector<long long>& bs,
+                      const std::vector<tncb_plan::GradPermute>& permutes, const void* dev, const char* ws, double2* out) {
+  int rc = TNCB_OK;
+  if (!items.empty())
+    rc = launch_grad_gather(ctx, (const GradItem*)dev, (const long long*)((const char*)dev + items.size() * sizeof(GradItem)),
+                            (int)items.size(), bs.back(), ws, out);
+  for (size_t i = 0; i < permutes.size() && !rc; i++) {
+    const auto& gp = permutes[i];
+    const SlotMeta& sm = P->S.slots[gp.slot];
+    rc = launch_permute(ctx, (const double2*)(ws + P->slot_off[gp.slot]), out + gp.dst, (int)sm.dims.size(), sm.dims.data(), gp.perm.data());
+  }
+  return rc;
+}
+} // namespace tncb
+
+// One forward-over-reverse pass on the staged leaves: leaf tangents in, the forward levels (forward pairs, tangent pairs,
+// sums), R and Ṙ out, the seed and its tangent in, the backward levels (backward pairs, backward-tangent pairs, sums),
+// the gathers of G and Ġ.  Nothing is kept between calls, so a call can be repeated and gives the same bits.
+int tncb_plan_hvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, const tncb_tensor* seed,
+                  const tncb_tensor* seed_tangent, tncb_tensor** value, tncb_tensor** tangent_out, tncb_tensor** grads,
+                  tncb_tensor** grad_tangents) {
+  using namespace tncb;
+  if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
+  if (!plan->hvp) return fail(TNCB_ERR_INVALID, "not a Hessian-vector plan (tncb_plan_create_hvp)");
+  int rc = jvp_args(plan, tangents, value || tangent_out || grads || grad_tangents, {plan->grad_elems});
+  if (rc) return rc;
+  const Schedule& S = plan->S;
+  const SlotMeta& rm = S.slots[S.result_slot];
+  if (seed) { if ((rc = seed_args(rm, seed, "seed"))) return rc; }
+  else if (!rm.dims.empty()) return fail(TNCB_ERR_INVALID, "a seed is needed for a result of rank " + std::to_string(rm.dims.size()));
+  if (seed_tangent && (rc = seed_args(rm, seed_tangent, "seed tangent"))) return rc;
+  if (plan->ctx != ctx || !plan->leaves_resident) return fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this plan and context");
+  TNCB_CUDA(cudaSetDevice(ctx->device));
+  const uint64_t ge = plan->grad_elems;
+  tncb_tensor *v = nullptr, *t = nullptr, *g = nullptr, *dg = nullptr;
+  if (value) rc = tensor_new(ctx, (int)rm.dims.size(), rm.dims.data(), &v);
+  if (!rc && tangent_out) rc = tensor_new(ctx, (int)rm.dims.size(), rm.dims.data(), &t);
+  if (!rc && grads) rc = tensor_new(ctx, 1, &ge, &g);
+  if (!rc && grad_tangents) rc = tensor_new(ctx, 1, &ge, &dg);
+  char* ws = (char*)plan->ws;
+  if (!rc) rc = stage_tangents(ctx, plan, tangents->ptr, ge, ws, 0, 1);
+  if (!rc) rc = enqueue_static(ctx, plan, ws, 1, 0, 0, plan->n_fwd_levels);
+  const size_t res_bytes = rm.elems * sizeof(double2);
+  for (auto [dst, slot] : {std::pair<tncb_tensor*, int>{v, S.result_slot}, {t, plan->tan_result}}) {
+    if (rc || !dst || !res_bytes) continue;
+    cudaError_t e = cudaMemcpyAsync(dst->ptr, ws + plan->slot_off[slot], res_bytes, cudaMemcpyDeviceToDevice, ctx->stream);
+    if (e != cudaSuccess) rc = fail(TNCB_ERR_CUDA, std::string("result copy: ") + cudaGetErrorString(e));
+  }
+  // the seed slots may reuse memory the forward levels freed: written after them, on the stream
+  if (!rc) {
+    static const double2 one = {1.0, 0.0};
+    char* s = ws + plan->slot_off[plan->seed_slot];
+    char* ds = ws + plan->slot_off[plan->seed_tan_slot];
+    cudaError_t e = seed ? cudaMemcpyAsync(s, seed->ptr, res_bytes, cudaMemcpyDeviceToDevice, ctx->stream)
+                         : cudaMemcpyAsync(s, &one, sizeof(double2), cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess)
+      e = seed_tangent ? cudaMemcpyAsync(ds, seed_tangent->ptr, res_bytes, cudaMemcpyDeviceToDevice, ctx->stream)
+                       : cudaMemsetAsync(ds, 0, res_bytes, ctx->stream);
+    if (e != cudaSuccess) rc = fail(TNCB_ERR_CUDA, std::string("seed copy: ") + cudaGetErrorString(e));
+  }
+  if (!rc) rc = enqueue_static(ctx, plan, ws, 1, 0, plan->n_fwd_levels, (int)plan->level_batched.size());
+  if (!rc && g) rc = gather_set(ctx, plan, plan->grad_items, plan->grad_block_start, plan->grad_permutes, plan->grad_dev, ws, g->ptr);
+  if (!rc && dg) rc = gather_set(ctx, plan, plan->dgrad_items, plan->dgrad_block_start, plan->dgrad_permutes, plan->dgrad_dev, ws, dg->ptr);
+  if (rc) {
+    for (tncb_tensor* x : {v, t, g, dg}) if (x) tncb_tensor_free(ctx, x);
+    return rc;
+  }
+  if (value) *value = v;
+  if (tangent_out) *tangent_out = t;
+  if (grads) *grads = g;
+  if (grad_tangents) *grad_tangents = dg;
+  return TNCB_OK;
+}
+
 // New payloads for some leaves of the staged network, straight from device memory: one launch on the ctx stream into the
 // leaf block the next run reads (a static plan's workspace block, which its graph replays also read; a non-static plan's
 // resident block; a sliced gradient plan's full block).  The static layout never releases its leaf block, so the new
@@ -1942,6 +2150,7 @@ int tncb_plan_stage_instances(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tmp
   using namespace tncb;
   if (!ctx || !plan || !tmpl || (n && (!leaf_index || !src || !instance_stride))) return fail(TNCB_ERR_INVALID, "null argument");
   if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan takes device payloads through tncb_plan_set_leaves");
+  if (plan->hvp) return hvp_refused();
   const Schedule& S = plan->S;
   for (int k : S.leaf_kind)
     if (k == TNCB_DATA_DEVICE) return fail(TNCB_ERR_UNSUPPORTED, "plans with device leaves cannot be staged (they are consumed per call)");
@@ -2049,11 +2258,12 @@ int tncb_plan_info(const tncb_plan* plan, uint64_t* n_pairs, double* flops, doub
     for (const tncb::Step& st : S.steps) k += st.plan.kernel_class == 1 ? 2 : 1;  // (K1: table build + GEMM)
     for (int nb : plan->level_batched) if (nb) k -= (uint64_t)(nb - 1);            // a batch is one launch
     if (!plan->grad_items.empty()) k++;                                            // the leaf-gradient gather
-    if (!plan->acc_items.empty()) k++;                                             // a slice's gradient accumulation
+    if (!plan->dgrad_items.empty()) k++;                                           // ... and of the gradients' tangents
+    if (!plan->acc_items.empty()) k++;                                            // a slice's gradient accumulation
     if (!plan->sl_items.empty()) k++;                                              // a slice's leaf extraction
     k += (plan->tan_leaves.size() + tncb::kStageItems - 1) / tncb::kStageItems;    // the leaf tangents' staging
     for (int ns : plan->sum_count) if (ns) k++;                                    // a level's tangent sums
-    *n_kernels = k + 2 * plan->grad_permutes.size();                               // (K3: tables + transpose)
+    *n_kernels = k + 2 * (plan->grad_permutes.size() + plan->dgrad_permutes.size());   // (K3: tables + transpose)
   }
   return TNCB_OK;
 }
@@ -2068,6 +2278,7 @@ void tncb_plan_release_device_state(tncb_plan* plan) {
   for (int i = 0; i < 2; i++) if (plan->exec[i]) { cudaGraphExecDestroy(plan->exec[i]); plan->exec[i] = nullptr; }
   if (plan->batch_dev) { ctx->arena.free(plan->batch_dev, plan->batch_bytes); plan->batch_dev = nullptr; }
   if (plan->grad_dev) { ctx->arena.free(plan->grad_dev, plan->grad_dev_bytes); plan->grad_dev = nullptr; }
+  if (plan->dgrad_dev) { ctx->arena.free(plan->dgrad_dev, plan->dgrad_dev_bytes); plan->dgrad_dev = nullptr; }
   if (plan->sum_dev) { ctx->arena.free(plan->sum_dev, plan->sum_dev_bytes); plan->sum_dev = nullptr; }
   if (plan->sl_dev) { ctx->arena.free(plan->sl_dev, plan->sl_dev_bytes); plan->sl_dev = nullptr; }
   if (plan->full_dev) { ctx->arena.free(plan->full_dev, plan->full_bytes); plan->full_dev = nullptr; }

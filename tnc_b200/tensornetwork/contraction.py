@@ -258,6 +258,14 @@ class NetworkPlan:
         return cls._derivative_plan("tncb_plan_create_jvp", tn, contract_path, wrt, ctx)
 
     @classmethod
+    def for_hvp(cls, tn: Tensor, contract_path: ContractionPath, wrt=None, ctx: Optional[Context] = None) -> "NetworkPlan":
+        """A Hessian-vector plan (tncb_plan_create_hvp): after `stage`, `hvp` returns the result, its directional
+        derivative, the gradient of the leaves `wrt` (indices into `leaves(tn)`; None = every leaf with a payload) and
+        that gradient's directional derivative along leaf and seed tangents: Hessian-vector products, in one
+        forward-over-reverse pass."""
+        return cls._derivative_plan("tncb_plan_create_hvp", tn, contract_path, wrt, ctx)
+
+    @classmethod
     def _derivative_plan(cls, create: str, tn: Tensor, contract_path: ContractionPath, wrt, ctx) -> "NetworkPlan":
         self = cls.__new__(cls)
         self.handle = None
@@ -374,6 +382,62 @@ class NetworkPlan:
         out = tan.to_numpy()
         tan.free()
         return res, out
+
+    def _result_input(self, x, what: str):
+        """(DeviceTensor, temporary to free) for an array, a torch CUDA tensor or a DeviceTensor with the result's shape"""
+        if x is None or isinstance(x, DeviceTensor):
+            return x, None
+        if type(x).__module__.split(".")[0] == "torch":
+            if tuple(x.shape) != tuple(self.result_dims):
+                raise ValueError(f"the {what} has shape {tuple(x.shape)}, the result {tuple(self.result_dims)}")
+            t = DeviceTensor.from_torch(self.ctx, x)
+        else:
+            t = DeviceTensor.from_numpy(self.ctx, np.asarray(x, dtype=np.complex128))
+        return t, t
+
+    def hvp_blocks(self, tangents: dict, seed=None, seed_tangent=None, outputs=(True, True, True, True)):
+        """One forward-over-reverse pass on the staged leaves of a Hessian-vector plan (tncb_plan_hvp), left on the
+        device: [value, tangent, grads, grad_tangents] as DeviceTensors, None where `outputs` is False.  value and
+        tangent have the result's shape (R and Ṙ, as jvp_block); grads and grad_tangents are [grad_elems] blocks at
+        grad_offsets() (G = vjp(seed) and Ġ, its derivative along the leaf tangents and the seed tangent).
+        tangents: {leaf index: array or torch CUDA tensor shaped like the leaf}, requested leaves left out have zero
+        tangent; seed / seed_tangent: array, torch CUDA tensor or DeviceTensor with the result's shape, seed None for a
+        scalar result (seed 1), seed_tangent None = zero.  No conjugation anywhere; a call repeats bit for bit."""
+        block = self._tangent_block(tangents)
+        tmp = []
+        try:
+            s, t = self._result_input(seed, "seed")
+            tmp.append(t)
+            ds, t = self._result_input(seed_tangent, "seed tangent")
+            tmp.append(t)
+            outs = [C.c_void_p() if want else None for want in outputs]
+            check(self.ctx._l.tncb_plan_hvp(self.ctx.handle, self.handle, block.handle,
+                                            s.handle if s is not None else None, ds.handle if ds is not None else None,
+                                            *[C.byref(o) if o is not None else None for o in outs]))
+        finally:
+            block.free()
+            for t in tmp:
+                if t is not None:
+                    t.free()
+        return [None if o is None else DeviceTensor.adopt(self.ctx, o) for o in outs]
+
+    def hvp(self, tangents: dict, seed=None, seed_tangent=None):
+        """`hvp_blocks` downloaded: (value, tangent, {leaf: G}, {leaf: Ġ}) as host arrays, value and tangent with the
+        result's shape, G and Ġ shaped like their leaf, for every requested leaf.  Ġ_l = sum_r Ṡ[r] dR[r]/dX_l +
+        sum_r S[r] sum_m d²R[r]/dX_l dX_m · Ẋ_m: with Ṡ = 0 that is the Hessian of sum_r S[r] R[r] times the tangents."""
+        host = []
+        for dt in self.hvp_blocks(tangents, seed, seed_tangent):
+            host.append(dt.to_numpy())
+            dt.free()
+        value, tangent, g, dg = host
+        offs = self.grad_offsets()
+        grads, grad_tangents = {}, {}
+        for i, (off, shape) in enumerate(zip(offs, self.leaf_shapes)):
+            if off >= 0:
+                size = int(np.prod(shape, dtype=np.int64))
+                grads[i] = g[off:off + size].reshape(shape)
+                grad_tangents[i] = dg[off:off + size].reshape(shape)
+        return value, tangent, grads, grad_tangents
 
     def jvp_batch_blocks(self, first: int = 0, count: Optional[int] = None, tangents: Optional[dict] = None,
                          values: bool = True):
