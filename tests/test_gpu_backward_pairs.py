@@ -35,10 +35,10 @@ Measured on an NVIDIA H100 80GB HBM3 at a 700 W power limit: bench.py's 553 dist
 slice's 595 (524 K0, 6 K0 split-K, 16 DMMA, 29 DMMA split-K, 20 K2) in 266 s, 4.5 GiB and 4.0 GiB; the whole gradient block
 in 46 s, with its reference replay on the host.
 
-Not covered here: tangent and Hessian-vector plans add no pair shapes (a tangent pair copies its forward step's PairPlan,
-which the forward tests cover; a backward-tangent pair copies its backward pair's, which section 2 covers), and a
-bench-scale element-wise Hessian-vector check does not fit beside its 36.5 GB workspace.  A whole-gradient reference for a
-Sycamore slice does not fit either: an autograd replay of a slice with 2^27-element intermediates does not."""
+Not covered here: Hessian-vector plans, whose pairs have the shapes of the forward and backward pairs (a tangent pair
+copies its forward step's PairPlan, a backward-tangent pair its backward pair's); test_gpu_hvp_bench.py asserts that and
+checks bench.py's whole Ġ block element by element.  A whole-gradient reference for a Sycamore slice does not fit: an
+autograd replay of a slice with 2^27-element intermediates does not."""
 import ctypes as C
 import functools
 import os
