@@ -9,7 +9,9 @@ network_function(..., sliced_legs=...)):
      value of vjp_sliced to run_slices, and repeated calls to each other;
   3. partial ranges (world = 2, 3) add up to the whole;
   4. bench.py's network with 2 sliced legs under TNCB_PLAN_WS_GB=8 (the unsliced gradient plan is refused there):
-     multilinearity in all 489 leaves, agreement with the unsliced gradient plan, the int8 engine;
+     multilinearity in all 489 leaves, agreement with the unsliced gradient plan, the int8 engine; element by element
+     in per-leaf units at 1, 2 and 3 sliced legs, partial ranges against replays of exactly their slices, and the
+     512-slice Sycamore-53 depth-12 gradient: test_gpu_vjp_sliced_bench.py;
   5. torch: gradcheck through a sliced network_function, gate-angle gradients equal to the unsliced function's;
   6. the error codes, with the arena's live bytes unchanged."""
 import ctypes as C
