@@ -2,6 +2,7 @@
 // (tnc/src/tensornetwork/contraction.rs:226-264, io/qasm/qasm_importer.rs:171-194,
 // builders/circuit_builder.rs:372-396, io/hdf5.rs:196-257).  Needs a GPU; run by tests/test_gpu_cpp_host.py.
 // `test_host_api --io <dir>` runs only the HDF5 tests, which need no GPU (tests/test_gpu_cpp_host.py::test_cpp_hdf5_io).
+// `test_host_api --deriv <dir>` writes the derivative methods' blocks (tests/test_gpu_general_networks.py).
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -178,8 +179,94 @@ static void test_file_leaf(Context& ctx, const std::string& dir) {
   for (int i = 0; i < 6; i++) EXPECT(e[i] == ref[i]);
 }
 
+// The derivative methods of NetworkPlan (ForGradients / vjp, ForTangents / jvp, ForHvp / hvp) on a nested network with
+// mixed extents, a dim-1 leg, a single-leaf composite and a rank-2 result, with a wrt subset.  Payloads, tangents, seed
+// and seed tangent come from small integer formulas (exact in double) that tests/test_gpu_general_networks.py
+// reproduces; every block is written raw to <dir> and compared there bit for bit with the Python plans' results.
+static Complex64 payload_at(size_t l, size_t e) { return {(double((7 * l + 3 * e) % 11) - 5.0) / 4.0, (double((5 * l + 2 * e) % 13) - 6.0) / 8.0}; }
+static Complex64 tangent_at(size_t l, size_t e) { return {(double((3 * l + 5 * e) % 7) - 3.0) / 2.0, (double((l + 4 * e) % 9) - 4.0) / 4.0}; }
+static Complex64 seed_at(size_t r) { return {(double((2 * r) % 5) - 2.0) / 2.0, (double((3 * r) % 7) - 3.0) / 4.0}; }
+static Complex64 seed_tangent_at(size_t r) { return {(double((r + 1) % 3) - 1.0) / 2.0, (double((5 * r) % 4) - 1.5) / 2.0}; }
+
+static Tensor formula_leaf(size_t l, std::vector<uint64_t> legs, std::vector<uint64_t> dims) {
+  size_t n = 1;
+  for (uint64_t d : dims) n *= d;
+  std::vector<Complex64> x(n);
+  for (size_t e = 0; e < n; e++) x[e] = payload_at(l, e);
+  Tensor t(std::move(legs), dims);
+  t.set_tensor_data(TensorData::new_from_data(dims, std::move(x)));
+  return t;
+}
+
+static void write_block(const std::string& path, const std::vector<Complex64>& v) {
+  FILE* f = std::fopen(path.c_str(), "wb");
+  EXPECT(f != nullptr);
+  if (!f) return;
+  EXPECT(std::fwrite(v.data(), sizeof(Complex64), v.size(), f) == v.size());
+  std::fclose(f);
+}
+
+static void test_derivative_methods(Context& ctx, const std::string& dir) {
+  // leaves in depth-first order: L0 (0:3, 1:2, 9:2) L1 (1:2, 2:5, 3:1) | L2 (2:5, 4:3, 5:2) | L3 (4:3, 0:3, 6:2, 3:1) |
+  // L4 (5:2, 7:7) L5 (7:7, 6:2, 8:3); open legs 9 and 8
+  Tensor c0 = Tensor::new_composite({formula_leaf(0, {0, 1, 9}, {3, 2, 2}), formula_leaf(1, {1, 2, 3}, {2, 5, 1})});
+  Tensor c1 = Tensor::new_composite({formula_leaf(2, {2, 4, 5}, {5, 3, 2})});
+  Tensor l3 = formula_leaf(3, {4, 0, 6, 3}, {3, 3, 2, 1});
+  Tensor c3 = Tensor::new_composite({formula_leaf(4, {5, 7}, {2, 7}), formula_leaf(5, {7, 6, 8}, {7, 2, 3})});
+  const Tensor tn = Tensor::new_composite({c0, c1, l3, c3});
+  ContractionPath path = ContractionPath::simple({{0, 1}, {0, 2}, {0, 3}});
+  path.nested[0] = ContractionPath::single(0, 1);
+  path.nested[1] = ContractionPath();
+  path.nested[3] = ContractionPath::single(0, 1);
+  const std::vector<size_t> wrt = {0, 2, 5};
+  const size_t leaf_elems[6] = {12, 10, 30, 18, 14, 42};
+  std::vector<Complex64> seed(6), seed_tangent(6);            // the result's 6 entries
+  for (size_t r = 0; r < 6; r++) { seed[r] = seed_at(r); seed_tangent[r] = seed_tangent_at(r); }
+  std::map<size_t, std::vector<Complex64>> tangents;
+  for (size_t l : wrt) {
+    tangents[l].resize(leaf_elems[l]);
+    for (size_t e = 0; e < leaf_elems[l]; e++) tangents[l][e] = tangent_at(l, e);
+  }
+  {
+    NetworkPlan plan(ctx, tn, path, NetworkPlan::ForGradients{wrt});
+    plan.stage(tn);
+    Tensor r = plan.run();
+    EXPECT((r.bond_dims == std::vector<uint64_t>{3, 2}) || (r.bond_dims == std::vector<uint64_t>{2, 3}));
+    write_block(dir + "/vjp_value.bin", r.elements());
+    auto g = plan.vjp(seed);
+    EXPECT(g.size() == wrt.size());
+    for (auto& [l, v] : g) {
+      EXPECT(v.size() == leaf_elems[l]);
+      write_block(dir + "/vjp_" + std::to_string(l) + ".bin", v);
+    }
+  }
+  {
+    NetworkPlan plan(ctx, tn, path, NetworkPlan::ForTangents{wrt});
+    plan.stage(tn);
+    auto [value, tangent] = plan.jvp(tangents);
+    write_block(dir + "/jvp_value.bin", value);
+    write_block(dir + "/jvp_tangent.bin", tangent);
+  }
+  {
+    NetworkPlan plan(ctx, tn, path, NetworkPlan::ForHvp{wrt});
+    plan.stage(tn);
+    auto h = plan.hvp(tangents, seed, seed_tangent);
+    write_block(dir + "/hvp_value.bin", h.value);
+    write_block(dir + "/hvp_tangent.bin", h.tangent);
+    EXPECT(h.grads.size() == wrt.size() && h.grad_tangents.size() == wrt.size());
+    for (auto& [l, v] : h.grads) write_block(dir + "/hvp_grad_" + std::to_string(l) + ".bin", v);
+    for (auto& [l, v] : h.grad_tangents) write_block(dir + "/hvp_dgrad_" + std::to_string(l) + ".bin", v);
+  }
+}
+
 int main(int argc, char** argv) {
   const std::string dir = argc > 2 ? argv[2] : "/tmp";
+  if (argc > 1 && std::strcmp(argv[1], "--deriv") == 0) {           // ForGradients / ForTangents / ForHvp (GPU)
+    try { Context ctx(0); test_derivative_methods(ctx, dir); } catch (const Error& e) { std::printf("FAIL uncaught tnc::Error %d: %s\n", e.status, e.what()); return 2; }
+    if (failures) { std::printf("%d failure(s)\n", failures); return 1; }
+    std::printf("HOST_DERIV_OK\n");
+    return 0;
+  }
   if (argc > 1 && std::strcmp(argv[1], "--io") == 0) {
     try { test_hdf5_write_read(dir); test_circuit_builder_structure(); } catch (const Error& e) { std::printf("FAIL uncaught tnc::Error %d: %s\n", e.status, e.what()); return 2; }
     if (failures) { std::printf("%d failure(s)\n", failures); return 1; }
