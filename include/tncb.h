@@ -482,6 +482,42 @@ int tncb_plan_create_hvp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path
 int tncb_plan_hvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, const tncb_tensor* seed,
                   const tncb_tensor* seed_tangent, tncb_tensor** value, tncb_tensor** tangent_out, tncb_tensor** grads,
                   tncb_tensor** grad_tangents);
+/* ---- sliced tangents and Hessian-vector products: networks whose tangent or Hessian-vector workspace does not fit ----
+ * By linearity, as for sliced gradients: R = sum_q R_q, so Ṙ = sum_q Ṙ_q; slice q's leaf (and its tangent) is q's
+ * fixed-index sub-block of the full leaf (and of its full-shape tangent), and q's G_l and Ġ_l add into q's sub-block of
+ * the full-shape blocks.  R_q depends on q's sub-blocks only, so there are no cross-slice Hessian terms.
+ * Creation as tncb_plan_create_vjp_sliced (the same sliced-leg checks and messages, ctx may be NULL), with the slice
+ * structure compiled exactly as tncb_plan_create_jvp / tncb_plan_create_hvp compile the host-sliced slice network:
+ * tncb_plan_info covers one slice's pass (with the leaf and tangent extraction and the accumulation launches) and
+ * peak_bytes is the per-slice workspace; a per-slice workspace above the static-workspace limit -> TNCB_ERR_UNSUPPORTED
+ * naming the bytes.  tncb_plan_grad_offsets packs the FULL leaves' shapes, for the tangents, G and Ġ alike.
+ * Use: tncb_plan_stage(ctx, plan, full tn) uploads the full leaves once; tncb_plan_run_slices runs the forward levels
+ * (with zero tangents) and returns a sum bit-identical to the plain sliced run.  Every other entry point (run, execute,
+ * stage_slices, run_batch, stage_batch, stage_instances, set_leaves, vjp, vjp_sliced, vjp_batch, jvp, jvp_batch, hvp)
+ * -> TNCB_ERR_UNSUPPORTED naming the call that runs the plan. */
+int tncb_plan_create_jvp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, size_t n_sliced,
+                                const uint64_t* sliced_legs, const uint8_t* wrt, tncb_plan** out);
+/* Per slice q = first, first+stride, ...: extract q's sub-blocks of the leaves that carry a sliced leg and of every
+ * requested leaf's tangent (one launch each), the forward levels with their tangent pairs, R += and Ṙ +=.  tangents:
+ * [tangent_elems] device tensor, every requested leaf's FULL-shape tangent at tncb_plan_grad_offsets.  *value (the
+ * sum of R_q, bit-identical to tncb_plan_run_slices) and *tangent_out (the sum of Ṙ_q) are new tensors with the result's
+ * dims; either may be NULL, not both.  An empty range (first >= slices) gives zeros; partial ranges add up, for ranks
+ * that all-reduce.  Not a sliced tangent plan, not staged on this context, stride 0, no output, NULL tangents ->
+ * TNCB_ERR_INVALID; tangent dims other than [tangent_elems] -> TNCB_ERR_SHAPE.  Errors leave the arena as they found it. */
+int tncb_plan_jvp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t stride, const tncb_tensor* tangents,
+                         tncb_tensor** value, tncb_tensor** tangent_out);
+int tncb_plan_create_hvp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, size_t n_sliced,
+                                const uint64_t* sliced_legs, const uint8_t* wrt, tncb_plan** out);
+/* As tncb_plan_jvp_sliced, then per slice: the seed (NULL only for a rank-0 result: 1) and the seed tangent (NULL: zero)
+ * written after the forward levels, the backward levels with their tangent pairs, K3 of the adjoints (and adjoint
+ * tangents) that need more than 8 leg groups, and the accumulation of G_l and then Ġ_l into q's sub-blocks of the
+ * full-shape [tangent_elems] blocks *grads and *grad_tangents (zeroed once per call).  The same seed and seed tangent
+ * serve every slice.  Each output may be NULL, not all four; the backward levels run only if *grads or *grad_tangents
+ * is wanted.  Errors as tncb_plan_jvp_sliced, seed errors as tncb_plan_hvp; not a sliced Hessian-vector plan ->
+ * TNCB_ERR_INVALID. */
+int tncb_plan_hvp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t stride, const tncb_tensor* tangents,
+                         const tncb_tensor* seed, const tncb_tensor* seed_tangent, tncb_tensor** value,
+                         tncb_tensor** tangent_out, tncb_tensor** grads, tncb_tensor** grad_tangents);
 void tncb_plan_destroy(tncb_plan* plan);
 
 /* ---- HDF5 tensor files: replaces tnc::io::hdf5 (tnc/src/io/hdf5.rs), which binds libhdf5 through hdf5-metno.

@@ -172,6 +172,24 @@ class SlicedPlan:
         leaf's gradient in the full leaf's shape, each slice extracted and accumulated on the device.  wrt: indices into
         `leaves(tn)`; None = every leaf with a payload.  Slice q is the row-major digit vector of q over `legs`, last leg
         fastest (the order of `slice_assignments`)."""
+        return cls._derivative("tncb_plan_create_vjp_sliced", tn, path, legs, wrt, ctx)
+
+    @classmethod
+    def for_tangents(cls, tn: Tensor, path: ContractionPath, legs: Sequence[int], wrt=None, ctx=None) -> "SlicedPlan":
+        """A sliced tangent plan (tncb_plan_create_jvp_sliced), built like `for_gradients`: after `stage(tn)`, `jvp`
+        returns the sum of the slices' results and of their directional derivatives along full-shape leaf tangents, each
+        slice's tangents extracted on the device.  `run` sums the slices' results."""
+        return cls._derivative("tncb_plan_create_jvp_sliced", tn, path, legs, wrt, ctx)
+
+    @classmethod
+    def for_hvp(cls, tn: Tensor, path: ContractionPath, legs: Sequence[int], wrt=None, ctx=None) -> "SlicedPlan":
+        """A sliced Hessian-vector plan (tncb_plan_create_hvp_sliced), built like `for_gradients`: after `stage(tn)`,
+        `hvp` returns R, Ṙ and every requested leaf's G and Ġ in the full leaf's shape, summed over the slices, each
+        slice's forward-over-reverse pass on the device.  `run` sums the slices' results."""
+        return cls._derivative("tncb_plan_create_hvp_sliced", tn, path, legs, wrt, ctx)
+
+    @classmethod
+    def _derivative(cls, create: str, tn: Tensor, path: ContractionPath, legs: Sequence[int], wrt, ctx) -> "SlicedPlan":
         import ctypes as C
         from .. import default_context
         from .._lib import check, u64_array
@@ -193,9 +211,13 @@ class SlicedPlan:
         c_tn, c_path = m.tn(tn), m.path(path)
         c_legs = u64_array(legs or [0])
         h = C.c_void_p()
-        check(self.ctx._l.tncb_plan_create_vjp_sliced(self.ctx.handle, C.byref(c_tn), C.byref(c_path), len(legs), c_legs, mask, C.byref(h)))
+        check(getattr(self.ctx._l, create)(self.ctx.handle, C.byref(c_tn), C.byref(c_path), len(legs), c_legs, mask, C.byref(h)))
         plan = NetworkPlan.__new__(NetworkPlan)
         plan.ctx, plan.handle, plan.leaf_shapes = self.ctx, h, shapes
+        n_out, out_legs, out_dims = C.c_int(), u64_array([0] * 64), u64_array([0] * 64)
+        check(self.ctx._l.tncb_network_out_legs(C.byref(c_tn), C.byref(c_path), C.byref(n_out), out_legs, out_dims))
+        plan.result_legs = [out_legs[i] for i in range(n_out.value)]
+        plan.result_dims = tuple(int(out_dims[i]) for i in range(n_out.value))
         self.plan = plan
         self._legs = None
         dim = {l: int(d) for t in lv for l, d in zip(t.legs, t.bond_dims)}
@@ -252,6 +274,86 @@ class SlicedPlan:
             check(ctx._l.tncb_comm_allreduce_sum(ctx.handle, value.handle))
             check(ctx._l.tncb_comm_allreduce_sum(ctx.handle, block.handle))
         return value, block
+
+    def _allreduce(self, blocks, world: int, allreduce: bool):
+        from .._lib import check
+        if world > 1 and allreduce:
+            for b in blocks:
+                if b is not None:
+                    check(self.ctx._l.tncb_comm_allreduce_sum(self.ctx.handle, b.handle))
+        return blocks
+
+    def jvp_block(self, tangents: dict, rank: int = 0, world: int = 1, allreduce: bool = True):
+        """A sliced tangent plan's forward-mode pass over the slices rank, rank + world, ... (tncb_plan_jvp_sliced), left on
+        the device: (value, tangent) DeviceTensors with the result's shape.  tangents: {leaf index: array or torch CUDA
+        tensor shaped like the FULL leaf}; requested leaves left out have zero tangent.  value equals `run` bit for bit.
+        With world > 1 and allreduce, both are summed over the ranks."""
+        import ctypes as C
+        from .. import DeviceTensor
+        from .._lib import check
+        block = self.plan._tangent_block(tangents)
+        val, tan = C.c_void_p(), C.c_void_p()
+        try:
+            check(self.ctx._l.tncb_plan_jvp_sliced(self.ctx.handle, self.plan.handle, int(rank), int(world), block.handle,
+                                                   C.byref(val), C.byref(tan)))
+        finally:
+            block.free()
+        return tuple(self._allreduce((DeviceTensor.adopt(self.ctx, val), DeviceTensor.adopt(self.ctx, tan)), world, allreduce))
+
+    def jvp(self, tangents: dict, rank: int = 0, world: int = 1, allreduce: bool = True):
+        """`jvp_block` with the derivative downloaded: (value Tensor on the device with the result's legs, tangent
+        ndarray), tangent[r] = sum_l sum_e dR[r]/dX_l[e] tangents[l][e] over the full leaves (no conjugation)."""
+        from ..tensornetwork.tensordata import TensorData
+        val, tan = self.jvp_block(tangents, rank, world, allreduce)
+        res = Tensor(list(self.plan.result_legs), val.shape)
+        res.set_tensor_data(TensorData.Matrix(val))
+        out = tan.to_numpy()
+        tan.free()
+        return res, out
+
+    def hvp_blocks(self, tangents: dict, seed=None, seed_tangent=None, rank: int = 0, world: int = 1, allreduce: bool = True,
+                   outputs=(True, True, True, True)):
+        """A sliced Hessian-vector plan's forward-over-reverse pass over the slices rank, rank + world, ...
+        (tncb_plan_hvp_sliced), left on the device: [value, tangent, grads, grad_tangents] as DeviceTensors, None where
+        `outputs` is False; grads and grad_tangents are full-shape blocks at grad_offsets().  Arguments as
+        NetworkPlan.hvp_blocks, with tangents shaped like the FULL leaves.  With world > 1 and allreduce, every returned
+        block is summed over the ranks."""
+        import ctypes as C
+        from .. import DeviceTensor
+        from .._lib import check
+        block = self.plan._tangent_block(tangents)
+        tmp = []
+        try:
+            s, t = self.plan._result_input(seed, "seed")
+            tmp.append(t)
+            ds, t = self.plan._result_input(seed_tangent, "seed tangent")
+            tmp.append(t)
+            outs = [C.c_void_p() if want else None for want in outputs]
+            check(self.ctx._l.tncb_plan_hvp_sliced(self.ctx.handle, self.plan.handle, int(rank), int(world), block.handle,
+                                                   s.handle if s is not None else None, ds.handle if ds is not None else None,
+                                                   *[C.byref(o) if o is not None else None for o in outs]))
+        finally:
+            block.free()
+            for t in tmp:
+                if t is not None:
+                    t.free()
+        return self._allreduce([None if o is None else DeviceTensor.adopt(self.ctx, o) for o in outs], world, allreduce)
+
+    def hvp(self, tangents: dict, seed=None, seed_tangent=None, rank: int = 0, world: int = 1, allreduce: bool = True):
+        """`hvp_blocks` downloaded: (value, tangent, {leaf: G}, {leaf: Ġ}) as host arrays, G and Ġ shaped like the full
+        leaf, for every requested leaf (see NetworkPlan.hvp)."""
+        host = []
+        for dt in self.hvp_blocks(tangents, seed, seed_tangent, rank, world, allreduce):
+            host.append(dt.to_numpy())
+            dt.free()
+        value, tangent, g, dg = host
+        grads, grad_tangents = {}, {}
+        for i, (off, shape) in enumerate(zip(self.plan.grad_offsets(), self.plan.leaf_shapes)):
+            if off >= 0:
+                size = int(np.prod(shape, dtype=np.int64))
+                grads[i] = g[off:off + size].reshape(shape)
+                grad_tangents[i] = dg[off:off + size].reshape(shape)
+        return value, tangent, grads, grad_tangents
 
     def set_leaves(self, payloads: dict) -> None:
         """New payloads for leaves of the staged FULL network straight from device memory ({leaf index: torch CUDA tensor

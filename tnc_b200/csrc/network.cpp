@@ -348,9 +348,13 @@ struct tncb_plan {
   tncb::Schedule full;                              // leaves only: kinds, dims, offsets in the full leaf block
   std::vector<tncb::SliceItem> sl_items, const_items, acc_items;   // extract (leaves with / without a sliced leg), accumulate
   std::vector<long long> sl_bs, const_bs, acc_bs;   // their block-count prefixes (n_items + 1 entries each)
+  // sliced tangent / Hessian-vector plans (sliced && tangent): extract of every requested leaf's tangent from the caller's
+  // full-shape tangent block, accumulate of the adjoints' tangents (Ġ)
+  std::vector<tncb::SliceItem> tan_items, dacc_items;
+  std::vector<long long> tan_bs, dacc_bs;
   size_t acc_scratch_elems = 0;                     // permute scratch of the leaves that take K3 before the accumulate
   void* sl_dev = nullptr; size_t sl_dev_bytes = 0;  // device copy of the items + prefixes, the seed 1, the permute scratch
-  size_t sl_off[7] = {};                            // byte offsets inside sl_dev: 3 item arrays, 3 prefixes, seed 1 (+ scratch)
+  size_t sl_off[11] = {};                           // byte offsets inside sl_dev: 5 item arrays, 5 prefixes, seed 1 (+ scratch)
   void* full_dev = nullptr; size_t full_bytes = 0;  // the staged full leaf block (outside the workspace)
   bool full_staged = false;
   // tncb_plan_stage_instances: the template's leaves that take no device payload, packed, in plan-owned pinned memory
@@ -419,6 +423,17 @@ static size_t static_ws_limit(size_t device_bytes) {
 
 // what every plan entry point but tncb_plan_stage / set_leaves / hvp / info / grad_offsets answers a Hessian-vector plan
 static int hvp_refused() { return fail(TNCB_ERR_UNSUPPORTED, "a Hessian-vector plan runs through tncb_plan_hvp"); }
+
+// a sliced tangent / Hessian-vector plan (tncb_plan_create_jvp_sliced / _hvp_sliced) runs through its own call only
+static bool sliced_tangent(const tncb_plan* P) { return P->sliced && P->tangent; }
+static int sliced_tangent_refused(const tncb_plan* P) {
+  return fail(TNCB_ERR_UNSUPPORTED, P->hvp ? "a sliced Hessian-vector plan runs through tncb_plan_hvp_sliced / tncb_plan_run_slices"
+                                           : "a sliced tangent plan runs through tncb_plan_jvp_sliced / tncb_plan_run_slices");
+}
+
+// the item sets of a sliced plan, in their sl_dev order: extract of the leaves with / without a sliced leg, accumulate of
+// the adjoints, extract of the leaf tangents, accumulate of the adjoints' tangents
+enum { kSlExtract, kSlConst, kSlAcc, kSlTan, kSlDacc, kSliceSets };
 
 static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) {
   Schedule& S = P->S;
@@ -621,19 +636,19 @@ static int plan_device_state(tncb_ctx* ctx, tncb_plan* P, bool workspace = true)
   }
   if (P->sliced && !P->sl_dev) {
     auto up16 = [](size_t b) { return (b + 15) / 16 * 16; };
-    const std::vector<SliceItem>* iv[3] = {&P->sl_items, &P->const_items, &P->acc_items};
-    const std::vector<long long>* bv[3] = {&P->sl_bs, &P->const_bs, &P->acc_bs};
+    const std::vector<SliceItem>* iv[kSliceSets] = {&P->sl_items, &P->const_items, &P->acc_items, &P->tan_items, &P->dacc_items};
+    const std::vector<long long>* bv[kSliceSets] = {&P->sl_bs, &P->const_bs, &P->acc_bs, &P->tan_bs, &P->dacc_bs};
     size_t off = 0;
-    for (int i = 0; i < 3; i++) { P->sl_off[i] = off; off = up16(off + iv[i]->size() * sizeof(SliceItem)); }
-    for (int i = 0; i < 3; i++) { P->sl_off[3 + i] = off; off = up16(off + bv[i]->size() * sizeof(long long)); }
-    P->sl_off[6] = off; off += sizeof(double2);
+    for (int i = 0; i < kSliceSets; i++) { P->sl_off[i] = off; off = up16(off + iv[i]->size() * sizeof(SliceItem)); }
+    for (int i = 0; i < kSliceSets; i++) { P->sl_off[kSliceSets + i] = off; off = up16(off + bv[i]->size() * sizeof(long long)); }
+    P->sl_off[2 * kSliceSets] = off; off += sizeof(double2);
     std::vector<char> host(off, 0);
-    for (int i = 0; i < 3; i++) {
+    for (int i = 0; i < kSliceSets; i++) {
       if (!iv[i]->empty()) std::memcpy(host.data() + P->sl_off[i], iv[i]->data(), iv[i]->size() * sizeof(SliceItem));
-      if (!bv[i]->empty()) std::memcpy(host.data() + P->sl_off[3 + i], bv[i]->data(), bv[i]->size() * sizeof(long long));
+      if (!bv[i]->empty()) std::memcpy(host.data() + P->sl_off[kSliceSets + i], bv[i]->data(), bv[i]->size() * sizeof(long long));
     }
     const double2 one = {1.0, 0.0};
-    std::memcpy(host.data() + P->sl_off[6], &one, sizeof(one));
+    std::memcpy(host.data() + P->sl_off[2 * kSliceSets], &one, sizeof(one));
     const size_t bytes = off + P->acc_scratch_elems * sizeof(double2);
     if ((rc = ctx->arena.alloc(bytes, &P->sl_dev))) return rc;
     P->sl_dev_bytes = bytes;
@@ -1005,14 +1020,23 @@ static void push_item(std::vector<SliceItem>& items, std::vector<long long>& bs,
 
 // The full leaves (P->full), the gradient offsets in full-leaf shapes, the extract items (after the layout fixed the leaf
 // slots) and the accumulate items of the leaf adjoints.  An accumulate item whose adjoint order needs more groups than an
-// item holds reads a K3-permuted copy of the adjoint (slice-leaf order) from the plan's permute scratch instead.
+// item holds reads a K3-permuted copy of the adjoint (slice-leaf order) from the plan's permute scratch instead.  A
+// tangent plan (leaf_adj empty) also gets the extract items of the requested leaves' tangents (full-shape tangent block
+// at the gradient offsets -> the tangent slots); a Hessian-vector plan also gets the accumulate items of the adjoints'
+// tangents (leaf_dadj), their K3 copies after the adjoints' in the same scratch.
 static int build_slice_items(tncb_plan* P, const std::vector<const tncb_tn*>& lv, const std::vector<uint64_t>& sl,
-                             const std::vector<uint64_t>& sdim, const std::vector<int>& leaf_adj) {
+                             const std::vector<uint64_t>& sdim, const std::vector<int>& leaf_adj,
+                             const std::vector<int>& leaf_dadj = {}) {
   const Schedule& S = P->S;
   Schedule& F = P->full;
   const size_t nl = S.n_leaves_total;
-  std::vector<int> sslot(nl, -1), fslot(nl, -1);
+  std::vector<int> sslot(nl, -1), fslot(nl, -1), leaf_tan(nl, -1);
   for (size_t s = 0; s < S.slots.size(); s++) if (S.slots[s].leaf_index >= 0) sslot[S.slots[s].leaf_index] = (int)s;
+  if (P->tangent) {                                // build_tangent: tan_leaves in leaf order, one per offset >= 0
+    size_t k = 0;
+    for (size_t li = 0; li < nl; li++) if (P->grad_offset[li] >= 0) leaf_tan[li] = P->tan_leaves[k++].slot;
+  }
+  auto wanted = [&](size_t li) { return leaf_adj.empty() ? leaf_tan[li] >= 0 : leaf_adj[li] >= 0; };
   F.n_leaves_total = nl;
   F.leaf_offset.assign(nl, 0);
   F.leaf_kind.assign(nl, TNCB_DATA_UNCONTRACTED);
@@ -1027,7 +1051,7 @@ static int build_slice_items(tncb_plan* P, const std::vector<const tncb_tn*>& lv
   P->grad_offset.assign(nl, -1);
   P->grad_elems = 0;
   for (size_t li = 0; li < nl; li++)
-    if (leaf_adj[li] >= 0) { P->grad_offset[li] = (int64_t)P->grad_elems; P->grad_elems += F.slots[fslot[li]].elems; }
+    if (wanted(li)) { P->grad_offset[li] = (int64_t)P->grad_elems; P->grad_elems += F.slots[fslot[li]].elems; }
   size_t scratch = 0;
   for (size_t li = 0; li < nl; li++) {
     if (sslot[li] < 0) continue;
@@ -1054,31 +1078,42 @@ static int build_slice_items(tncb_plan* P, const std::vector<const tncb_tn*>& lv
     if (!fuse_slice_groups(ex, d, rm, fst))
       return fail(TNCB_ERR_UNSUPPORTED, "leaf " + std::to_string(li) + " needs more than " + std::to_string(kSliceGroups) + " leg groups to address its slices");
     if (ex.ns) push_item(P->sl_items, P->sl_bs, ex); else push_item(P->const_items, P->const_bs, ex);
-    if (leaf_adj[li] < 0) continue;
-    // accumulate: the adjoint slot (pair output order) -> q's sub-block of the full-shape gradient
-    const int gs = leaf_adj[li];
-    const SlotMeta& g = S.slots[gs];
-    std::vector<long long> gst(g.legs.size());
-    { long long s = 1; for (size_t j = g.legs.size(); j-- > 0;) { gst[j] = s; s *= (long long)g.dims[j]; } }
-    std::vector<int> perm(sm.legs.size());
-    std::vector<long long> ast(sm.legs.size());
-    for (size_t i = 0; i < sm.legs.size(); i++) {
-      perm[i] = (int)(std::find(g.legs.begin(), g.legs.end(), sm.legs[i]) - g.legs.begin());
-      ast[i] = gst[perm[i]];
+    if (!wanted(li)) continue;
+    if (leaf_tan[li] >= 0) {                         // the leaf's tangent: caller's full-shape block -> its tangent slot
+      SliceItem tx = ex;
+      tx.slot = (long long)P->slot_off[leaf_tan[li]]; tx.full = (long long)P->grad_offset[li];
+      push_item(P->tan_items, P->tan_bs, tx);
     }
-    SliceItem ac = it;
-    ac.full = (long long)P->grad_offset[li];
-    ac.slot = (long long)P->slot_off[gs];
-    if (!fuse_slice_groups(ac, d, ast, fst)) {       // many groups: K3 into the scratch, then the same kernel
-      ac.from_scratch = 1; ac.slot = (long long)scratch;
-      fuse_slice_groups(ac, d, rm, fst);            // (the extract item fitted with the same groups)
-      P->grad_permutes.push_back({gs, (int64_t)scratch, perm});
-      scratch += sm.elems;
-    }
-    push_item(P->acc_items, P->acc_bs, ac);
+    if (leaf_adj.empty()) continue;
+    // accumulate: the adjoint slot (pair output order) -> q's sub-block of the full-shape gradient; the same for the
+    // adjoint's tangent, which has the adjoint's legs
+    auto accumulate = [&](int gs, std::vector<SliceItem>& items, std::vector<long long>& bs,
+                          std::vector<tncb_plan::GradPermute>& permutes) {
+      const SlotMeta& g = S.slots[gs];
+      std::vector<long long> gst(g.legs.size());
+      { long long s = 1; for (size_t j = g.legs.size(); j-- > 0;) { gst[j] = s; s *= (long long)g.dims[j]; } }
+      std::vector<int> perm(sm.legs.size());
+      std::vector<long long> ast(sm.legs.size());
+      for (size_t i = 0; i < sm.legs.size(); i++) {
+        perm[i] = (int)(std::find(g.legs.begin(), g.legs.end(), sm.legs[i]) - g.legs.begin());
+        ast[i] = gst[perm[i]];
+      }
+      SliceItem ac = it;
+      ac.full = (long long)P->grad_offset[li];
+      ac.slot = (long long)P->slot_off[gs];
+      if (!fuse_slice_groups(ac, d, ast, fst)) {     // many groups: K3 into the scratch, then the same kernel
+        ac.from_scratch = 1; ac.slot = (long long)scratch;
+        fuse_slice_groups(ac, d, rm, fst);          // (the extract item fitted with the same groups)
+        permutes.push_back({gs, (int64_t)scratch, perm});
+        scratch += sm.elems;
+      }
+      push_item(items, bs, ac);
+    };
+    accumulate(leaf_adj[li], P->acc_items, P->acc_bs, P->grad_permutes);
+    if (!leaf_dadj.empty()) accumulate(leaf_dadj[li], P->dacc_items, P->dacc_bs, P->dgrad_permutes);
   }
   P->acc_scratch_elems = scratch;
-  for (const auto* bs : {&P->sl_bs, &P->const_bs, &P->acc_bs})
+  for (const auto* bs : {&P->sl_bs, &P->const_bs, &P->acc_bs, &P->tan_bs, &P->dacc_bs})
     if (!bs->empty() && bs->back() > 0x7fffffffLL) return fail(TNCB_ERR_UNSUPPORTED, "slice leaves too large for one launch");
   return TNCB_OK;
 }
@@ -1087,40 +1122,70 @@ static int build_slice_items(tncb_plan* P, const std::vector<const tncb_tn*>& lv
 // backward levels, K3 of the many-group adjoints and the accumulation into the full-shape gradient (zeroed here).  The
 // leaves without a sliced leg are the same in every slice: they are copied once per call (the leaf block is never
 // released by the layout, so they stay in place across slices).
-static int run_sliced(tncb_ctx* ctx, tncb_plan* P, size_t first, size_t stride, const double2* seed, double2* value, double2* grad) {
+// A sliced tangent / Hessian-vector plan also extracts slice q's sub-block of every requested leaf's tangent (tangents:
+// the caller's full-shape block) before the forward levels, adds the result's tangent into tan_value, writes the seed
+// tangent with the seed (NULL: zero) and accumulates the adjoints' tangents into dgrad after the adjoints.  The tangent
+// slots are released by the layout after their last read, so every tangent is extracted per slice.  Any output may be
+// NULL; the backward levels run only if grad or dgrad is wanted.
+struct SliceRun {
+  const double2 *seed = nullptr, *seed_tan = nullptr, *tangents = nullptr;
+  double2 *value = nullptr, *tan_value = nullptr, *grad = nullptr, *dgrad = nullptr;
+};
+static int run_sliced(tncb_ctx* ctx, tncb_plan* P, size_t first, size_t stride, const SliceRun& io) {
   const Schedule& S = P->S;
   char* ws = (char*)P->ws;
   char* dev = (char*)P->sl_dev;
   const SlotMeta& rm = S.slots[S.result_slot];
-  const size_t vbytes = std::max<size_t>(rm.elems, 1) * sizeof(double2);
+  const size_t vbytes = std::max<size_t>(rm.elems, 1) * sizeof(double2), rbytes = rm.elems * sizeof(double2);
   auto items = [&](int i) { return (const SliceItem*)(dev + P->sl_off[i]); };
-  auto bs = [&](int i) { return (const long long*)(dev + P->sl_off[3 + i]); };
-  double2* scratch = (double2*)(dev + P->sl_off[6] + sizeof(double2));
+  auto bs = [&](int i) { return (const long long*)(dev + P->sl_off[kSliceSets + i]); };
+  const double2* one = (const double2*)(dev + P->sl_off[2 * kSliceSets]);
+  double2* scratch = (double2*)(dev + P->sl_off[2 * kSliceSets] + sizeof(double2));
   const double2* full = (const double2*)P->full_dev;
+  const size_t gbytes = std::max<uint64_t>(P->grad_elems, 1) * sizeof(double2);
   P->fwd_ready = false;
-  if (grad) TNCB_CUDA(cudaMemsetAsync(grad, 0, std::max<uint64_t>(P->grad_elems, 1) * sizeof(double2), ctx->stream));
+  for (double2* g : {io.grad, io.dgrad}) if (g) TNCB_CUDA(cudaMemsetAsync(g, 0, gbytes, ctx->stream));
   if (first >= P->n_sl) {                          // more ranks than slices
-    TNCB_CUDA(cudaMemsetAsync(value, 0, vbytes, ctx->stream));
+    for (double2* v : {io.value, io.tan_value}) if (v) TNCB_CUDA(cudaMemsetAsync(v, 0, vbytes, ctx->stream));
     return TNCB_OK;
   }
-  int rc = launch_slice_extract(ctx, items(1), bs(1), (int)P->const_items.size(), P->const_items.empty() ? 0 : P->const_bs.back(), full, ws, 0);
-  for (size_t q = first; q < P->n_sl && !rc; q += stride) {
-    if (!P->sl_items.empty() && (rc = launch_slice_extract(ctx, items(0), bs(0), (int)P->sl_items.size(), P->sl_bs.back(), full, ws, q))) break;
-    if ((rc = enqueue_static(ctx, P, ws, 1, 0, 0, P->n_fwd_levels))) break;
-    const double2* r = (const double2*)(ws + P->slot_off[S.result_slot]);
-    if (q == first) TNCB_CUDA(cudaMemcpyAsync(value, r, rm.elems * sizeof(double2), cudaMemcpyDeviceToDevice, ctx->stream));
-    else if ((rc = launch_add(ctx, value, r, rm.elems))) break;
-    if (!grad) continue;
-    TNCB_CUDA(cudaMemcpyAsync(ws + P->slot_off[P->seed_slot], seed ? seed : (const double2*)(dev + P->sl_off[6]),
-                              rm.elems * sizeof(double2), cudaMemcpyDeviceToDevice, ctx->stream));
-    if ((rc = enqueue_static(ctx, P, ws, 1, 0, P->n_fwd_levels, (int)P->level_batched.size()))) break;
-    for (size_t i = 0; i < P->grad_permutes.size() && !rc; i++) {
-      const auto& gp = P->grad_permutes[i];
+  const bool backward = io.grad || io.dgrad;
+  auto accumulate = [&](const std::vector<tncb_plan::GradPermute>& permutes) {
+    int rc = TNCB_OK;
+    for (size_t i = 0; i < permutes.size() && !rc; i++) {
+      const auto& gp = permutes[i];
       const SlotMeta& sm = S.slots[gp.slot];
       rc = launch_permute(ctx, (const double2*)(ws + P->slot_off[gp.slot]), scratch + gp.dst, (int)sm.dims.size(), sm.dims.data(), gp.perm.data());
     }
-    if (!rc && !P->acc_items.empty())
-      rc = launch_grad_accumulate(ctx, items(2), bs(2), (int)P->acc_items.size(), P->acc_bs.back(), ws, scratch, grad, q);
+    return rc;
+  };
+  int rc = launch_slice_extract(ctx, items(kSlConst), bs(kSlConst), (int)P->const_items.size(), P->const_items.empty() ? 0 : P->const_bs.back(), full, ws, 0);
+  for (size_t q = first; q < P->n_sl && !rc; q += stride) {
+    if (!P->sl_items.empty() && (rc = launch_slice_extract(ctx, items(kSlExtract), bs(kSlExtract), (int)P->sl_items.size(), P->sl_bs.back(), full, ws, q))) break;
+    if (!P->tan_items.empty() &&
+        (rc = launch_slice_extract(ctx, items(kSlTan), bs(kSlTan), (int)P->tan_items.size(), P->tan_bs.back(), io.tangents, ws, q))) break;
+    if ((rc = enqueue_static(ctx, P, ws, 1, 0, 0, P->n_fwd_levels))) break;
+    for (auto [sum, slot] : {std::pair<double2*, int>{io.value, S.result_slot}, {io.tan_value, P->tan_result}}) {
+      if (!sum || rc) continue;
+      const double2* r = (const double2*)(ws + P->slot_off[slot]);
+      if (q != first) rc = launch_add(ctx, sum, r, rm.elems);
+      else if (cudaMemcpyAsync(sum, r, rbytes, cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess)
+        rc = fail(TNCB_ERR_CUDA, "result copy failed");
+    }
+    if (rc || !backward) continue;
+    // the seed slots may reuse memory the forward levels freed: written after them, on the stream
+    TNCB_CUDA(cudaMemcpyAsync(ws + P->slot_off[P->seed_slot], io.seed ? io.seed : one, rbytes, cudaMemcpyDeviceToDevice, ctx->stream));
+    if (P->seed_tan_slot >= 0) {
+      char* ds = ws + P->slot_off[P->seed_tan_slot];
+      TNCB_CUDA(io.seed_tan ? cudaMemcpyAsync(ds, io.seed_tan, rbytes, cudaMemcpyDeviceToDevice, ctx->stream)
+                            : cudaMemsetAsync(ds, 0, rbytes, ctx->stream));
+    }
+    if ((rc = enqueue_static(ctx, P, ws, 1, 0, P->n_fwd_levels, (int)P->level_batched.size()))) break;
+    if ((io.grad && (rc = accumulate(P->grad_permutes))) || (io.dgrad && (rc = accumulate(P->dgrad_permutes)))) break;
+    if (io.grad && !P->acc_items.empty())
+      rc = launch_grad_accumulate(ctx, items(kSlAcc), bs(kSlAcc), (int)P->acc_items.size(), P->acc_bs.back(), ws, scratch, io.grad, q);
+    if (!rc && io.dgrad && !P->dacc_items.empty())
+      rc = launch_grad_accumulate(ctx, items(kSlDacc), bs(kSlDacc), (int)P->dacc_items.size(), P->dacc_bs.back(), ws, scratch, io.dgrad, q);
   }
   return rc;
 }
@@ -1385,18 +1450,16 @@ int tncb_plan_create_vjp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path
   return TNCB_OK;
 }
 
-// A sliced gradient plan: the gradient plan of one slice's structure (compiled exactly as tncb_plan_create_vjp compiles
-// the host-sliced slice network), plus the extract / accumulate items that move slice q's sub-blocks between the full
-// leaves and the workspace.
-int tncb_plan_create_vjp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, size_t n_sliced,
-                                const uint64_t* sliced_legs, const uint8_t* wrt, tncb_plan** out) {
-  using namespace tncb;
-  if (!tn || !out || (n_sliced && !sliced_legs)) return fail(TNCB_ERR_INVALID, "null argument");
-  std::vector<const tncb_tn*> lv;
-  collect_leaf_nodes(tn, lv);
+namespace tncb {
+// The checks every sliced creator makes on the network and its sliced legs: no device leaves (`plans` names the plan
+// kind in the message), every sliced leg listed once, joining two tensors, of non-zero dimension, and a slice count that
+// fits 64 bits.  Fills the legs' dims and the slice count.
+static int check_sliced_legs(const std::vector<const tncb_tn*>& lv, const char* plans, size_t n_sliced, const uint64_t* sliced_legs,
+                             std::vector<uint64_t>& sl, std::vector<uint64_t>& sdim, uint64_t* n_slices) {
   for (const tncb_tn* l : lv)
-    if (l->kind == TNCB_DATA_DEVICE) return fail(TNCB_ERR_UNSUPPORTED, "gradient plans do not take device leaves (they are consumed per call)");
-  std::vector<uint64_t> sl(sliced_legs, sliced_legs + n_sliced), sdim(n_sliced, 0);
+    if (l->kind == TNCB_DATA_DEVICE) return fail(TNCB_ERR_UNSUPPORTED, std::string(plans) + " plans do not take device leaves (they are consumed per call)");
+  sl.assign(sliced_legs, sliced_legs + n_sliced);
+  sdim.assign(n_sliced, 0);
   uint64_t n_sl = 1;
   bool overflow = false;
   for (size_t k = 0; k < n_sliced; k++) {
@@ -1414,15 +1477,40 @@ int tncb_plan_create_vjp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_pat
     else n_sl *= sdim[k];
   }
   if (overflow) return fail(TNCB_ERR_INVALID, "the slice count overflows 64 bits");
+  *n_slices = n_sl;
+  return TNCB_OK;
+}
+
+// A sliced derivative plan of the given kind: the gradient, tangent or Hessian-vector plan of one slice's structure,
+// compiled with the calls tncb_plan_create_vjp / _jvp / _hvp make on the host-sliced slice network, plus the slice items.
+enum class SlicedKind { vjp, jvp, hvp };
+static int create_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, size_t n_sliced, const uint64_t* sliced_legs,
+                         const uint8_t* wrt, SlicedKind kind, tncb_plan** out) {
+  if (!tn || !out || (n_sliced && !sliced_legs)) return fail(TNCB_ERR_INVALID, "null argument");
+  static const char* const noun[3] = {"gradient", "tangent", "Hessian-vector"};
+  const int ki = (int)kind;
+  std::vector<const tncb_tn*> lv;
+  collect_leaf_nodes(tn, lv);
+  std::vector<uint64_t> sl, sdim;
+  uint64_t n_sl = 1;
+  int rc = check_sliced_legs(lv, noun[ki], n_sliced, sliced_legs, sl, sdim, &n_sl);
+  if (rc) return rc;
   SliceTree keep;
   tncb_tn st;
   slice_tree(tn, &st, sl, keep);
   tncb_plan* p = new tncb_plan();
-  p->grad = p->sliced = true;
+  p->sliced = true;
+  p->grad = kind != SlicedKind::jvp;
+  p->tangent = kind != SlicedKind::vjp;
+  p->hvp = kind == SlicedKind::hvp;
   p->n_sl = n_sl;
-  std::vector<int> leaf_adj;
-  int rc = build_schedule(&st, path, p->S);
-  if (!rc) rc = build_backward(p, wrt, leaf_adj, p->S.steps.size());
+  std::vector<int> tan, leaf_adj, leaf_dadj;
+  rc = build_schedule(&st, path, p->S);
+  const size_t n_fwd = p->S.steps.size();
+  size_t b0 = n_fwd;
+  if (!rc && p->tangent) { rc = build_tangent(p, wrt, &tan); b0 = p->S.steps.size(); }
+  if (!rc && p->grad) rc = build_backward(p, wrt, leaf_adj, n_fwd);
+  if (!rc && p->hvp) rc = build_backward_tangent(p, b0, tan, leaf_adj, leaf_dadj);
   if (rc) { delete p; return rc; }
   size_t dev_free = 0, dev_total = 0;
   if (ctx) { cudaSetDevice(ctx->device); if (cudaMemGetInfo(&dev_free, &dev_total) != cudaSuccess) { dev_total = 0; cudaGetLastError(); } }
@@ -1430,12 +1518,33 @@ int tncb_plan_create_vjp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_pat
   if (!p->is_static) {
     const size_t need = p->ws_bytes, limit = static_ws_limit(dev_total);
     delete p;
-    return fail(TNCB_ERR_UNSUPPORTED, "the gradient workspace of one slice needs " + std::to_string(need) + " bytes, above the static-workspace limit of " +
-                                      std::to_string(limit) + " bytes (TNCB_PLAN_WS_GB)");
+    return fail(TNCB_ERR_UNSUPPORTED, std::string("the ") + noun[ki] + " workspace of one slice needs " + std::to_string(need) +
+                                      " bytes, above the static-workspace limit of " + std::to_string(limit) + " bytes (TNCB_PLAN_WS_GB)");
   }
-  if ((rc = build_slice_items(p, lv, sl, sdim, leaf_adj))) { delete p; return rc; }
+  if ((rc = build_slice_items(p, lv, sl, sdim, leaf_adj, leaf_dadj))) { delete p; return rc; }
   *out = p;
   return TNCB_OK;
+}
+} // namespace tncb
+
+// A sliced gradient plan: the gradient plan of one slice's structure (compiled exactly as tncb_plan_create_vjp compiles
+// the host-sliced slice network), plus the extract / accumulate items that move slice q's sub-blocks between the full
+// leaves and the workspace.
+int tncb_plan_create_vjp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, size_t n_sliced,
+                                const uint64_t* sliced_legs, const uint8_t* wrt, tncb_plan** out) {
+  return tncb::create_sliced(ctx, tn, path, n_sliced, sliced_legs, wrt, tncb::SlicedKind::vjp, out);
+}
+
+// Sliced tangent and Hessian-vector plans: the tangent / Hessian-vector plan of one slice's structure plus the items that
+// also move the leaf tangents in and the adjoints' tangents out per slice.
+int tncb_plan_create_jvp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, size_t n_sliced,
+                                const uint64_t* sliced_legs, const uint8_t* wrt, tncb_plan** out) {
+  return tncb::create_sliced(ctx, tn, path, n_sliced, sliced_legs, wrt, tncb::SlicedKind::jvp, out);
+}
+
+int tncb_plan_create_hvp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, size_t n_sliced,
+                                const uint64_t* sliced_legs, const uint8_t* wrt, tncb_plan** out) {
+  return tncb::create_sliced(ctx, tn, path, n_sliced, sliced_legs, wrt, tncb::SlicedKind::hvp, out);
 }
 
 int tncb_plan_grad_offsets(const tncb_plan* plan, int64_t* offsets) {
@@ -1450,6 +1559,7 @@ int tncb_plan_grad_offsets(const tncb_plan* plan, int64_t* offsets) {
 int tncb_plan_vjp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* seed, tncb_tensor** grads) {
   using namespace tncb;
   if (!ctx || !plan || !grads) return fail(TNCB_ERR_INVALID, "null argument");
+  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
   if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_vjp_sliced");
   if (plan->hvp) return hvp_refused();
   if (plan->tangent) return fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp");
@@ -1497,6 +1607,7 @@ int tncb_plan_vjp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t st
                          tncb_tensor** value, tncb_tensor** grads) {
   using namespace tncb;
   if (!ctx || !plan || !value || !grads || stride == 0) return fail(TNCB_ERR_INVALID, "bad argument");
+  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
   if (plan->hvp) return hvp_refused();
   if (plan->tangent) return fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp");
   if (!plan->sliced) return fail(TNCB_ERR_INVALID, "not a sliced gradient plan (tncb_plan_create_vjp_sliced)");
@@ -1514,7 +1625,11 @@ int tncb_plan_vjp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t st
   const uint64_t n = plan->grad_elems;
   int rc = tensor_new(ctx, (int)rm.dims.size(), rm.dims.data(), &v);
   if (!rc) rc = tensor_new(ctx, 1, &n, &g);
-  if (!rc) rc = run_sliced(ctx, plan, first, stride, seed ? seed->ptr : nullptr, v->ptr, g->ptr);
+  if (!rc) {
+    SliceRun io;
+    io.seed = seed ? seed->ptr : nullptr; io.value = v->ptr; io.grad = g->ptr;
+    rc = run_sliced(ctx, plan, first, stride, io);
+  }
   if (rc) {
     if (v) tncb_tensor_free(ctx, v);
     if (g) tncb_tensor_free(ctx, g);
@@ -1526,6 +1641,7 @@ int tncb_plan_vjp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t st
 
 int tncb_plan_execute(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tn, tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   if (!ctx || !plan || !tn) return tncb::fail(TNCB_ERR_INVALID, "null argument");
+  if (tncb::sliced_tangent(plan)) return tncb::sliced_tangent_refused(plan);
   if (plan->sliced) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_run_slices / tncb_plan_vjp_sliced");
   if (plan->hvp) return tncb::hvp_refused();
   if (plan->tangent) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp");
@@ -1597,6 +1713,7 @@ int tncb_plan_stage(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tn) {
 
 int tncb_plan_run(tncb_ctx* ctx, tncb_plan* plan, tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   if (!ctx || !plan) return tncb::fail(TNCB_ERR_INVALID, "null argument");
+  if (tncb::sliced_tangent(plan)) return tncb::sliced_tangent_refused(plan);
   if (plan->sliced) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_run_slices / tncb_plan_vjp_sliced");
   if (plan->hvp) return tncb::hvp_refused();
   if (plan->tangent) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp");
@@ -1615,6 +1732,7 @@ int tncb_plan_run(tncb_ctx* ctx, tncb_plan* plan, tncb_tensor** out, int* n_out,
 // block (KBs), the plan's kernels (batched / graph as usual), one accumulation kernel.
 int tncb_plan_stage_slices(tncb_ctx* ctx, tncb_plan* plan, size_t n_slices, const tncb_tn* const* slice_tns) {
   if (!ctx || !plan || !slice_tns || n_slices == 0) return tncb::fail(TNCB_ERR_INVALID, "null argument");
+  if (tncb::sliced_tangent(plan)) return tncb::sliced_tangent_refused(plan);
   if (plan->sliced) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan stages its full network once (tncb_plan_stage)");
   if (plan->hvp) return tncb::hvp_refused();
   if (plan->grad) return tncb::fail(TNCB_ERR_UNSUPPORTED, "gradient plans run one staged network at a time");
@@ -1625,21 +1743,30 @@ int tncb_plan_stage_slices(tncb_ctx* ctx, tncb_plan* plan, size_t n_slices, cons
 
 int tncb_plan_run_slices(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t stride, tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   if (!ctx || !plan || stride == 0) return tncb::fail(TNCB_ERR_INVALID, "bad argument");
-  if (plan->hvp) return tncb::hvp_refused();
-  if (plan->tangent) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp / tncb_plan_jvp_batch");
   if (plan->sliced) {         // forward levels only, slices extracted on the device from the staged full leaves
     if (plan->ctx != ctx || !plan->full_staged) return tncb::fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this context");
     const tncb::SlotMeta& rm = plan->S.slots[plan->S.result_slot];
     TNCB_CUDA(cudaSetDevice(ctx->device));
-    tncb_tensor* sum = nullptr;
+    tncb_tensor *sum = nullptr, *zero = nullptr;
     int rc = tncb::tensor_new(ctx, (int)rm.dims.size(), rm.dims.data(), &sum);
-    if (!rc) rc = tncb::run_sliced(ctx, plan, first, stride, nullptr, sum->ptr, nullptr);
+    tncb::SliceRun io;
+    io.value = sum ? sum->ptr : nullptr;
+    if (!rc && tncb::sliced_tangent(plan)) {   // the tangent pairs share the forward levels: they read zero tangents
+      rc = tncb::tensor_new(ctx, 1, &plan->grad_elems, &zero);
+      if (!rc && cudaMemsetAsync(zero->ptr, 0, zero->elems * sizeof(double2), ctx->stream) != cudaSuccess)
+        rc = tncb::fail(TNCB_ERR_CUDA, "tangent block: memset failed");
+      if (!rc) io.tangents = zero->ptr;
+    }
+    if (!rc) rc = tncb::run_sliced(ctx, plan, first, stride, io);
+    if (zero) tncb_tensor_free(ctx, zero);      // (stream-ordered: the arena hands it out behind this call's kernels)
     if (rc) { if (sum) tncb_tensor_free(ctx, sum); return rc; }
     if (out) *out = sum; else tncb_tensor_free(ctx, sum);
     if (n_out) *n_out = (int)rm.legs.size();
     if (out_legs) for (size_t i = 0; i < rm.legs.size(); i++) out_legs[i] = rm.legs[i];
     return TNCB_OK;
   }
+  if (plan->hvp) return tncb::hvp_refused();
+  if (plan->tangent) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp / tncb_plan_jvp_batch");
   if (plan->grad) return tncb::fail(TNCB_ERR_UNSUPPORTED, "gradient plans run one staged network at a time");
   if (!plan->slices_dev || plan->ctx != ctx) return tncb::fail(TNCB_ERR_INVALID, "tncb_plan_stage_slices has not been called on this context");
   const tncb::Schedule& S = plan->S;
@@ -1679,6 +1806,7 @@ int tncb_plan_run_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
                         tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   using namespace tncb;
   if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
+  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
   if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_run_slices / tncb_plan_vjp_sliced");
   if (plan->hvp) return hvp_refused();
   if (plan->grad) return fail(TNCB_ERR_UNSUPPORTED, "gradient plans run one staged network at a time");
@@ -1727,6 +1855,7 @@ int tncb_plan_run_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
 int tncb_plan_stage_batch(tncb_ctx* ctx, tncb_plan* plan, size_t n, const tncb_tn* const* tns) {
   using namespace tncb;
   if (!ctx || !plan || !tns || n == 0) return fail(TNCB_ERR_INVALID, "null argument");
+  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
   if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan has no batched gradients");
   if (plan->hvp) return hvp_refused();
   if (!plan->grad && !plan->tangent)
@@ -1742,6 +1871,7 @@ int tncb_plan_vjp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
                         tncb_tensor** values, tncb_tensor** grad_rows, tncb_tensor** grad_sum) {
   using namespace tncb;
   if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
+  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
   if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan has no batched gradients");
   if (plan->hvp) return hvp_refused();
   if (plan->tangent) return fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp_batch");
@@ -1909,6 +2039,7 @@ static int stage_tangents(tncb_ctx* ctx, const tncb_plan* P, const double2* tang
 int tncb_plan_jvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, tncb_tensor** value, tncb_tensor** tangent_out) {
   using namespace tncb;
   if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
+  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
   if (plan->hvp) return hvp_refused();
   int rc = jvp_args(plan, tangents, value || tangent_out, {plan->grad_elems});
   if (rc) return rc;
@@ -1945,6 +2076,7 @@ int tncb_plan_jvp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
                         tncb_tensor** values, tncb_tensor** tangent_rows) {
   using namespace tncb;
   if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
+  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
   if (plan->hvp) return hvp_refused();
   if (!plan->tangent) return fail(TNCB_ERR_INVALID, "not a tangent plan (tncb_plan_create_jvp)");
   if (!plan->slices_dev || plan->ctx != ctx)
@@ -2064,6 +2196,7 @@ int tncb_plan_hvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, c
                   tncb_tensor** grad_tangents) {
   using namespace tncb;
   if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
+  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
   if (!plan->hvp) return fail(TNCB_ERR_INVALID, "not a Hessian-vector plan (tncb_plan_create_hvp)");
   int rc = jvp_args(plan, tangents, value || tangent_out || grads || grad_tangents, {plan->grad_elems});
   if (rc) return rc;
@@ -2115,6 +2248,67 @@ int tncb_plan_hvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, c
   return TNCB_OK;
 }
 
+namespace tncb {
+// tncb_plan_jvp_sliced / tncb_plan_hvp_sliced: the arguments, the outputs (any may be NULL), one run_sliced
+static int sliced_tangent_call(tncb_ctx* ctx, tncb_plan* plan, bool hvp, size_t first, size_t stride, const tncb_tensor* tangents,
+                               const tncb_tensor* seed, const tncb_tensor* seed_tangent, tncb_tensor** value,
+                               tncb_tensor** tangent_out, tncb_tensor** grads, tncb_tensor** grad_tangents) {
+  if (!ctx || !plan || stride == 0) return fail(TNCB_ERR_INVALID, "bad argument");
+  if (!sliced_tangent(plan) || plan->hvp != hvp)
+    return fail(TNCB_ERR_INVALID, hvp ? "not a sliced Hessian-vector plan (tncb_plan_create_hvp_sliced)"
+                                      : "not a sliced tangent plan (tncb_plan_create_jvp_sliced)");
+  int rc = jvp_args(plan, tangents, value || tangent_out || grads || grad_tangents, {plan->grad_elems});
+  if (rc) return rc;
+  const Schedule& S = plan->S;
+  const SlotMeta& rm = S.slots[S.result_slot];
+  if (hvp) {                                       // the seed checks of tncb_plan_hvp
+    if (seed) { if ((rc = seed_args(rm, seed, "seed"))) return rc; }
+    else if (!rm.dims.empty()) return fail(TNCB_ERR_INVALID, "a seed is needed for a result of rank " + std::to_string(rm.dims.size()));
+    if (seed_tangent && (rc = seed_args(rm, seed_tangent, "seed tangent"))) return rc;
+  }
+  if (plan->ctx != ctx || !plan->full_staged) return fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this context");
+  TNCB_CUDA(cudaSetDevice(ctx->device));
+  const uint64_t ge = plan->grad_elems;
+  tncb_tensor *v = nullptr, *t = nullptr, *g = nullptr, *dg = nullptr;
+  if (value) rc = tensor_new(ctx, (int)rm.dims.size(), rm.dims.data(), &v);
+  if (!rc && tangent_out) rc = tensor_new(ctx, (int)rm.dims.size(), rm.dims.data(), &t);
+  if (!rc && grads) rc = tensor_new(ctx, 1, &ge, &g);
+  if (!rc && grad_tangents) rc = tensor_new(ctx, 1, &ge, &dg);
+  if (!rc) {
+    SliceRun io;
+    io.tangents = tangents->ptr;
+    io.seed = seed ? seed->ptr : nullptr; io.seed_tan = seed_tangent ? seed_tangent->ptr : nullptr;
+    io.value = v ? v->ptr : nullptr; io.tan_value = t ? t->ptr : nullptr;
+    io.grad = g ? g->ptr : nullptr; io.dgrad = dg ? dg->ptr : nullptr;
+    rc = run_sliced(ctx, plan, first, stride, io);
+  }
+  if (rc) {
+    for (tncb_tensor* x : {v, t, g, dg}) if (x) tncb_tensor_free(ctx, x);
+    return rc;
+  }
+  if (value) *value = v;
+  if (tangent_out) *tangent_out = t;
+  if (grads) *grads = g;
+  if (grad_tangents) *grad_tangents = dg;
+  return TNCB_OK;
+}
+} // namespace tncb
+
+// Per slice first, first+stride, ...: extract (sliced leaves, every leaf tangent), forward levels with their tangent
+// pairs, R += and Ṙ +=.  No host work per slice; slices run in stream order, so a call repeats bit for bit.
+int tncb_plan_jvp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t stride, const tncb_tensor* tangents,
+                         tncb_tensor** value, tncb_tensor** tangent_out) {
+  return tncb::sliced_tangent_call(ctx, plan, false, first, stride, tangents, nullptr, nullptr, value, tangent_out, nullptr, nullptr);
+}
+
+// As tncb_plan_jvp_sliced, then per slice the seed and its tangent, the backward levels with their tangent pairs, K3 of the
+// many-group adjoints and adjoint tangents, and the accumulation of G and Ġ into the full-shape blocks.
+int tncb_plan_hvp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t stride, const tncb_tensor* tangents,
+                         const tncb_tensor* seed, const tncb_tensor* seed_tangent, tncb_tensor** value,
+                         tncb_tensor** tangent_out, tncb_tensor** grads, tncb_tensor** grad_tangents) {
+  return tncb::sliced_tangent_call(ctx, plan, true, first, stride, tangents, seed, seed_tangent, value, tangent_out, grads, grad_tangents);
+}
+
 // New payloads for some leaves of the staged network, straight from device memory: one launch on the ctx stream into the
 // leaf block the next run reads (a static plan's workspace block, which its graph replays also read; a non-static plan's
 // resident block; a sliced gradient plan's full block).  The static layout never releases its leaf block, so the new
@@ -2122,6 +2316,7 @@ int tncb_plan_hvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, c
 int tncb_plan_set_leaves(tncb_ctx* ctx, tncb_plan* plan, size_t n, const uint64_t* leaf_index, const void* const* src) {
   using namespace tncb;
   if (!ctx || !plan || (n && (!leaf_index || !src))) return fail(TNCB_ERR_INVALID, "null argument");
+  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
   for (int k : plan->S.leaf_kind)
     if (k == TNCB_DATA_DEVICE) return fail(TNCB_ERR_UNSUPPORTED, "plans with device leaves cannot be staged (they are consumed per call)");
   const Schedule* S = &plan->S;
@@ -2149,6 +2344,7 @@ int tncb_plan_stage_instances(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tmp
                               const uint64_t* leaf_index, const void* const* src, const uint64_t* instance_stride) {
   using namespace tncb;
   if (!ctx || !plan || !tmpl || (n && (!leaf_index || !src || !instance_stride))) return fail(TNCB_ERR_INVALID, "null argument");
+  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
   if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan takes device payloads through tncb_plan_set_leaves");
   if (plan->hvp) return hvp_refused();
   const Schedule& S = plan->S;
@@ -2261,7 +2457,9 @@ int tncb_plan_info(const tncb_plan* plan, uint64_t* n_pairs, double* flops, doub
     if (!plan->dgrad_items.empty()) k++;                                           // ... and of the gradients' tangents
     if (!plan->acc_items.empty()) k++;                                            // a slice's gradient accumulation
     if (!plan->sl_items.empty()) k++;                                              // a slice's leaf extraction
-    k += (plan->tan_leaves.size() + tncb::kStageItems - 1) / tncb::kStageItems;    // the leaf tangents' staging
+    if (!plan->dacc_items.empty()) k++;                                            // ... accumulation of the adjoints' tangents
+    if (plan->sliced) k += !plan->tan_items.empty();                               // ... and extraction of the leaf tangents
+    else k += (plan->tan_leaves.size() + tncb::kStageItems - 1) / tncb::kStageItems;   // the leaf tangents' staging
     for (int ns : plan->sum_count) if (ns) k++;                                    // a level's tangent sums
     *n_kernels = k + 2 * (plan->grad_permutes.size() + plan->dgrad_permutes.size());   // (K3: tables + transpose)
   }
