@@ -465,7 +465,7 @@ int tncb_plan_jvp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
  * every leaf requested, in one walk over the levels.  Arguments and refusals as tncb_plan_create_jvp (the message of
  * a workspace above the limit states the bytes needed); ctx may be NULL (host-only compile: tncb_plan_info and
  * tncb_plan_grad_offsets).  Always static, never graphed, no pair-by-pair fallback.  Every other plan entry point but
- * tncb_plan_stage / set_leaves / info / grad_offsets -> TNCB_ERR_UNSUPPORTED on a Hessian-vector plan. */
+ * tncb_plan_stage / set_leaves / hvp_batch / info / grad_offsets -> TNCB_ERR_UNSUPPORTED on a Hessian-vector plan. */
 int tncb_plan_create_hvp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, const uint8_t* wrt, tncb_plan** out);
 /* One forward-over-reverse pass on the leaves staged by tncb_plan_stage (and overwritten by tncb_plan_set_leaves).
  * tangents:     [tangent_elems] device tensor at tncb_plan_grad_offsets (the gradient block's layout)
@@ -482,6 +482,32 @@ int tncb_plan_create_hvp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path
 int tncb_plan_hvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, const tncb_tensor* seed,
                   const tncb_tensor* seed_tangent, tncb_tensor** value, tncb_tensor** tangent_out, tncb_tensor** grads,
                   tncb_tensor** grad_tangents);
+/* count forward-over-reverse passes in one walk over the levels, in passes of as many workspace copies as fit beside
+ * the plan's own (as tncb_plan_run_batch): many directions of one network (a Hessian block, block Lanczos), or one
+ * direction per sampled network (a loss over bitstrings or input states).  Instance i < count is the network staged
+ * by tncb_plan_stage (and tncb_plan_set_leaves), except leaves leaf_index[0..n): instance i reads src[k] +
+ * i * instance_stride[k] elements (stride 0 = the same device payload in every instance), validated as
+ * tncb_plan_stage_instances validates its sources, before any launch.  n == 0: count copies of the staged network.
+ *   tangents:      [count, tangent_elems], row i for instance i at tncb_plan_grad_offsets
+ *   seeds:         [count, result dims..]; NULL only for a rank-0 result (every seed 1)
+ *   seed_tangents: [count, result dims..]; NULL = zero
+ *   *values, *tangent_rows:           new [count, result dims..], R and Ṙ of every instance
+ *   *grad_rows, *grad_tangent_rows:   new [count, tangent_elems], G and Ġ of every instance
+ *   *grad_sum, *grad_tangent_sum:     new [tangent_elems], the left fold 0 + row 0 + row 1 + ... in instance order
+ * Each output may be NULL, not all six; the backward levels run only if one of the four G / Ġ outputs is wanted.  Row i
+ * of every output is bit-identical to tncb_plan_set_leaves(instance i's payloads) + tncb_plan_hvp(tangent row i, seed
+ * i, seed tangent i): every launch decision is the single-network one, and int8-engine steps run instance by instance.
+ * The plan's staged leaves and workspace are left as they are, so tncb_plan_hvp before and after gives the same bits.
+ * The sums can be combined across ranks with tncb_comm_allreduce_sum.  Not a Hessian-vector plan, not staged on this
+ * context, count == 0, no output, NULL tangents, a NULL seed for a result of rank > 0, a result of rank 64 ->
+ * TNCB_ERR_INVALID; a sliced Hessian-vector or tangent plan -> TNCB_ERR_UNSUPPORTED; device-source errors as
+ * tncb_plan_stage_instances; tangent, seed or seed-tangent dims that do not match -> TNCB_ERR_SHAPE; not even one
+ * workspace copy fits beside the plan's -> TNCB_ERR_OOM.  Errors leave the arena and the staged plan as they found them. */
+int tncb_plan_hvp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t count, size_t n, const uint64_t* leaf_index,
+                        const void* const* src, const uint64_t* instance_stride, const tncb_tensor* tangents,
+                        const tncb_tensor* seeds, const tncb_tensor* seed_tangents, tncb_tensor** values,
+                        tncb_tensor** tangent_rows, tncb_tensor** grad_rows, tncb_tensor** grad_sum,
+                        tncb_tensor** grad_tangent_rows, tncb_tensor** grad_tangent_sum);
 /* ---- sliced tangents and Hessian-vector products: networks whose tangent or Hessian-vector workspace does not fit ----
  * By linearity, as for sliced gradients: R = sum_q R_q, so Ṙ = sum_q Ṙ_q; slice q's leaf (and its tangent) is q's
  * fixed-index sub-block of the full leaf (and of its full-shape tangent), and q's G_l and Ġ_l add into q's sub-block of
@@ -493,7 +519,8 @@ int tncb_plan_hvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, c
  * naming the bytes.  tncb_plan_grad_offsets packs the FULL leaves' shapes, for the tangents, G and Ġ alike.
  * Use: tncb_plan_stage(ctx, plan, full tn) uploads the full leaves once; tncb_plan_run_slices runs the forward levels
  * (with zero tangents) and returns a sum bit-identical to the plain sliced run.  Every other entry point (run, execute,
- * stage_slices, run_batch, stage_batch, stage_instances, set_leaves, vjp, vjp_sliced, vjp_batch, jvp, jvp_batch, hvp)
+ * stage_slices, run_batch, stage_batch, stage_instances, set_leaves, vjp, vjp_sliced, vjp_batch, jvp, jvp_batch, hvp,
+ * hvp_batch)
  * -> TNCB_ERR_UNSUPPORTED naming the call that runs the plan. */
 int tncb_plan_create_jvp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, size_t n_sliced,
                                 const uint64_t* sliced_legs, const uint8_t* wrt, tncb_plan** out);

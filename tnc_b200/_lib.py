@@ -123,6 +123,8 @@ SIGNATURES = {
     "tncb_plan_jvp_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, vpp, vpp]),
     "tncb_plan_create_hvp": (C.c_int, [C.c_void_p, C.POINTER(TncbTn), C.POINTER(TncbPath), C.POINTER(C.c_uint8), vpp]),
     "tncb_plan_hvp": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, vpp, vpp, vpp, vpp]),
+    "tncb_plan_hvp_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, u64p, vpp, u64p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, vpp, vpp, vpp, vpp, vpp, vpp]),
     "tncb_plan_create_jvp_sliced": (C.c_int, [C.c_void_p, C.POINTER(TncbTn), C.POINTER(TncbPath), C.c_size_t, u64p,
                                               C.POINTER(C.c_uint8), vpp]),
     "tncb_plan_jvp_sliced": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, vpp, vpp]),

@@ -1270,6 +1270,28 @@ static int batch_copy(tncb_ctx* ctx, const BatchBlock& B, char* dst, size_t dpit
   return e == cudaSuccess ? TNCB_OK : fail(TNCB_ERR_CUDA, std::string("batched copy: ") + cudaGetErrorString(e));
 }
 
+// One gather set (grad_* or dgrad_*) of a pass of n instances whose workspaces lie `stride` bytes apart: instance i's
+// leaf blocks into rows + i * row_elems (rows != nullptr) and/or added to `sum` in instance order, in one launch; the
+// leaves with more fused groups than a GradItem holds take K3 per instance, in instance order, the sum through `scratch`
+static int gather_set_batch(tncb_ctx* ctx, const tncb_plan* P, const std::vector<GradItem>& items, const std::vector<long long>& bs,
+                            const std::vector<tncb_plan::GradPermute>& permutes, const void* dev, const char* base, size_t stride,
+                            size_t n, double2* rows, uint64_t row_elems, double2* sum, double2* scratch) {
+  int rc = TNCB_OK;
+  if (!items.empty())
+    rc = launch_grad_gather_batch(ctx, (const GradItem*)dev, (const long long*)((const char*)dev + items.size() * sizeof(GradItem)),
+                                  (int)items.size(), bs.back(), base, (long long)stride, (int)n, rows, (long long)row_elems, sum);
+  for (size_t i = 0; i < n && !rc; i++)
+    for (size_t k = 0; k < permutes.size() && !rc; k++) {
+      const auto& gp = permutes[k];
+      const SlotMeta& sm = P->S.slots[gp.slot];
+      const double2* adj = (const double2*)(base + i * stride + P->slot_off[gp.slot]);
+      if (rows) rc = launch_permute(ctx, adj, rows + i * row_elems + gp.dst, (int)sm.dims.size(), sm.dims.data(), gp.perm.data());
+      if (!rc && sum) rc = launch_permute(ctx, adj, scratch, (int)sm.dims.size(), sm.dims.data(), gp.perm.data());
+      if (!rc && sum) rc = launch_add(ctx, sum + gp.dst, scratch, sm.elems);
+    }
+  return rc;
+}
+
 // ---- leaf payloads from device memory (tncb_plan_set_leaves / tncb_plan_stage_instances) ----
 // cuMemGetAddressRange, resolved through the runtime as crt.cu resolves cuTensorMapEncodeTiled: the allocation that holds
 // a device address, so that a source range running past its end is refused before anything is launched
@@ -1328,6 +1350,19 @@ static int device_items(const tncb_ctx* ctx, const Schedule& S, size_t n_inst, s
     items.push_back({(const double2*)p, st, (long long)S.leaf_offset[li], (long long)e});
   }
   return TNCB_OK;
+}
+
+// The runs of a leaf block of `block` elements that the device items do not cover (sorted by dst here): run r covers
+// block elements [start, start + len) and sits at `packed` once the runs are packed back to back
+struct LeafRun { long long start, len, packed; };
+static std::vector<LeafRun> leaf_runs(std::vector<LeafStageItem>& items, long long block) {
+  std::vector<LeafRun> runs;
+  std::sort(items.begin(), items.end(), [](const LeafStageItem& x, const LeafStageItem& y) { return x.dst < y.dst; });
+  long long pos = 0, packed = 0;
+  auto gap = [&](long long end) { if (end > pos) { runs.push_back({pos, end - pos, packed}); packed += end - pos; } };
+  for (const LeafStageItem& it : items) { gap(it.dst); pos = std::max(pos, it.dst + it.elems); }
+  gap(block);
+  return runs;
 }
 
 } // namespace tncb
@@ -1939,8 +1974,6 @@ int tncb_plan_vjp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
   const size_t block_bytes = std::max<size_t>(S.leaf_block_elems, 1) * sizeof(double2);
   const size_t res_bytes = rm.elems * sizeof(double2);
   const int n_levels = (int)plan->level_batched.size();
-  const GradItem* d_items = (const GradItem*)plan->grad_dev;
-  const long long* d_bs = (const long long*)((char*)plan->grad_dev + plan->grad_items.size() * sizeof(GradItem));
   for (size_t done = 0; done < count && !rc; done += c) {
     const size_t n = std::min(c, count - done);
     const char* src = (const char*)plan->slices_dev + (first + done) * block_bytes;
@@ -1953,19 +1986,8 @@ int tncb_plan_vjp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
     if (seeds) { if (res_bytes && (rc = batch_copy(ctx, B, seed_dst, ws, (const char*)seeds->ptr + done * res_bytes, res_bytes, res_bytes, n))) break; }
     else if ((rc = batch_copy(ctx, B, seed_dst, ws, (const char*)d_one, sizeof(double2), sizeof(double2), n))) break;
     if ((rc = enqueue_static(ctx, plan, base, (int)n, (long long)ws, plan->n_fwd_levels, n_levels))) break;
-    if (!plan->grad_items.empty() &&
-        (rc = launch_grad_gather_batch(ctx, d_items, d_bs, (int)plan->grad_items.size(), plan->grad_block_start.back(), base,
-                                       (long long)ws, (int)n, gr ? gr->ptr + done * ge : nullptr, (long long)ge, gs ? gs->ptr : nullptr))) break;
-    // leaves with more fused groups than a GradItem holds: K3 per instance, in instance order
-    for (size_t i = 0; i < n && !rc; i++)
-      for (size_t k = 0; k < plan->grad_permutes.size() && !rc; k++) {
-        const auto& gp = plan->grad_permutes[k];
-        const SlotMeta& sm = S.slots[gp.slot];
-        const double2* adj = (const double2*)(base + i * ws + plan->slot_off[gp.slot]);
-        if (gr) rc = launch_permute(ctx, adj, gr->ptr + (done + i) * ge + gp.dst, (int)sm.dims.size(), sm.dims.data(), gp.perm.data());
-        if (!rc && gs) rc = launch_permute(ctx, adj, d_scratch, (int)sm.dims.size(), sm.dims.data(), gp.perm.data());
-        if (!rc && gs) rc = launch_add(ctx, gs->ptr + gp.dst, d_scratch, sm.elems);
-      }
+    rc = gather_set_batch(ctx, plan, plan->grad_items, plan->grad_block_start, plan->grad_permutes, plan->grad_dev, base, ws, n,
+                          gr ? gr->ptr + done * ge : nullptr, ge, gs ? gs->ptr : nullptr, d_scratch);
   }
   if (rc) { cleanup(); return rc; }
   batch_free(ctx, &B);
@@ -2248,6 +2270,139 @@ int tncb_plan_hvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, c
   return TNCB_OK;
 }
 
+// Instance-batched forward over reverse.  Per pass of c instances on c workspace copies beside the plan's own: one launch
+// fills every copy's leaf block (the device payloads, and the staged block's runs between them at stride 0), the leaf
+// tangents, the forward levels, R and Ṙ out, seeds and seed tangents in, the backward levels, the gathers of G and Ġ
+// into rows and/or sums.  Every launch decision is the single-network one, so row i is bit-identical to set_leaves +
+// tncb_plan_hvp of instance i; passes run in stream order, so the sums are the left folds of the rows in instance order.
+int tncb_plan_hvp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t count, size_t n, const uint64_t* leaf_index,
+                        const void* const* src, const uint64_t* instance_stride, const tncb_tensor* tangents,
+                        const tncb_tensor* seeds, const tncb_tensor* seed_tangents, tncb_tensor** values,
+                        tncb_tensor** tangent_rows, tncb_tensor** grad_rows, tncb_tensor** grad_sum,
+                        tncb_tensor** grad_tangent_rows, tncb_tensor** grad_tangent_sum) {
+  using namespace tncb;
+  if (!ctx || !plan || (n && (!leaf_index || !src || !instance_stride))) return fail(TNCB_ERR_INVALID, "null argument");
+  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
+  if (!plan->hvp) return fail(TNCB_ERR_INVALID, "not a Hessian-vector plan (tncb_plan_create_hvp)");
+  if (count == 0) return fail(TNCB_ERR_INVALID, "count is 0");
+  const bool backward = grad_rows || grad_sum || grad_tangent_rows || grad_tangent_sum;
+  const uint64_t ge = plan->grad_elems;
+  int rc = jvp_args(plan, tangents, values || tangent_rows || backward, {(uint64_t)count, ge});
+  if (rc) return rc;
+  const Schedule& S = plan->S;
+  const SlotMeta& rm = S.slots[S.result_slot];
+  const int r = (int)rm.dims.size();
+  if (r + 1 > kMaxLegs) return fail(TNCB_ERR_INVALID, "a result of rank 64 leaves no room for the instance dimension");
+  std::vector<uint64_t> rdims(r + 1);
+  rdims[0] = count;
+  for (int i = 0; i < r; i++) rdims[i + 1] = rm.dims[i];
+  for (auto [t, what] : {std::pair<const tncb_tensor*, const char*>{seeds, "seeds"}, {seed_tangents, "seed tangents"}}) {
+    if (!t) continue;
+    bool same = t->rank == r + 1;
+    for (int i = 0; same && i <= r; i++) same = t->dims[i] == rdims[i];
+    if (!same) return fail(TNCB_ERR_SHAPE, std::string("the ") + what + "' dims differ from [count, result dims]");
+    if (!t->ptr) return fail(TNCB_ERR_UNCONTRACTED, std::string("the ") + what + " tensor has no storage");
+  }
+  if (!seeds && r > 0) return fail(TNCB_ERR_INVALID, "seeds are needed for a result of rank " + std::to_string(r));
+  if (plan->ctx != ctx || !plan->leaves_resident) return fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this plan and context");
+  TNCB_CUDA(cudaSetDevice(ctx->device));
+  std::vector<LeafStageItem> dev_items;
+  if ((rc = device_items(ctx, S, count, n, leaf_index, src, instance_stride, dev_items))) return rc;
+  const size_t block = std::max<size_t>(S.leaf_block_elems, 1);
+  const double2* staged = (const double2*)((const char*)plan->ws + plan->leaf_off);
+  const std::vector<LeafRun> runs = leaf_runs(dev_items, (long long)block);
+  BatchBlock B;
+  if ((rc = batch_size(ctx, plan, count, &B))) return rc;
+  tncb_tensor *v = nullptr, *t = nullptr, *gr = nullptr, *gs = nullptr, *dgr = nullptr, *dgs = nullptr;
+  void* aux = nullptr;                 // the seed 1 of every copy (scalar result, NULL seeds), the K3 scratch of the sums
+  size_t aux_bytes = 0;
+  auto cleanup = [&]() {
+    batch_free(ctx, &B);
+    if (aux) ctx->arena.free(aux, aux_bytes);
+    for (tncb_tensor* x : {v, t, gr, gs, dgr, dgs}) if (x) tncb_tensor_free(ctx, x);
+  };
+  const uint64_t row_dims[2] = {(uint64_t)count, ge};
+  if (values) rc = tensor_new(ctx, r + 1, rdims.data(), &v);
+  if (!rc && tangent_rows) rc = tensor_new(ctx, r + 1, rdims.data(), &t);
+  if (!rc && grad_rows) rc = tensor_new(ctx, 2, row_dims, &gr);
+  if (!rc && grad_sum) rc = tensor_new(ctx, 1, &ge, &gs);
+  if (!rc && grad_tangent_rows) rc = tensor_new(ctx, 2, row_dims, &dgr);
+  if (!rc && grad_tangent_sum) rc = tensor_new(ctx, 1, &ge, &dgs);
+  if (!rc) rc = batch_alloc(ctx, &B);
+  const size_t ws = B.ws, c = B.c;
+  const size_t ones = backward && !seeds ? c : 0;
+  size_t scratch = 0;
+  if (grad_sum) for (const auto& gp : plan->grad_permutes) scratch = std::max<size_t>(scratch, S.slots[gp.slot].elems);
+  if (grad_tangent_sum) for (const auto& gp : plan->dgrad_permutes) scratch = std::max<size_t>(scratch, S.slots[gp.slot].elems);
+  if (!rc && (ones || scratch)) {
+    aux_bytes = (ones + scratch) * sizeof(double2);
+    rc = ctx->arena.alloc(aux_bytes, &aux);
+    if (!rc && ones) {
+      const std::vector<double2> one(ones, double2{1.0, 0.0});
+      cudaError_t e = cudaMemcpyAsync(aux, one.data(), ones * sizeof(double2), cudaMemcpyHostToDevice, ctx->stream);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);      // `one` dies with this scope
+      if (e != cudaSuccess) rc = fail(TNCB_ERR_CUDA, std::string("seed copy: ") + cudaGetErrorString(e));
+    }
+  }
+  for (tncb_tensor* x : {gs, dgs}) {
+    if (rc || !x) continue;
+    cudaError_t e = cudaMemsetAsync(x->ptr, 0, std::max<uint64_t>(ge, 1) * sizeof(double2), ctx->stream);
+    if (e != cudaSuccess) rc = fail(TNCB_ERR_CUDA, std::string("gradient sum: ") + cudaGetErrorString(e));
+  }
+  if (rc) { cleanup(); return rc; }
+  char* base = (char*)B.blk;
+  const double2* d_one = (const double2*)aux;
+  double2* d_scratch = (double2*)aux + ones;
+  const size_t res_bytes = rm.elems * sizeof(double2);
+  const int n_levels = (int)plan->level_batched.size();
+  std::vector<LeafStageItem> items;
+  for (size_t done = 0; done < count && !rc; done += c) {
+    const size_t m = std::min(c, count - done);
+    // every copy's leaf block: the device payloads of instances done .. done+m-1, the staged block between them
+    items.clear();
+    for (const LeafStageItem& it : dev_items) items.push_back({it.src + done * it.src_stride, it.src_stride, it.dst, it.elems});
+    for (const LeafRun& lr : runs) items.push_back({staged + lr.start, 0, lr.start, lr.len});
+    if ((rc = launch_leaf_stage(ctx, items.data(), items.size(), (double2*)(base + plan->leaf_off), (long long)(ws / sizeof(double2)), m))) break;
+    if ((rc = stage_tangents(ctx, plan, tangents->ptr + done * ge, ge, base, (long long)ws, m))) break;
+    if ((rc = enqueue_static(ctx, plan, base, (int)m, (long long)ws, 0, plan->n_fwd_levels))) break;
+    if (v && res_bytes &&
+        (rc = batch_copy(ctx, B, (char*)v->ptr + done * res_bytes, res_bytes, base + plan->slot_off[S.result_slot], ws, res_bytes, m))) break;
+    if (t && res_bytes &&
+        (rc = batch_copy(ctx, B, (char*)t->ptr + done * res_bytes, res_bytes, base + plan->slot_off[plan->tan_result], ws, res_bytes, m))) break;
+    if (!backward) continue;
+    // the seed slots may reuse memory the forward levels freed: written after them, on the stream
+    char* seed_dst = base + plan->slot_off[plan->seed_slot];
+    char* seed_tan_dst = base + plan->slot_off[plan->seed_tan_slot];
+    if (seeds) { if (res_bytes && (rc = batch_copy(ctx, B, seed_dst, ws, (const char*)seeds->ptr + done * res_bytes, res_bytes, res_bytes, m))) break; }
+    else if ((rc = batch_copy(ctx, B, seed_dst, ws, (const char*)d_one, sizeof(double2), sizeof(double2), m))) break;
+    if (seed_tangents) {
+      if (res_bytes && (rc = batch_copy(ctx, B, seed_tan_dst, ws, (const char*)seed_tangents->ptr + done * res_bytes, res_bytes, res_bytes, m))) break;
+    } else if (res_bytes) {
+      cudaError_t e = cudaSuccess;
+      if (B.strided) e = cudaMemset2DAsync(seed_tan_dst, ws, 0, res_bytes, m, ctx->stream);
+      else for (size_t i = 0; i < m && e == cudaSuccess; i++) e = cudaMemsetAsync(seed_tan_dst + i * ws, 0, res_bytes, ctx->stream);
+      if (e != cudaSuccess) { rc = fail(TNCB_ERR_CUDA, std::string("seed tangent: ") + cudaGetErrorString(e)); break; }
+    }
+    if ((rc = enqueue_static(ctx, plan, base, (int)m, (long long)ws, plan->n_fwd_levels, n_levels))) break;
+    if ((gr || gs) &&
+        (rc = gather_set_batch(ctx, plan, plan->grad_items, plan->grad_block_start, plan->grad_permutes, plan->grad_dev, base, ws, m,
+                               gr ? gr->ptr + done * ge : nullptr, ge, gs ? gs->ptr : nullptr, d_scratch))) break;
+    if (dgr || dgs)
+      rc = gather_set_batch(ctx, plan, plan->dgrad_items, plan->dgrad_block_start, plan->dgrad_permutes, plan->dgrad_dev, base, ws, m,
+                            dgr ? dgr->ptr + done * ge : nullptr, ge, dgs ? dgs->ptr : nullptr, d_scratch);
+  }
+  if (rc) { cleanup(); return rc; }
+  batch_free(ctx, &B);
+  if (aux) ctx->arena.free(aux, aux_bytes);
+  if (values) *values = v;
+  if (tangent_rows) *tangent_rows = t;
+  if (grad_rows) *grad_rows = gr;
+  if (grad_sum) *grad_sum = gs;
+  if (grad_tangent_rows) *grad_tangent_rows = dgr;
+  if (grad_tangent_sum) *grad_tangent_sum = dgs;
+  return TNCB_OK;
+}
+
 namespace tncb {
 // tncb_plan_jvp_sliced / tncb_plan_hvp_sliced: the arguments, the outputs (any may be NULL), one run_sliced
 static int sliced_tangent_call(tncb_ctx* ctx, tncb_plan* plan, bool hvp, size_t first, size_t stride, const tncb_tensor* tangents,
@@ -2363,17 +2518,8 @@ int tncb_plan_stage_instances(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tmp
   const size_t block = std::max<size_t>(S.leaf_block_elems, 1);
   size_t bytes = 0;
   if (__builtin_mul_overflow(n_instances, block * sizeof(double2), &bytes)) return fail(TNCB_ERR_OOM, "the instances' leaf blocks overflow 64 bits");
-  // the runs of the leaf block between the device payloads come from the template: run r covers block elements
-  // [start, start + len) and sits at `packed` in the packed template
-  struct Run { long long start, len, packed; };
-  std::vector<Run> runs;
-  std::sort(items.begin(), items.end(), [](const LeafStageItem& x, const LeafStageItem& y) { return x.dst < y.dst; });
-  {
-    long long pos = 0, packed = 0;
-    auto gap = [&](long long end) { if (end > pos) { runs.push_back({pos, end - pos, packed}); packed += end - pos; } };
-    for (const LeafStageItem& it : items) { gap(it.dst); pos = std::max(pos, it.dst + it.elems); }
-    gap((long long)block);
-  }
+  // the runs of the leaf block between the device payloads come from the template, packed
+  const std::vector<LeafRun> runs = leaf_runs(items, (long long)block);
   if ((rc = plan_device_state(ctx, plan, !plan->grad && !plan->tangent))) return rc;
   if (!plan->tmpl_host) {
     plan->tmpl_bytes = block * sizeof(double2);
@@ -2390,7 +2536,7 @@ int tncb_plan_stage_instances(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tmp
   for (size_t li = 0; li < leaves.size(); li++) {
     if (device_leaf[li] || S.leaf_kind[li] == TNCB_DATA_UNCONTRACTED) continue;
     const long long off = (long long)S.leaf_offset[li];
-    const Run& r = *(std::upper_bound(runs.begin(), runs.end(), off, [](long long o, const Run& x) { return o < x.start; }) - 1);
+    const LeafRun& r = *(std::upper_bound(runs.begin(), runs.end(), off, [](long long o, const LeafRun& x) { return o < x.start; }) - 1);
     if ((rc = stage_leaf(leaves[li], host + r.packed + (off - r.start)))) return rc;
   }
   void* blk = nullptr;
@@ -2402,7 +2548,7 @@ int tncb_plan_stage_instances(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tmp
     if (e != cudaSuccess) { ctx->arena.free(blk, bytes); return fail(TNCB_ERR_CUDA, std::string("template upload: ") + cudaGetErrorString(e)); }
     plan->tmpl_busy = true;
   }
-  for (const Run& r : runs) items.push_back({(const double2*)plan->tmpl_dev + r.packed, 0, r.start, r.len});
+  for (const LeafRun& r : runs) items.push_back({(const double2*)plan->tmpl_dev + r.packed, 0, r.start, r.len});
   if ((rc = launch_leaf_stage(ctx, items.data(), items.size(), (double2*)blk, (long long)block, n_instances))) {
     ctx->arena.free(blk, bytes);
     return rc;

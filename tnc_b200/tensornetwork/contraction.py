@@ -439,6 +439,81 @@ class NetworkPlan:
                 grad_tangents[i] = dg[off:off + size].reshape(shape)
         return value, tangent, grads, grad_tangents
 
+    def _rows_input(self, x, shape, what: str):
+        """(DeviceTensor, temporary to free) for an array, a torch CUDA tensor or a DeviceTensor shaped `shape`; an array
+        or torch tensor of another shape raises ValueError before anything reaches the device (a DeviceTensor is checked
+        by the library)"""
+        if x is None or isinstance(x, DeviceTensor):
+            return x, None
+        on_device = type(x).__module__.split(".")[0] == "torch"
+        if not on_device:
+            x = np.asarray(x, dtype=np.complex128)
+        if tuple(x.shape) != tuple(shape):
+            raise ValueError(f"the {what} have shape {tuple(x.shape)}, expected {tuple(shape)}")
+        t = DeviceTensor.from_torch(self.ctx, x) if on_device else DeviceTensor.from_numpy(self.ctx, x)
+        return t, t
+
+    def hvp_batch_blocks(self, count: int, tangents, seeds=None, seed_tangents=None, payloads: Optional[dict] = None,
+                         outputs=(True,) * 6):
+        """`count` forward-over-reverse passes in one walk over the levels (tncb_plan_hvp_batch), left on the device:
+        [values, tangent_rows, grad_rows, grad_sum, grad_tangent_rows, grad_tangent_sum] as DeviceTensors, None where
+        `outputs` is False.  Values and tangent rows are [count, *result dims] (R, Ṙ), the G / Ġ rows [count, grad_elems]
+        at grad_offsets(), the sums [grad_elems] (the left fold of the rows in instance order).
+        Instance i is the staged network, with payloads = {leaf: torch CUDA tensor [count, *leaf shape] (row i for
+        instance i) or [*leaf shape] (shared)} replacing leaves from device memory.
+        tangents: {leaf: [count, *leaf shape] or [*leaf shape]} as jvp_batch takes them, or an already packed
+        [count, grad_elems] array, torch CUDA tensor or DeviceTensor (a Hessian block: np.eye(grad_elems)[rows]).
+        seeds / seed_tangents: [count, *result dims] array, torch CUDA tensor or DeviceTensor; seeds None for a scalar
+        result (every seed 1), seed_tangents None = zero.  Row i equals set_leaves(instance i's payloads) + hvp(tangent
+        row i, seed i, seed tangent i) bit for bit; the plan's staged leaves are left as they are."""
+        count = int(count)
+        offs = self.grad_offsets()
+        te = sum(int(np.prod(s, dtype=np.int64)) for off, s in zip(offs, self.leaf_shapes) if off >= 0)
+        rdims = (count,) + tuple(self.result_dims)
+        tmp = []
+        try:
+            if isinstance(tangents, dict):
+                block = self._tangent_block(tangents, count)
+                tmp.append(block)
+            else:
+                block, t = self._rows_input(tangents, (count, te), "tangents")
+                tmp.append(t)
+            s, t = self._rows_input(seeds, rdims, "seeds")
+            tmp.append(t)
+            ds, t = self._rows_input(seed_tangents, rdims, "seed tangents")
+            tmp.append(t)
+            idx, ptrs, strides, keep = _device_sources(self.ctx, self.leaf_shapes, payloads, count) if payloads else ([], [], [], [])
+            c_ptrs = (C.c_void_p * max(len(ptrs), 1))(*ptrs)
+            outs = [C.c_void_p() if want else None for want in outputs]
+            h = lambda x: x.handle if x is not None else None
+            call = lambda: self.ctx._l.tncb_plan_hvp_batch(
+                self.ctx.handle, self.handle, count, len(idx), u64_array(idx), c_ptrs, u64_array(strides), h(block), h(s), h(ds),
+                *[C.byref(o) if o is not None else None for o in outs])
+            if keep:
+                _call_after_torch(self.ctx, keep, call)
+            else:
+                check(call())
+        finally:
+            for t in tmp:
+                if t is not None:
+                    t.free()
+        return [None if o is None else DeviceTensor.adopt(self.ctx, o) for o in outs]
+
+    def hvp_batch(self, count: int, tangents, seeds=None, seed_tangents=None, payloads: Optional[dict] = None,
+                  outputs=(True,) * 6):
+        """`hvp_batch_blocks` downloaded: (legs of one instance, values [count, *dims], tangent rows [count, *dims],
+        {leaf: G rows [count, *leaf shape]}, {leaf: G sum}, {leaf: Ġ rows}, {leaf: Ġ sum}) as host arrays, None where
+        not requested."""
+        host = []
+        for dt in self.hvp_batch_blocks(count, tangents, seeds, seed_tangents, payloads, outputs):
+            host.append(None if dt is None else dt.to_numpy())
+            if dt is not None:
+                dt.free()
+        offs = self.grad_offsets()
+        rows, one = (int(count),), ()
+        return (list(self.result_legs), host[0], host[1], self._unpack(offs, host[2], rows), self._unpack(offs, host[3], one),
+                self._unpack(offs, host[4], rows), self._unpack(offs, host[5], one))
+
     def jvp_batch_blocks(self, first: int = 0, count: Optional[int] = None, tangents: Optional[dict] = None,
                          values: bool = True):
         """`jvp_batch` left on the device: [values [count, *dims] or None, tangents [count, *dims]] as DeviceTensors"""
@@ -518,17 +593,18 @@ class NetworkPlan:
             dt.free()
         vals, row_block, sum_block = host
         offs = self.grad_offsets()
+        return (list(self.result_legs), vals, self._unpack(offs, row_block, (int(count),)), self._unpack(offs, sum_block, ()))
 
-        def unpack(block, lead):
-            if block is None:
-                return None
-            out = {}
-            for i, (off, shape) in enumerate(zip(offs, self.leaf_shapes)):
-                if off >= 0:
-                    size = int(np.prod(shape, dtype=np.int64))
-                    out[i] = block[..., off:off + size].reshape(lead + tuple(shape))
-            return out
-        return (list(self.result_legs), vals, unpack(row_block, (int(count),)), unpack(sum_block, ()))
+    def _unpack(self, offs, block, lead):
+        """{leaf: lead + leaf shape} views of a host block [*lead, grad_elems] at the offsets `offs`; None stays None"""
+        if block is None:
+            return None
+        out = {}
+        for i, (off, shape) in enumerate(zip(offs, self.leaf_shapes)):
+            if off >= 0:
+                size = int(np.prod(shape, dtype=np.int64))
+                out[i] = block[..., off:off + size].reshape(lead + tuple(shape))
+        return out
 
     def vjp_batch_blocks(self, first: int = 0, count: Optional[int] = None, seeds=None, rows: bool = True,
                          sum: bool = False, values: bool = True):
