@@ -265,7 +265,28 @@ int tncb_network_out_legs(const tncb_tn* tn, const tncb_path* path, int* n_out, 
 
 /* Compile once / execute many: the same circuit with different payloads
  * (e.g. other bitstrings or angles) re-uses the schedule, arena layout and the
- * captured CUDA graph. */
+ * captured CUDA graph.
+ * A plan has one of seven kinds: plain (tncb_plan_create), vjp, jvp, hvp (tncb_plan_create_vjp / _jvp / _hvp) and sliced
+ * vjp, jvp, hvp (the _sliced creators).  Every call that takes a plan checks its kind first, right after its null
+ * checks: "." takes it; U (TNCB_ERR_UNSUPPORTED) and I (TNCB_ERR_INVALID) refuse it with a message that names the call
+ * that runs the plan, or the creator the call wants.  tncb_plan_info and tncb_plan_destroy take every kind.
+ *                        plain  vjp  jvp  hvp  sliced vjp  sliced jvp  sliced hvp
+ *   stage                  .     .    .    .       .           .           .
+ *   run, execute           .     .    U    U       U           U           U
+ *   stage_slices           .     U    U    U       U           U           U
+ *   run_slices             .     U    U    U       .           .           .
+ *   run_batch              .     U    U    U       U           U           U
+ *   vjp                    I     .    U    U       U           U           U
+ *   vjp_sliced             I     I    U    U       .           U           U
+ *   stage_batch            I     .    .    U       U           U           U
+ *   vjp_batch              I     .    U    U       U           U           U
+ *   jvp, jvp_batch         I     I    .    U       I           U           U
+ *   jvp_sliced             I     I    I    I       I           .           I
+ *   hvp, hvp_batch         I     I    I    .       I           U           U
+ *   hvp_sliced             I     I    I    I       I           I           .
+ *   stage_instances        .     .    .    U       U           U           U
+ *   set_leaves             .     .    .    .       .           U           U
+ *   grad_offsets           I     .    .    .       .           .           .          */
 int tncb_plan_create(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, tncb_plan** out);
 /* `tn` must have the structure the plan was compiled from: every leaf is re-validated (kind, rank,
  * dims, non-null payload, live device handle) -> TNCB_ERR_INVALID / TNCB_ERR_SHAPE /
@@ -322,9 +343,7 @@ int tncb_plan_create_vjp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path
  * seed: device tensor with the result's dims (else TNCB_ERR_SHAPE); NULL only for a rank-0 result (seed 1).
  * *grads: new rank-1 device tensor holding every requested G_l back to back (tncb_plan_grad_offsets).
  * TNCB_ERR_INVALID without such a forward run on the currently staged leaves, and for a second call after one (the
- * backward slots reuse freed forward memory).  tncb_plan_stage_slices / run_slices / run_batch on a gradient plan ->
- * TNCB_ERR_UNSUPPORTED; many networks of its structure go through tncb_plan_stage_batch / tncb_plan_vjp_batch.  Errors
- * leave the arena as they found it. */
+ * backward slots reuse freed forward memory).  Errors leave the arena as they found it. */
 int tncb_plan_vjp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* seed, tncb_tensor** grads);
 /* Element offset of each leaf's gradient inside *grads, -1 for leaves not requested (n_leaves entries); host only.
  * For a sliced gradient plan the offsets pack the FULL leaves' shapes; for a tangent plan they place each requested
@@ -345,9 +364,7 @@ int tncb_plan_grad_offsets(const tncb_plan* plan, int64_t* offsets);
  * Use: tncb_plan_stage(ctx, plan, full tn) validates against the full structure and uploads the full leaf block once
  * into a plan-owned block outside the workspace (re-staging replaces it); tncb_plan_run_slices(ctx, plan, first,
  * stride, ...) runs the forward levels of slices first, first+stride, ... and returns their sum, bit-identical to a
- * plain plan of the host-sliced networks staged with tncb_plan_stage_slices; tncb_plan_vjp_sliced adds the backward.
- * tncb_plan_run / tncb_plan_execute / tncb_plan_vjp / tncb_plan_stage_slices / tncb_plan_run_batch on such a plan ->
- * TNCB_ERR_UNSUPPORTED. */
+ * plain plan of the host-sliced networks staged with tncb_plan_stage_slices; tncb_plan_vjp_sliced adds the backward. */
 int tncb_plan_create_vjp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, size_t n_sliced,
                                 const uint64_t* sliced_legs, const uint8_t* wrt, tncb_plan** out);
 /* Per slice q = first, first+stride, ...: extract q's sub-blocks of the leaves that carry a sliced leg (one launch),
@@ -357,16 +374,14 @@ int tncb_plan_create_vjp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_pat
  * *value: new tensor, the sum of the slices' results, bit-identical to tncb_plan_run_slices(first, stride).
  * *grads: new rank-1 tensor, every requested full-shape G_l back to back (tncb_plan_grad_offsets).  An empty range
  * (more ranks than slices) gives zeros for both; partial ranges add up, so ranks of a multi-GPU job pass (rank, world)
- * and run tncb_comm_allreduce_sum on both tensors.  Not staged on this context / not a sliced gradient plan / stride 0
+ * and run tncb_comm_allreduce_sum on both tensors.  Not staged on this context / stride 0
  * -> TNCB_ERR_INVALID; seed errors as tncb_plan_vjp.  Errors leave the arena as they found it. */
 int tncb_plan_vjp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t stride, const tncb_tensor* seed,
                          tncb_tensor** value, tncb_tensor** grads);
 /* ---- batched gradients: many networks of one gradient plan's structure (sampled bitstrings, angle sets, input states)
  * Stage n networks of a (non-sliced) gradient plan's structure for tncb_plan_vjp_batch: every leaf validated and
  * materialised, one H2D; the structure-validation errors are those of tncb_plan_stage_slices.  The plan's own staged
- * leaves (tncb_plan_stage) and forward state are untouched.  Tangent plans take it as well (for tncb_plan_jvp_batch).
- * Not a gradient or tangent plan -> TNCB_ERR_INVALID (plain plans use tncb_plan_stage_slices); a sliced gradient plan -> TNCB_ERR_UNSUPPORTED.  tncb_plan_stage_slices / run_slices /
- * run_batch stay TNCB_ERR_UNSUPPORTED on gradient plans. */
+ * leaves (tncb_plan_stage) and forward state are untouched.  Tangent plans take it as well (for tncb_plan_jvp_batch). */
 int tncb_plan_stage_batch(tncb_ctx* ctx, tncb_plan* plan, size_t n, const tncb_tn* const* tns);
 /* Instances first .. first+count-1, each contracted forward and backward on its own with the instance as a grid
  * dimension of every kernel, in passes of as many workspace copies as fit (as tncb_plan_run_batch; a gradient workspace
@@ -380,9 +395,9 @@ int tncb_plan_stage_batch(tncb_ctx* ctx, tncb_plan* plan, size_t n, const tncb_t
  * grad_rows == grad_sum == NULL: forward levels only.  The plan's workspace, staged leaves and forward state are left
  * alone, so stage + run + tncb_plan_vjp_batch + tncb_plan_vjp works.  Ranks of a multi-GPU job may split [first, count)
  * and combine their grad_sum with tncb_comm_allreduce_sum.
- * Not a gradient plan, nothing staged by tncb_plan_stage_batch on this context, count == 0, a range past the staged
- * networks, every output NULL, NULL seeds for a non-scalar result with gradients requested, a result of rank 64 ->
- * TNCB_ERR_INVALID; a sliced gradient plan -> TNCB_ERR_UNSUPPORTED; seed dims other than [count, result dims] ->
+ * Nothing staged by tncb_plan_stage_batch on this context, count == 0, a range past the staged networks, every output
+ * NULL, NULL seeds for a non-scalar result with gradients requested, a result of rank 64 -> TNCB_ERR_INVALID; seed dims
+ * other than [count, result dims] ->
  * TNCB_ERR_SHAPE; not even one workspace copy fits -> TNCB_ERR_OOM.  Errors leave the arena as they found it. */
 int tncb_plan_vjp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t count, const tncb_tensor* seeds,
                         tncb_tensor** values, tncb_tensor** grad_rows, tncb_tensor** grad_sum);
@@ -409,8 +424,7 @@ int tncb_plan_set_leaves(tncb_ctx* ctx, tncb_plan* plan, size_t n, const uint64_
  * tncb_plan_stage_slices (feeds run_slices / run_batch; needs a static plan, else TNCB_ERR_UNSUPPORTED).  Gradient plans:
  * replaces tncb_plan_stage_batch (feeds vjp_batch; the plan's own workspace is not allocated); tangent plans likewise
  * (feeds jvp_batch).  Staged instances are
- * bit-identical to the host-staged networks with the same payloads.  n_instances == 0 -> TNCB_ERR_INVALID; a sliced
- * gradient plan -> TNCB_ERR_UNSUPPORTED (it uses tncb_plan_set_leaves). */
+ * bit-identical to the host-staged networks with the same payloads.  n_instances == 0 -> TNCB_ERR_INVALID. */
 int tncb_plan_stage_instances(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tmpl, size_t n_instances,
                               size_t n, const uint64_t* leaf_index, const void* const* src, const uint64_t* instance_stride);
 /* ---- directional derivatives with respect to the leaves (forward mode) ----
@@ -428,14 +442,13 @@ int tncb_plan_stage_instances(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tmp
  * TNCB_ERR_UNSUPPORTED: device leaves, networks without pairs, and a static workspace above the static-workspace limit
  * (TNCB_PLAN_WS_GB; the message states the bytes needed).  wrt selecting no leaf, or a leaf without a payload ->
  * TNCB_ERR_INVALID.  Tangent plans always run on their static layout, are never captured into a CUDA graph and have no
- * pair-by-pair fallback.  tncb_plan_run / execute / run_slices / run_batch / stage_slices / vjp / vjp_sliced /
- * vjp_batch on a tangent plan -> TNCB_ERR_UNSUPPORTED. */
+ * pair-by-pair fallback. */
 int tncb_plan_create_jvp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, const uint8_t* wrt, tncb_plan** out);
 /* One forward-mode pass on the leaves staged by tncb_plan_stage (and overwritten by tncb_plan_set_leaves).
  * tangents: [tangent_elems] device tensor (tangent_elems = the sum of the requested leaves' sizes).
  * *value: new tensor with the result's dims, bit-identical to a plain plan's tncb_plan_run on the same leaves.
  * *tangent_out: new tensor with the result's dims, Ṙ.  Either may be NULL, not both.  Each call is self-contained and
- * repeats bit for bit.  Not a tangent plan, not staged on this context, both outputs NULL, NULL tangents ->
+ * repeats bit for bit.  Not staged on this context, both outputs NULL, NULL tangents ->
  * TNCB_ERR_INVALID; tangent dims other than [tangent_elems] -> TNCB_ERR_SHAPE.  Errors leave the arena as they found it. */
 int tncb_plan_jvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, tncb_tensor** value, tncb_tensor** tangent_out);
 /* Instances first .. first+count-1 staged by tncb_plan_stage_batch or tncb_plan_stage_instances, each with its own
@@ -445,7 +458,7 @@ int tncb_plan_jvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, t
  *   *tangent_rows: new [count, result dims..]; row i bit-identical to tncb_plan_jvp of instance i with tangent row i
  * Either output may be NULL, not both.  Many directions of one network: stage count instances of it with
  * tncb_plan_stage_instances (every device source at stride 0, or the host template alone) and pass one tangent row per
- * direction.  Not a tangent plan, nothing staged on this context, count == 0, a range past the staged networks, both
+ * direction.  Nothing staged on this context, count == 0, a range past the staged networks, both
  * outputs NULL, NULL tangents, a result of rank 64 -> TNCB_ERR_INVALID; tangent dims other than [count, tangent_elems]
  * -> TNCB_ERR_SHAPE; not even one workspace copy fits -> TNCB_ERR_OOM.  Errors leave the arena as they found it. */
 int tncb_plan_jvp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t count, const tncb_tensor* tangents,
@@ -464,8 +477,7 @@ int tncb_plan_jvp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
  * the same engines and backward level, summed in that order when both exist.  Cost: about nine forward passes with
  * every leaf requested, in one walk over the levels.  Arguments and refusals as tncb_plan_create_jvp (the message of
  * a workspace above the limit states the bytes needed); ctx may be NULL (host-only compile: tncb_plan_info and
- * tncb_plan_grad_offsets).  Always static, never graphed, no pair-by-pair fallback.  Every other plan entry point but
- * tncb_plan_stage / set_leaves / hvp_batch / info / grad_offsets -> TNCB_ERR_UNSUPPORTED on a Hessian-vector plan. */
+ * tncb_plan_grad_offsets).  Always static, never graphed, no pair-by-pair fallback. */
 int tncb_plan_create_hvp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, const uint8_t* wrt, tncb_plan** out);
 /* One forward-over-reverse pass on the leaves staged by tncb_plan_stage (and overwritten by tncb_plan_set_leaves).
  * tangents:     [tangent_elems] device tensor at tncb_plan_grad_offsets (the gradient block's layout)
@@ -475,8 +487,8 @@ int tncb_plan_create_hvp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path
  *   (bit-identical to tncb_plan_jvp with the same tangents)
  * *grads, *grad_tangents: new [tangent_elems] tensors at tncb_plan_grad_offsets, G (bit-identical to tncb_plan_vjp(seed)
  *   of a gradient plan after a run) and Ġ
- * Each output may be NULL, not all four.  Each call is self-contained and repeats bit for bit.  Not a Hessian-vector
- * plan, not staged on this context, no output, NULL tangents, a NULL seed for a result of rank > 0 ->
+ * Each output may be NULL, not all four.  Each call is self-contained and repeats bit for bit.  Not staged on this
+ * context, no output, NULL tangents, a NULL seed for a result of rank > 0 ->
  * TNCB_ERR_INVALID; tangent, seed or seed-tangent dims that do not match -> TNCB_ERR_SHAPE.  Errors leave the arena as
  * they found it. */
 int tncb_plan_hvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, const tncb_tensor* seed,
@@ -498,9 +510,8 @@ int tncb_plan_hvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, c
  * of every output is bit-identical to tncb_plan_set_leaves(instance i's payloads) + tncb_plan_hvp(tangent row i, seed
  * i, seed tangent i): every launch decision is the single-network one, and int8-engine steps run instance by instance.
  * The plan's staged leaves and workspace are left as they are, so tncb_plan_hvp before and after gives the same bits.
- * The sums can be combined across ranks with tncb_comm_allreduce_sum.  Not a Hessian-vector plan, not staged on this
- * context, count == 0, no output, NULL tangents, a NULL seed for a result of rank > 0, a result of rank 64 ->
- * TNCB_ERR_INVALID; a sliced Hessian-vector or tangent plan -> TNCB_ERR_UNSUPPORTED; device-source errors as
+ * The sums can be combined across ranks with tncb_comm_allreduce_sum.  Not staged on this context, count == 0, no output, NULL tangents, a NULL seed for a result of rank > 0, a result of rank 64 ->
+ * TNCB_ERR_INVALID; device-source errors as
  * tncb_plan_stage_instances; tangent, seed or seed-tangent dims that do not match -> TNCB_ERR_SHAPE; not even one
  * workspace copy fits beside the plan's -> TNCB_ERR_OOM.  Errors leave the arena and the staged plan as they found them. */
 int tncb_plan_hvp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t count, size_t n, const uint64_t* leaf_index,
@@ -518,10 +529,7 @@ int tncb_plan_hvp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t count, size_t n, 
  * peak_bytes is the per-slice workspace; a per-slice workspace above the static-workspace limit -> TNCB_ERR_UNSUPPORTED
  * naming the bytes.  tncb_plan_grad_offsets packs the FULL leaves' shapes, for the tangents, G and Ġ alike.
  * Use: tncb_plan_stage(ctx, plan, full tn) uploads the full leaves once; tncb_plan_run_slices runs the forward levels
- * (with zero tangents) and returns a sum bit-identical to the plain sliced run.  Every other entry point (run, execute,
- * stage_slices, run_batch, stage_batch, stage_instances, set_leaves, vjp, vjp_sliced, vjp_batch, jvp, jvp_batch, hvp,
- * hvp_batch)
- * -> TNCB_ERR_UNSUPPORTED naming the call that runs the plan. */
+ * (with zero tangents) and returns a sum bit-identical to the plain sliced run. */
 int tncb_plan_create_jvp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, size_t n_sliced,
                                 const uint64_t* sliced_legs, const uint8_t* wrt, tncb_plan** out);
 /* Per slice q = first, first+stride, ...: extract q's sub-blocks of the leaves that carry a sliced leg and of every
@@ -529,7 +537,7 @@ int tncb_plan_create_jvp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_pat
  * [tangent_elems] device tensor, every requested leaf's FULL-shape tangent at tncb_plan_grad_offsets.  *value (the
  * sum of R_q, bit-identical to tncb_plan_run_slices) and *tangent_out (the sum of Ṙ_q) are new tensors with the result's
  * dims; either may be NULL, not both.  An empty range (first >= slices) gives zeros; partial ranges add up, for ranks
- * that all-reduce.  Not a sliced tangent plan, not staged on this context, stride 0, no output, NULL tangents ->
+ * that all-reduce.  Not staged on this context, stride 0, no output, NULL tangents ->
  * TNCB_ERR_INVALID; tangent dims other than [tangent_elems] -> TNCB_ERR_SHAPE.  Errors leave the arena as they found it. */
 int tncb_plan_jvp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t stride, const tncb_tensor* tangents,
                          tncb_tensor** value, tncb_tensor** tangent_out);
@@ -540,8 +548,7 @@ int tncb_plan_create_hvp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_pat
  * tangents) that need more than 8 leg groups, and the accumulation of G_l and then Ġ_l into q's sub-blocks of the
  * full-shape [tangent_elems] blocks *grads and *grad_tangents (zeroed once per call).  The same seed and seed tangent
  * serve every slice.  Each output may be NULL, not all four; the backward levels run only if *grads or *grad_tangents
- * is wanted.  Errors as tncb_plan_jvp_sliced, seed errors as tncb_plan_hvp; not a sliced Hessian-vector plan ->
- * TNCB_ERR_INVALID. */
+ * is wanted.  Errors as tncb_plan_jvp_sliced, seed errors as tncb_plan_hvp. */
 int tncb_plan_hvp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t stride, const tncb_tensor* tangents,
                          const tncb_tensor* seed, const tncb_tensor* seed_tangent, tncb_tensor** value,
                          tncb_tensor** tangent_out, tncb_tensor** grads, tncb_tensor** grad_tangents);

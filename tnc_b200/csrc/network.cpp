@@ -328,9 +328,16 @@ struct tncb_plan {
   size_t resident_bytes = 0;
   void* slices_dev = nullptr;        // tncb_plan_stage_slices: n_slices leaf blocks, back to back
   size_t n_slices = 0, slices_bytes = 0;
+  // the plan kind (tncb_plan_create / _vjp / _jvp / _hvp), sliced or not (the _sliced creators; never plain).  Only the
+  // routing table asks which kind a plan is; everything else asks what it has: backward levels and leaf adjoints
+  // (grad), tangent pairs (tangent)
+  enum class Kind { plain, vjp, jvp, hvp };
+  Kind kind = Kind::plain;
+  bool sliced = false;
+  bool grad() const { return kind == Kind::vjp || kind == Kind::hvp; }
+  bool tangent() const { return kind == Kind::jvp || kind == Kind::hvp; }
   // gradient plans (tncb_plan_create_vjp): the backward pairs follow the forward ones in S.steps and occupy the levels
   // from n_fwd_levels on; always static, never graphed
-  bool grad = false;
   int n_fwd_levels = 0;              // levels [0, n_fwd_levels) are the forward pass (all levels of a plain plan)
   int seed_slot = -1;
   std::vector<int64_t> grad_offset;  // per leaf (collect order): element offset in the gradient block, -1 = not requested
@@ -343,7 +350,6 @@ struct tncb_plan {
   bool fwd_ready = false;            // a forward run left its state in the workspace for one tncb_plan_vjp
   // sliced gradient plans (tncb_plan_create_vjp_sliced): S is the structure of one slice, `full` holds the full
   // network's leaves; tncb_plan_stage uploads the full leaf block once and every slice is extracted from it on the device
-  bool sliced = false;
   uint64_t n_sl = 1;                                // slices: the product of the sliced legs' dims
   tncb::Schedule full;                              // leaves only: kinds, dims, offsets in the full leaf block
   std::vector<tncb::SliceItem> sl_items, const_items, acc_items;   // extract (leaves with / without a sliced leg), accumulate
@@ -364,7 +370,6 @@ struct tncb_plan {
   bool tmpl_busy = false;
   // tangent plans (tncb_plan_create_jvp): the tangent pairs follow the forward ones in S.steps, each on its forward
   // step's level; grad_offset / grad_elems give the packing of the leaf tangents.  Always static, never graphed.
-  bool tangent = false;
   int tan_result = -1;                              // the slot of the result's tangent
   struct TanLeaf { int slot; int64_t off; };        // a requested leaf's tangent slot and its offset in a tangent row
   std::vector<TanLeaf> tan_leaves;
@@ -378,7 +383,6 @@ struct tncb_plan {
   // Hessian-vector plans (tncb_plan_create_hvp) are gradient and tangent plans at once: S.steps holds the forward,
   // tangent, backward and backward-tangent pairs; tan_sums holds the sums of both tangent passes.  grad_* gathers the
   // leaf adjoints (G), dgrad_* their tangents (Ġ), both at grad_offset.
-  bool hvp = false;
   int seed_tan_slot = -1;                           // Ṡ, written (or zeroed) by tncb_plan_hvp before the backward levels
   std::vector<tncb::GradItem> dgrad_items;
   std::vector<long long> dgrad_block_start;
@@ -421,14 +425,68 @@ static size_t static_ws_limit(size_t device_bytes) {
   return limit;
 }
 
-// what every plan entry point but tncb_plan_stage / set_leaves / hvp / info / grad_offsets answers a Hessian-vector plan
-static int hvp_refused() { return fail(TNCB_ERR_UNSUPPORTED, "a Hessian-vector plan runs through tncb_plan_hvp"); }
+// the size of ctx's device (0: no context, or the device does not answer), which scales the static-workspace limit
+static size_t device_bytes(tncb_ctx* ctx) {
+  size_t dev_free = 0, dev_total = 0;
+  if (ctx) { cudaSetDevice(ctx->device); if (cudaMemGetInfo(&dev_free, &dev_total) != cudaSuccess) { dev_total = 0; cudaGetLastError(); } }
+  return dev_total;
+}
 
-// a sliced tangent / Hessian-vector plan (tncb_plan_create_jvp_sliced / _hvp_sliced) runs through its own call only
-static bool sliced_tangent(const tncb_plan* P) { return P->sliced && P->tangent; }
-static int sliced_tangent_refused(const tncb_plan* P) {
-  return fail(TNCB_ERR_UNSUPPORTED, P->hvp ? "a sliced Hessian-vector plan runs through tncb_plan_hvp_sliced / tncb_plan_run_slices"
-                                           : "a sliced tangent plan runs through tncb_plan_jvp_sliced / tncb_plan_run_slices");
+// ---- which call takes which plan kind (the table in tncb.h) ----
+// The calls that take a plan, in the order of kRoutes' rows
+enum class Call { stage, run, execute, stage_slices, run_slices, run_batch, vjp, vjp_sliced, stage_batch, vjp_batch, jvp,
+                  jvp_batch, jvp_sliced, hvp, hvp_batch, hvp_sliced, stage_instances, set_leaves, grad_offsets, count };
+struct Refusal { int status; const char* msg; };
+static const Refusal
+    kHvpRuns{TNCB_ERR_UNSUPPORTED, "a Hessian-vector plan runs through tncb_plan_hvp"},
+    kSlJvpRuns{TNCB_ERR_UNSUPPORTED, "a sliced tangent plan runs through tncb_plan_jvp_sliced / tncb_plan_run_slices"},
+    kSlHvpRuns{TNCB_ERR_UNSUPPORTED, "a sliced Hessian-vector plan runs through tncb_plan_hvp_sliced / tncb_plan_run_slices"},
+    kSlVjpRuns{TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_run_slices / tncb_plan_vjp_sliced"},
+    kSlVjpGrads{TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_vjp_sliced"},
+    kSlVjpStage{TNCB_ERR_UNSUPPORTED, "a sliced gradient plan stages its full network once (tncb_plan_stage)"},
+    kSlVjpNoBatch{TNCB_ERR_UNSUPPORTED, "a sliced gradient plan has no batched gradients"},
+    kSlVjpLeaves{TNCB_ERR_UNSUPPORTED, "a sliced gradient plan takes device payloads through tncb_plan_set_leaves"},
+    kVjpOne{TNCB_ERR_UNSUPPORTED, "gradient plans run one staged network at a time"},
+    kJvpRuns{TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp"},
+    kJvpBatch{TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp_batch"},
+    kJvpEither{TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp / tncb_plan_jvp_batch"},
+    kJvpStage{TNCB_ERR_UNSUPPORTED, "tangent plans stage many networks with tncb_plan_stage_batch"},
+    kNotVjp{TNCB_ERR_INVALID, "not a gradient plan (tncb_plan_create_vjp)"},
+    kNotJvp{TNCB_ERR_INVALID, "not a tangent plan (tncb_plan_create_jvp)"},
+    kNotHvp{TNCB_ERR_INVALID, "not a Hessian-vector plan (tncb_plan_create_hvp)"},
+    kNotSlVjp{TNCB_ERR_INVALID, "not a sliced gradient plan (tncb_plan_create_vjp_sliced)"},
+    kNotSlJvp{TNCB_ERR_INVALID, "not a sliced tangent plan (tncb_plan_create_jvp_sliced)"},
+    kNotSlHvp{TNCB_ERR_INVALID, "not a sliced Hessian-vector plan (tncb_plan_create_hvp_sliced)"},
+    kNotDerivStage{TNCB_ERR_INVALID, "not a gradient or tangent plan (plain plans stage many networks with tncb_plan_stage_slices)"},
+    kNotDeriv{TNCB_ERR_INVALID, "not a gradient or tangent plan (tncb_plan_create_vjp / _jvp)"};
+static const Refusal* const kTakes = nullptr;
+static const Refusal* const kRoutes[(int)Call::count][7] = {
+  //                    plain            vjp             jvp           hvp          sliced vjp      sliced jvp    sliced hvp
+  /* stage */           {kTakes,          kTakes,         kTakes,       kTakes,      kTakes,         kTakes,       kTakes},
+  /* run */             {kTakes,          kTakes,         &kJvpRuns,    &kHvpRuns,   &kSlVjpRuns,    &kSlJvpRuns,  &kSlHvpRuns},
+  /* execute */         {kTakes,          kTakes,         &kJvpRuns,    &kHvpRuns,   &kSlVjpRuns,    &kSlJvpRuns,  &kSlHvpRuns},
+  /* stage_slices */    {kTakes,          &kVjpOne,       &kJvpStage,   &kHvpRuns,   &kSlVjpStage,   &kSlJvpRuns,  &kSlHvpRuns},
+  /* run_slices */      {kTakes,          &kVjpOne,       &kJvpEither,  &kHvpRuns,   kTakes,         kTakes,       kTakes},
+  /* run_batch */       {kTakes,          &kVjpOne,       &kJvpBatch,   &kHvpRuns,   &kSlVjpRuns,    &kSlJvpRuns,  &kSlHvpRuns},
+  /* vjp */             {&kNotVjp,        kTakes,         &kJvpRuns,    &kHvpRuns,   &kSlVjpGrads,   &kSlJvpRuns,  &kSlHvpRuns},
+  /* vjp_sliced */      {&kNotSlVjp,      &kNotSlVjp,     &kJvpRuns,    &kHvpRuns,   kTakes,         &kSlJvpRuns,  &kSlHvpRuns},
+  /* stage_batch */     {&kNotDerivStage, kTakes,         kTakes,       &kHvpRuns,   &kSlVjpNoBatch, &kSlJvpRuns,  &kSlHvpRuns},
+  /* vjp_batch */       {&kNotVjp,        kTakes,         &kJvpBatch,   &kHvpRuns,   &kSlVjpNoBatch, &kSlJvpRuns,  &kSlHvpRuns},
+  /* jvp */             {&kNotJvp,        &kNotJvp,       kTakes,       &kHvpRuns,   &kNotJvp,       &kSlJvpRuns,  &kSlHvpRuns},
+  /* jvp_batch */       {&kNotJvp,        &kNotJvp,       kTakes,       &kHvpRuns,   &kNotJvp,       &kSlJvpRuns,  &kSlHvpRuns},
+  /* jvp_sliced */      {&kNotSlJvp,      &kNotSlJvp,     &kNotSlJvp,   &kNotSlJvp,  &kNotSlJvp,     kTakes,       &kNotSlJvp},
+  /* hvp */             {&kNotHvp,        &kNotHvp,       &kNotHvp,     kTakes,      &kNotHvp,       &kSlJvpRuns,  &kSlHvpRuns},
+  /* hvp_batch */       {&kNotHvp,        &kNotHvp,       &kNotHvp,     kTakes,      &kNotHvp,       &kSlJvpRuns,  &kSlHvpRuns},
+  /* hvp_sliced */      {&kNotSlHvp,      &kNotSlHvp,     &kNotSlHvp,   &kNotSlHvp,  &kNotSlHvp,     &kNotSlHvp,   kTakes},
+  /* stage_instances */ {kTakes,          kTakes,         kTakes,       &kHvpRuns,   &kSlVjpLeaves,  &kSlJvpRuns,  &kSlHvpRuns},
+  /* set_leaves */      {kTakes,          kTakes,         kTakes,       kTakes,      kTakes,         &kSlJvpRuns,  &kSlHvpRuns},
+  /* grad_offsets */    {&kNotDeriv,      kTakes,         kTakes,       kTakes,      kTakes,         kTakes,       kTakes},
+};
+
+// TNCB_OK if `c` takes P's kind, else the cell's refusal.  Every plan-taking call asks first, right after its null checks.
+static int route(const tncb_plan* P, Call c) {
+  const Refusal* r = kRoutes[(int)c][(int)P->kind + (P->sliced ? 3 : 0)];
+  return r ? fail(r->status, r->msg) : TNCB_OK;
 }
 
 // the item sets of a sliced plan, in their sl_dev order: extract of the leaves with / without a sliced leg, accumulate of
@@ -437,7 +495,7 @@ enum { kSlExtract, kSlConst, kSlAcc, kSlTan, kSlDacc, kSliceSets };
 
 static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) {
   Schedule& S = P->S;
-  P->is_static = !S.steps.empty() && (P->grad || P->tangent || std::getenv("TNCB_NO_STATIC") == nullptr);
+  P->is_static = !S.steps.empty() && (P->grad() || P->tangent() || std::getenv("TNCB_NO_STATIC") == nullptr);
   for (int k : S.leaf_kind) if (k == TNCB_DATA_DEVICE) P->is_static = false;   // addresses change per call
   if (!P->is_static) return;
   // ---- levels: a step's level is 1 + the deepest level among its operands' producers (leaves: 0); backward pairs
@@ -506,7 +564,7 @@ static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) 
     P->slot_off[tl.slot] = A.alloc(sz[tl.slot]);
   }
   for (int l = 0; l < n_levels; l++) {
-    if (P->grad && l == P->n_fwd_levels) {         // the seed, written by tncb_plan_vjp before the backward levels
+    if (P->grad() && l == P->n_fwd_levels) {       // the seed, written by tncb_plan_vjp before the backward levels
       sz[P->seed_slot] = std::max<size_t>(S.slots[P->seed_slot].elems * sizeof(double2), 16);
       P->slot_off[P->seed_slot] = A.alloc(sz[P->seed_slot]);
       if (P->seed_tan_slot >= 0) {                 // a Hessian-vector plan's seed tangent, written with the seed
@@ -548,7 +606,7 @@ static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) 
     }
     P->block_start.push_back(blocks);
   }
-  if (P->tangent) {
+  if (P->tangent()) {
     P->sum_first.assign(n_levels, 0); P->sum_count.assign(n_levels, 0); P->sum_bs_first.assign(n_levels, 0);
     for (int l = 0; l < n_levels; l++) {
       P->sum_first[l] = (int)P->sum_items.size(); P->sum_bs_first[l] = P->sum_bs.size();
@@ -565,7 +623,7 @@ static void plan_static_layout(tncb_plan* P, int sm_count, size_t device_bytes) 
       if (P->sum_count[l]) P->sum_bs.push_back(blocks);
     }
   }
-  P->graphable = !P->grad && !P->tangent && std::getenv("TNCB_NO_GRAPH") == nullptr && P->ws_bytes <= ((size_t)1 << 30);   // graphs are for small networks
+  P->graphable = !P->grad() && !P->tangent() && std::getenv("TNCB_NO_GRAPH") == nullptr && P->ws_bytes <= ((size_t)1 << 30);   // graphs are for small networks
   for (const Step& st : S.steps) if (st.plan.kernel_class == 1) { P->graphable = false; break; }   // K1/K1' use ctx-owned tables / arena scratch
 }
 
@@ -593,6 +651,20 @@ static int stage_leaves(const Schedule& S, const std::vector<const tncb_tn*>& le
   return TNCB_OK;
 }
 
+// one descriptor set on the device, once: `items` followed by its block-count prefixes `bs`
+template <class Item, class Prefix>
+static int upload(tncb_ctx* ctx, const std::vector<Item>& items, const std::vector<Prefix>& bs, void** dev, size_t* bytes) {
+  if (*dev || items.empty()) return TNCB_OK;
+  const size_t ib = items.size() * sizeof(Item), bb = bs.size() * sizeof(Prefix);
+  int rc = ctx->arena.alloc(ib + bb, dev);
+  if (rc) return rc;
+  *bytes = ib + bb;
+  TNCB_CUDA(cudaMemcpyAsync(*dev, items.data(), ib, cudaMemcpyHostToDevice, ctx->stream));
+  TNCB_CUDA(cudaMemcpyAsync((char*)*dev + ib, bs.data(), bb, cudaMemcpyHostToDevice, ctx->stream));
+  TNCB_CUDA(cudaStreamSynchronize(ctx->stream));   // (pageable sources)
+  return TNCB_OK;
+}
+
 // workspace, pinned staging and the device copy of the batch descriptors (once per plan and context).  workspace =
 // false: the descriptors only (a gradient plan's batched pass runs on workspace copies of its own)
 static int plan_device_state(tncb_ctx* ctx, tncb_plan* P, bool workspace = true) {
@@ -602,38 +674,11 @@ static int plan_device_state(tncb_ctx* ctx, tncb_plan* P, bool workspace = true)
   if (workspace && !P->ws && (rc = ctx->arena.alloc(P->ws_bytes, &P->ws))) return rc;
   const size_t block_bytes = std::max<size_t>(P->S.leaf_block_elems * sizeof(double2), 16);
   if (workspace && !P->stage) TNCB_CUDA(cudaMallocHost(&P->stage, block_bytes));
-  if (!P->batch_dev && !P->items.empty()) {
-    const size_t ib = P->items.size() * sizeof(K0BatchItem), bb = P->block_start.size() * sizeof(int);
-    P->batch_bytes = ib + bb;
-    if ((rc = ctx->arena.alloc(P->batch_bytes, &P->batch_dev))) return rc;
-    TNCB_CUDA(cudaMemcpyAsync(P->batch_dev, P->items.data(), ib, cudaMemcpyHostToDevice, ctx->stream));
-    TNCB_CUDA(cudaMemcpyAsync((char*)P->batch_dev + ib, P->block_start.data(), bb, cudaMemcpyHostToDevice, ctx->stream));
-    TNCB_CUDA(cudaStreamSynchronize(ctx->stream));   // (pageable sources)
-  }
-  if (!P->grad_dev && !P->grad_items.empty()) {
-    const size_t ib = P->grad_items.size() * sizeof(GradItem), bb = P->grad_block_start.size() * sizeof(long long);
-    if ((rc = ctx->arena.alloc(ib + bb, &P->grad_dev))) return rc;
-    P->grad_dev_bytes = ib + bb;
-    TNCB_CUDA(cudaMemcpyAsync(P->grad_dev, P->grad_items.data(), ib, cudaMemcpyHostToDevice, ctx->stream));
-    TNCB_CUDA(cudaMemcpyAsync((char*)P->grad_dev + ib, P->grad_block_start.data(), bb, cudaMemcpyHostToDevice, ctx->stream));
-    TNCB_CUDA(cudaStreamSynchronize(ctx->stream));
-  }
-  if (!P->dgrad_dev && !P->dgrad_items.empty()) {
-    const size_t ib = P->dgrad_items.size() * sizeof(GradItem), bb = P->dgrad_block_start.size() * sizeof(long long);
-    if ((rc = ctx->arena.alloc(ib + bb, &P->dgrad_dev))) return rc;
-    P->dgrad_dev_bytes = ib + bb;
-    TNCB_CUDA(cudaMemcpyAsync(P->dgrad_dev, P->dgrad_items.data(), ib, cudaMemcpyHostToDevice, ctx->stream));
-    TNCB_CUDA(cudaMemcpyAsync((char*)P->dgrad_dev + ib, P->dgrad_block_start.data(), bb, cudaMemcpyHostToDevice, ctx->stream));
-    TNCB_CUDA(cudaStreamSynchronize(ctx->stream));
-  }
-  if (!P->sum_dev && !P->sum_items.empty()) {
-    const size_t ib = P->sum_items.size() * sizeof(TangentSumItem), bb = P->sum_bs.size() * sizeof(long long);
-    if ((rc = ctx->arena.alloc(ib + bb, &P->sum_dev))) return rc;
-    P->sum_dev_bytes = ib + bb;
-    TNCB_CUDA(cudaMemcpyAsync(P->sum_dev, P->sum_items.data(), ib, cudaMemcpyHostToDevice, ctx->stream));
-    TNCB_CUDA(cudaMemcpyAsync((char*)P->sum_dev + ib, P->sum_bs.data(), bb, cudaMemcpyHostToDevice, ctx->stream));
-    TNCB_CUDA(cudaStreamSynchronize(ctx->stream));
-  }
+  if ((rc = upload(ctx, P->items, P->block_start, &P->batch_dev, &P->batch_bytes)) ||
+      (rc = upload(ctx, P->grad_items, P->grad_block_start, &P->grad_dev, &P->grad_dev_bytes)) ||
+      (rc = upload(ctx, P->dgrad_items, P->dgrad_block_start, &P->dgrad_dev, &P->dgrad_dev_bytes)) ||
+      (rc = upload(ctx, P->sum_items, P->sum_bs, &P->sum_dev, &P->sum_dev_bytes)))
+    return rc;
   if (P->sliced && !P->sl_dev) {
     auto up16 = [](size_t b) { return (b + 15) / 16 * 16; };
     const std::vector<SliceItem>* iv[kSliceSets] = {&P->sl_items, &P->const_items, &P->acc_items, &P->tan_items, &P->dacc_items};
@@ -678,7 +723,7 @@ static int enqueue_static(tncb_ctx* ctx, tncb_plan* P, char* ws, int count, long
       rc = launch_pair(ctx, st.plan, (const double2*)(ws + P->slot_off[st.a]), (const double2*)(ws + P->slot_off[st.b]),
                        (double2*)(ws + P->slot_off[st.out]), count, stride);
     }
-    if (!rc && P->tangent && P->sum_count[l]) {    // a tangent plan: the level's tangent sums, after its pairs
+    if (!rc && P->tangent() && P->sum_count[l]) {  // a tangent plan: the level's tangent sums, after its pairs
       const TangentSumItem* d_sum = (const TangentSumItem*)P->sum_dev;
       const long long* d_sbs = (const long long*)((char*)P->sum_dev + P->sum_items.size() * sizeof(TangentSumItem));
       const int ns = P->sum_count[l];
@@ -745,7 +790,7 @@ static int execute_static(tncb_ctx* ctx, tncb_plan* P, const tncb_tn* tn, tncb_t
     }
     if ((rc = enqueue_static(ctx, P, ws, 1, 0, 0, P->n_fwd_levels))) return rc;
   }
-  P->fwd_ready = P->grad;      // the forward operands the backward levels read are in the workspace now
+  P->fwd_ready = P->grad();    // the forward operands the backward levels read are in the workspace now
   tncb_tensor* result = nullptr;
   if (S.result_slot >= 0) {
     const SlotMeta& rm = S.slots[S.result_slot];
@@ -1032,7 +1077,7 @@ static int build_slice_items(tncb_plan* P, const std::vector<const tncb_tn*>& lv
   const size_t nl = S.n_leaves_total;
   std::vector<int> sslot(nl, -1), fslot(nl, -1), leaf_tan(nl, -1);
   for (size_t s = 0; s < S.slots.size(); s++) if (S.slots[s].leaf_index >= 0) sslot[S.slots[s].leaf_index] = (int)s;
-  if (P->tangent) {                                // build_tangent: tan_leaves in leaf order, one per offset >= 0
+  if (P->tangent()) {                              // build_tangent: tan_leaves in leaf order, one per offset >= 0
     size_t k = 0;
     for (size_t li = 0; li < nl; li++) if (P->grad_offset[li] >= 0) leaf_tan[li] = P->tan_leaves[k++].slot;
   }
@@ -1365,6 +1410,244 @@ static std::vector<LeafRun> leaf_runs(std::vector<LeafStageItem>& items, long lo
   return runs;
 }
 
+// ---- the arguments and outputs of the derivative calls ----
+// the checks every call of a tangent plan makes: an output, tangents shaped `want` with storage
+static int jvp_args(const tncb_tensor* tangents, bool any_out, const std::vector<uint64_t>& want) {
+  if (!any_out) return fail(TNCB_ERR_INVALID, "no output requested");
+  if (!tangents) return fail(TNCB_ERR_INVALID, "tangents are needed");
+  bool same = tangents->rank == (int)want.size();
+  for (size_t i = 0; same && i < want.size(); i++) same = tangents->dims[i] == want[i];
+  if (!same) {
+    std::string w;
+    for (uint64_t d : want) w += (w.empty() ? "" : ", ") + std::to_string(d);
+    return fail(TNCB_ERR_SHAPE, "the tangents' dims differ from [" + w + "]");
+  }
+  if (!tangents->ptr) return fail(TNCB_ERR_UNCONTRACTED, "the tangent tensor has no storage");
+  return TNCB_OK;
+}
+
+// a seed or seed tangent: the result's dims, with storage.  NULL: needed (a seed) unless the result is a scalar
+static int seed_args(const SlotMeta& rm, const tncb_tensor* t, const char* what, bool needed = false) {
+  if (!t) {
+    if (needed && !rm.dims.empty()) return fail(TNCB_ERR_INVALID, "a seed is needed for a result of rank " + std::to_string(rm.dims.size()));
+    return TNCB_OK;
+  }
+  bool same = t->rank == (int)rm.dims.size();
+  for (int i = 0; same && i < t->rank; i++) same = t->dims[i] == rm.dims[i];
+  if (!same) return fail(TNCB_ERR_SHAPE, std::string("the ") + what + "'s dims differ from the result's");
+  if (!t->ptr) return fail(TNCB_ERR_UNCONTRACTED, std::string("the ") + what + " tensor has no storage");
+  return TNCB_OK;
+}
+
+// the instances [first, first + count) of a batched call: within the staged networks
+static int instance_range(const tncb_plan* P, size_t first, size_t count) {
+  if (count == 0 || first > P->n_slices || count > P->n_slices - first)
+    return fail(TNCB_ERR_INVALID, "instances [" + std::to_string(first) + ", " + std::to_string(first + count) + ") are not within the " +
+                                  std::to_string(P->n_slices) + " staged networks");
+  return TNCB_OK;
+}
+
+// the dims of a batched call's value rows: [count, result dims]
+static int result_rows(const tncb_plan* P, size_t count, std::vector<uint64_t>& dims) {
+  const SlotMeta& rm = P->S.slots[P->S.result_slot];
+  if (rm.dims.size() + 1 > (size_t)kMaxLegs) return fail(TNCB_ERR_INVALID, "a result of rank 64 leaves no room for the instance dimension");
+  dims.assign(1, count);
+  dims.insert(dims.end(), rm.dims.begin(), rm.dims.end());
+  return TNCB_OK;
+}
+
+// seed or seed-tangent rows of a batched call: shaped `rows` (result_rows), with storage
+static int seed_rows(const tncb_tensor* t, const std::vector<uint64_t>& rows, const char* what, const char* noun) {
+  bool same = t->rank == (int)rows.size();
+  for (size_t i = 0; same && i < rows.size(); i++) same = t->dims[i] == rows[i];
+  if (!same) return fail(TNCB_ERR_SHAPE, std::string("the ") + what + "' dims differ from [count, result dims]");
+  if (!t->ptr) return fail(TNCB_ERR_UNCONTRACTED, std::string("the ") + noun + " tensor has no storage");
+  return TNCB_OK;
+}
+
+// The output tensors of a call: one per requested (non-null) destination, handed out together on success and all freed
+// on an error, so that a failed call leaves the caller's pointers as they were.  After a failed allocation add() makes
+// nothing more and rc holds the error.
+struct Outputs {
+  tncb_ctx* ctx;
+  int rc = TNCB_OK;
+  std::vector<std::pair<tncb_tensor**, tncb_tensor*>> made;
+  tncb_tensor* add(tncb_tensor** dst, int rank, const uint64_t* dims) {
+    tncb_tensor* t = nullptr;
+    if (dst && !rc && !(rc = tensor_new(ctx, rank, dims, &t))) made.push_back({dst, t});
+    return t;
+  }
+  int finish(int status) {
+    for (auto [dst, t] : made) if (status) tncb_tensor_free(ctx, t); else *dst = t;
+    return status;
+  }
+};
+
+// the leaf tangents of n instances (rows of `row_elems` elements from `tangents` on) into the workspaces at `ws`,
+// `stride` bytes apart: one leaf_stage_kernel launch, the instance a grid dimension
+static int stage_tangents(tncb_ctx* ctx, const tncb_plan* P, const double2* tangents, unsigned long long row_elems,
+                          char* ws, long long stride, size_t n) {
+  std::vector<LeafStageItem> items;
+  for (const auto& tl : P->tan_leaves)
+    items.push_back({tangents + tl.off, n > 1 ? row_elems : 0, (long long)(P->slot_off[tl.slot] / sizeof(double2)),
+                     (long long)P->S.slots[tl.slot].elems});
+  return launch_leaf_stage(ctx, items.data(), items.size(), (double2*)ws, stride / (long long)sizeof(double2), n);
+}
+
+// the result and its tangent (either may be null) out of the workspace `ws`
+static int copy_results(tncb_ctx* ctx, const tncb_plan* P, const char* ws, tncb_tensor* value, tncb_tensor* tangent) {
+  const size_t res_bytes = P->S.slots[P->S.result_slot].elems * sizeof(double2);
+  for (auto [dst, slot] : {std::pair<tncb_tensor*, int>{value, P->S.result_slot}, {tangent, P->tan_result}}) {
+    if (!dst || !res_bytes) continue;
+    cudaError_t e = cudaMemcpyAsync(dst->ptr, ws + P->slot_off[slot], res_bytes, cudaMemcpyDeviceToDevice, ctx->stream);
+    if (e != cudaSuccess) return fail(TNCB_ERR_CUDA, std::string("result copy: ") + cudaGetErrorString(e));
+  }
+  return TNCB_OK;
+}
+
+// the seed (NULL: the 1 of a scalar result) and a Hessian-vector plan's seed tangent (NULL: zero) into the workspace `ws`.
+// The seed slots may reuse memory the forward levels freed: written after them, on the stream.
+static int write_seed(tncb_ctx* ctx, const tncb_plan* P, char* ws, const tncb_tensor* seed, const tncb_tensor* seed_tangent) {
+  static const double2 one = {1.0, 0.0};
+  const size_t res_bytes = P->S.slots[P->S.result_slot].elems * sizeof(double2);
+  char* s = ws + P->slot_off[P->seed_slot];
+  cudaError_t e = seed ? cudaMemcpyAsync(s, seed->ptr, res_bytes, cudaMemcpyDeviceToDevice, ctx->stream)
+                       : cudaMemcpyAsync(s, &one, sizeof(double2), cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess && P->seed_tan_slot >= 0) {
+    char* ds = ws + P->slot_off[P->seed_tan_slot];
+    e = seed_tangent ? cudaMemcpyAsync(ds, seed_tangent->ptr, res_bytes, cudaMemcpyDeviceToDevice, ctx->stream)
+                     : cudaMemsetAsync(ds, 0, res_bytes, ctx->stream);
+  }
+  return e == cudaSuccess ? TNCB_OK : fail(TNCB_ERR_CUDA, std::string("seed copy: ") + cudaGetErrorString(e));
+}
+
+// one gather set (grad_* or dgrad_*) from the workspace into the packed block `out`: one grad_gather_kernel launch, K3
+// for the leaves with more fused groups than a GradItem holds
+static int gather_set(tncb_ctx* ctx, const tncb_plan* P, const std::vector<GradItem>& items, const std::vector<long long>& bs,
+                      const std::vector<tncb_plan::GradPermute>& permutes, const void* dev, const char* ws, double2* out) {
+  int rc = TNCB_OK;
+  if (!items.empty())
+    rc = launch_grad_gather(ctx, (const GradItem*)dev, (const long long*)((const char*)dev + items.size() * sizeof(GradItem)),
+                            (int)items.size(), bs.back(), ws, out);
+  for (size_t i = 0; i < permutes.size() && !rc; i++) {
+    const auto& gp = permutes[i];
+    const SlotMeta& sm = P->S.slots[gp.slot];
+    rc = launch_permute(ctx, (const double2*)(ws + P->slot_off[gp.slot]), out + gp.dst, (int)sm.dims.size(), sm.dims.data(), gp.perm.data());
+  }
+  return rc;
+}
+
+// ---- instance-batched passes (tncb_plan_run_batch / _vjp_batch / _jvp_batch / _hvp_batch) ----
+// Where a pass's leaf blocks come from: the staged instance blocks from `first` on (dev == nullptr), or the device
+// payloads `dev` (sorted by leaf_runs) with the `runs` between them from the plan's staged leaf block, at stride 0
+struct InstanceFill {
+  size_t first = 0;
+  const std::vector<LeafStageItem>* dev = nullptr;
+  const std::vector<LeafRun>* runs = nullptr;
+};
+// The inputs (rows of the instances: a tangent plan's tangents, seeds, seed tangents; NULL seeds: 1, NULL seed tangents:
+// zero) and the outputs, each made if its destination is non-null
+struct InstanceIO {
+  const tncb_tensor *tangents = nullptr, *seeds = nullptr, *seed_tangents = nullptr;
+  tncb_tensor **values = nullptr, **tangent_rows = nullptr, **grad_rows = nullptr, **grad_sum = nullptr,
+              **grad_tangent_rows = nullptr, **grad_tangent_sum = nullptr;
+};
+
+// rows[0] instances with value rows of dims `rows` (result_rows), in passes of c instances on c copies of the plan's
+// workspace (BatchBlock).  Per pass: the leaf blocks, a tangent plan's leaf tangents, the forward levels, values and
+// tangent rows out; if a G or Ġ output is wanted, the seeds and seed tangents, the backward levels and the gathers of G,
+// then Ġ, into rows and/or sums.  Every launch decision is the single-network one, so row i is bit-identical to the
+// single-network call on instance i; passes run in stream order, so a sum is the left fold of its rows in instance order.
+static int run_instances(tncb_ctx* ctx, tncb_plan* P, const std::vector<uint64_t>& rows, const InstanceFill& fill,
+                         const InstanceIO& io) {
+  const Schedule& S = P->S;
+  const size_t count = rows[0];
+  const uint64_t ge = P->grad_elems, row_dims[2] = {(uint64_t)count, ge};
+  const bool backward = io.grad_rows || io.grad_sum || io.grad_tangent_rows || io.grad_tangent_sum;
+  TNCB_CUDA(cudaSetDevice(ctx->device));
+  BatchBlock B;
+  int rc = batch_size(ctx, P, count, &B);
+  if (rc) return rc;
+  Outputs out{ctx};
+  tncb_tensor* v = out.add(io.values, (int)rows.size(), rows.data());
+  tncb_tensor* t = out.add(io.tangent_rows, (int)rows.size(), rows.data());
+  tncb_tensor* gr = out.add(io.grad_rows, 2, row_dims);
+  tncb_tensor* gs = out.add(io.grad_sum, 1, &ge);
+  tncb_tensor* dgr = out.add(io.grad_tangent_rows, 2, row_dims);
+  tncb_tensor* dgs = out.add(io.grad_tangent_sum, 1, &ge);
+  if (!(rc = out.rc)) rc = batch_alloc(ctx, &B);
+  const size_t ws = B.ws, c = B.c;
+  void* aux = nullptr;                 // the seed 1 of every copy (scalar result, NULL seeds), the K3 scratch of the sums
+  const size_t ones = backward && !io.seeds ? c : 0;
+  size_t scratch = 0;
+  if (gs) for (const auto& gp : P->grad_permutes) scratch = std::max<size_t>(scratch, S.slots[gp.slot].elems);
+  if (dgs) for (const auto& gp : P->dgrad_permutes) scratch = std::max<size_t>(scratch, S.slots[gp.slot].elems);
+  const size_t aux_bytes = (ones + scratch) * sizeof(double2);
+  if (!rc && aux_bytes) {
+    rc = ctx->arena.alloc(aux_bytes, &aux);
+    if (!rc && ones) {
+      const std::vector<double2> one(ones, double2{1.0, 0.0});
+      cudaError_t e = cudaMemcpyAsync(aux, one.data(), ones * sizeof(double2), cudaMemcpyHostToDevice, ctx->stream);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);      // `one` dies with this scope
+      if (e != cudaSuccess) rc = fail(TNCB_ERR_CUDA, std::string("seed copy: ") + cudaGetErrorString(e));
+    }
+  }
+  for (tncb_tensor* x : {gs, dgs}) {
+    if (rc || !x) continue;
+    cudaError_t e = cudaMemsetAsync(x->ptr, 0, std::max<uint64_t>(ge, 1) * sizeof(double2), ctx->stream);
+    if (e != cudaSuccess) rc = fail(TNCB_ERR_CUDA, std::string("gradient sum: ") + cudaGetErrorString(e));
+  }
+  char* base = (char*)B.blk;
+  const double2* d_one = (const double2*)aux;
+  double2* d_scratch = (double2*)aux + ones;
+  const size_t block_bytes = std::max<size_t>(S.leaf_block_elems, 1) * sizeof(double2);
+  const size_t res_bytes = S.slots[S.result_slot].elems * sizeof(double2);
+  std::vector<LeafStageItem> items;
+  for (size_t done = 0; done < count && !rc; done += c) {
+    const size_t n = std::min(c, count - done);
+    if (!fill.dev) {
+      const char* src = (const char*)P->slices_dev + (fill.first + done) * block_bytes;
+      if ((rc = batch_copy(ctx, B, base + P->leaf_off, ws, src, block_bytes, block_bytes, n))) break;
+    } else {          // every copy's leaf block: the device payloads of instances done .. done+n-1, the staged block between
+      const double2* staged = (const double2*)((const char*)P->ws + P->leaf_off);
+      items.clear();
+      for (const LeafStageItem& it : *fill.dev) items.push_back({it.src + done * it.src_stride, it.src_stride, it.dst, it.elems});
+      for (const LeafRun& lr : *fill.runs) items.push_back({staged + lr.start, 0, lr.start, lr.len});
+      if ((rc = launch_leaf_stage(ctx, items.data(), items.size(), (double2*)(base + P->leaf_off), (long long)(ws / sizeof(double2)), n))) break;
+    }
+    if (P->tangent() && (rc = stage_tangents(ctx, P, io.tangents->ptr + done * ge, ge, base, (long long)ws, n))) break;
+    if ((rc = enqueue_static(ctx, P, base, (int)n, (long long)ws, 0, P->n_fwd_levels))) break;
+    for (auto [x, slot] : {std::pair<tncb_tensor*, int>{v, S.result_slot}, {t, P->tan_result}})
+      if (!rc && x && res_bytes) rc = batch_copy(ctx, B, (char*)x->ptr + done * res_bytes, res_bytes, base + P->slot_off[slot], ws, res_bytes, n);
+    if (rc || !backward) continue;
+    // the seed slots may reuse memory the forward levels freed: written after them, on the stream
+    char* seed_dst = base + P->slot_off[P->seed_slot];
+    if (io.seeds) { if (res_bytes && (rc = batch_copy(ctx, B, seed_dst, ws, (const char*)io.seeds->ptr + done * res_bytes, res_bytes, res_bytes, n))) break; }
+    else if ((rc = batch_copy(ctx, B, seed_dst, ws, (const char*)d_one, sizeof(double2), sizeof(double2), n))) break;
+    if (P->seed_tan_slot >= 0) {
+      char* seed_tan_dst = base + P->slot_off[P->seed_tan_slot];
+      if (io.seed_tangents) {
+        if (res_bytes && (rc = batch_copy(ctx, B, seed_tan_dst, ws, (const char*)io.seed_tangents->ptr + done * res_bytes, res_bytes, res_bytes, n))) break;
+      } else if (res_bytes) {
+        cudaError_t e = cudaSuccess;
+        if (B.strided) e = cudaMemset2DAsync(seed_tan_dst, ws, 0, res_bytes, n, ctx->stream);
+        else for (size_t i = 0; i < n && e == cudaSuccess; i++) e = cudaMemsetAsync(seed_tan_dst + i * ws, 0, res_bytes, ctx->stream);
+        if (e != cudaSuccess) { rc = fail(TNCB_ERR_CUDA, std::string("seed tangent: ") + cudaGetErrorString(e)); break; }
+      }
+    }
+    if ((rc = enqueue_static(ctx, P, base, (int)n, (long long)ws, P->n_fwd_levels, (int)P->level_batched.size()))) break;
+    if ((gr || gs) &&
+        (rc = gather_set_batch(ctx, P, P->grad_items, P->grad_block_start, P->grad_permutes, P->grad_dev, base, ws, n,
+                               gr ? gr->ptr + done * ge : nullptr, ge, gs ? gs->ptr : nullptr, d_scratch))) break;
+    if (dgr || dgs)
+      rc = gather_set_batch(ctx, P, P->dgrad_items, P->dgrad_block_start, P->dgrad_permutes, P->dgrad_dev, base, ws, n,
+                            dgr ? dgr->ptr + done * ge : nullptr, ge, dgs ? dgs->ptr : nullptr, d_scratch);
+  }
+  batch_free(ctx, &B);
+  if (aux) ctx->arena.free(aux, aux_bytes);
+  return out.finish(rc);
+}
+
 } // namespace tncb
 
 extern "C" {
@@ -1448,51 +1731,16 @@ int tncb_plan_create(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, tn
   tncb_plan* p = new tncb_plan();
   int rc = tncb::build_schedule(tn, path, p->S);
   if (rc) { delete p; return rc; }
-  size_t dev_free = 0, dev_total = 0;
-  if (ctx) { cudaSetDevice(ctx->device); if (cudaMemGetInfo(&dev_free, &dev_total) != cudaSuccess) { dev_total = 0; cudaGetLastError(); } }
-  tncb::plan_static_layout(p, ctx ? ctx->sm_count : 132, dev_total);
-  *out = p;
-  return TNCB_OK;
-}
-
-// A gradient plan: the forward schedule, the backward pairs of the `wrt` leaves and the leaf-gradient gather, in one
-// static layout.  There is no pair-by-pair fallback: a layout above the static-workspace limit is refused here.
-int tncb_plan_create_vjp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, const uint8_t* wrt, tncb_plan** out) {
-  if (!tn || !out) return tncb::fail(TNCB_ERR_INVALID, "null argument");
-  {
-    std::vector<const tncb_tn*> lv;
-    tncb::collect_leaf_nodes(tn, lv);
-    for (const tncb_tn* l : lv)
-      if (l->kind == TNCB_DATA_DEVICE) return tncb::fail(TNCB_ERR_UNSUPPORTED, "gradient plans do not take device leaves (they are consumed per call)");
-  }
-  tncb_plan* p = new tncb_plan();
-  p->grad = true;
-  std::vector<int> leaf_adj;
-  int rc = tncb::build_schedule(tn, path, p->S);
-  if (!rc) rc = tncb::build_backward(p, wrt, leaf_adj, p->S.steps.size());
-  if (rc) { delete p; return rc; }
-  size_t dev_free = 0, dev_total = 0;
-  if (ctx) { cudaSetDevice(ctx->device); if (cudaMemGetInfo(&dev_free, &dev_total) != cudaSuccess) { dev_total = 0; cudaGetLastError(); } }
-  tncb::plan_static_layout(p, ctx ? ctx->sm_count : 132, dev_total);
-  if (!p->is_static) {
-    const size_t need = p->ws_bytes, limit = tncb::static_ws_limit(dev_total);
-    delete p;
-    return tncb::fail(TNCB_ERR_UNSUPPORTED, "the gradient workspace needs " + std::to_string(need) + " bytes, above the static-workspace limit of " +
-                                           std::to_string(limit) + " bytes (TNCB_PLAN_WS_GB)");
-  }
-  if ((rc = tncb::build_gather(p, leaf_adj, p->grad_items, p->grad_block_start, p->grad_permutes))) { delete p; return rc; }
+  tncb::plan_static_layout(p, ctx ? ctx->sm_count : 132, tncb::device_bytes(ctx));
   *out = p;
   return TNCB_OK;
 }
 
 namespace tncb {
-// The checks every sliced creator makes on the network and its sliced legs: no device leaves (`plans` names the plan
-// kind in the message), every sliced leg listed once, joining two tensors, of non-zero dimension, and a slice count that
-// fits 64 bits.  Fills the legs' dims and the slice count.
-static int check_sliced_legs(const std::vector<const tncb_tn*>& lv, const char* plans, size_t n_sliced, const uint64_t* sliced_legs,
+// The checks every sliced creator makes on the sliced legs: every sliced leg listed once, joining two tensors, of
+// non-zero dimension, and a slice count that fits 64 bits.  Fills the legs' dims and the slice count.
+static int check_sliced_legs(const std::vector<const tncb_tn*>& lv, size_t n_sliced, const uint64_t* sliced_legs,
                              std::vector<uint64_t>& sl, std::vector<uint64_t>& sdim, uint64_t* n_slices) {
-  for (const tncb_tn* l : lv)
-    if (l->kind == TNCB_DATA_DEVICE) return fail(TNCB_ERR_UNSUPPORTED, std::string(plans) + " plans do not take device leaves (they are consumed per call)");
   sl.assign(sliced_legs, sliced_legs + n_sliced);
   sdim.assign(n_sliced, 0);
   uint64_t n_sl = 1;
@@ -1516,75 +1764,98 @@ static int check_sliced_legs(const std::vector<const tncb_tn*>& lv, const char* 
   return TNCB_OK;
 }
 
-// A sliced derivative plan of the given kind: the gradient, tangent or Hessian-vector plan of one slice's structure,
-// compiled with the calls tncb_plan_create_vjp / _jvp / _hvp make on the host-sliced slice network, plus the slice items.
-enum class SlicedKind { vjp, jvp, hvp };
-static int create_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, size_t n_sliced, const uint64_t* sliced_legs,
-                         const uint8_t* wrt, SlicedKind kind, tncb_plan** out) {
+// A derivative plan of a kind other than plain, in one static layout: the forward schedule plus the tangent pairs
+// (build_tangent), backward pairs (build_backward) and backward-tangent pairs (build_backward_tangent) the kind has, and
+// the gathers of G (and Ġ).  Sliced (n_sliced legs, possibly none): the plan of one slice's structure, compiled exactly
+// so on the host-sliced slice network, plus the slice items instead of the gathers.  There is no pair-by-pair fallback:
+// a layout above the static-workspace limit is refused here.
+static int create(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, tncb_plan::Kind kind, bool sliced, size_t n_sliced,
+                  const uint64_t* sliced_legs, const uint8_t* wrt, tncb_plan** out) {
   if (!tn || !out || (n_sliced && !sliced_legs)) return fail(TNCB_ERR_INVALID, "null argument");
-  static const char* const noun[3] = {"gradient", "tangent", "Hessian-vector"};
-  const int ki = (int)kind;
+  static const char* const noun[4] = {nullptr, "gradient", "tangent", "Hessian-vector"};
+  const std::string what = noun[(int)kind];
   std::vector<const tncb_tn*> lv;
   collect_leaf_nodes(tn, lv);
+  for (const tncb_tn* l : lv)
+    if (l->kind == TNCB_DATA_DEVICE) return fail(TNCB_ERR_UNSUPPORTED, what + " plans do not take device leaves (they are consumed per call)");
   std::vector<uint64_t> sl, sdim;
   uint64_t n_sl = 1;
-  int rc = check_sliced_legs(lv, noun[ki], n_sliced, sliced_legs, sl, sdim, &n_sl);
-  if (rc) return rc;
   SliceTree keep;
   tncb_tn st;
-  slice_tree(tn, &st, sl, keep);
+  if (sliced) {
+    int rc = check_sliced_legs(lv, n_sliced, sliced_legs, sl, sdim, &n_sl);
+    if (rc) return rc;
+    slice_tree(tn, &st, sl, keep);
+  }
   tncb_plan* p = new tncb_plan();
-  p->sliced = true;
-  p->grad = kind != SlicedKind::jvp;
-  p->tangent = kind != SlicedKind::vjp;
-  p->hvp = kind == SlicedKind::hvp;
+  p->kind = kind;
+  p->sliced = sliced;
   p->n_sl = n_sl;
   std::vector<int> tan, leaf_adj, leaf_dadj;
-  rc = build_schedule(&st, path, p->S);
+  int rc = build_schedule(sliced ? &st : tn, path, p->S);
   const size_t n_fwd = p->S.steps.size();
   size_t b0 = n_fwd;
-  if (!rc && p->tangent) { rc = build_tangent(p, wrt, &tan); b0 = p->S.steps.size(); }
-  if (!rc && p->grad) rc = build_backward(p, wrt, leaf_adj, n_fwd);
-  if (!rc && p->hvp) rc = build_backward_tangent(p, b0, tan, leaf_adj, leaf_dadj);
+  if (!rc && p->tangent()) { rc = build_tangent(p, wrt, &tan); b0 = p->S.steps.size(); }
+  if (!rc && p->grad()) rc = build_backward(p, wrt, leaf_adj, n_fwd);
+  if (!rc && kind == tncb_plan::Kind::hvp) rc = build_backward_tangent(p, b0, tan, leaf_adj, leaf_dadj);
   if (rc) { delete p; return rc; }
-  size_t dev_free = 0, dev_total = 0;
-  if (ctx) { cudaSetDevice(ctx->device); if (cudaMemGetInfo(&dev_free, &dev_total) != cudaSuccess) { dev_total = 0; cudaGetLastError(); } }
+  const size_t dev_total = device_bytes(ctx);
   plan_static_layout(p, ctx ? ctx->sm_count : 132, dev_total);
   if (!p->is_static) {
     const size_t need = p->ws_bytes, limit = static_ws_limit(dev_total);
     delete p;
-    return fail(TNCB_ERR_UNSUPPORTED, std::string("the ") + noun[ki] + " workspace of one slice needs " + std::to_string(need) +
+    return fail(TNCB_ERR_UNSUPPORTED, "the " + what + (sliced ? " workspace of one slice needs " : " workspace needs ") + std::to_string(need) +
                                       " bytes, above the static-workspace limit of " + std::to_string(limit) + " bytes (TNCB_PLAN_WS_GB)");
   }
-  if ((rc = build_slice_items(p, lv, sl, sdim, leaf_adj, leaf_dadj))) { delete p; return rc; }
+  if (sliced) rc = build_slice_items(p, lv, sl, sdim, leaf_adj, leaf_dadj);
+  else {
+    if (p->grad()) rc = build_gather(p, leaf_adj, p->grad_items, p->grad_block_start, p->grad_permutes);
+    if (!rc && kind == tncb_plan::Kind::hvp) rc = build_gather(p, leaf_dadj, p->dgrad_items, p->dgrad_block_start, p->dgrad_permutes);
+  }
+  if (rc) { delete p; return rc; }
   *out = p;
   return TNCB_OK;
 }
 } // namespace tncb
 
-// A sliced gradient plan: the gradient plan of one slice's structure (compiled exactly as tncb_plan_create_vjp compiles
-// the host-sliced slice network), plus the extract / accumulate items that move slice q's sub-blocks between the full
-// leaves and the workspace.
+// A gradient plan: the forward schedule, the backward pairs of the `wrt` leaves and the leaf-gradient gather.
+int tncb_plan_create_vjp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, const uint8_t* wrt, tncb_plan** out) {
+  return tncb::create(ctx, tn, path, tncb_plan::Kind::vjp, false, 0, nullptr, wrt, out);
+}
+
+// A tangent plan: the forward schedule and the tangent pairs of the `wrt` leaves, on the forward levels.
+int tncb_plan_create_jvp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, const uint8_t* wrt, tncb_plan** out) {
+  return tncb::create(ctx, tn, path, tncb_plan::Kind::jvp, false, 0, nullptr, wrt, out);
+}
+
+// A Hessian-vector plan: the forward schedule, the tangent pairs, the backward pairs and the backward-tangent pairs of
+// the `wrt` leaves, plus the gathers of G and Ġ.
+int tncb_plan_create_hvp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, const uint8_t* wrt, tncb_plan** out) {
+  return tncb::create(ctx, tn, path, tncb_plan::Kind::hvp, false, 0, nullptr, wrt, out);
+}
+
+// A sliced gradient plan: the gradient plan of one slice's structure plus the extract / accumulate items that move slice
+// q's sub-blocks between the full leaves and the workspace.
 int tncb_plan_create_vjp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, size_t n_sliced,
                                 const uint64_t* sliced_legs, const uint8_t* wrt, tncb_plan** out) {
-  return tncb::create_sliced(ctx, tn, path, n_sliced, sliced_legs, wrt, tncb::SlicedKind::vjp, out);
+  return tncb::create(ctx, tn, path, tncb_plan::Kind::vjp, true, n_sliced, sliced_legs, wrt, out);
 }
 
 // Sliced tangent and Hessian-vector plans: the tangent / Hessian-vector plan of one slice's structure plus the items that
 // also move the leaf tangents in and the adjoints' tangents out per slice.
 int tncb_plan_create_jvp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, size_t n_sliced,
                                 const uint64_t* sliced_legs, const uint8_t* wrt, tncb_plan** out) {
-  return tncb::create_sliced(ctx, tn, path, n_sliced, sliced_legs, wrt, tncb::SlicedKind::jvp, out);
+  return tncb::create(ctx, tn, path, tncb_plan::Kind::jvp, true, n_sliced, sliced_legs, wrt, out);
 }
 
 int tncb_plan_create_hvp_sliced(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, size_t n_sliced,
                                 const uint64_t* sliced_legs, const uint8_t* wrt, tncb_plan** out) {
-  return tncb::create_sliced(ctx, tn, path, n_sliced, sliced_legs, wrt, tncb::SlicedKind::hvp, out);
+  return tncb::create(ctx, tn, path, tncb_plan::Kind::hvp, true, n_sliced, sliced_legs, wrt, out);
 }
 
 int tncb_plan_grad_offsets(const tncb_plan* plan, int64_t* offsets) {
   if (!plan || !offsets) return tncb::fail(TNCB_ERR_INVALID, "null argument");
-  if (!plan->grad && !plan->tangent) return tncb::fail(TNCB_ERR_INVALID, "not a gradient or tangent plan (tncb_plan_create_vjp / _jvp)");
+  if (int rc = tncb::route(plan, tncb::Call::grad_offsets)) return rc;
   for (size_t i = 0; i < plan->grad_offset.size(); i++) offsets[i] = plan->grad_offset[i];
   return TNCB_OK;
 }
@@ -1594,46 +1865,22 @@ int tncb_plan_grad_offsets(const tncb_plan* plan, int64_t* offsets) {
 int tncb_plan_vjp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* seed, tncb_tensor** grads) {
   using namespace tncb;
   if (!ctx || !plan || !grads) return fail(TNCB_ERR_INVALID, "null argument");
-  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
-  if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_vjp_sliced");
-  if (plan->hvp) return hvp_refused();
-  if (plan->tangent) return fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp");
-  if (!plan->grad) return fail(TNCB_ERR_INVALID, "not a gradient plan (tncb_plan_create_vjp)");
+  int rc = route(plan, Call::vjp);
+  if (rc) return rc;
   if (plan->ctx != ctx || !plan->fwd_ready)
     return fail(TNCB_ERR_INVALID, "tncb_plan_vjp needs a forward run (tncb_plan_run / tncb_plan_execute) of the plan on this context "
                                   "since its leaves were staged or its last tncb_plan_vjp");
-  const Schedule& S = plan->S;
-  const SlotMeta& rm = S.slots[S.result_slot];
-  if (seed) {
-    bool same = seed->rank == (int)rm.dims.size();
-    for (int i = 0; same && i < seed->rank; i++) same = seed->dims[i] == rm.dims[i];
-    if (!same) return fail(TNCB_ERR_SHAPE, "the seed's dims differ from the result's");
-    if (!seed->ptr) return fail(TNCB_ERR_UNCONTRACTED, "the seed tensor has no storage");
-  } else if (!rm.dims.empty()) return fail(TNCB_ERR_INVALID, "a seed is needed for a result of rank " + std::to_string(rm.dims.size()));
+  if ((rc = seed_args(plan->S.slots[plan->S.result_slot], seed, "seed", true))) return rc;
   TNCB_CUDA(cudaSetDevice(ctx->device));
-  const uint64_t n = plan->grad_elems;
-  tncb_tensor* g = nullptr;
-  int rc = tensor_new(ctx, 1, &n, &g);
-  if (rc) return rc;
+  Outputs out{ctx};
+  tncb_tensor* g = out.add(grads, 1, &plan->grad_elems);
+  if (out.rc) return out.rc;
   char* ws = (char*)plan->ws;
-  static const double2 one = {1.0, 0.0};
-  cudaError_t ce = seed ? cudaMemcpyAsync(ws + plan->slot_off[plan->seed_slot], seed->ptr, rm.elems * sizeof(double2), cudaMemcpyDeviceToDevice, ctx->stream)
-                        : cudaMemcpyAsync(ws + plan->slot_off[plan->seed_slot], &one, sizeof(double2), cudaMemcpyHostToDevice, ctx->stream);
-  if (ce != cudaSuccess) rc = fail(TNCB_ERR_CUDA, std::string("seed copy: ") + cudaGetErrorString(ce));
+  rc = write_seed(ctx, plan, ws, seed, nullptr);
   plan->fwd_ready = false;
   if (!rc) rc = enqueue_static(ctx, plan, ws, 1, 0, plan->n_fwd_levels, (int)plan->level_batched.size());
-  if (!rc && !plan->grad_items.empty())
-    rc = launch_grad_gather(ctx, (const GradItem*)plan->grad_dev,
-                            (const long long*)((char*)plan->grad_dev + plan->grad_items.size() * sizeof(GradItem)),
-                            (int)plan->grad_items.size(), plan->grad_block_start.back(), ws, g->ptr);
-  for (size_t i = 0; i < plan->grad_permutes.size() && !rc; i++) {
-    const auto& gp = plan->grad_permutes[i];
-    const SlotMeta& sm = S.slots[gp.slot];
-    rc = launch_permute(ctx, (const double2*)(ws + plan->slot_off[gp.slot]), g->ptr + gp.dst, (int)sm.dims.size(), sm.dims.data(), gp.perm.data());
-  }
-  if (rc) { tncb_tensor_free(ctx, g); return rc; }
-  *grads = g;
-  return TNCB_OK;
+  if (!rc) rc = gather_set(ctx, plan, plan->grad_items, plan->grad_block_start, plan->grad_permutes, plan->grad_dev, ws, g->ptr);
+  return out.finish(rc);
 }
 
 // Per slice first, first+stride, ...: extract, forward levels, seed copy, backward levels, accumulate into the
@@ -1642,45 +1889,27 @@ int tncb_plan_vjp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t st
                          tncb_tensor** value, tncb_tensor** grads) {
   using namespace tncb;
   if (!ctx || !plan || !value || !grads || stride == 0) return fail(TNCB_ERR_INVALID, "bad argument");
-  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
-  if (plan->hvp) return hvp_refused();
-  if (plan->tangent) return fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp");
-  if (!plan->sliced) return fail(TNCB_ERR_INVALID, "not a sliced gradient plan (tncb_plan_create_vjp_sliced)");
+  int rc = route(plan, Call::vjp_sliced);
+  if (rc) return rc;
   if (plan->ctx != ctx || !plan->full_staged) return fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this context");
-  const Schedule& S = plan->S;
-  const SlotMeta& rm = S.slots[S.result_slot];
-  if (seed) {
-    bool same = seed->rank == (int)rm.dims.size();
-    for (int i = 0; same && i < seed->rank; i++) same = seed->dims[i] == rm.dims[i];
-    if (!same) return fail(TNCB_ERR_SHAPE, "the seed's dims differ from the result's");
-    if (!seed->ptr) return fail(TNCB_ERR_UNCONTRACTED, "the seed tensor has no storage");
-  } else if (!rm.dims.empty()) return fail(TNCB_ERR_INVALID, "a seed is needed for a result of rank " + std::to_string(rm.dims.size()));
+  const SlotMeta& rm = plan->S.slots[plan->S.result_slot];
+  if ((rc = seed_args(rm, seed, "seed", true))) return rc;
   TNCB_CUDA(cudaSetDevice(ctx->device));
-  tncb_tensor *v = nullptr, *g = nullptr;
-  const uint64_t n = plan->grad_elems;
-  int rc = tensor_new(ctx, (int)rm.dims.size(), rm.dims.data(), &v);
-  if (!rc) rc = tensor_new(ctx, 1, &n, &g);
-  if (!rc) {
+  Outputs out{ctx};
+  tncb_tensor* v = out.add(value, (int)rm.dims.size(), rm.dims.data());
+  tncb_tensor* g = out.add(grads, 1, &plan->grad_elems);
+  if (!(rc = out.rc)) {
     SliceRun io;
     io.seed = seed ? seed->ptr : nullptr; io.value = v->ptr; io.grad = g->ptr;
     rc = run_sliced(ctx, plan, first, stride, io);
   }
-  if (rc) {
-    if (v) tncb_tensor_free(ctx, v);
-    if (g) tncb_tensor_free(ctx, g);
-    return rc;
-  }
-  *value = v; *grads = g;
-  return TNCB_OK;
+  return out.finish(rc);
 }
 
 int tncb_plan_execute(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tn, tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   if (!ctx || !plan || !tn) return tncb::fail(TNCB_ERR_INVALID, "null argument");
-  if (tncb::sliced_tangent(plan)) return tncb::sliced_tangent_refused(plan);
-  if (plan->sliced) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_run_slices / tncb_plan_vjp_sliced");
-  if (plan->hvp) return tncb::hvp_refused();
-  if (plan->tangent) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp");
-  if (plan->grad) return tncb::execute_static(ctx, plan, tn, out, n_out, out_legs);   // forward levels only, no fallback
+  if (int rc = tncb::route(plan, tncb::Call::execute)) return rc;
+  if (plan->grad()) return tncb::execute_static(ctx, plan, tn, out, n_out, out_legs);   // forward levels only, no fallback
   static const bool trace = std::getenv("TNCB_TRACE") != nullptr;   // per-step times come from the pair-by-pair executor
   if (plan->is_static && !trace && (plan->ctx == nullptr || plan->ctx == ctx)) {
     int rc = tncb::execute_static(ctx, plan, tn, out, n_out, out_legs);
@@ -1695,6 +1924,7 @@ int tncb_plan_execute(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tn, tncb_te
 // block of sliced execution).
 int tncb_plan_stage(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tn) {
   if (!ctx || !plan || !tn) return tncb::fail(TNCB_ERR_INVALID, "null argument");
+  if (int rc = tncb::route(plan, tncb::Call::stage)) return rc;
   const tncb::Schedule& S = plan->S;
   for (int k : S.leaf_kind) if (k == TNCB_DATA_DEVICE) return tncb::fail(TNCB_ERR_UNSUPPORTED, "plans with device leaves cannot be staged (they are consumed per call)");
   if (plan->ctx && plan->ctx != ctx) return tncb::fail(TNCB_ERR_INVALID, "plan belongs to another context");
@@ -1723,7 +1953,7 @@ int tncb_plan_stage(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tn) {
   const size_t bytes = std::max<size_t>(S.leaf_block_elems * sizeof(double2), 16);
   std::vector<std::complex<double>> host(std::max<size_t>(S.leaf_block_elems, 1));
   if (plan->is_static && (rc = tncb::plan_device_state(ctx, plan))) {
-    if (rc != TNCB_ERR_OOM || plan->ws || plan->grad || plan->tangent) return rc;
+    if (rc != TNCB_ERR_OOM || plan->ws || plan->grad() || plan->tangent()) return rc;
     plan->is_static = false;    // the static workspace does not fit: resident leaf block + pair-by-pair executor
   }
   if (plan->is_static) {      // the leaf block lives inside the plan workspace
@@ -1748,13 +1978,10 @@ int tncb_plan_stage(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tn) {
 
 int tncb_plan_run(tncb_ctx* ctx, tncb_plan* plan, tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   if (!ctx || !plan) return tncb::fail(TNCB_ERR_INVALID, "null argument");
-  if (tncb::sliced_tangent(plan)) return tncb::sliced_tangent_refused(plan);
-  if (plan->sliced) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_run_slices / tncb_plan_vjp_sliced");
-  if (plan->hvp) return tncb::hvp_refused();
-  if (plan->tangent) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp");
+  if (int rc = tncb::route(plan, tncb::Call::run)) return rc;
   static const bool trace = std::getenv("TNCB_TRACE") != nullptr;
   if (plan->is_static && plan->leaves_resident && plan->ctx == ctx) {
-    if (!trace || plan->grad) return tncb::execute_static(ctx, plan, nullptr, out, n_out, out_legs);
+    if (!trace || plan->grad()) return tncb::execute_static(ctx, plan, nullptr, out, n_out, out_legs);
     return tncb::execute(ctx, plan->S, nullptr, out, n_out, out_legs, (const double2*)((char*)plan->ws + plan->leaf_off));
   }
   if (!plan->resident || plan->ctx != ctx) return tncb::fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this context");
@@ -1767,17 +1994,14 @@ int tncb_plan_run(tncb_ctx* ctx, tncb_plan* plan, tncb_tensor** out, int* n_out,
 // block (KBs), the plan's kernels (batched / graph as usual), one accumulation kernel.
 int tncb_plan_stage_slices(tncb_ctx* ctx, tncb_plan* plan, size_t n_slices, const tncb_tn* const* slice_tns) {
   if (!ctx || !plan || !slice_tns || n_slices == 0) return tncb::fail(TNCB_ERR_INVALID, "null argument");
-  if (tncb::sliced_tangent(plan)) return tncb::sliced_tangent_refused(plan);
-  if (plan->sliced) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan stages its full network once (tncb_plan_stage)");
-  if (plan->hvp) return tncb::hvp_refused();
-  if (plan->grad) return tncb::fail(TNCB_ERR_UNSUPPORTED, "gradient plans run one staged network at a time");
-  if (plan->tangent) return tncb::fail(TNCB_ERR_UNSUPPORTED, "tangent plans stage many networks with tncb_plan_stage_batch");
+  if (int rc = tncb::route(plan, tncb::Call::stage_slices)) return rc;
   if (!plan->is_static) return tncb::fail(TNCB_ERR_UNSUPPORTED, "sliced execution needs a plan with a static layout (no device leaves)");
   return tncb::stage_networks(ctx, plan, n_slices, slice_tns, true);
 }
 
 int tncb_plan_run_slices(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t stride, tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   if (!ctx || !plan || stride == 0) return tncb::fail(TNCB_ERR_INVALID, "bad argument");
+  if (int rc = tncb::route(plan, tncb::Call::run_slices)) return rc;
   if (plan->sliced) {         // forward levels only, slices extracted on the device from the staged full leaves
     if (plan->ctx != ctx || !plan->full_staged) return tncb::fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this context");
     const tncb::SlotMeta& rm = plan->S.slots[plan->S.result_slot];
@@ -1786,7 +2010,7 @@ int tncb_plan_run_slices(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t st
     int rc = tncb::tensor_new(ctx, (int)rm.dims.size(), rm.dims.data(), &sum);
     tncb::SliceRun io;
     io.value = sum ? sum->ptr : nullptr;
-    if (!rc && tncb::sliced_tangent(plan)) {   // the tangent pairs share the forward levels: they read zero tangents
+    if (!rc && plan->tangent()) {   // the tangent pairs share the forward levels: they read zero tangents
       rc = tncb::tensor_new(ctx, 1, &plan->grad_elems, &zero);
       if (!rc && cudaMemsetAsync(zero->ptr, 0, zero->elems * sizeof(double2), ctx->stream) != cudaSuccess)
         rc = tncb::fail(TNCB_ERR_CUDA, "tangent block: memset failed");
@@ -1800,9 +2024,6 @@ int tncb_plan_run_slices(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t st
     if (out_legs) for (size_t i = 0; i < rm.legs.size(); i++) out_legs[i] = rm.legs[i];
     return TNCB_OK;
   }
-  if (plan->hvp) return tncb::hvp_refused();
-  if (plan->tangent) return tncb::fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp / tncb_plan_jvp_batch");
-  if (plan->grad) return tncb::fail(TNCB_ERR_UNSUPPORTED, "gradient plans run one staged network at a time");
   if (!plan->slices_dev || plan->ctx != ctx) return tncb::fail(TNCB_ERR_INVALID, "tncb_plan_stage_slices has not been called on this context");
   const tncb::Schedule& S = plan->S;
   if (S.result_slot < 0) return tncb::fail(TNCB_ERR_INVALID, "plan has no result");
@@ -1841,47 +2062,22 @@ int tncb_plan_run_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
                         tncb_tensor** out, int* n_out, uint64_t* out_legs) {
   using namespace tncb;
   if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
-  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
-  if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan runs through tncb_plan_run_slices / tncb_plan_vjp_sliced");
-  if (plan->hvp) return hvp_refused();
-  if (plan->grad) return fail(TNCB_ERR_UNSUPPORTED, "gradient plans run one staged network at a time");
-  if (plan->tangent) return fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp_batch");
+  int rc = route(plan, Call::run_batch);
+  if (rc) return rc;
   if (!plan->is_static) return fail(TNCB_ERR_UNSUPPORTED, "batched execution needs a plan with a static layout (no device leaves)");
   if (!plan->slices_dev || plan->ctx != ctx) return fail(TNCB_ERR_INVALID, "tncb_plan_stage_slices has not been called on this context");
-  if (count == 0 || first > plan->n_slices || count > plan->n_slices - first)
-    return fail(TNCB_ERR_INVALID, "instances [" + std::to_string(first) + ", " + std::to_string(first + count) + ") are not within the " +
-                                  std::to_string(plan->n_slices) + " staged networks");
-  const Schedule& S = plan->S;
-  if (S.result_slot < 0) return fail(TNCB_ERR_INVALID, "plan has no result");
-  const SlotMeta& rm = S.slots[S.result_slot];
-  const int r = (int)rm.dims.size();
-  if (r + 1 > kMaxLegs) return fail(TNCB_ERR_INVALID, "a result of rank 64 leaves no room for the instance dimension");
-  TNCB_CUDA(cudaSetDevice(ctx->device));
-  BatchBlock B;
-  int rc = batch_size(ctx, plan, count, &B);
-  if (rc) return rc;
-  std::vector<uint64_t> dims(r + 1);
-  dims[0] = count;
-  for (int i = 0; i < r; i++) dims[i + 1] = rm.dims[i];
+  if ((rc = instance_range(plan, first, count))) return rc;
+  if (plan->S.result_slot < 0) return fail(TNCB_ERR_INVALID, "plan has no result");
+  std::vector<uint64_t> rows;
+  if ((rc = result_rows(plan, count, rows))) return rc;
   tncb_tensor* res = nullptr;
-  if ((rc = tensor_new(ctx, r + 1, dims.data(), &res))) return rc;
-  if ((rc = batch_alloc(ctx, &B))) { tncb_tensor_free(ctx, res); return rc; }
-  const size_t ws = B.ws, c = B.c;
-  char* base = (char*)B.blk;
-  const size_t block_bytes = std::max<size_t>(S.leaf_block_elems, 1) * sizeof(double2);
-  const size_t res_bytes = rm.elems * sizeof(double2);
-  for (size_t done = 0; done < count && !rc; done += c) {
-    const size_t n = std::min(c, count - done);
-    const char* src = (const char*)plan->slices_dev + (first + done) * block_bytes;
-    if ((rc = batch_copy(ctx, B, base + plan->leaf_off, ws, src, block_bytes, block_bytes, n))) break;
-    if ((rc = enqueue_static(ctx, plan, base, (int)n, (long long)ws, 0, (int)plan->level_batched.size()))) break;
-    if (res_bytes) rc = batch_copy(ctx, B, (char*)res->ptr + done * res_bytes, res_bytes, base + plan->slot_off[S.result_slot], ws, res_bytes, n);
-  }
-  batch_free(ctx, &B);
-  if (rc) { tncb_tensor_free(ctx, res); return rc; }
+  InstanceIO io;
+  io.values = &res;
+  if ((rc = run_instances(ctx, plan, rows, {first}, io))) return rc;
+  const SlotMeta& rm = plan->S.slots[plan->S.result_slot];
   if (out) *out = res; else tncb_tensor_free(ctx, res);
-  if (n_out) *n_out = r;
-  if (out_legs) for (int i = 0; i < r; i++) out_legs[i] = rm.legs[i];
+  if (n_out) *n_out = (int)rm.legs.size();
+  if (out_legs) for (size_t i = 0; i < rm.legs.size(); i++) out_legs[i] = rm.legs[i];
   return TNCB_OK;
 }
 
@@ -1890,325 +2086,73 @@ int tncb_plan_run_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t cou
 int tncb_plan_stage_batch(tncb_ctx* ctx, tncb_plan* plan, size_t n, const tncb_tn* const* tns) {
   using namespace tncb;
   if (!ctx || !plan || !tns || n == 0) return fail(TNCB_ERR_INVALID, "null argument");
-  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
-  if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan has no batched gradients");
-  if (plan->hvp) return hvp_refused();
-  if (!plan->grad && !plan->tangent)
-    return fail(TNCB_ERR_INVALID, "not a gradient or tangent plan (plain plans stage many networks with tncb_plan_stage_slices)");
+  if (int rc = route(plan, Call::stage_batch)) return rc;
   return stage_networks(ctx, plan, n, tns, false);
 }
 
-// Instance-batched reverse mode.  Per pass of c instances on c workspace copies: leaf blocks in, forward levels, values
-// out, seeds in, backward levels, one gather launch that writes gradient rows and/or folds them into the sum.  Every
-// launch decision is the single-network one, so each instance is bit-identical to stage + run + tncb_plan_vjp; passes
-// run in stream order, so the sum is the left fold of the rows in instance order.
+// Instance-batched reverse mode (run_instances): leaf blocks in, forward levels, values out, seeds in, backward levels,
+// one gather launch that writes gradient rows and/or folds them into the sum.  Each instance is bit-identical to
+// stage + run + tncb_plan_vjp.
 int tncb_plan_vjp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t count, const tncb_tensor* seeds,
                         tncb_tensor** values, tncb_tensor** grad_rows, tncb_tensor** grad_sum) {
   using namespace tncb;
   if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
-  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
-  if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan has no batched gradients");
-  if (plan->hvp) return hvp_refused();
-  if (plan->tangent) return fail(TNCB_ERR_UNSUPPORTED, "a tangent plan runs through tncb_plan_jvp_batch");
-  if (!plan->grad) return fail(TNCB_ERR_INVALID, "not a gradient plan (tncb_plan_create_vjp)");
-  if (!plan->slices_dev || plan->ctx != ctx) return fail(TNCB_ERR_INVALID, "tncb_plan_stage_batch has not been called on this context");
-  if (count == 0 || first > plan->n_slices || count > plan->n_slices - first)
-    return fail(TNCB_ERR_INVALID, "instances [" + std::to_string(first) + ", " + std::to_string(first + count) + ") are not within the " +
-                                  std::to_string(plan->n_slices) + " staged networks");
-  if (!values && !grad_rows && !grad_sum) return fail(TNCB_ERR_INVALID, "no output requested");
-  const Schedule& S = plan->S;
-  const SlotMeta& rm = S.slots[S.result_slot];
-  const int r = (int)rm.dims.size();
-  if (r + 1 > kMaxLegs) return fail(TNCB_ERR_INVALID, "a result of rank 64 leaves no room for the instance dimension");
-  const bool grad = grad_rows || grad_sum;
-  if (seeds) {
-    bool same = seeds->rank == r + 1 && seeds->dims[0] == count;
-    for (int i = 0; same && i < r; i++) same = seeds->dims[i + 1] == rm.dims[i];
-    if (!same) return fail(TNCB_ERR_SHAPE, "the seeds' dims differ from [count, result dims]");
-    if (!seeds->ptr) return fail(TNCB_ERR_UNCONTRACTED, "the seed tensor has no storage");
-  } else if (grad && r > 0) return fail(TNCB_ERR_INVALID, "seeds are needed for a result of rank " + std::to_string(r));
-  TNCB_CUDA(cudaSetDevice(ctx->device));
-  BatchBlock B;
-  int rc = batch_size(ctx, plan, count, &B);
+  int rc = route(plan, Call::vjp_batch);
   if (rc) return rc;
-  tncb_tensor *v = nullptr, *gr = nullptr, *gs = nullptr;
-  void* aux = nullptr;                 // the seed 1 of every copy (scalar result, NULL seeds), the K3 scratch of the sum
-  size_t aux_bytes = 0;
-  auto cleanup = [&]() {
-    batch_free(ctx, &B);
-    if (aux) ctx->arena.free(aux, aux_bytes);
-    for (tncb_tensor* t : {v, gr, gs}) if (t) tncb_tensor_free(ctx, t);
-  };
-  const uint64_t ge = plan->grad_elems;
-  if (values) {
-    std::vector<uint64_t> dims(r + 1);
-    dims[0] = count;
-    for (int i = 0; i < r; i++) dims[i + 1] = rm.dims[i];
-    rc = tensor_new(ctx, r + 1, dims.data(), &v);
-  }
-  if (!rc && grad_rows) { const uint64_t dims[2] = {count, ge}; rc = tensor_new(ctx, 2, dims, &gr); }
-  if (!rc && grad_sum) rc = tensor_new(ctx, 1, &ge, &gs);
-  if (!rc) rc = batch_alloc(ctx, &B);
-  const size_t ws = B.ws, c = B.c;
-  const size_t ones = grad && !seeds ? c : 0;
-  size_t scratch = 0;
-  if (grad_sum) for (const auto& gp : plan->grad_permutes) scratch = std::max<size_t>(scratch, S.slots[gp.slot].elems);
-  if (!rc && (ones || scratch)) {
-    aux_bytes = (ones + scratch) * sizeof(double2);
-    rc = ctx->arena.alloc(aux_bytes, &aux);
-    if (!rc && ones) {
-      const std::vector<double2> one(ones, double2{1.0, 0.0});
-      cudaError_t e = cudaMemcpyAsync(aux, one.data(), ones * sizeof(double2), cudaMemcpyHostToDevice, ctx->stream);
-      if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);      // `one` dies with this scope
-      if (e != cudaSuccess) rc = fail(TNCB_ERR_CUDA, std::string("seed copy: ") + cudaGetErrorString(e));
-    }
-  }
-  if (!rc && gs) {
-    cudaError_t e = cudaMemsetAsync(gs->ptr, 0, std::max<uint64_t>(ge, 1) * sizeof(double2), ctx->stream);
-    if (e != cudaSuccess) rc = fail(TNCB_ERR_CUDA, std::string("gradient sum: ") + cudaGetErrorString(e));
-  }
-  if (rc) { cleanup(); return rc; }
-  char* base = (char*)B.blk;
-  const double2* d_one = (const double2*)aux;
-  double2* d_scratch = (double2*)aux + ones;
-  const size_t block_bytes = std::max<size_t>(S.leaf_block_elems, 1) * sizeof(double2);
-  const size_t res_bytes = rm.elems * sizeof(double2);
-  const int n_levels = (int)plan->level_batched.size();
-  for (size_t done = 0; done < count && !rc; done += c) {
-    const size_t n = std::min(c, count - done);
-    const char* src = (const char*)plan->slices_dev + (first + done) * block_bytes;
-    if ((rc = batch_copy(ctx, B, base + plan->leaf_off, ws, src, block_bytes, block_bytes, n))) break;
-    if ((rc = enqueue_static(ctx, plan, base, (int)n, (long long)ws, 0, plan->n_fwd_levels))) break;
-    if (v && res_bytes &&
-        (rc = batch_copy(ctx, B, (char*)v->ptr + done * res_bytes, res_bytes, base + plan->slot_off[S.result_slot], ws, res_bytes, n))) break;
-    if (!grad) continue;
-    char* seed_dst = base + plan->slot_off[plan->seed_slot];
-    if (seeds) { if (res_bytes && (rc = batch_copy(ctx, B, seed_dst, ws, (const char*)seeds->ptr + done * res_bytes, res_bytes, res_bytes, n))) break; }
-    else if ((rc = batch_copy(ctx, B, seed_dst, ws, (const char*)d_one, sizeof(double2), sizeof(double2), n))) break;
-    if ((rc = enqueue_static(ctx, plan, base, (int)n, (long long)ws, plan->n_fwd_levels, n_levels))) break;
-    rc = gather_set_batch(ctx, plan, plan->grad_items, plan->grad_block_start, plan->grad_permutes, plan->grad_dev, base, ws, n,
-                          gr ? gr->ptr + done * ge : nullptr, ge, gs ? gs->ptr : nullptr, d_scratch);
-  }
-  if (rc) { cleanup(); return rc; }
-  batch_free(ctx, &B);
-  if (aux) ctx->arena.free(aux, aux_bytes);
-  if (values) *values = v;
-  if (grad_rows) *grad_rows = gr;
-  if (grad_sum) *grad_sum = gs;
-  return TNCB_OK;
+  if (!plan->slices_dev || plan->ctx != ctx) return fail(TNCB_ERR_INVALID, "tncb_plan_stage_batch has not been called on this context");
+  if ((rc = instance_range(plan, first, count))) return rc;
+  if (!values && !grad_rows && !grad_sum) return fail(TNCB_ERR_INVALID, "no output requested");
+  std::vector<uint64_t> rows;
+  if ((rc = result_rows(plan, count, rows))) return rc;
+  if (seeds) { if ((rc = seed_rows(seeds, rows, "seeds", "seed"))) return rc; }
+  else if ((grad_rows || grad_sum) && rows.size() > 1)
+    return fail(TNCB_ERR_INVALID, "seeds are needed for a result of rank " + std::to_string(rows.size() - 1));
+  InstanceIO io;
+  io.seeds = seeds;
+  io.values = values; io.grad_rows = grad_rows; io.grad_sum = grad_sum;
+  return run_instances(ctx, plan, rows, {first}, io);
 }
-
-// A tangent plan: the forward schedule and the tangent pairs of the `wrt` leaves, on the forward levels of one static
-// layout.  There is no pair-by-pair fallback: a layout above the static-workspace limit is refused here.
-int tncb_plan_create_jvp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, const uint8_t* wrt, tncb_plan** out) {
-  using namespace tncb;
-  if (!tn || !out) return fail(TNCB_ERR_INVALID, "null argument");
-  {
-    std::vector<const tncb_tn*> lv;
-    collect_leaf_nodes(tn, lv);
-    for (const tncb_tn* l : lv)
-      if (l->kind == TNCB_DATA_DEVICE) return fail(TNCB_ERR_UNSUPPORTED, "tangent plans do not take device leaves (they are consumed per call)");
-  }
-  tncb_plan* p = new tncb_plan();
-  p->tangent = true;
-  int rc = build_schedule(tn, path, p->S);
-  if (!rc) rc = build_tangent(p, wrt);
-  if (rc) { delete p; return rc; }
-  size_t dev_free = 0, dev_total = 0;
-  if (ctx) { cudaSetDevice(ctx->device); if (cudaMemGetInfo(&dev_free, &dev_total) != cudaSuccess) { dev_total = 0; cudaGetLastError(); } }
-  plan_static_layout(p, ctx ? ctx->sm_count : 132, dev_total);
-  if (!p->is_static) {
-    const size_t need = p->ws_bytes, limit = static_ws_limit(dev_total);
-    delete p;
-    return fail(TNCB_ERR_UNSUPPORTED, "the tangent workspace needs " + std::to_string(need) + " bytes, above the static-workspace limit of " +
-                                      std::to_string(limit) + " bytes (TNCB_PLAN_WS_GB)");
-  }
-  *out = p;
-  return TNCB_OK;
-}
-
-namespace tncb {
-// the checks tncb_plan_jvp and tncb_plan_jvp_batch share: a tangent plan, an output, tangents shaped `want` with storage
-static int jvp_args(const tncb_plan* plan, const tncb_tensor* tangents, bool any_out, const std::vector<uint64_t>& want) {
-  if (!plan->tangent) return fail(TNCB_ERR_INVALID, "not a tangent plan (tncb_plan_create_jvp)");
-  if (!any_out) return fail(TNCB_ERR_INVALID, "no output requested");
-  if (!tangents) return fail(TNCB_ERR_INVALID, "tangents are needed");
-  bool same = tangents->rank == (int)want.size();
-  for (size_t i = 0; same && i < want.size(); i++) same = tangents->dims[i] == want[i];
-  if (!same) {
-    std::string w;
-    for (uint64_t d : want) w += (w.empty() ? "" : ", ") + std::to_string(d);
-    return fail(TNCB_ERR_SHAPE, "the tangents' dims differ from [" + w + "]");
-  }
-  if (!tangents->ptr) return fail(TNCB_ERR_UNCONTRACTED, "the tangent tensor has no storage");
-  return TNCB_OK;
-}
-
-// the leaf tangents of n instances (rows of `row_elems` elements from `tangents` on) into the workspaces at `ws`,
-// `stride` bytes apart: one leaf_stage_kernel launch, the instance a grid dimension
-static int stage_tangents(tncb_ctx* ctx, const tncb_plan* P, const double2* tangents, unsigned long long row_elems,
-                          char* ws, long long stride, size_t n) {
-  std::vector<LeafStageItem> items;
-  for (const auto& tl : P->tan_leaves)
-    items.push_back({tangents + tl.off, n > 1 ? row_elems : 0, (long long)(P->slot_off[tl.slot] / sizeof(double2)),
-                     (long long)P->S.slots[tl.slot].elems});
-  return launch_leaf_stage(ctx, items.data(), items.size(), (double2*)ws, stride / (long long)sizeof(double2), n);
-}
-} // namespace tncb
 
 // One forward-mode pass on the staged leaves: leaf tangents in, every level (forward pairs, tangent pairs, sums), the
 // result and its tangent out.  Nothing is kept between calls, so a call can be repeated and gives the same bits.
 int tncb_plan_jvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, tncb_tensor** value, tncb_tensor** tangent_out) {
   using namespace tncb;
   if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
-  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
-  if (plan->hvp) return hvp_refused();
-  int rc = jvp_args(plan, tangents, value || tangent_out, {plan->grad_elems});
-  if (rc) return rc;
+  int rc = route(plan, Call::jvp);
+  if (rc || (rc = jvp_args(tangents, value || tangent_out, {plan->grad_elems}))) return rc;
   if (plan->ctx != ctx || !plan->leaves_resident) return fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this plan and context");
   TNCB_CUDA(cudaSetDevice(ctx->device));
-  const Schedule& S = plan->S;
-  const SlotMeta& rm = S.slots[S.result_slot];
-  tncb_tensor *v = nullptr, *t = nullptr;
-  if (value) rc = tensor_new(ctx, (int)rm.dims.size(), rm.dims.data(), &v);
-  if (!rc && tangent_out) rc = tensor_new(ctx, (int)rm.dims.size(), rm.dims.data(), &t);
+  const SlotMeta& rm = plan->S.slots[plan->S.result_slot];
+  Outputs out{ctx};
+  tncb_tensor* v = out.add(value, (int)rm.dims.size(), rm.dims.data());
+  tncb_tensor* t = out.add(tangent_out, (int)rm.dims.size(), rm.dims.data());
   char* ws = (char*)plan->ws;
-  if (!rc) rc = stage_tangents(ctx, plan, tangents->ptr, plan->grad_elems, ws, 0, 1);
+  if (!(rc = out.rc)) rc = stage_tangents(ctx, plan, tangents->ptr, plan->grad_elems, ws, 0, 1);
   if (!rc) rc = enqueue_static(ctx, plan, ws, 1, 0, 0, (int)plan->level_batched.size());
-  const size_t res_bytes = rm.elems * sizeof(double2);
-  for (auto [dst, slot] : {std::pair<tncb_tensor*, int>{v, S.result_slot}, {t, plan->tan_result}}) {
-    if (rc || !dst || !res_bytes) continue;
-    cudaError_t e = cudaMemcpyAsync(dst->ptr, ws + plan->slot_off[slot], res_bytes, cudaMemcpyDeviceToDevice, ctx->stream);
-    if (e != cudaSuccess) rc = fail(TNCB_ERR_CUDA, std::string("result copy: ") + cudaGetErrorString(e));
-  }
-  if (rc) {
-    for (tncb_tensor* x : {v, t}) if (x) tncb_tensor_free(ctx, x);
-    return rc;
-  }
-  if (value) *value = v;
-  if (tangent_out) *tangent_out = t;
-  return TNCB_OK;
+  if (!rc) rc = copy_results(ctx, plan, ws, v, t);
+  return out.finish(rc);
 }
 
-// Instance-batched forward mode over the networks staged by tncb_plan_stage_batch / tncb_plan_stage_instances.  Per pass
-// of c instances on c workspace copies: leaf blocks in, leaf tangents in (row i of `tangents` for instance i), every
-// level, values and tangents out.  Every launch decision is the single-network one, so row i is bit-identical to
-// tncb_plan_jvp of instance i with tangent row i.
+// Instance-batched forward mode (run_instances) over the networks staged by tncb_plan_stage_batch /
+// tncb_plan_stage_instances: leaf blocks in, leaf tangents in (row i of `tangents` for instance i), every level, values
+// and tangents out.  Row i is bit-identical to tncb_plan_jvp of instance i with tangent row i.
 int tncb_plan_jvp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t count, const tncb_tensor* tangents,
                         tncb_tensor** values, tncb_tensor** tangent_rows) {
   using namespace tncb;
   if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
-  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
-  if (plan->hvp) return hvp_refused();
-  if (!plan->tangent) return fail(TNCB_ERR_INVALID, "not a tangent plan (tncb_plan_create_jvp)");
+  int rc = route(plan, Call::jvp_batch);
+  if (rc) return rc;
   if (!plan->slices_dev || plan->ctx != ctx)
     return fail(TNCB_ERR_INVALID, "tncb_plan_stage_batch / tncb_plan_stage_instances has not been called on this context");
-  if (count == 0 || first > plan->n_slices || count > plan->n_slices - first)
-    return fail(TNCB_ERR_INVALID, "instances [" + std::to_string(first) + ", " + std::to_string(first + count) + ") are not within the " +
-                                  std::to_string(plan->n_slices) + " staged networks");
-  const Schedule& S = plan->S;
-  const SlotMeta& rm = S.slots[S.result_slot];
-  const int r = (int)rm.dims.size();
-  if (r + 1 > kMaxLegs) return fail(TNCB_ERR_INVALID, "a result of rank 64 leaves no room for the instance dimension");
-  int rc = jvp_args(plan, tangents, values || tangent_rows, {(uint64_t)count, plan->grad_elems});
-  if (rc) return rc;
-  TNCB_CUDA(cudaSetDevice(ctx->device));
-  BatchBlock B;
-  if ((rc = batch_size(ctx, plan, count, &B))) return rc;
-  std::vector<uint64_t> dims(r + 1);
-  dims[0] = count;
-  for (int i = 0; i < r; i++) dims[i + 1] = rm.dims[i];
-  tncb_tensor *v = nullptr, *t = nullptr;
-  if (values) rc = tensor_new(ctx, r + 1, dims.data(), &v);
-  if (!rc && tangent_rows) rc = tensor_new(ctx, r + 1, dims.data(), &t);
-  if (!rc) rc = batch_alloc(ctx, &B);
-  const size_t ws = B.ws, c = B.c;
-  char* base = (char*)B.blk;
-  const size_t block_bytes = std::max<size_t>(S.leaf_block_elems, 1) * sizeof(double2);
-  const size_t res_bytes = rm.elems * sizeof(double2);
-  const uint64_t te = plan->grad_elems;
-  for (size_t done = 0; done < count && !rc; done += c) {
-    const size_t n = std::min(c, count - done);
-    const char* src = (const char*)plan->slices_dev + (first + done) * block_bytes;
-    if ((rc = batch_copy(ctx, B, base + plan->leaf_off, ws, src, block_bytes, block_bytes, n))) break;
-    if ((rc = stage_tangents(ctx, plan, tangents->ptr + done * te, te, base, (long long)ws, n))) break;
-    if ((rc = enqueue_static(ctx, plan, base, (int)n, (long long)ws, 0, (int)plan->level_batched.size()))) break;
-    if (!res_bytes) continue;
-    if (v && (rc = batch_copy(ctx, B, (char*)v->ptr + done * res_bytes, res_bytes, base + plan->slot_off[S.result_slot], ws, res_bytes, n))) break;
-    if (t && (rc = batch_copy(ctx, B, (char*)t->ptr + done * res_bytes, res_bytes, base + plan->slot_off[plan->tan_result], ws, res_bytes, n))) break;
-  }
-  batch_free(ctx, &B);
-  if (rc) {
-    for (tncb_tensor* x : {v, t}) if (x) tncb_tensor_free(ctx, x);
+  std::vector<uint64_t> rows;
+  if ((rc = instance_range(plan, first, count)) || (rc = result_rows(plan, count, rows)) ||
+      (rc = jvp_args(tangents, values || tangent_rows, {(uint64_t)count, plan->grad_elems})))
     return rc;
-  }
-  if (values) *values = v;
-  if (tangent_rows) *tangent_rows = t;
-  return TNCB_OK;
+  InstanceIO io;
+  io.tangents = tangents;
+  io.values = values; io.tangent_rows = tangent_rows;
+  return run_instances(ctx, plan, rows, {first}, io);
 }
-
-// A Hessian-vector plan: the forward schedule, the tangent pairs (build_tangent), the backward pairs (build_backward) and
-// the backward-tangent pairs of the `wrt` leaves, plus the gathers of G and Ġ, in one static layout.  There is no
-// pair-by-pair fallback: a layout above the static-workspace limit is refused here.
-int tncb_plan_create_hvp(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, const uint8_t* wrt, tncb_plan** out) {
-  using namespace tncb;
-  if (!tn || !out) return fail(TNCB_ERR_INVALID, "null argument");
-  {
-    std::vector<const tncb_tn*> lv;
-    collect_leaf_nodes(tn, lv);
-    for (const tncb_tn* l : lv)
-      if (l->kind == TNCB_DATA_DEVICE) return fail(TNCB_ERR_UNSUPPORTED, "Hessian-vector plans do not take device leaves (they are consumed per call)");
-  }
-  tncb_plan* p = new tncb_plan();
-  p->hvp = p->grad = p->tangent = true;
-  std::vector<int> tan, leaf_adj, leaf_dadj;
-  int rc = build_schedule(tn, path, p->S);
-  size_t n_fwd = 0, b0 = 0;
-  if (!rc) { n_fwd = p->S.steps.size(); rc = build_tangent(p, wrt, &tan); }
-  if (!rc) { b0 = p->S.steps.size(); rc = build_backward(p, wrt, leaf_adj, n_fwd); }
-  if (!rc) rc = build_backward_tangent(p, b0, tan, leaf_adj, leaf_dadj);
-  if (rc) { delete p; return rc; }
-  size_t dev_free = 0, dev_total = 0;
-  if (ctx) { cudaSetDevice(ctx->device); if (cudaMemGetInfo(&dev_free, &dev_total) != cudaSuccess) { dev_total = 0; cudaGetLastError(); } }
-  plan_static_layout(p, ctx ? ctx->sm_count : 132, dev_total);
-  if (!p->is_static) {
-    const size_t need = p->ws_bytes, limit = static_ws_limit(dev_total);
-    delete p;
-    return fail(TNCB_ERR_UNSUPPORTED, "the Hessian-vector workspace needs " + std::to_string(need) + " bytes, above the static-workspace limit of " +
-                                      std::to_string(limit) + " bytes (TNCB_PLAN_WS_GB)");
-  }
-  if ((rc = build_gather(p, leaf_adj, p->grad_items, p->grad_block_start, p->grad_permutes)) ||
-      (rc = build_gather(p, leaf_dadj, p->dgrad_items, p->dgrad_block_start, p->dgrad_permutes))) { delete p; return rc; }
-  *out = p;
-  return TNCB_OK;
-}
-
-namespace tncb {
-// a seed or seed tangent: the result's dims, with storage
-static int seed_args(const SlotMeta& rm, const tncb_tensor* t, const char* what) {
-  bool same = t->rank == (int)rm.dims.size();
-  for (int i = 0; same && i < t->rank; i++) same = t->dims[i] == rm.dims[i];
-  if (!same) return fail(TNCB_ERR_SHAPE, std::string("the ") + what + "'s dims differ from the result's");
-  if (!t->ptr) return fail(TNCB_ERR_UNCONTRACTED, std::string("the ") + what + " tensor has no storage");
-  return TNCB_OK;
-}
-
-// one gather set (grad_* or dgrad_*) from the workspace into the packed block `out`: one grad_gather_kernel launch, K3
-// for the leaves with more fused groups than a GradItem holds
-static int gather_set(tncb_ctx* ctx, const tncb_plan* P, const std::vector<GradItem>& items, const std::vector<long long>& bs,
-                      const std::vector<tncb_plan::GradPermute>& permutes, const void* dev, const char* ws, double2* out) {
-  int rc = TNCB_OK;
-  if (!items.empty())
-    rc = launch_grad_gather(ctx, (const GradItem*)dev, (const long long*)((const char*)dev + items.size() * sizeof(GradItem)),
-                            (int)items.size(), bs.back(), ws, out);
-  for (size_t i = 0; i < permutes.size() && !rc; i++) {
-    const auto& gp = permutes[i];
-    const SlotMeta& sm = P->S.slots[gp.slot];
-    rc = launch_permute(ctx, (const double2*)(ws + P->slot_off[gp.slot]), out + gp.dst, (int)sm.dims.size(), sm.dims.data(), gp.perm.data());
-  }
-  return rc;
-}
-} // namespace tncb
 
 // One forward-over-reverse pass on the staged leaves: leaf tangents in, the forward levels (forward pairs, tangent pairs,
 // sums), R and Ṙ out, the seed and its tangent in, the backward levels (backward pairs, backward-tangent pairs, sums),
@@ -2218,63 +2162,33 @@ int tncb_plan_hvp(tncb_ctx* ctx, tncb_plan* plan, const tncb_tensor* tangents, c
                   tncb_tensor** grad_tangents) {
   using namespace tncb;
   if (!ctx || !plan) return fail(TNCB_ERR_INVALID, "null argument");
-  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
-  if (!plan->hvp) return fail(TNCB_ERR_INVALID, "not a Hessian-vector plan (tncb_plan_create_hvp)");
-  int rc = jvp_args(plan, tangents, value || tangent_out || grads || grad_tangents, {plan->grad_elems});
-  if (rc) return rc;
-  const Schedule& S = plan->S;
-  const SlotMeta& rm = S.slots[S.result_slot];
-  if (seed) { if ((rc = seed_args(rm, seed, "seed"))) return rc; }
-  else if (!rm.dims.empty()) return fail(TNCB_ERR_INVALID, "a seed is needed for a result of rank " + std::to_string(rm.dims.size()));
-  if (seed_tangent && (rc = seed_args(rm, seed_tangent, "seed tangent"))) return rc;
+  int rc = route(plan, Call::hvp);
+  if (rc || (rc = jvp_args(tangents, value || tangent_out || grads || grad_tangents, {plan->grad_elems}))) return rc;
+  const SlotMeta& rm = plan->S.slots[plan->S.result_slot];
+  if ((rc = seed_args(rm, seed, "seed", true)) || (rc = seed_args(rm, seed_tangent, "seed tangent"))) return rc;
   if (plan->ctx != ctx || !plan->leaves_resident) return fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this plan and context");
   TNCB_CUDA(cudaSetDevice(ctx->device));
   const uint64_t ge = plan->grad_elems;
-  tncb_tensor *v = nullptr, *t = nullptr, *g = nullptr, *dg = nullptr;
-  if (value) rc = tensor_new(ctx, (int)rm.dims.size(), rm.dims.data(), &v);
-  if (!rc && tangent_out) rc = tensor_new(ctx, (int)rm.dims.size(), rm.dims.data(), &t);
-  if (!rc && grads) rc = tensor_new(ctx, 1, &ge, &g);
-  if (!rc && grad_tangents) rc = tensor_new(ctx, 1, &ge, &dg);
+  Outputs out{ctx};
+  tncb_tensor* v = out.add(value, (int)rm.dims.size(), rm.dims.data());
+  tncb_tensor* t = out.add(tangent_out, (int)rm.dims.size(), rm.dims.data());
+  tncb_tensor* g = out.add(grads, 1, &ge);
+  tncb_tensor* dg = out.add(grad_tangents, 1, &ge);
   char* ws = (char*)plan->ws;
-  if (!rc) rc = stage_tangents(ctx, plan, tangents->ptr, ge, ws, 0, 1);
+  if (!(rc = out.rc)) rc = stage_tangents(ctx, plan, tangents->ptr, ge, ws, 0, 1);
   if (!rc) rc = enqueue_static(ctx, plan, ws, 1, 0, 0, plan->n_fwd_levels);
-  const size_t res_bytes = rm.elems * sizeof(double2);
-  for (auto [dst, slot] : {std::pair<tncb_tensor*, int>{v, S.result_slot}, {t, plan->tan_result}}) {
-    if (rc || !dst || !res_bytes) continue;
-    cudaError_t e = cudaMemcpyAsync(dst->ptr, ws + plan->slot_off[slot], res_bytes, cudaMemcpyDeviceToDevice, ctx->stream);
-    if (e != cudaSuccess) rc = fail(TNCB_ERR_CUDA, std::string("result copy: ") + cudaGetErrorString(e));
-  }
-  // the seed slots may reuse memory the forward levels freed: written after them, on the stream
-  if (!rc) {
-    static const double2 one = {1.0, 0.0};
-    char* s = ws + plan->slot_off[plan->seed_slot];
-    char* ds = ws + plan->slot_off[plan->seed_tan_slot];
-    cudaError_t e = seed ? cudaMemcpyAsync(s, seed->ptr, res_bytes, cudaMemcpyDeviceToDevice, ctx->stream)
-                         : cudaMemcpyAsync(s, &one, sizeof(double2), cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess)
-      e = seed_tangent ? cudaMemcpyAsync(ds, seed_tangent->ptr, res_bytes, cudaMemcpyDeviceToDevice, ctx->stream)
-                       : cudaMemsetAsync(ds, 0, res_bytes, ctx->stream);
-    if (e != cudaSuccess) rc = fail(TNCB_ERR_CUDA, std::string("seed copy: ") + cudaGetErrorString(e));
-  }
+  if (!rc) rc = copy_results(ctx, plan, ws, v, t);
+  if (!rc) rc = write_seed(ctx, plan, ws, seed, seed_tangent);
   if (!rc) rc = enqueue_static(ctx, plan, ws, 1, 0, plan->n_fwd_levels, (int)plan->level_batched.size());
   if (!rc && g) rc = gather_set(ctx, plan, plan->grad_items, plan->grad_block_start, plan->grad_permutes, plan->grad_dev, ws, g->ptr);
   if (!rc && dg) rc = gather_set(ctx, plan, plan->dgrad_items, plan->dgrad_block_start, plan->dgrad_permutes, plan->dgrad_dev, ws, dg->ptr);
-  if (rc) {
-    for (tncb_tensor* x : {v, t, g, dg}) if (x) tncb_tensor_free(ctx, x);
-    return rc;
-  }
-  if (value) *value = v;
-  if (tangent_out) *tangent_out = t;
-  if (grads) *grads = g;
-  if (grad_tangents) *grad_tangents = dg;
-  return TNCB_OK;
+  return out.finish(rc);
 }
 
-// Instance-batched forward over reverse.  Per pass of c instances on c workspace copies beside the plan's own: one launch
-// fills every copy's leaf block (the device payloads, and the staged block's runs between them at stride 0), the leaf
-// tangents, the forward levels, R and Ṙ out, seeds and seed tangents in, the backward levels, the gathers of G and Ġ
-// into rows and/or sums.  Every launch decision is the single-network one, so row i is bit-identical to set_leaves +
-// tncb_plan_hvp of instance i; passes run in stream order, so the sums are the left folds of the rows in instance order.
+// Instance-batched forward over reverse (run_instances) on c workspace copies beside the plan's own: one launch fills
+// every copy's leaf block (the device payloads, and the staged block's runs between them at stride 0), the leaf tangents,
+// the forward levels, R and Ṙ out, seeds and seed tangents in, the backward levels, the gathers of G and Ġ into rows
+// and/or sums.  Row i is bit-identical to set_leaves + tncb_plan_hvp of instance i.
 int tncb_plan_hvp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t count, size_t n, const uint64_t* leaf_index,
                         const void* const* src, const uint64_t* instance_stride, const tncb_tensor* tangents,
                         const tncb_tensor* seeds, const tncb_tensor* seed_tangents, tncb_tensor** values,
@@ -2282,125 +2196,26 @@ int tncb_plan_hvp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t count, size_t n, 
                         tncb_tensor** grad_tangent_rows, tncb_tensor** grad_tangent_sum) {
   using namespace tncb;
   if (!ctx || !plan || (n && (!leaf_index || !src || !instance_stride))) return fail(TNCB_ERR_INVALID, "null argument");
-  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
-  if (!plan->hvp) return fail(TNCB_ERR_INVALID, "not a Hessian-vector plan (tncb_plan_create_hvp)");
-  if (count == 0) return fail(TNCB_ERR_INVALID, "count is 0");
-  const bool backward = grad_rows || grad_sum || grad_tangent_rows || grad_tangent_sum;
-  const uint64_t ge = plan->grad_elems;
-  int rc = jvp_args(plan, tangents, values || tangent_rows || backward, {(uint64_t)count, ge});
+  int rc = route(plan, Call::hvp_batch);
   if (rc) return rc;
-  const Schedule& S = plan->S;
-  const SlotMeta& rm = S.slots[S.result_slot];
-  const int r = (int)rm.dims.size();
-  if (r + 1 > kMaxLegs) return fail(TNCB_ERR_INVALID, "a result of rank 64 leaves no room for the instance dimension");
-  std::vector<uint64_t> rdims(r + 1);
-  rdims[0] = count;
-  for (int i = 0; i < r; i++) rdims[i + 1] = rm.dims[i];
-  for (auto [t, what] : {std::pair<const tncb_tensor*, const char*>{seeds, "seeds"}, {seed_tangents, "seed tangents"}}) {
-    if (!t) continue;
-    bool same = t->rank == r + 1;
-    for (int i = 0; same && i <= r; i++) same = t->dims[i] == rdims[i];
-    if (!same) return fail(TNCB_ERR_SHAPE, std::string("the ") + what + "' dims differ from [count, result dims]");
-    if (!t->ptr) return fail(TNCB_ERR_UNCONTRACTED, std::string("the ") + what + " tensor has no storage");
-  }
-  if (!seeds && r > 0) return fail(TNCB_ERR_INVALID, "seeds are needed for a result of rank " + std::to_string(r));
+  if (count == 0) return fail(TNCB_ERR_INVALID, "count is 0");
+  const bool any_out = values || tangent_rows || grad_rows || grad_sum || grad_tangent_rows || grad_tangent_sum;
+  std::vector<uint64_t> rows;
+  if ((rc = jvp_args(tangents, any_out, {(uint64_t)count, plan->grad_elems})) || (rc = result_rows(plan, count, rows)) ||
+      (seeds && (rc = seed_rows(seeds, rows, "seeds", "seeds"))) ||
+      (seed_tangents && (rc = seed_rows(seed_tangents, rows, "seed tangents", "seed tangents"))))
+    return rc;
+  if (!seeds && rows.size() > 1) return fail(TNCB_ERR_INVALID, "seeds are needed for a result of rank " + std::to_string(rows.size() - 1));
   if (plan->ctx != ctx || !plan->leaves_resident) return fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this plan and context");
   TNCB_CUDA(cudaSetDevice(ctx->device));
   std::vector<LeafStageItem> dev_items;
-  if ((rc = device_items(ctx, S, count, n, leaf_index, src, instance_stride, dev_items))) return rc;
-  const size_t block = std::max<size_t>(S.leaf_block_elems, 1);
-  const double2* staged = (const double2*)((const char*)plan->ws + plan->leaf_off);
-  const std::vector<LeafRun> runs = leaf_runs(dev_items, (long long)block);
-  BatchBlock B;
-  if ((rc = batch_size(ctx, plan, count, &B))) return rc;
-  tncb_tensor *v = nullptr, *t = nullptr, *gr = nullptr, *gs = nullptr, *dgr = nullptr, *dgs = nullptr;
-  void* aux = nullptr;                 // the seed 1 of every copy (scalar result, NULL seeds), the K3 scratch of the sums
-  size_t aux_bytes = 0;
-  auto cleanup = [&]() {
-    batch_free(ctx, &B);
-    if (aux) ctx->arena.free(aux, aux_bytes);
-    for (tncb_tensor* x : {v, t, gr, gs, dgr, dgs}) if (x) tncb_tensor_free(ctx, x);
-  };
-  const uint64_t row_dims[2] = {(uint64_t)count, ge};
-  if (values) rc = tensor_new(ctx, r + 1, rdims.data(), &v);
-  if (!rc && tangent_rows) rc = tensor_new(ctx, r + 1, rdims.data(), &t);
-  if (!rc && grad_rows) rc = tensor_new(ctx, 2, row_dims, &gr);
-  if (!rc && grad_sum) rc = tensor_new(ctx, 1, &ge, &gs);
-  if (!rc && grad_tangent_rows) rc = tensor_new(ctx, 2, row_dims, &dgr);
-  if (!rc && grad_tangent_sum) rc = tensor_new(ctx, 1, &ge, &dgs);
-  if (!rc) rc = batch_alloc(ctx, &B);
-  const size_t ws = B.ws, c = B.c;
-  const size_t ones = backward && !seeds ? c : 0;
-  size_t scratch = 0;
-  if (grad_sum) for (const auto& gp : plan->grad_permutes) scratch = std::max<size_t>(scratch, S.slots[gp.slot].elems);
-  if (grad_tangent_sum) for (const auto& gp : plan->dgrad_permutes) scratch = std::max<size_t>(scratch, S.slots[gp.slot].elems);
-  if (!rc && (ones || scratch)) {
-    aux_bytes = (ones + scratch) * sizeof(double2);
-    rc = ctx->arena.alloc(aux_bytes, &aux);
-    if (!rc && ones) {
-      const std::vector<double2> one(ones, double2{1.0, 0.0});
-      cudaError_t e = cudaMemcpyAsync(aux, one.data(), ones * sizeof(double2), cudaMemcpyHostToDevice, ctx->stream);
-      if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);      // `one` dies with this scope
-      if (e != cudaSuccess) rc = fail(TNCB_ERR_CUDA, std::string("seed copy: ") + cudaGetErrorString(e));
-    }
-  }
-  for (tncb_tensor* x : {gs, dgs}) {
-    if (rc || !x) continue;
-    cudaError_t e = cudaMemsetAsync(x->ptr, 0, std::max<uint64_t>(ge, 1) * sizeof(double2), ctx->stream);
-    if (e != cudaSuccess) rc = fail(TNCB_ERR_CUDA, std::string("gradient sum: ") + cudaGetErrorString(e));
-  }
-  if (rc) { cleanup(); return rc; }
-  char* base = (char*)B.blk;
-  const double2* d_one = (const double2*)aux;
-  double2* d_scratch = (double2*)aux + ones;
-  const size_t res_bytes = rm.elems * sizeof(double2);
-  const int n_levels = (int)plan->level_batched.size();
-  std::vector<LeafStageItem> items;
-  for (size_t done = 0; done < count && !rc; done += c) {
-    const size_t m = std::min(c, count - done);
-    // every copy's leaf block: the device payloads of instances done .. done+m-1, the staged block between them
-    items.clear();
-    for (const LeafStageItem& it : dev_items) items.push_back({it.src + done * it.src_stride, it.src_stride, it.dst, it.elems});
-    for (const LeafRun& lr : runs) items.push_back({staged + lr.start, 0, lr.start, lr.len});
-    if ((rc = launch_leaf_stage(ctx, items.data(), items.size(), (double2*)(base + plan->leaf_off), (long long)(ws / sizeof(double2)), m))) break;
-    if ((rc = stage_tangents(ctx, plan, tangents->ptr + done * ge, ge, base, (long long)ws, m))) break;
-    if ((rc = enqueue_static(ctx, plan, base, (int)m, (long long)ws, 0, plan->n_fwd_levels))) break;
-    if (v && res_bytes &&
-        (rc = batch_copy(ctx, B, (char*)v->ptr + done * res_bytes, res_bytes, base + plan->slot_off[S.result_slot], ws, res_bytes, m))) break;
-    if (t && res_bytes &&
-        (rc = batch_copy(ctx, B, (char*)t->ptr + done * res_bytes, res_bytes, base + plan->slot_off[plan->tan_result], ws, res_bytes, m))) break;
-    if (!backward) continue;
-    // the seed slots may reuse memory the forward levels freed: written after them, on the stream
-    char* seed_dst = base + plan->slot_off[plan->seed_slot];
-    char* seed_tan_dst = base + plan->slot_off[plan->seed_tan_slot];
-    if (seeds) { if (res_bytes && (rc = batch_copy(ctx, B, seed_dst, ws, (const char*)seeds->ptr + done * res_bytes, res_bytes, res_bytes, m))) break; }
-    else if ((rc = batch_copy(ctx, B, seed_dst, ws, (const char*)d_one, sizeof(double2), sizeof(double2), m))) break;
-    if (seed_tangents) {
-      if (res_bytes && (rc = batch_copy(ctx, B, seed_tan_dst, ws, (const char*)seed_tangents->ptr + done * res_bytes, res_bytes, res_bytes, m))) break;
-    } else if (res_bytes) {
-      cudaError_t e = cudaSuccess;
-      if (B.strided) e = cudaMemset2DAsync(seed_tan_dst, ws, 0, res_bytes, m, ctx->stream);
-      else for (size_t i = 0; i < m && e == cudaSuccess; i++) e = cudaMemsetAsync(seed_tan_dst + i * ws, 0, res_bytes, ctx->stream);
-      if (e != cudaSuccess) { rc = fail(TNCB_ERR_CUDA, std::string("seed tangent: ") + cudaGetErrorString(e)); break; }
-    }
-    if ((rc = enqueue_static(ctx, plan, base, (int)m, (long long)ws, plan->n_fwd_levels, n_levels))) break;
-    if ((gr || gs) &&
-        (rc = gather_set_batch(ctx, plan, plan->grad_items, plan->grad_block_start, plan->grad_permutes, plan->grad_dev, base, ws, m,
-                               gr ? gr->ptr + done * ge : nullptr, ge, gs ? gs->ptr : nullptr, d_scratch))) break;
-    if (dgr || dgs)
-      rc = gather_set_batch(ctx, plan, plan->dgrad_items, plan->dgrad_block_start, plan->dgrad_permutes, plan->dgrad_dev, base, ws, m,
-                            dgr ? dgr->ptr + done * ge : nullptr, ge, dgs ? dgs->ptr : nullptr, d_scratch);
-  }
-  if (rc) { cleanup(); return rc; }
-  batch_free(ctx, &B);
-  if (aux) ctx->arena.free(aux, aux_bytes);
-  if (values) *values = v;
-  if (tangent_rows) *tangent_rows = t;
-  if (grad_rows) *grad_rows = gr;
-  if (grad_sum) *grad_sum = gs;
-  if (grad_tangent_rows) *grad_tangent_rows = dgr;
-  if (grad_tangent_sum) *grad_tangent_sum = dgs;
-  return TNCB_OK;
+  if ((rc = device_items(ctx, plan->S, count, n, leaf_index, src, instance_stride, dev_items))) return rc;
+  const std::vector<LeafRun> runs = leaf_runs(dev_items, (long long)std::max<size_t>(plan->S.leaf_block_elems, 1));
+  InstanceIO io;
+  io.tangents = tangents; io.seeds = seeds; io.seed_tangents = seed_tangents;
+  io.values = values; io.tangent_rows = tangent_rows; io.grad_rows = grad_rows; io.grad_sum = grad_sum;
+  io.grad_tangent_rows = grad_tangent_rows; io.grad_tangent_sum = grad_tangent_sum;
+  return run_instances(ctx, plan, rows, {0, &dev_items, &runs}, io);
 }
 
 namespace tncb {
@@ -2409,27 +2224,19 @@ static int sliced_tangent_call(tncb_ctx* ctx, tncb_plan* plan, bool hvp, size_t 
                                const tncb_tensor* seed, const tncb_tensor* seed_tangent, tncb_tensor** value,
                                tncb_tensor** tangent_out, tncb_tensor** grads, tncb_tensor** grad_tangents) {
   if (!ctx || !plan || stride == 0) return fail(TNCB_ERR_INVALID, "bad argument");
-  if (!sliced_tangent(plan) || plan->hvp != hvp)
-    return fail(TNCB_ERR_INVALID, hvp ? "not a sliced Hessian-vector plan (tncb_plan_create_hvp_sliced)"
-                                      : "not a sliced tangent plan (tncb_plan_create_jvp_sliced)");
-  int rc = jvp_args(plan, tangents, value || tangent_out || grads || grad_tangents, {plan->grad_elems});
-  if (rc) return rc;
-  const Schedule& S = plan->S;
-  const SlotMeta& rm = S.slots[S.result_slot];
-  if (hvp) {                                       // the seed checks of tncb_plan_hvp
-    if (seed) { if ((rc = seed_args(rm, seed, "seed"))) return rc; }
-    else if (!rm.dims.empty()) return fail(TNCB_ERR_INVALID, "a seed is needed for a result of rank " + std::to_string(rm.dims.size()));
-    if (seed_tangent && (rc = seed_args(rm, seed_tangent, "seed tangent"))) return rc;
-  }
+  int rc = route(plan, hvp ? Call::hvp_sliced : Call::jvp_sliced);
+  if (rc || (rc = jvp_args(tangents, value || tangent_out || grads || grad_tangents, {plan->grad_elems}))) return rc;
+  const SlotMeta& rm = plan->S.slots[plan->S.result_slot];
+  if (hvp && ((rc = seed_args(rm, seed, "seed", true)) || (rc = seed_args(rm, seed_tangent, "seed tangent")))) return rc;
   if (plan->ctx != ctx || !plan->full_staged) return fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this context");
   TNCB_CUDA(cudaSetDevice(ctx->device));
   const uint64_t ge = plan->grad_elems;
-  tncb_tensor *v = nullptr, *t = nullptr, *g = nullptr, *dg = nullptr;
-  if (value) rc = tensor_new(ctx, (int)rm.dims.size(), rm.dims.data(), &v);
-  if (!rc && tangent_out) rc = tensor_new(ctx, (int)rm.dims.size(), rm.dims.data(), &t);
-  if (!rc && grads) rc = tensor_new(ctx, 1, &ge, &g);
-  if (!rc && grad_tangents) rc = tensor_new(ctx, 1, &ge, &dg);
-  if (!rc) {
+  Outputs out{ctx};
+  tncb_tensor* v = out.add(value, (int)rm.dims.size(), rm.dims.data());
+  tncb_tensor* t = out.add(tangent_out, (int)rm.dims.size(), rm.dims.data());
+  tncb_tensor* g = out.add(grads, 1, &ge);
+  tncb_tensor* dg = out.add(grad_tangents, 1, &ge);
+  if (!(rc = out.rc)) {
     SliceRun io;
     io.tangents = tangents->ptr;
     io.seed = seed ? seed->ptr : nullptr; io.seed_tan = seed_tangent ? seed_tangent->ptr : nullptr;
@@ -2437,15 +2244,7 @@ static int sliced_tangent_call(tncb_ctx* ctx, tncb_plan* plan, bool hvp, size_t 
     io.grad = g ? g->ptr : nullptr; io.dgrad = dg ? dg->ptr : nullptr;
     rc = run_sliced(ctx, plan, first, stride, io);
   }
-  if (rc) {
-    for (tncb_tensor* x : {v, t, g, dg}) if (x) tncb_tensor_free(ctx, x);
-    return rc;
-  }
-  if (value) *value = v;
-  if (tangent_out) *tangent_out = t;
-  if (grads) *grads = g;
-  if (grad_tangents) *grad_tangents = dg;
-  return TNCB_OK;
+  return out.finish(rc);
 }
 } // namespace tncb
 
@@ -2471,7 +2270,7 @@ int tncb_plan_hvp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t st
 int tncb_plan_set_leaves(tncb_ctx* ctx, tncb_plan* plan, size_t n, const uint64_t* leaf_index, const void* const* src) {
   using namespace tncb;
   if (!ctx || !plan || (n && (!leaf_index || !src))) return fail(TNCB_ERR_INVALID, "null argument");
-  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
+  if (int rc = route(plan, Call::set_leaves)) return rc;
   for (int k : plan->S.leaf_kind)
     if (k == TNCB_DATA_DEVICE) return fail(TNCB_ERR_UNSUPPORTED, "plans with device leaves cannot be staged (they are consumed per call)");
   const Schedule* S = &plan->S;
@@ -2499,13 +2298,11 @@ int tncb_plan_stage_instances(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tmp
                               const uint64_t* leaf_index, const void* const* src, const uint64_t* instance_stride) {
   using namespace tncb;
   if (!ctx || !plan || !tmpl || (n && (!leaf_index || !src || !instance_stride))) return fail(TNCB_ERR_INVALID, "null argument");
-  if (sliced_tangent(plan)) return sliced_tangent_refused(plan);
-  if (plan->sliced) return fail(TNCB_ERR_UNSUPPORTED, "a sliced gradient plan takes device payloads through tncb_plan_set_leaves");
-  if (plan->hvp) return hvp_refused();
+  if (int rc = route(plan, Call::stage_instances)) return rc;
   const Schedule& S = plan->S;
   for (int k : S.leaf_kind)
     if (k == TNCB_DATA_DEVICE) return fail(TNCB_ERR_UNSUPPORTED, "plans with device leaves cannot be staged (they are consumed per call)");
-  if (!plan->grad && !plan->is_static) return fail(TNCB_ERR_UNSUPPORTED, "many networks need a plan with a static layout");
+  if (!plan->grad() && !plan->is_static) return fail(TNCB_ERR_UNSUPPORTED, "many networks need a plan with a static layout");
   if (plan->ctx && plan->ctx != ctx) return fail(TNCB_ERR_INVALID, "plan belongs to another context");
   if (n_instances == 0) return fail(TNCB_ERR_INVALID, "n_instances is 0");
   TNCB_CUDA(cudaSetDevice(ctx->device));
@@ -2520,7 +2317,7 @@ int tncb_plan_stage_instances(tncb_ctx* ctx, tncb_plan* plan, const tncb_tn* tmp
   if (__builtin_mul_overflow(n_instances, block * sizeof(double2), &bytes)) return fail(TNCB_ERR_OOM, "the instances' leaf blocks overflow 64 bits");
   // the runs of the leaf block between the device payloads come from the template, packed
   const std::vector<LeafRun> runs = leaf_runs(items, (long long)block);
-  if ((rc = plan_device_state(ctx, plan, !plan->grad && !plan->tangent))) return rc;
+  if ((rc = plan_device_state(ctx, plan, !plan->grad() && !plan->tangent()))) return rc;
   if (!plan->tmpl_host) {
     plan->tmpl_bytes = block * sizeof(double2);
     TNCB_CUDA(cudaMallocHost(&plan->tmpl_host, plan->tmpl_bytes));
@@ -2584,7 +2381,7 @@ int tncb_plan_info(const tncb_plan* plan, uint64_t* n_pairs, double* flops, doub
   if (n_pairs) *n_pairs = S.steps.size();
   if (flops) *flops = S.flops;
   if (bytes) *bytes = S.bytes;
-  if (peak_bytes && (plan->grad || plan->tangent)) *peak_bytes = plan->ws_bytes;   // the whole pass lives in its static workspace
+  if (peak_bytes && (plan->grad() || plan->tangent())) *peak_bytes = plan->ws_bytes;   // the whole pass lives in its static workspace
   else if (peak_bytes) { // replay the liveness: leaves + live intermediates
     size_t live = S.leaf_block_elems * 16, peak = live;
     std::vector<size_t> sz(S.slots.size(), 0);
@@ -2620,11 +2417,10 @@ void tncb_plan_release_device_state(tncb_plan* plan) {
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
   for (int i = 0; i < 2; i++) if (plan->exec[i]) { cudaGraphExecDestroy(plan->exec[i]); plan->exec[i] = nullptr; }
-  if (plan->batch_dev) { ctx->arena.free(plan->batch_dev, plan->batch_bytes); plan->batch_dev = nullptr; }
-  if (plan->grad_dev) { ctx->arena.free(plan->grad_dev, plan->grad_dev_bytes); plan->grad_dev = nullptr; }
-  if (plan->dgrad_dev) { ctx->arena.free(plan->dgrad_dev, plan->dgrad_dev_bytes); plan->dgrad_dev = nullptr; }
-  if (plan->sum_dev) { ctx->arena.free(plan->sum_dev, plan->sum_dev_bytes); plan->sum_dev = nullptr; }
-  if (plan->sl_dev) { ctx->arena.free(plan->sl_dev, plan->sl_dev_bytes); plan->sl_dev = nullptr; }
+  for (auto [dev, bytes] : {std::pair<void**, size_t>{&plan->batch_dev, plan->batch_bytes}, {&plan->grad_dev, plan->grad_dev_bytes},
+                            {&plan->dgrad_dev, plan->dgrad_dev_bytes}, {&plan->sum_dev, plan->sum_dev_bytes},
+                            {&plan->sl_dev, plan->sl_dev_bytes}})
+    if (*dev) { ctx->arena.free(*dev, bytes); *dev = nullptr; }
   if (plan->full_dev) { ctx->arena.free(plan->full_dev, plan->full_bytes); plan->full_dev = nullptr; }
   plan->full_staged = false;
   plan->fwd_ready = false;
