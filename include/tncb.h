@@ -201,6 +201,12 @@ int tncb_tensor_add(tncb_ctx* ctx, tncb_tensor* dst, const tncb_tensor* src);
  *      Host-side; writes 4 or 16 interleaved complex values, *rank = 2 or 4. ---- */
 int tncb_gate_matrix(const char* name, const double* angles, int n_angles, int adjoint,
                      double* out_re_im, int* rank);
+/* The derivative of that matrix with respect to its angles, for the six gates that take angles (u, rx, ry, rz, cp,
+ * fsim): dU/da_slot (slot2 < 0) or d²U/da_slot da_slot2, in the same element order, adjointed when adjoint != 0 (the
+ * angles are real, so d(U†) = (dU)†).  The errors of tncb_gate_matrix, plus TNCB_ERR_GATE "slot out of range for this
+ * gate" for a slot (or slot2 >= 0) at or past the gate's angle count -- every slot of a gate without angles. */
+int tncb_gate_derivative(const char* name, const double* angles, int n_angles, int adjoint, int slot, int slot2,
+                         double* out_re_im, int* rank);
 
 /* ---- networks: mirrors tnc::tensornetwork::tensor::Tensor (tensor.rs:21-37) and
  *      tnc::contractionpath::ContractionPath (contractionpath.rs:29-35) as plain
@@ -553,6 +559,65 @@ int tncb_plan_hvp_sliced(tncb_ctx* ctx, tncb_plan* plan, size_t first, size_t st
                          const tncb_tensor* seed, const tncb_tensor* seed_tangent, tncb_tensor** value,
                          tncb_tensor** tangent_out, tncb_tensor** grads, tncb_tensor** grad_tangents);
 void tncb_plan_destroy(tncb_plan* plan);
+
+/* ---- angle maps: derivatives with respect to the angles of Gate leaves ----
+ * A circuit's gates are functions of real angles; these calls turn a parameter vector θ into Gate-leaf payloads, leaf
+ * tangents and, from the leaf gradients of a plan, the gradient with respect to θ, all on the device.  They add no plan
+ * kind: they produce and read blocks that the plan calls above take.
+ * A ref fixes angle slot `slot` of Gate leaf `leaf` (collect order, as wrt) to scale * θ[param].  Slots no ref names keep
+ * the leaf's own angle, captured at creation.  Several refs may share a param (tied angles: rx(2β) on every qubit, the
+ * ket and bra copies of a gate in an expectation network).
+ * offsets (one per network leaf, -1 = not in the block) place each leaf's elements in a block of block_elems complex
+ * elements; every block the calls below read or write has this layout.  The intended source is tncb_plan_grad_offsets
+ * with block_elems = the plan's tangent / gradient block size: then gate rows, tangent blocks, G and Ġ share the plan's
+ * layout.  offsets NULL: the referenced leaves packed in leaf order (block_elems 0 = their total).
+ * Creation is host-only and refuses, naming the offending ref: a leaf out of range or not a Gate leaf; a gate without
+ * angles, with the wrong angle count or shape, or a slot past its angle count (TNCB_ERR_GATE / TNCB_ERR_SHAPE); param >=
+ * n_params; the same (leaf, slot) twice; a non-finite scale; a referenced leaf at offset -1, whose elements run past
+ * block_elems or overlap another's (TNCB_ERR_INVALID).  n_params == 0 or n_refs == 0 -> TNCB_ERR_INVALID.
+ * A map may be destroyed before or after the contexts it was used on, as plans may. */
+typedef struct { uint64_t leaf; uint32_t slot; uint32_t param; double scale; } tncb_angle_ref;
+typedef struct tncb_angles tncb_angles;
+int tncb_angles_create(const tncb_tn* tn, size_t n_params, size_t n_refs, const tncb_angle_ref* refs,
+                       const int64_t* offsets, size_t block_elems, tncb_angles** out);
+int tncb_angles_destroy(tncb_angles* a);
+/* n_params, block_elems and the offsets of every network leaf (any may be NULL). */
+int tncb_angles_layout(const tncb_angles* a, size_t* n_params, size_t* block_elems, int64_t* offsets);
+/* The device calls.  theta, theta_dot and direction are device double rows: row i at p + i * stride (stride 0 = one row
+ * shared by all count rows), validated as tncb_plan_set_leaves validates its sources (non-null, 8-byte aligned, device
+ * memory of the ctx's device, every byte inside its allocation; a non-zero stride below n_params) -> TNCB_ERR_INVALID.
+ * The map's tables are uploaded once per context.  Every call is asynchronous on the ctx stream; count == 0 ->
+ * TNCB_ERR_INVALID.  Non-finite angles give non-finite rows and are not refused.  Errors leave the arena as they found it.
+ * <A, B> = sum_e A[e] B[e] (no conjugation); r runs over refs, l_r, s_r, p_r, c_r are its leaf, slot, param and scale.
+ *   gates:     *rows = new [count, block_elems]; row i holds X_l(θ_i) of every referenced leaf at its offset, zeros elsewhere
+ *   tangents:  *rows = new [count, block_elems]; Ẋ_l = sum_{r on l} c_r θ̇[p_r] dU_l/da_{s_r}, zeros elsewhere
+ *   pullback:  g[p] = sum_{r: p_r = p} c_r <G_l, dU_l/da_{s_r}>; with G = vjp(S) this is sum_r S[r] dR[r]/dθ_p (complex:
+ *              θ is real).  With grad_tangents Ġ and direction v (both or neither) it gives instead the derivative of g
+ *              along v:  ġ[p] = sum_{r: p_r = p} c_r ( <Ġ_l, dU_l/da_{s_r}> + sum_{r' on l_r} c_r' v[p_r'] <G_l, d²U_l/da_{s_r} da_{s_r'}> );
+ *              with G and Ġ from tncb_plan_hvp on tangents(θ, v) and a zero seed tangent, that is (H_θ v)[p] of S·R.
+ *              grads (and grad_tangents) are [block_elems] (shared) or [count, block_elems].  *rows = new [count,
+ *              n_params], *sum = new [n_params]; either may be NULL, not both.  Shape errors -> TNCB_ERR_SHAPE.
+ * Determinism: no atomics; each param folds its refs in (param, leaf, slot) order; row i of any call is bit-identical to
+ * the same call on row i alone; sum is the left fold 0 + row_0 + row_1 + ... bit for bit; calls repeat bit for bit.
+ * How the calls compose with plans (no route is added to the table above):
+ *   R(θ) without the host:      gates -> tncb_plan_set_leaves(src = row + offset) -> run / run_slices
+ *   d(S·R)/dθ:                   gates -> set_leaves -> run -> tncb_plan_vjp(S) -> pullback(G)
+ *   sliced:                      gates -> set_leaves on a sliced gradient plan -> vjp_sliced -> pullback of the full G
+ *   B angle sets:                gates(B rows) -> stage_instances(src = rows + offset, stride = block_elems) ->
+ *                                vjp_batch(seeds) -> pullback(grad rows) with the θ rows
+ *   one θ for all instances:     vjp_batch grad_sum -> pullback with count = 1
+ *   Ṙ along θ̇; the Jacobian:     tangents -> jvp; tangents(θ, eye(P)) -> jvp_batch over P instances at stride 0
+ *   H_θ v, many v:               tangents(θ, v) -> hvp -> pullback(G, Ġ, v); hvp_batch with rows
+ *   sliced tangent / Hessian-vector plans take no device payloads, so the angles arrive by staging the Gate network;
+ *   then tangents -> jvp_sliced / hvp_sliced -> pullback. */
+int tncb_angles_gates(tncb_ctx* ctx, const tncb_angles* a, const double* theta, size_t theta_stride, size_t count,
+                      tncb_tensor** rows);
+int tncb_angles_tangents(tncb_ctx* ctx, const tncb_angles* a, const double* theta, size_t theta_stride,
+                         const double* theta_dot, size_t dot_stride, size_t count, tncb_tensor** rows);
+int tncb_angles_pullback(tncb_ctx* ctx, const tncb_angles* a, const double* theta, size_t theta_stride, size_t count,
+                         const tncb_tensor* grads, const tncb_tensor* grad_tangents,
+                         const double* direction, size_t direction_stride,
+                         tncb_tensor** rows, tncb_tensor** sum);
 
 /* ---- HDF5 tensor files: replaces tnc::io::hdf5 (tnc/src/io/hdf5.rs), which binds libhdf5 through hdf5-metno.
  *      Neither is available here; csrc/hdf5io.cpp restates the published file format for the subset those calls produce

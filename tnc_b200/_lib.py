@@ -98,6 +98,7 @@ SIGNATURES = {
     "tncb_conjugate": (C.c_int, [C.c_void_p, C.c_void_p]),
     "tncb_tensor_add": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "tncb_gate_matrix": (C.c_int, [C.c_char_p, f64p, C.c_int, C.c_int, f64p, i32p]),
+    "tncb_gate_derivative": (C.c_int, [C.c_char_p, f64p, C.c_int, C.c_int, C.c_int, C.c_int, f64p, i32p]),
     "tncb_contract_tensor_network": (C.c_int, [C.c_void_p, C.POINTER(TncbTn), C.POINTER(TncbPath), vpp, i32p, u64p]),
     "tncb_network_out_legs": (C.c_int, [C.POINTER(TncbTn), C.POINTER(TncbPath), i32p, u64p, u64p]),
     "tncb_plan_create": (C.c_int, [C.c_void_p, C.POINTER(TncbTn), C.POINTER(TncbPath), vpp]),
@@ -133,6 +134,13 @@ SIGNATURES = {
     "tncb_plan_hvp_sliced": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
                                        vpp, vpp, vpp, vpp]),
     "tncb_plan_destroy": (None, [C.c_void_p]),
+    "tncb_angles_create": (C.c_int, [C.POINTER(TncbTn), C.c_size_t, C.c_size_t, C.c_void_p, C.POINTER(C.c_int64), C.c_size_t, vpp]),
+    "tncb_angles_destroy": (C.c_int, [C.c_void_p]),
+    "tncb_angles_layout": (C.c_int, [C.c_void_p, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(C.c_int64)]),
+    "tncb_angles_gates": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, vpp]),
+    "tncb_angles_tangents": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, vpp]),
+    "tncb_angles_pullback": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_size_t, vpp, vpp]),
     "tncb_comm_unique_id": (C.c_int, [C.c_void_p]),
     "tncb_comm_init": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     "tncb_comm_send": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),

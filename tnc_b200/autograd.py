@@ -4,8 +4,9 @@
     amp = f(u3, u7)                                 # torch complex128 tensors shaped like those leaves
     (amp.abs() ** 2).backward()                     # u3.grad, u7.grad
 
-Gate angles differentiate through ordinary torch code that builds the gate matrices; the library needs no
-angle-derivative table.  One backward pass gives the gradient of every input, at about two forward passes of cost.
+Gate angles differentiate either through ordinary torch code that builds the gate matrices as Matrix leaves, or with
+circuit_function (at the end of this module), which takes the angles themselves and computes the gates and their
+derivatives on the device (tnc_b200.angles).  One backward pass gives the gradient of every input, at about two forward passes of cost.
 With `sliced_legs`, a network whose gradient workspace does not fit unsliced runs slice by slice (SlicedPlan.for_gradients).
 With `batched`, B networks that differ in some leaves (bitstrings, input states) run in one batched pass
 (NetworkPlan.vjp_batch) and the result gets a leading dimension B.  With `on_device=True`, CUDA inputs are copied into the
@@ -17,12 +18,14 @@ Forward mode (torch.autograd.forward_ad, torch.func.jvp) runs on a tangent plan 
 pass through the network from Hessian-vector products of a forward-over-reverse plan (NetworkPlan.for_hvp)."""
 from __future__ import annotations
 
+import ctypes
 from typing import Optional, Sequence
 
 import numpy as np
 import torch
 
 from . import Context, DeviceTensor, check_cuda_tensor, default_context
+from ._lib import check
 from .contractionpath import ContractionPath
 from .contractionpath.slicing import SlicedPlan
 from .tensornetwork import NetworkPlan, PreparedNetwork, Tensor, leaves
@@ -532,3 +535,141 @@ def network_function(tn: Tensor, path: ContractionPath, wrt: Sequence[int], ctx:
     NetworkPlan.stage_instances of the network marshalled once with `batched`), ordered against torch's current stream
     both ways.  Values and gradients equal those of on_device=False bit for bit."""
     return NetworkFunction(tn, path, wrt, ctx, sliced_legs, batched, on_device)
+
+
+class _CircuitFn(torch.autograd.Function):
+    @staticmethod
+    def forward(runner, theta):
+        return runner._forward(theta)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        ctx.runner = inputs[0]
+        ctx.save_for_backward(inputs[1])
+        ctx.save_for_forward(inputs[1])
+
+    @staticmethod
+    def jvp(ctx, _runner_tangent, theta_dot):
+        with torch._C._DisableFuncTorch():   # (see _NetworkFn.jvp)
+            return ctx.runner._jvp(ctx.saved_tensors[0], theta_dot)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        (theta,) = ctx.saved_tensors
+        if torch.is_grad_enabled():
+            raise NotImplementedError("second-order derivatives (create_graph=True) are not supported by circuit_function")
+        return None, ctx.runner._backward(theta, grad_out)
+
+
+class CircuitFunction:
+    """See circuit_function."""
+
+    def __init__(self, tn: Tensor, path: ContractionPath, angle_map, ctx: Optional[Context] = None, sliced_legs: Sequence[int] = ()):
+        from .angles import Angles
+        self.ctx = ctx or default_context()
+        self.tn, self.path, self.map = tn, path, angle_map
+        self.sliced_legs = [int(l) for l in sliced_legs]
+        wrt = angle_map.leaves()
+        if self.sliced_legs:
+            self.plan = SlicedPlan.for_gradients(tn, path, self.sliced_legs, wrt=wrt, ctx=self.ctx)
+        else:
+            self.plan = NetworkPlan.for_gradients(tn, path, wrt=wrt, ctx=self.ctx)
+        self.plan.stage(tn)
+        self.angles = Angles(self.ctx, tn, angle_map, self.plan)
+        self.template = PreparedNetwork(tn)
+        self.result_dims = tuple(self.plan.plan.result_dims if self.sliced_legs else self.plan.result_dims)
+        self._tplan = self._tangles = None
+
+    def _theta(self, theta) -> int:
+        """the batch size B of a [B, P] θ, 0 for a [P] one; ValueError for anything else"""
+        check_cuda_tensor(self.ctx, theta, "theta")
+        P = self.angles.n_params
+        if theta.dtype != torch.float64:
+            raise ValueError(f"theta must be float64, got {theta.dtype}")
+        if theta.dim() == 1 and theta.shape[0] == P:
+            return 0
+        if theta.dim() == 2 and theta.shape[1] == P and theta.shape[0] >= 1:
+            if self.sliced_legs:
+                raise ValueError("theta must be [P] with sliced_legs")
+            return int(theta.shape[0])
+        raise ValueError(f"theta has shape {tuple(theta.shape)}, expected [{P}] or [B, {P}]")
+
+    def _forward(self, theta):
+        B = self._theta(theta)
+        if B:
+            self.angles.stage_instances(self.plan, self.template, theta)
+            vals = self.plan.vjp_batch_blocks(0, B, rows=False, sum=False, values=True)[0]
+            return vals.to_torch()
+        self.angles.set_leaves(self.plan, theta)
+        return self.plan.run().tensordata.matrix.to_torch()
+
+    def _backward(self, theta, grad_out):
+        B = self._theta(theta)
+        seed = DeviceTensor.from_torch(self.ctx, torch.conj_physical(grad_out.to(torch.complex128)))
+        try:
+            if B:
+                self.angles.stage_instances(self.plan, self.template, theta)
+                G = self.plan.vjp_batch_blocks(0, B, seeds=seed, rows=True, sum=False, values=False)[1]
+            else:
+                self.angles.set_leaves(self.plan, theta)
+                if self.sliced_legs:
+                    value, G = self.plan.vjp_blocks(seed)
+                    value.free()
+                else:
+                    self.plan.run()
+                    G = self.plan.vjp_block(seed)
+            rows = self.angles.pullback(theta, G)[0]
+            G.free()
+        finally:
+            seed.free()
+        g = rows.to_torch().real
+        rows.free()
+        return g if B else g[0]
+
+    def _jvp(self, theta, theta_dot):
+        from .angles import Angles
+        if self.sliced_legs:
+            raise NotImplementedError("forward mode is not supported by circuit_function with sliced_legs")
+        B = self._theta(theta)
+        if theta_dot is None:
+            theta_dot = torch.zeros_like(theta)
+        if self._tplan is None:
+            self._tplan = NetworkPlan.for_tangents(self.tn, self.path, wrt=self.map.leaves(), ctx=self.ctx)
+            self._tplan.stage(self.tn)
+            self._tangles = Angles(self.ctx, self.tn, self.map, self._tplan)
+        tdot = theta_dot.detach().to(torch.float64)
+        l, plan = self.ctx._l, self._tplan
+        out = ctypes.c_void_p()
+        if B:
+            self._tangles.stage_instances(plan, self.template, theta)
+            tan = self._tangles.tangents(theta, tdot)
+            rc = l.tncb_plan_jvp_batch(self.ctx.handle, plan.handle, 0, B, tan.handle, None, ctypes.byref(out))
+        else:
+            self._tangles.set_leaves(plan, theta)
+            tan = self._tangles.tangents(theta, tdot)
+            rc = l.tncb_plan_jvp(self.ctx.handle, plan.handle, tan.handle, None, ctypes.byref(out))
+        tan.free()
+        check(rc)
+        rdot = DeviceTensor.adopt(self.ctx, out)
+        res = rdot.to_torch()
+        rdot.free()
+        return res
+
+    def __call__(self, theta: torch.Tensor) -> torch.Tensor:
+        return _CircuitFn.apply(self, theta)
+
+
+def circuit_function(tn: Tensor, path: ContractionPath, angle_map, ctx: Optional[Context] = None,
+                     sliced_legs: Sequence[int] = ()) -> CircuitFunction:
+    """A torch.autograd.Function of the gate angles of the circuit network `tn` contracted along `path`: the returned
+    callable takes θ, a CUDA float64 tensor [P] (P = angle_map.n_params, see tnc_b200.angles.AngleMap), and returns R(θ)
+    as a complex128 CUDA tensor; θ of shape [B, P] runs B angle sets as instances of one batched pass and returns
+    [B, *R].  Nothing goes through the host: the Gate leaves are computed on the device (Angles.gates) and copied into
+    a gradient plan staged once.
+
+    Backward (torch's convention for a real input): grad_θ = Re(pullback(vjp(conj(grad_out)))), through the plan's vjp,
+    vjp_batch rows for [B, P], or vjp_sliced with `sliced_legs`.  The backward re-stages the angles and runs the forward
+    again, so it is right whatever ran in between.  Forward mode (torch.autograd.forward_ad, torch.func.jvp) runs
+    Angles.tangents and a tangent plan's jvp / jvp_batch, compiled on first use.  Second order (create_graph=True) and
+    forward mode with sliced_legs raise NotImplementedError; vmap is not supported."""
+    return CircuitFunction(tn, path, angle_map, ctx, sliced_legs)

@@ -3,6 +3,7 @@
 // materialised on the host and travel to the device inside the single leaf upload of a
 // network (network.cpp), not one call per pair as in the reference (tensordata.rs:50-56).
 #include "internal.h"
+#include "gate_angles.h"
 #include <cmath>
 #include <complex>
 #include <cstring>
@@ -11,7 +12,23 @@ namespace tncb {
 
 typedef std::complex<double> cd;
 
-static inline cd expi(double x) { return cd(std::cos(x), std::sin(x)); } // Complex64::new(0,x).exp()
+// the table index of a gate that takes angles (gate_angles.h), -1 for the others
+int angle_gate(const char* name) {
+  static const char* const names[ga::kGates] = {"u", "rx", "ry", "rz", "cp", "fsim"};
+  for (int g = 0; g < ga::kGates; g++) if (name && std::strcmp(name, names[g]) == 0) return g;
+  return -1;
+}
+
+// every entry of U (s < 0), dU/da_s (t < 0) or d²U/da_s da_t of angle gate g into out; returns 4 or 16
+static int angle_entries(int g, const double* ang, int s, int t, bool adjoint, cd* out) {
+  const int cnt = ga::dim(g) * ga::dim(g), n = ga::n_angles(g);
+  const ga::Trig T = ga::trig(g, ang[0], n > 1 ? ang[1] : 0.0, n > 2 ? ang[2] : 0.0);
+  for (int e = 0; e < cnt; e++) {
+    const ga::Cplx v = ga::element(g, T, s, t, adjoint, e);
+    out[e] = cd(v.re, v.im);
+  }
+  return cnt;
+}
 
 // Returns number of complex entries written (4 or 16) or a negative status.
 int gate_matrix(const char* name, const double* ang, int n_ang, bool adjoint, cd* out) {
@@ -25,41 +42,23 @@ int gate_matrix(const char* name, const double* ang, int n_ang, bool adjoint, cd
   auto set4 = [&](cd a, cd b, cd c, cd d) { out[0] = a; out[1] = b; out[2] = c; out[3] = d; cnt = 4; };
   auto set16 = [&](const cd (&m)[16]) { for (int q = 0; q < 16; q++) out[q] = m[q]; cnt = 16; };
   std::string g(name ? name : "");
+  const int ag = angle_gate(name);
+  if (ag >= 0) {                       // u, rx, ry, rz, cp, fsim: gate_angles.h, adjoint included
+    if (!need(ga::n_angles(ag))) return TNCB_ERR_GATE;
+    return angle_entries(ag, ang, -1, -1, adjoint, out);
+  }
   if (g == "x") { if (!need(0)) return TNCB_ERR_GATE; set4(z, o, o, z); }
   else if (g == "y") { if (!need(0)) return TNCB_ERR_GATE; set4(z, -i, i, z); }
   else if (g == "z") { if (!need(0)) return TNCB_ERR_GATE; set4(o, z, z, -o); }
   else if (g == "h") { if (!need(0)) return TNCB_ERR_GATE; set4(cd(h, 0), cd(h, 0), cd(h, 0), cd(-h, 0)); }
   else if (g == "t") { if (!need(0)) return TNCB_ERR_GATE; set4(o, z, z, cd(h, h)); }
-  else if (g == "u") {
-    if (!need(3)) return TNCB_ERR_GATE;
-    const double s = std::sin(ang[0] / 2), c = std::cos(ang[0] / 2);
-    set4(cd(c, 0), -expi(ang[2]) * s, expi(ang[1]) * s, expi(ang[1] + ang[2]) * c);
-  }
   else if (g == "sx") { if (!need(0)) return TNCB_ERR_GATE; set4(cd(.5, .5), cd(.5, -.5), cd(.5, -.5), cd(.5, .5)); }
   else if (g == "sy") { if (!need(0)) return TNCB_ERR_GATE; set4(cd(.5, .5), cd(-.5, -.5), cd(.5, .5), cd(.5, .5)); }
   else if (g == "sz") { if (!need(0)) return TNCB_ERR_GATE; set4(o, z, z, i); }
-  else if (g == "rx") {
-    if (!need(1)) return TNCB_ERR_GATE;
-    const double s = std::sin(ang[0] / 2), c = std::cos(ang[0] / 2);
-    set4(o * c, -i * s, -i * s, o * c);
-  }
-  else if (g == "ry") {
-    if (!need(1)) return TNCB_ERR_GATE;
-    const double s = std::sin(ang[0] / 2), c = std::cos(ang[0] / 2);
-    set4(o * c, -o * s, o * s, o * c);
-  }
-  else if (g == "rz") { if (!need(1)) return TNCB_ERR_GATE; set4(expi(-ang[0] / 2), z, z, expi(ang[0] / 2)); }
   else if (g == "cx") { if (!need(0)) return TNCB_ERR_GATE; const cd m[16] = {o, z, z, z, z, o, z, z, z, z, z, o, z, z, o, z}; set16(m); }
   else if (g == "cz") { if (!need(0)) return TNCB_ERR_GATE; const cd m[16] = {o, z, z, z, z, o, z, z, z, z, o, z, z, z, z, -o}; set16(m); }
   else if (g == "swap") { if (!need(0)) return TNCB_ERR_GATE; const cd m[16] = {o, z, z, z, z, z, o, z, z, o, z, z, z, z, z, o}; set16(m); }
-  else if (g == "cp") { if (!need(1)) return TNCB_ERR_GATE; const cd e = expi(ang[0]); const cd m[16] = {o, z, z, z, z, o, z, z, z, z, o, z, z, z, z, e}; set16(m); }
   else if (g == "iswap") { if (!need(0)) return TNCB_ERR_GATE; const cd m[16] = {o, z, z, z, z, z, i, z, z, i, z, z, z, z, z, o}; set16(m); }
-  else if (g == "fsim") {
-    if (!need(2)) return TNCB_ERR_GATE;
-    const cd a(std::cos(ang[0]), 0), b(0, -std::sin(ang[0])), c = expi(-ang[1]);
-    const cd m[16] = {o, z, z, z, z, a, b, z, z, b, a, z, z, z, z, c};
-    set16(m);
-  }
   else return fail(TNCB_ERR_GATE, "Gate '" + g + "' not found.");
   if (adjoint) { // matrix_adjoint_inplace, gates.rs:82-99: swap dim halves, conjugate
     const int d = cnt == 4 ? 2 : 4;
@@ -78,6 +77,23 @@ extern "C" int tncb_gate_matrix(const char* name, const double* angles, int n_an
   tncb::cd buf[16];
   int cnt = tncb::gate_matrix(name, angles, n_angles, adjoint != 0, buf);
   if (cnt < 0) return cnt;
+  for (int q = 0; q < cnt; q++) { out_re_im[2 * q] = buf[q].real(); out_re_im[2 * q + 1] = buf[q].imag(); }
+  if (rank) *rank = cnt == 4 ? 2 : 4;
+  return TNCB_OK;
+}
+
+extern "C" int tncb_gate_derivative(const char* name, const double* angles, int n_angles, int adjoint, int slot, int slot2,
+                                    double* out_re_im, int* rank) {
+  if (!name || !out_re_im || (n_angles > 0 && !angles)) return tncb::fail(TNCB_ERR_INVALID, "null argument");
+  tncb::cd buf[16];
+  int cnt = tncb::gate_matrix(name, angles, n_angles, adjoint != 0, buf);    // the errors of tncb_gate_matrix
+  if (cnt < 0) return cnt;
+  const int g = tncb::angle_gate(name);
+  const int n = g < 0 ? 0 : tncb::ga::n_angles(g);
+  if (slot < 0 || slot >= n || slot2 >= n)
+    return tncb::fail(TNCB_ERR_GATE, "slot out of range for this gate: '" + std::string(name) + "' takes " + std::to_string(n) +
+                                         " angles, slots " + std::to_string(slot) + ", " + std::to_string(slot2));
+  cnt = tncb::angle_entries(g, angles, slot, slot2 < 0 ? -1 : slot2, adjoint != 0, buf);
   for (int q = 0; q < cnt; q++) { out_re_im[2 * q] = buf[q].real(); out_re_im[2 * q + 1] = buf[q].imag(); }
   if (rank) *rank = cnt == 4 ? 2 : 4;
   return TNCB_OK;

@@ -5,6 +5,7 @@
 #include <string>
 #include <vector>
 #include <map>
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include "../../include/tncb.h"
 
@@ -115,9 +116,12 @@ struct tncb_ctx {
   // structure-keyed cache of plans behind tncb_contract_tensor_network (most recently used last)
   struct CachedPlan { std::vector<uint64_t> key; struct tncb_plan* plan; };
   std::vector<CachedPlan> plan_cache;
+  // angle maps whose tables live in this context's arena; detached by tncb_ctx_destroy
+  std::vector<struct tncb_angles*> angle_maps;
 };
 
 extern "C" void tncb_plan_release_device_state(struct tncb_plan* plan);
+namespace tncb { void angles_release(struct tncb_angles* a, tncb_ctx* ctx); }   // angles.cu
 
 namespace tncb {
 // ---- kernel launchers (kernels.cu) ---------------------------------------------------
@@ -222,6 +226,12 @@ struct LeafStageBatch {
 // instance i's leaf block at dst + i * block_elems; any number of items and instances (several launches if needed)
 int launch_leaf_stage(tncb_ctx* ctx, const LeafStageItem* items, size_t n_items, double2* dst, long long block_elems,
                       size_t n_instances);
+// cuMemGetAddressRange, resolved through the runtime (network.cpp); nullptr when the driver does not offer it
+typedef CUresult (*MemRangeFn)(CUdeviceptr*, size_t*, CUdeviceptr);
+MemRangeFn get_mem_range();
+
+// the table index (gate_angles.h) of a gate that takes angles, -1 for the others (gates.cpp)
+int angle_gate(const char* name);
 
 // ---- tangent sums of a tangent plan: every two-sided forward step of one level, out = t1 + t2, in ONE launch; count
 // instances whose workspaces lie `stride` bytes apart (the instance a grid dimension) ----

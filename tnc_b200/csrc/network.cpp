@@ -1340,8 +1340,7 @@ static int gather_set_batch(tncb_ctx* ctx, const tncb_plan* P, const std::vector
 // ---- leaf payloads from device memory (tncb_plan_set_leaves / tncb_plan_stage_instances) ----
 // cuMemGetAddressRange, resolved through the runtime as crt.cu resolves cuTensorMapEncodeTiled: the allocation that holds
 // a device address, so that a source range running past its end is refused before anything is launched
-typedef CUresult (*MemRangeFn)(CUdeviceptr*, size_t*, CUdeviceptr);
-static MemRangeFn get_mem_range() {
+MemRangeFn get_mem_range() {
   static const MemRangeFn fn = [] {
     cudaDriverEntryPointQueryResult q;
     void* p = nullptr;

@@ -175,6 +175,7 @@ void tncb_ctx_destroy(tncb_ctx* ctx) {
   for (auto& c : ctx->plan_cache) tncb_plan_destroy(c.plan);                         // the contract_tensor_network plan cache
   ctx->plan_cache.clear();
   while (!ctx->plans.empty()) tncb_plan_release_device_state(ctx->plans.back());   // plans may outlive the ctx
+  while (!ctx->angle_maps.empty()) tncb::angles_release(ctx->angle_maps.back(), ctx);   // so may angle maps
   tncb_comm_destroy(ctx);
   if (ctx->tab) cudaFree(ctx->tab);
   if (ctx->partial) cudaFree(ctx->partial);
