@@ -9,8 +9,9 @@ circuit_function (at the end of this module), which takes the angles themselves 
 derivatives on the device (tnc_b200.angles).  One backward pass gives the gradient of every input, at about two forward passes of cost.
 With `sliced_legs`, a network whose gradient workspace does not fit unsliced runs slice by slice (SlicedPlan.for_gradients).
 With `batched`, B networks that differ in some leaves (bitstrings, input states) run in one batched pass
-(NetworkPlan.vjp_batch) and the result gets a leading dimension B.  With `on_device=True`, CUDA inputs are copied into the
-staged plan on the device and the result and gradients come back as CUDA tensors.
+(NetworkPlan.vjp_batch) and the result gets a leading dimension B.  The network is staged once; every call copies the
+inputs into the staged plan on the device, CPU inputs after one upload of them all.  With `on_device=True`, the inputs
+must be CUDA tensors and the result and gradients come back as CUDA tensors.
 
 Forward mode (torch.autograd.forward_ad, torch.func.jvp) runs on a tangent plan (NetworkPlan.for_tangents).  Without
 `batched` or `sliced_legs`, the backward is itself differentiable: `grad(..., create_graph=True)` followed by another
@@ -19,9 +20,9 @@ pass through the network from Hessian-vector products of a forward-over-reverse 
 from __future__ import annotations
 
 import ctypes
+import math
 from typing import Optional, Sequence
 
-import numpy as np
 import torch
 
 from . import Context, DeviceTensor, check_cuda_tensor, default_context
@@ -49,8 +50,7 @@ class _NetworkFn(torch.autograd.Function):
     # forward / setup_context (rather than forward(ctx, ...)) so that torch.func transforms (torch.func.jvp) accept it
     @staticmethod
     def forward(runner, *xs):
-        runner._forward_device(xs) if runner.on_device else runner._forward(xs)
-        return runner._result
+        return runner._forward(xs)
 
     @staticmethod
     def setup_context(ctx, inputs, output):
@@ -80,18 +80,7 @@ class _NetworkFn(torch.autograd.Function):
             what = "batched inputs" if runner.batched else "sliced_legs"
             raise NotImplementedError(f"second-order derivatives (create_graph=True) are not supported with {what}: "
                                       "Hessian-vector plans are neither batched nor sliced")
-        if runner.on_device:
-            return (None,) + runner._backward_device(ctx, grad_out, xs)
-        seed = np.conj(grad_out.detach().to(torch.complex128).cpu().numpy())
-        if runner.batched:               # vjp_batch runs forward and backward of every instance: it only needs them staged
-            if runner._token != ctx.token:
-                ctx.token = runner._stage_batch(xs)
-            return (None,) + runner._batch_grads(seed, xs)
-        # sliced: vjp_sliced re-runs every slice's forward, it only needs these inputs staged
-        if runner._token != ctx.token:
-            ctx.token = runner._stage(xs)
-        g = runner.plan.vjp(seed)[1]
-        return (None,) + tuple(torch.from_numpy(np.conj(g[i])).to(x.device) for i, x in zip(runner.wrt, xs))
+        return (None,) + runner._backward(ctx, grad_out, xs)
 
 
 class _GradFn(torch.autograd.Function):
@@ -157,6 +146,16 @@ class _HessFn(torch.autograd.Function):
         return (None, None) + (None,) * len(xs) + tuple(torch.conj_physical(g) for g in gdot)
 
 
+def _to_torch(blocks) -> list:
+    """the DeviceTensors `blocks` as torch CUDA tensors, each freed; None stays None"""
+    out = []
+    for b in blocks:
+        out.append(None if b is None else b.to_torch())
+        if b is not None:
+            b.free()
+    return out
+
+
 class NetworkFunction:
     """The callable network_function returns: inputs -> contracted result, differentiable in every input."""
 
@@ -179,196 +178,47 @@ class NetworkFunction:
         self.inputs = self.wrt + [i for i in self.batched if i not in self.wrt]
         self.shapes = [tuple(int(d) for d in lv[i].bond_dims) for i in self.inputs]
         self.tn, self.path = tn, path
+        self._ctx = ctx or default_context()
         self.sliced = len(sliced_legs) > 0
         if self.sliced:
-            self.plan = SlicedPlan.for_gradients(tn, path, sliced_legs, self.wrt, ctx=ctx or default_context())
+            self.plan = SlicedPlan.for_gradients(tn, path, sliced_legs, self.wrt, ctx=self._ctx)
         else:
-            self.plan = NetworkPlan.for_gradients(tn, path, self.wrt, ctx=ctx or default_context())
-        self._token, self._count, self._result = None, 0, None
+            self.plan = NetworkPlan.for_gradients(tn, path, self.wrt, ctx=self._ctx)
+        self._token = None               # the staging the gradient plan's state belongs to
         self.on_device = bool(on_device)
-        self._staged = False             # on_device: the template network is staged (unbatched and sliced)
-        self._template = None            # on_device, batched: the network marshalled once
+        self._staged = []                # the plans `tn` is staged in (unbatched and sliced)
+        self._template = None            # batched: the network marshalled once
         self._offsets = None
-        self._ctx = ctx or default_context()
-        self._sliced_legs = tuple(sliced_legs)
         self._tplan = None               # the tangent plan, compiled on the first forward-mode call
-        self._tstaged = False            # on_device, unbatched: the tangent plan has `tn` staged
         self._hplan = None               # the Hessian-vector plan, compiled on the first second-order call
-        self._hstaged = False            # on_device: the Hessian-vector plan has `tn` staged
 
-    # ---- on_device: inputs, results and gradients stay on the GPU ----
-    def _check_device(self, xs):
-        for i, x in zip(self.inputs, xs):
-            check_cuda_tensor(self.plan.ctx, x, f"input for leaf {i}")
-
-    def _set_device(self, xs):
-        """the inputs as the wrt leaves' payloads, copied on the device into the staged network (staged once, from the
-        network's own payloads, on first use)"""
-        self._check_device(xs)
-        for i, shape, x in zip(self.wrt, self.shapes, xs):
-            if tuple(x.shape) != shape:
-                raise ValueError(f"input for leaf {i} has shape {tuple(x.shape)}, the leaf {shape}")
-        if not self._staged:
-            self.plan.stage(self.tn)
-            self._staged = True
-        self.plan.set_leaves(dict(zip(self.wrt, xs)))
-        self._count += 1
-        self._token = self._count
-        return self._token
-
-    def _stage_instances(self, xs):
-        """B instances staged from device memory: batched inputs row by row, the others shared"""
-        self._check_device(xs)
-        b = self._batch_size(xs)
-        if self._template is None:
-            self._template = PreparedNetwork(self.tn)
-        self.plan.stage_instances(self._template, dict(zip(self.inputs, xs)), b)
-        self._count += 1
-        self._token = self._count
-        return self._token
-
-    def _split(self, block, lead=()):
-        """{wrt leaf: its slice of a [..., grad_elems] torch gradient block, shaped lead + leaf shape}"""
-        if self._offsets is None:
-            self._offsets = self.plan.grad_offsets()
-        out = {}
-        for i, shape in zip(self.wrt, self.shapes):
-            off = self._offsets[i]
-            out[i] = block[..., off:off + int(np.prod(shape, dtype=np.int64))].reshape(tuple(lead) + shape)
+    # ---- inputs, staging and gradients: the plans run on the context's device, whatever device the inputs are on ----
+    def _to_ctx(self, ts, names) -> list:
+        """the torch tensors `ts` as physical complex128 tensors on the context's device.  on_device: each must be there
+        already (else ValueError, naming it from `names`).  Else the ones elsewhere are packed into one buffer per
+        device they are on, moved in one copy and split into views: networks have hundreds of inputs, and a copy each
+        would cost more than the contraction of a small one."""
+        if self.on_device:
+            for t, name in zip(ts, names):
+                check_cuda_tensor(self._ctx, t, name)
+        dev = torch.device("cuda", self._ctx.device)
+        out, away = [], {}
+        for k, t in enumerate(ts):
+            if t.dtype != torch.complex128 or t.is_conj() or t.is_neg():
+                t = t.detach().to(torch.complex128).resolve_conj().resolve_neg()
+            out.append(t)
+            if t.device != dev:
+                away.setdefault(t.device, []).append(k)
+        for ks in away.values():
+            buf = torch.cat([out[k].reshape(-1) for k in ks]).to(dev)
+            for k, part in zip(ks, buf.split([out[k].numel() for k in ks])):
+                out[k] = part.view(out[k].shape)
         return out
 
-    def _forward_device(self, xs):
-        if self.batched:
-            token = self._stage_instances(xs)
-            vals = self.plan.vjp_batch_blocks(0, None, rows=False, sum=False, values=True)[0]
-        else:
-            token = self._set_device(xs)
-            vals = self.plan.run().tensordata.matrix
-        self._result = vals.to_torch()
-        vals.free()
-        return token
-
-    def _backward_device(self, fctx, grad_out, xs):
-        """the gradients of batched or sliced inputs (torch's convention, conj of the holomorphic vjp)"""
-        seed = DeviceTensor.from_torch(self.plan.ctx, torch.conj_physical(grad_out.detach().to(torch.complex128)))
-        try:
-            if self.batched:
-                if self._token != fctx.token:
-                    fctx.token = self._stage_instances(xs)
-                return self._batch_grads_device(seed, xs)
-            if self._token != fctx.token:
-                fctx.token = self._set_device(xs)
-            value, block = self.plan.vjp_blocks(seed)
-            value.free()
-            flat = torch.conj_physical(block.to_torch())
-            block.free()
-        finally:
-            seed.free()
-        g = self._split(flat)
-        return tuple(g[i] for i in self.wrt)
-
-    def _grads(self, fctx, seed, xs):
-        """G_i = sum_r seed[r] dR[r]/dx_i (holomorphic, no conjugation) of the unbatched, unsliced plan, one per wrt input:
-        the forward of the _NetworkFn call `fctx` (re-run when another call used the plan's state since), then vjp"""
-        seed = seed.detach().to(torch.complex128)
-        if self.on_device:
-            s = DeviceTensor.from_torch(self.plan.ctx, seed)
-            try:
-                if self._token != fctx.token:
-                    fctx.token = self._forward_device(xs)
-                self._token = None
-                block = self.plan.vjp_block(s)
-                flat = block.to_torch()
-                block.free()
-            finally:
-                s.free()
-            g = self._split(flat)
-            return tuple(g[i] for i in self.wrt)
-        if self._token != fctx.token:    # another forward (or an earlier backward) used the plan's state since
-            fctx.token = self._forward(xs)
-        self._token = None               # the backward levels overwrite the forward state
-        g = self.plan.vjp(seed.cpu().numpy())
-        return tuple(torch.from_numpy(g[i]).to(x.device) for i, x in zip(self.wrt, xs))
-
-    # ---- second order (create_graph=True, torch.autograd.functional.hvp / hessian, torch.func.jvp of torch.func.grad):
-    # a Hessian-vector plan, compiled on the first second-order call ----
-    def _hvp(self, xs, seed, tangents: dict, seed_tangent, want_rdot: bool):
-        """(Ṙ or None, (Ġ_i per wrt input)) of one NetworkPlan.hvp_blocks pass on the inputs xs with seed `seed`, leaf
-        tangents {wrt leaf: tensor} (left out: zero) and seed tangent `seed_tangent` (None: zero); no conjugation"""
-        if self._hplan is None:
-            self._hplan = NetworkPlan.for_hvp(self.tn, self.path, self.wrt, ctx=self._ctx)
-        plan = self._hplan
-        for i, shape, x in zip(self.wrt, self.shapes, xs):
-            if tuple(x.shape) != shape:
-                raise ValueError(f"input for leaf {i} has shape {tuple(x.shape)}, the leaf {shape}")
-        outputs = (False, want_rdot, False, True)
-
-        def phys(t):
-            return t.detach().to(torch.complex128).resolve_conj()
-        if self.on_device:
-            self._check_device(xs)
-            for i, t in tangents.items():
-                check_cuda_tensor(plan.ctx, t, f"tangent for leaf {i}")
-            if not self._hstaged:
-                plan.stage(self.tn)
-                self._hstaged = True
-            plan.set_leaves(dict(zip(self.wrt, xs)))
-            _, rdot, _, gdot = plan.hvp_blocks({i: phys(t) for i, t in tangents.items()}, phys(seed),
-                                               None if seed_tangent is None else phys(seed_tangent), outputs)
-            out = []
-            for dt in (rdot, gdot):
-                out.append(None if dt is None else dt.to_torch())
-                if dt is not None:
-                    dt.free()
-            g = self._split(out[1])
-            return out[0], tuple(g[i] for i in self.wrt)
-
-        def host(t):                     # (np.ascontiguousarray would make a rank-0 seed rank 1)
-            return phys(t).contiguous().cpu().numpy()
-        plan.stage(_with_payloads(self.tn, {i: host(x) for i, x in zip(self.wrt, xs)}, [0]))
-        _, rdot, _, gdot = plan.hvp_blocks({i: host(t) for i, t in tangents.items()}, host(seed),
-                                           None if seed_tangent is None else host(seed_tangent), outputs)
-        out = []
-        for dt in (rdot, gdot):
-            out.append(None if dt is None else torch.from_numpy(dt.to_numpy()).to(seed.device))
-            if dt is not None:
-                dt.free()
-        g = self._split(out[1])
-        return out[0], tuple(g[i].to(x.device) for i, x in zip(self.wrt, xs))
-
-    def _batch_grads_device(self, seed, xs):
-        want_rows = any(i in self.batched for i in self.wrt)
-        want_sum = any(i not in self.batched for i in self.wrt)
-        _, rows, total = self.plan.vjp_batch_blocks(0, None, seeds=seed, rows=want_rows, sum=want_sum, values=False)
-        blocks = []
-        for dt in (rows, total):
-            blocks.append(None if dt is None else torch.conj_physical(dt.to_torch()))
-            if dt is not None:
-                dt.free()
-        rows_g = self._split(blocks[0], (self.plan.n_staged,)) if want_rows else {}
-        sum_g = self._split(blocks[1]) if want_sum else {}
-        grads = []
-        for i in self.inputs:
-            if i not in self.wrt:
-                grads.append(None)
-            else:
-                grads.append(rows_g[i] if i in self.batched else sum_g[i])
-        return tuple(grads)
-
-    def _stage(self, xs):
-        """stage the inputs as the wrt leaves' payloads (through the host)"""
-        pay = {}
-        for i, shape, x in zip(self.wrt, self.shapes, xs):
-            if tuple(x.shape) != shape:
-                raise ValueError(f"input for leaf {i} has shape {tuple(x.shape)}, the leaf {shape}")
-            pay[i] = np.ascontiguousarray(x.detach().to(torch.complex128).cpu().numpy())
-        self.plan.stage(_with_payloads(self.tn, pay, [0]))
-        self._count += 1
-        self._token = self._count
-        return self._token
-
-    def _batch_size(self, xs) -> int:
-        """the common leading dimension B of the batched inputs; every input's shape checked"""
+    def _inputs(self, xs):
+        """(the inputs on the context's device, B or None without `batched`), every shape checked: a wrt leaf's input
+        shaped like the leaf, a batched leaf's [B, *leaf shape] with one B >= 1 for all of them"""
+        dxs = self._to_ctx(xs, [f"input for leaf {i}" for i in self.inputs])
         b = None
         for i, shape, x in zip(self.inputs, self.shapes, xs):
             want = shape
@@ -381,55 +231,122 @@ class NetworkFunction:
                     raise ValueError(f"batched input for leaf {i} has {int(x.shape[0])} instances, an earlier one {b}")
                 want = (b,) + shape
             if tuple(x.shape) != want:
-                raise ValueError(f"input for leaf {i} has shape {tuple(x.shape)}, expected {want}")
+                raise ValueError(f"input for leaf {i} has shape {tuple(x.shape)}, "
+                                 + (f"expected {want}" if self.batched else f"the leaf {shape}"))
         if b == 0:
             raise ValueError("batched inputs hold no instance")
-        return b
+        return dxs, b
 
-    def _stage_batch(self, xs):
-        """stage B networks: batched leaves take their row b, the others the same payload in every instance"""
-        b = self._batch_size(xs)
-        arrs = [np.ascontiguousarray(x.detach().to(torch.complex128).cpu().numpy()) for x in xs]
-        nets = []
-        for k in range(b):
-            pay = {i: (a[k] if i in self.batched else a) for i, a in zip(self.inputs, arrs)}
-            nets.append(_with_payloads(self.tn, pay, [0]))
-        self.plan.stage_batch(nets)
-        self._count += 1
-        self._token = self._count
-        return self._token
+    def _stage(self, plan, xs) -> None:
+        """the inputs into `plan`: with `batched`, B instances of the network marshalled once (stage_instances), batched
+        inputs row by row, the others shared; else `tn` itself, staged on the plan's first use, with the wrt leaves
+        copied in on the device (set_leaves)"""
+        dxs, b = self._inputs(xs)
+        if self.batched:
+            if self._template is None:
+                self._template = PreparedNetwork(self.tn)
+            plan.stage_instances(self._template, dict(zip(self.inputs, dxs)), b)
+            return
+        if plan not in self._staged:
+            plan.stage(self.tn)
+            self._staged.append(plan)
+        plan.set_leaves(dict(zip(self.wrt, dxs)))
 
-    def _batch_grads(self, seed, xs):
-        """conj of the rows (batched leaves in wrt) or of the sum (shared leaves in wrt); None for the other inputs"""
-        want_rows = any(i in self.batched for i in self.wrt)
-        want_sum = any(i not in self.batched for i in self.wrt)
-        _, _, rows, total = self.plan.vjp_batch(0, None, seeds=seed, rows=want_rows, sum=want_sum, values=False)
-        grads = []
-        for i, x in zip(self.inputs, xs):
-            if i not in self.wrt:
-                grads.append(None)
-            else:
-                g = rows[i] if i in self.batched else total[i]
-                grads.append(torch.from_numpy(np.conj(g)).to(x.device))
-        return tuple(grads)
+    def _split(self, block, inputs: dict, lead=()) -> dict:
+        """{leaf: its slice of a [*lead, grad_elems] torch gradient block, shaped lead + leaf shape} for the leaves of
+        `inputs` ({wrt leaf: input}), each on its input's device: the whole block is copied once to each other device"""
+        if self._offsets is None:
+            self._offsets = self.plan.grad_offsets()
+        shapes = dict(zip(self.inputs, self.shapes))
+        blocks = {block.device: block}
+        out = {}
+        for i, x in inputs.items():
+            if x.device not in blocks:
+                blocks[x.device] = block.to(x.device)
+            off, shape = self._offsets[i], shapes[i]
+            out[i] = blocks[x.device][..., off:off + math.prod(shape)].reshape(tuple(lead) + shape)
+        return out
 
     def _forward(self, xs):
         """stage the inputs and run the forward levels (every slice's, summed, on a sliced plan; every instance's, one
-        per row, with batched inputs)"""
+        per row, with batched inputs); returns the result, on the host unless on_device.  Not kept here: the result's
+        graph refers to this object, and a reference back would make a cycle that holds the plans' device memory until
+        the garbage collector runs."""
+        self._stage(self.plan, xs)
+        self._token = object()
         if self.batched:
-            token = self._stage_batch(xs)
-            _, vals, _, _ = self.plan.vjp_batch(0, None, rows=False, sum=False, values=True)
-            self._result = torch.from_numpy(np.asarray(vals).copy())
-            return token
-        token = self._stage(xs)
-        res = self.plan.run()
-        self._result = torch.from_numpy(np.asarray(res.to_numpy()).copy())
-        return token
+            vals = self.plan.vjp_batch_blocks(0, None, rows=False, sum=False, values=True)[0]
+        else:
+            vals = self.plan.run().tensordata.matrix
+        (res,) = _to_torch([vals])
+        return res if self.on_device else res.cpu()
+
+    def _backward(self, fctx, grad_out, xs):
+        """the gradients of batched or sliced inputs (torch's convention, conj of the holomorphic vjp), None for batched
+        inputs not in wrt: per-instance rows for batched inputs, their sum over the instances for shared ones"""
+        (s,) = self._to_ctx([torch.conj_physical(grad_out)], ["the seed"])
+        seed = DeviceTensor.from_torch(self._ctx, s)
+        try:
+            # vjp_batch and vjp_sliced re-run every forward: they only need these inputs staged
+            if self._token != fctx.token:
+                self._stage(self.plan, xs)
+                fctx.token = self._token = object()
+            if self.batched:
+                _, rows, total = self.plan.vjp_batch_blocks(0, None, seeds=seed, rows=any(i in self.batched for i in self.wrt),
+                                                            sum=any(i not in self.batched for i in self.wrt), values=False)
+            else:
+                value, total = self.plan.vjp_blocks(seed)
+                value.free()
+                rows = None
+        finally:
+            seed.free()
+        rows, total = (None if b is None else torch.conj_physical(b) for b in _to_torch([rows, total]))
+        wrt = dict(zip(self.wrt, xs))
+        g = {}
+        if rows is not None:
+            g.update(self._split(rows, {i: x for i, x in wrt.items() if i in self.batched}, (self.plan.n_staged,)))
+        if total is not None:
+            g.update(self._split(total, {i: x for i, x in wrt.items() if i not in self.batched}))
+        return tuple(g.get(i) for i in self.inputs)
+
+    def _grads(self, fctx, seed, xs):
+        """G_i = sum_r seed[r] dR[r]/dx_i (holomorphic, no conjugation) of the unbatched, unsliced plan, one per wrt input:
+        the forward of the _NetworkFn call `fctx` (re-run when another call used the plan's state since), then vjp"""
+        (s,) = self._to_ctx([seed], ["the seed"])
+        s = DeviceTensor.from_torch(self._ctx, s)
+        try:
+            if self._token != fctx.token:
+                self._forward(xs)
+                fctx.token = self._token
+            self._token = None           # the backward levels overwrite the forward state
+            (flat,) = _to_torch([self.plan.vjp_block(s)])
+        finally:
+            s.free()
+        return tuple(self._split(flat, dict(zip(self.wrt, xs))).values())
+
+    # ---- second order (create_graph=True, torch.autograd.functional.hvp / hessian, torch.func.jvp of torch.func.grad):
+    # a Hessian-vector plan, compiled on the first second-order call ----
+    def _hvp(self, xs, seed, tangents: dict, seed_tangent, want_rdot: bool):
+        """(Ṙ or None, (Ġ_i per wrt input)) of one NetworkPlan.hvp_blocks pass on the inputs xs with seed `seed`, leaf
+        tangents {wrt leaf: tensor} (left out: zero) and seed tangent `seed_tangent` (None: zero); no conjugation.  Ṙ
+        comes back on the seed's device, Ġ_i on its input's."""
+        if self._hplan is None:
+            self._hplan = NetworkPlan.for_hvp(self.tn, self.path, self.wrt, ctx=self._ctx)
+        self._stage(self._hplan, xs)
+        n = len(tangents)
+        ts = self._to_ctx(list(tangents.values()) + [seed] + ([] if seed_tangent is None else [seed_tangent]),
+                          [f"tangent for leaf {i}" for i in tangents] + ["the seed", "the seed tangent"])
+        _, rdot, _, gdot = self._hplan.hvp_blocks(dict(zip(tangents, ts[:n])), ts[n], ts[n + 1] if seed_tangent is not None else None,
+                                                  (False, want_rdot, False, True))
+        rdot, gdot = _to_torch([rdot, gdot])
+        g = self._split(gdot, dict(zip(self.wrt, xs)))
+        return None if rdot is None else rdot.to(seed.device), tuple(g.values())
 
     # ---- forward mode (torch.autograd.forward_ad, torch.func.jvp): a tangent plan, compiled on first use ----
     def _jvp(self, xs, tangents, out_meta):
         """Ṙ for the tangents of the inputs (None = zero; tangents of inputs not in wrt are ignored, as backward gives
-        them no gradient): the tangent plan staged with the inputs, then NetworkPlan.jvp / jvp_batch"""
+        them no gradient) on the result's device: the tangent plan staged with the inputs, then NetworkPlan.jvp_block /
+        jvp_batch_blocks"""
         if self.sliced:
             raise NotImplementedError("forward-mode AD (jvp) is not supported with sliced_legs: tangent plans are not sliced")
         shape, device = out_meta
@@ -438,47 +355,14 @@ class NetworkFunction:
             return torch.zeros(shape, dtype=torch.complex128, device=device)
         if self._tplan is None:
             self._tplan = NetworkPlan.for_tangents(self.tn, self.path, self.wrt, ctx=self._ctx)
-        plan = self._tplan
-        if self.on_device:
-            self._check_device(xs)
-            for i, t in tans.items():
-                check_cuda_tensor(plan.ctx, t, f"tangent for leaf {i}")
-            if self.batched:
-                if self._template is None:
-                    self._template = PreparedNetwork(self.tn)
-                plan.stage_instances(self._template, dict(zip(self.inputs, xs)), self._batch_size(xs))
-                _, rows = plan.jvp_batch_blocks(0, None, tans, values=False)
-                out = rows.to_torch()
-                rows.free()
-                return out
-            for i, shape_i, x in zip(self.wrt, self.shapes, xs):
-                if tuple(x.shape) != shape_i:
-                    raise ValueError(f"input for leaf {i} has shape {tuple(x.shape)}, the leaf {shape_i}")
-            if not self._tstaged:
-                plan.stage(self.tn)
-                self._tstaged = True
-            plan.set_leaves(dict(zip(self.wrt, xs)))
-            val, tan = plan.jvp_block(tans)
-            val.free()
-            out = tan.to_torch()
-            tan.free()
-            return out
-        host = {i: np.ascontiguousarray(t.detach().to(torch.complex128).resolve_conj().cpu().numpy()) for i, t in tans.items()}
+        self._stage(self._tplan, xs)
+        tans = dict(zip(tans, self._to_ctx(list(tans.values()), [f"tangent for leaf {i}" for i in tans])))
         if self.batched:
-            b = self._batch_size(xs)
-            arrs = [np.ascontiguousarray(x.detach().to(torch.complex128).resolve_conj().cpu().numpy()) for x in xs]
-            plan.stage_batch([_with_payloads(self.tn, {i: (a[k] if i in self.batched else a) for i, a in zip(self.inputs, arrs)}, [0])
-                              for k in range(b)])
-            _, _, rows = plan.jvp_batch(0, None, host, values=False)
-            return torch.from_numpy(rows).to(device)
-        pay = {}
-        for i, shape_i, x in zip(self.wrt, self.shapes, xs):
-            if tuple(x.shape) != shape_i:
-                raise ValueError(f"input for leaf {i} has shape {tuple(x.shape)}, the leaf {shape_i}")
-            pay[i] = np.ascontiguousarray(x.detach().to(torch.complex128).resolve_conj().cpu().numpy())
-        plan.stage(_with_payloads(self.tn, pay, [0]))
-        _, tan = plan.jvp(host)
-        return torch.from_numpy(tan).to(device)
+            _, tan = self._tplan.jvp_batch_blocks(0, None, tans, values=False)
+        else:
+            val, tan = self._tplan.jvp_block(tans)
+            val.free()
+        return _to_torch([tan])[0].to(device)
 
     def __call__(self, *xs: torch.Tensor) -> torch.Tensor:
         if len(xs) != len(self.inputs):
@@ -493,10 +377,16 @@ def network_function(tn: Tensor, path: ContractionPath, wrt: Sequence[int], ctx:
     contracted result as a torch tensor.  Its backward is conj(vjp(conj(grad_out))) of the gradient plan, torch's
     convention for complex inputs.
 
-    Forward = stage + run: the inputs are copied to the host and staged the way NetworkPlan.stage stages any payload
-    (with on_device=False, the default; see below).  A backward needs the plan's forward state: when another call of the
-    same function ran in between, or a retained graph is differentiated again, the backward re-runs the forward from
-    the saved inputs first.  A second backward through a graph that was not retained raises torch's error.
+    Forward = stage + run, on the context's device whatever device the inputs are on.  The first call stages `tn`
+    itself; every call then copies the inputs into the staged network on the device (NetworkPlan.set_leaves, or
+    NetworkPlan.stage_instances of the network marshalled once with `batched`), ordered against torch's current stream
+    both ways.  So the payloads of the leaves that are not inputs are read once, at the first call: changing them in
+    `tn` afterwards does not change the function.  With on_device=False (the default), inputs may be on any device:
+    those elsewhere are packed into one buffer and arrive in one copy.  The result comes back on the CPU, each gradient
+    on its input's device and a forward-mode tangent on the result's.  A backward needs the plan's forward state: when
+    another call of the same function ran in between, or a retained graph is differentiated again, the backward re-runs
+    the forward from the saved inputs first.  A second backward through a graph that was not retained raises torch's
+    error.
 
     sliced_legs: legs of `tn` to slice (e.g. from contractionpath.slicing.find_slices), for networks whose gradient
     workspace does not fit unsliced.  Forward = stage + the forward levels of every slice, summed on the device;
@@ -507,8 +397,8 @@ def network_function(tn: Tensor, path: ContractionPath, wrt: Sequence[int], ctx:
     batched: Matrix leaves whose payload differs per instance, e.g. bitstring projectors or per-sample input states; they
     may include leaves not in `wrt`.  The callable then takes one tensor per `wrt` leaf followed by one per batched leaf
     not in `wrt`, in the order given; a batched leaf's tensor is [B, *leaf shape] with one B for all of them, the others
-    are [*leaf shape] and shared by every instance.  It returns [B, *result].  Forward = stage_batch + the forward pass
-    of every instance (NetworkPlan.vjp_batch, values only); backward = vjp_batch with seeds conj(grad_out), a forward
+    are [*leaf shape] and shared by every instance.  It returns [B, *result].  Forward = stage_instances + the forward
+    pass of every instance (NetworkPlan.vjp_batch, values only); backward = vjp_batch with seeds conj(grad_out), a forward
     plus backward pass of every instance: per-instance gradient rows for batched inputs in `wrt`, their sum over the
     instances for shared ones.  About 4 forward passes per forward + backward in all, against about 3 for one
     unbatched network; the instances share every launch.  Not combinable with sliced_legs.
@@ -530,10 +420,8 @@ def network_function(tn: Tensor, path: ContractionPath, wrt: Sequence[int], ctx:
     without a graph.  torch.func.hessian / jacrev / jacfwd need a vmap rule the function does not have.
 
     on_device=True: the inputs must be torch CUDA tensors on the context's device (else ValueError), and the result and
-    the gradients are CUDA tensors there; no payload, result or gradient goes through the host.  The first call stages
-    `tn` itself; every call then copies the inputs into the staged network on the device (NetworkPlan.set_leaves, or
-    NetworkPlan.stage_instances of the network marshalled once with `batched`), ordered against torch's current stream
-    both ways.  Values and gradients equal those of on_device=False bit for bit."""
+    the gradients are CUDA tensors there; no payload, result or gradient goes through the host.  Values and gradients
+    equal those of on_device=False bit for bit."""
     return NetworkFunction(tn, path, wrt, ctx, sliced_legs, batched, on_device)
 
 

@@ -190,37 +190,16 @@ class SlicedPlan:
 
     @classmethod
     def _derivative(cls, create: str, tn: Tensor, path: ContractionPath, legs: Sequence[int], wrt, ctx) -> "SlicedPlan":
-        import ctypes as C
         from .. import default_context
-        from .._lib import check, u64_array
-        from ..tensornetwork.contraction import NetworkPlan, _Marshal, leaves
+        from .._lib import u64_array
+        from ..tensornetwork.contraction import NetworkPlan, leaves
         self = cls.__new__(cls)
         self.ctx = ctx or default_context()
         self.sn = None
-        lv = leaves(tn)
-        shapes = [tuple(int(d) for d in leaf.bond_dims) for leaf in lv]
-        mask = None
-        if wrt is not None:
-            mask = (C.c_uint8 * max(len(shapes), 1))()
-            for i in wrt:
-                if not 0 <= int(i) < len(shapes):
-                    raise IndexError(f"leaf index {i} out of range ({len(shapes)} leaves)")
-                mask[int(i)] = 1
         legs = [int(l) for l in legs]
-        m = _Marshal()
-        c_tn, c_path = m.tn(tn), m.path(path)
-        c_legs = u64_array(legs or [0])
-        h = C.c_void_p()
-        check(getattr(self.ctx._l, create)(self.ctx.handle, C.byref(c_tn), C.byref(c_path), len(legs), c_legs, mask, C.byref(h)))
-        plan = NetworkPlan.__new__(NetworkPlan)
-        plan.ctx, plan.handle, plan.leaf_shapes = self.ctx, h, shapes
-        n_out, out_legs, out_dims = C.c_int(), u64_array([0] * 64), u64_array([0] * 64)
-        check(self.ctx._l.tncb_network_out_legs(C.byref(c_tn), C.byref(c_path), C.byref(n_out), out_legs, out_dims))
-        plan.result_legs = [out_legs[i] for i in range(n_out.value)]
-        plan.result_dims = tuple(int(out_dims[i]) for i in range(n_out.value))
-        self.plan = plan
+        self.plan = NetworkPlan._derivative_plan(create, tn, path, wrt, self.ctx, len(legs), u64_array(legs or [0]))
         self._legs = None
-        dim = {l: int(d) for t in lv for l, d in zip(t.legs, t.bond_dims)}
+        dim = {l: int(d) for t in leaves(tn) for l, d in zip(t.legs, t.bond_dims)}
         self.n_slices = int(np.prod([dim[l] for l in legs], dtype=object)) if legs else 1
         return self
 
@@ -239,14 +218,11 @@ class SlicedPlan:
         """(value, {leaf index: G}) summed over the slices rank, rank + world, ...: value is bit-identical to `run`, G has
         the full leaf's shape with G[e] = sum_r seed[r] dR[r]/dX[e] (no conjugation).  seed: array or DeviceTensor with
         the result's shape, None for a scalar result.  With world > 1 and allreduce, both are summed over the ranks."""
+        from ..tensornetwork.contraction import _download
         from ..tensornetwork.tensordata import TensorData
         value, block = self.vjp_blocks(seed, rank, world, allreduce)
-        flat = block.to_numpy()
-        block.free()
-        grads = {}
-        for i, (off, shape) in enumerate(zip(self.plan.grad_offsets(), self.plan.leaf_shapes)):
-            if off >= 0:
-                grads[i] = flat[off:off + int(np.prod(shape, dtype=np.int64))].reshape(shape)
+        (flat,) = _download([block])
+        grads = self.plan._unpack(self.plan.grad_offsets(), flat, ())
         if self._legs is None:        # the result's leg order: an empty slice range returns it without running a kernel
             self._legs = list(self.plan.run_slices(self.n_slices, 1).legs)
         res = Tensor(self._legs, value.shape)
@@ -269,11 +245,7 @@ class SlicedPlan:
         finally:
             if tmp is not None:
                 tmp.free()
-        value, block = DeviceTensor.adopt(ctx, val), DeviceTensor.adopt(ctx, out)
-        if world > 1 and allreduce:
-            check(ctx._l.tncb_comm_allreduce_sum(ctx.handle, value.handle))
-            check(ctx._l.tncb_comm_allreduce_sum(ctx.handle, block.handle))
-        return value, block
+        return tuple(self._allreduce((DeviceTensor.adopt(ctx, val), DeviceTensor.adopt(ctx, out)), world, allreduce))
 
     def _allreduce(self, blocks, world: int, allreduce: bool):
         from .._lib import check
@@ -303,13 +275,12 @@ class SlicedPlan:
     def jvp(self, tangents: dict, rank: int = 0, world: int = 1, allreduce: bool = True):
         """`jvp_block` with the derivative downloaded: (value Tensor on the device with the result's legs, tangent
         ndarray), tangent[r] = sum_l sum_e dR[r]/dX_l[e] tangents[l][e] over the full leaves (no conjugation)."""
+        from ..tensornetwork.contraction import _download
         from ..tensornetwork.tensordata import TensorData
         val, tan = self.jvp_block(tangents, rank, world, allreduce)
         res = Tensor(list(self.plan.result_legs), val.shape)
         res.set_tensor_data(TensorData.Matrix(val))
-        out = tan.to_numpy()
-        tan.free()
-        return res, out
+        return res, _download([tan])[0]
 
     def hvp_blocks(self, tangents: dict, seed=None, seed_tangent=None, rank: int = 0, world: int = 1, allreduce: bool = True,
                    outputs=(True, True, True, True)):
@@ -342,18 +313,10 @@ class SlicedPlan:
     def hvp(self, tangents: dict, seed=None, seed_tangent=None, rank: int = 0, world: int = 1, allreduce: bool = True):
         """`hvp_blocks` downloaded: (value, tangent, {leaf: G}, {leaf: Ġ}) as host arrays, G and Ġ shaped like the full
         leaf, for every requested leaf (see NetworkPlan.hvp)."""
-        host = []
-        for dt in self.hvp_blocks(tangents, seed, seed_tangent, rank, world, allreduce):
-            host.append(dt.to_numpy())
-            dt.free()
-        value, tangent, g, dg = host
-        grads, grad_tangents = {}, {}
-        for i, (off, shape) in enumerate(zip(self.plan.grad_offsets(), self.plan.leaf_shapes)):
-            if off >= 0:
-                size = int(np.prod(shape, dtype=np.int64))
-                grads[i] = g[off:off + size].reshape(shape)
-                grad_tangents[i] = dg[off:off + size].reshape(shape)
-        return value, tangent, grads, grad_tangents
+        from ..tensornetwork.contraction import _download
+        value, tangent, g, dg = _download(self.hvp_blocks(tangents, seed, seed_tangent, rank, world, allreduce))
+        offs = self.plan.grad_offsets()
+        return value, tangent, self.plan._unpack(offs, g, ()), self.plan._unpack(offs, dg, ())
 
     def set_leaves(self, payloads: dict) -> None:
         """New payloads for leaves of the staged FULL network straight from device memory ({leaf index: torch CUDA tensor

@@ -6,6 +6,7 @@ upload and every pair kernel run inside libtncb200."""
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 from itertools import chain
 from typing import List, Optional
@@ -197,11 +198,16 @@ def _device_sources(ctx: Context, shapes, payloads: dict, count: Optional[int] =
             raise IndexError(f"leaf index {leaf} out of range ({len(shapes)} leaves)")
         check_cuda_tensor(ctx, x, f"the payload of leaf {leaf}")
         shape = tuple(shapes[leaf])
-        elems = int(np.prod(shape, dtype=np.int64))
+        elems = math.prod(shape)
+        x = x.detach()
+        # a lazily conjugated or negated view keeps its bit through .to and .contiguous, and its data_ptr is the
+        # memory without it
+        if x.dtype != torch.complex128 or x.is_conj() or x.is_neg():
+            x = x.to(torch.complex128).resolve_conj().resolve_neg()
         if tuple(x.shape) == shape:
-            src, stride = x.detach().to(torch.complex128).contiguous(), 0
+            src, stride = x.contiguous(), 0
         elif count is not None and tuple(x.shape) == (int(count),) + shape:
-            src = x.detach().to(torch.complex128)
+            src = x
             if count > 1 and src[0].is_contiguous() and src.stride(0) >= elems:
                 stride = src.stride(0)
             else:
@@ -214,6 +220,16 @@ def _device_sources(ctx: Context, shapes, payloads: dict, count: Optional[int] =
         strides.append(stride)
         keep.append(src)
     return idx, ptrs, strides, keep
+
+
+def _download(blocks) -> list:
+    """the DeviceTensors `blocks` as host arrays, each freed; None stays None"""
+    out = []
+    for b in blocks:
+        out.append(None if b is None else b.to_numpy())
+        if b is not None:
+            b.free()
+    return out
 
 
 def _call_after_torch(ctx: Context, keep, call) -> None:
@@ -266,7 +282,8 @@ class NetworkPlan:
         return cls._derivative_plan("tncb_plan_create_hvp", tn, contract_path, wrt, ctx)
 
     @classmethod
-    def _derivative_plan(cls, create: str, tn: Tensor, contract_path: ContractionPath, wrt, ctx) -> "NetworkPlan":
+    def _derivative_plan(cls, create: str, tn: Tensor, contract_path: ContractionPath, wrt, ctx, *extra) -> "NetworkPlan":
+        """a plan from the creator `create`, called with `extra` (a sliced creator's legs) between the path and the mask"""
         self = cls.__new__(cls)
         self.handle = None
         self.ctx = ctx or default_context()
@@ -281,7 +298,7 @@ class NetworkPlan:
         m = _Marshal()
         c_tn, c_path = m.tn(tn), m.path(contract_path)
         h = C.c_void_p()
-        check(getattr(self.ctx._l, create)(self.ctx.handle, C.byref(c_tn), C.byref(c_path), mask, C.byref(h)))
+        check(getattr(self.ctx._l, create)(self.ctx.handle, C.byref(c_tn), C.byref(c_path), *extra, mask, C.byref(h)))
         self.handle = h
         self.leaf_shapes = shapes
         n_out, legs, dims = C.c_int(), u64_array([0] * 64), u64_array([0] * 64)
@@ -300,14 +317,8 @@ class NetworkPlan:
         """After a forward `run`/`execute` of a gradient plan: {leaf index: G} for every requested leaf, G shaped like
         the leaf with G[e] = sum_r seed[r] dR[r]/dX[e] (no conjugation).  seed: array or DeviceTensor with the result's
         shape; None for a scalar result (seed 1).  One device-to-host copy of the whole gradient block."""
-        block = self.vjp_block(seed)
-        flat = block.to_numpy()
-        block.free()
-        grads = {}
-        for i, (off, shape) in enumerate(zip(self.grad_offsets(), self.leaf_shapes)):
-            if off >= 0:
-                grads[i] = flat[off:off + int(np.prod(shape, dtype=np.int64))].reshape(shape)
-        return grads
+        (flat,) = _download([self.vjp_block(seed)])
+        return self._unpack(self.grad_offsets(), flat, ())
 
     def vjp_block(self, seed=None) -> DeviceTensor:
         """`vjp` left on the device: the rank-1 block of every requested leaf's G at grad_offsets()"""
@@ -379,9 +390,7 @@ class NetworkPlan:
         val, tan = self.jvp_block(tangents)
         res = Tensor(list(self.result_legs), val.shape)
         res.set_tensor_data(TensorData.Matrix(val))
-        out = tan.to_numpy()
-        tan.free()
-        return res, out
+        return res, _download([tan])[0]
 
     def _result_input(self, x, what: str):
         """(DeviceTensor, temporary to free) for an array, a torch CUDA tensor or a DeviceTensor with the result's shape"""
@@ -425,19 +434,9 @@ class NetworkPlan:
         """`hvp_blocks` downloaded: (value, tangent, {leaf: G}, {leaf: Ġ}) as host arrays, value and tangent with the
         result's shape, G and Ġ shaped like their leaf, for every requested leaf.  Ġ_l = sum_r Ṡ[r] dR[r]/dX_l +
         sum_r S[r] sum_m d²R[r]/dX_l dX_m · Ẋ_m: with Ṡ = 0 that is the Hessian of sum_r S[r] R[r] times the tangents."""
-        host = []
-        for dt in self.hvp_blocks(tangents, seed, seed_tangent):
-            host.append(dt.to_numpy())
-            dt.free()
-        value, tangent, g, dg = host
+        value, tangent, g, dg = _download(self.hvp_blocks(tangents, seed, seed_tangent))
         offs = self.grad_offsets()
-        grads, grad_tangents = {}, {}
-        for i, (off, shape) in enumerate(zip(offs, self.leaf_shapes)):
-            if off >= 0:
-                size = int(np.prod(shape, dtype=np.int64))
-                grads[i] = g[off:off + size].reshape(shape)
-                grad_tangents[i] = dg[off:off + size].reshape(shape)
-        return value, tangent, grads, grad_tangents
+        return value, tangent, self._unpack(offs, g, ()), self._unpack(offs, dg, ())
 
     def _rows_input(self, x, shape, what: str):
         """(DeviceTensor, temporary to free) for an array, a torch CUDA tensor or a DeviceTensor shaped `shape`; an array
@@ -504,11 +503,7 @@ class NetworkPlan:
         """`hvp_batch_blocks` downloaded: (legs of one instance, values [count, *dims], tangent rows [count, *dims],
         {leaf: G rows [count, *leaf shape]}, {leaf: G sum}, {leaf: Ġ rows}, {leaf: Ġ sum}) as host arrays, None where
         not requested."""
-        host = []
-        for dt in self.hvp_batch_blocks(count, tangents, seeds, seed_tangents, payloads, outputs):
-            host.append(None if dt is None else dt.to_numpy())
-            if dt is not None:
-                dt.free()
+        host = _download(self.hvp_batch_blocks(count, tangents, seeds, seed_tangents, payloads, outputs))
         offs = self.grad_offsets()
         rows, one = (int(count),), ()
         return (list(self.result_legs), host[0], host[1], self._unpack(offs, host[2], rows), self._unpack(offs, host[3], one),
@@ -535,12 +530,8 @@ class NetworkPlan:
         instance, values [count, *dims] or None, tangents [count, *dims]); row i equals jvp of instance i with its
         tangent rows, bit for bit.  Many directions of one network: stage_instances of it with count copies, one
         tangent row per direction."""
-        host = []
-        for dt in self.jvp_batch_blocks(first, count, tangents, values):
-            host.append(None if dt is None else dt.to_numpy())
-            if dt is not None:
-                dt.free()
-        return list(self.result_legs), host[0], host[1]
+        vals, tans = _download(self.jvp_batch_blocks(first, count, tangents, values))
+        return list(self.result_legs), vals, tans
 
     def set_leaves(self, payloads: dict) -> None:
         """New payloads for leaves of the staged network straight from device memory (tncb_plan_set_leaves): {leaf index
@@ -584,14 +575,7 @@ class NetworkPlan:
         the sum is the left fold of the rows in instance order, also bit for bit."""
         if count is None:
             count = max(0, getattr(self, "n_staged", 0) - int(first))
-        host = []
-        for dt in self.vjp_batch_blocks(first, count, seeds, rows, sum, values):
-            if dt is None:
-                host.append(None)
-                continue
-            host.append(dt.to_numpy())
-            dt.free()
-        vals, row_block, sum_block = host
+        vals, row_block, sum_block = _download(self.vjp_batch_blocks(first, count, seeds, rows, sum, values))
         offs = self.grad_offsets()
         return (list(self.result_legs), vals, self._unpack(offs, row_block, (int(count),)), self._unpack(offs, sum_block, ()))
 
