@@ -18,7 +18,8 @@ from typing import List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import Context, DeviceTensor, check_cuda_tensor, default_context
-from ._lib import check, u64_array
+from ._lib import check
+from .tensornetwork.contraction import PreparedNetwork, _library_call
 
 ANGLE_GATES = {"u": 3, "rx": 1, "ry": 1, "rz": 1, "cp": 1, "fsim": 2}
 
@@ -123,18 +124,12 @@ class Angles:
         want = f"[{P}] or [count, {P}]" if count is None else f"[{P}] or [{count}, {P}]"
         raise ValueError(f"{what} has shape {tuple(x.shape)}, expected {want}")
 
-    def _call(self, keep, fn) -> None:
-        from .tensornetwork.contraction import _call_after_torch
-        _call_after_torch(self.ctx, keep, fn)
-
     # ---- the three calls ----
     def gates(self, theta) -> DeviceTensor:
         """[count, block_elems] rows: row i holds every referenced leaf's gate at θ_i, zeros elsewhere"""
         th, st, n = self._rows(theta, "theta")
-        out = C.c_void_p()
-        self._call([th], lambda: self.ctx._l.tncb_angles_gates(self.ctx.handle, self.handle, C.c_void_p(th.data_ptr()), st, n,
-                                                               C.byref(out)))
-        return DeviceTensor.adopt(self.ctx, out)
+        return _library_call(self.ctx, "tncb_angles_gates", [self.ctx.handle, self.handle, C.c_void_p(th.data_ptr()), st, n],
+                             (True,), [th])[0]
 
     def tangents(self, theta, theta_dot) -> DeviceTensor:
         """[count, block_elems] rows of leaf tangents Ẋ_l = sum_{r on l} scale_r θ̇[param_r] dU_l/da_{slot_r}; theta and
@@ -145,10 +140,8 @@ class Angles:
         n = max(n, nd)
         if nd == 1:
             sd = 0
-        out = C.c_void_p()
-        self._call([th, td], lambda: self.ctx._l.tncb_angles_tangents(
-            self.ctx.handle, self.handle, C.c_void_p(th.data_ptr()), st, C.c_void_p(td.data_ptr()), sd, n, C.byref(out)))
-        rows = DeviceTensor.adopt(self.ctx, out)
+        rows = _library_call(self.ctx, "tncb_angles_tangents", [self.ctx.handle, self.handle, C.c_void_p(th.data_ptr()), st,
+                                                                C.c_void_p(td.data_ptr()), sd, n], (True,), [th, td])[0]
         if theta.dim() == 1 and theta_dot.dim() == 1:
             return _vector(rows)
         return rows
@@ -169,19 +162,16 @@ class Angles:
             if nv == 1:
                 sv = 0
             keep.append(dv)
-        outs = [C.c_void_p() if want else None for want in (rows, sum)]
-        self._call(keep, lambda: self.ctx._l.tncb_angles_pullback(
+        return tuple(_library_call(self.ctx, "tncb_angles_pullback", [
             self.ctx.handle, self.handle, C.c_void_p(th.data_ptr()), st, n, grads.handle,
-            grad_tangents.handle if grad_tangents is not None else None,
-            C.c_void_p(dv.data_ptr()) if dv is not None else None, sv,
-            *[C.byref(o) if o is not None else None for o in outs]))
-        return tuple(None if o is None else DeviceTensor.adopt(self.ctx, o) for o in outs)
+            grad_tangents.handle if grad_tangents is not None else None, C.c_void_p(dv.data_ptr()) if dv is not None else None,
+            sv], (rows, sum), keep))
 
     # ---- into plans ----
-    def _sources(self, rows: DeviceTensor):
+    def _gate_ptrs(self, rows: DeviceTensor) -> list:
+        """the device address of every referenced leaf's gate in each row of `rows`"""
         base = rows.device_ptr()
-        idx = self.leaf_index
-        return len(idx), u64_array(idx), (C.c_void_p * max(len(idx), 1))(*[base + 16 * self.offsets[l] for l in idx])
+        return [base + 16 * self.offsets[l] for l in self.leaf_index]
 
     def set_leaves(self, plan, theta) -> None:
         """The referenced leaves of the staged `plan` (NetworkPlan or sliced gradient SlicedPlan) set to their gates at
@@ -189,25 +179,20 @@ class Angles:
         plan = getattr(plan, "plan", plan)
         rows = self.gates(theta)
         try:
-            n, idx, src = self._sources(rows)
-            check(self.ctx._l.tncb_plan_set_leaves(self.ctx.handle, plan.handle, n, idx, src))
+            plan._set_leaves(self.leaf_index, self._gate_ptrs(rows))
         finally:
             rows.free()                  # (the arena reuses it in stream order, after the copy)
 
     def stage_instances(self, plan, template, theta_rows) -> None:
         """count = len(theta_rows) instances of `plan`: every leaf from `template` (a Tensor or PreparedNetwork of the
         plan's structure) except the referenced leaves, which take their gates at θ_i: gates + tncb_plan_stage_instances"""
-        from .tensornetwork.contraction import PreparedNetwork
         tmpl = template if isinstance(template, PreparedNetwork) else PreparedNetwork(template)
         rows = self.gates(theta_rows)
-        count = rows.shape[0]
         try:
-            n, idx, src = self._sources(rows)
-            check(self.ctx._l.tncb_plan_stage_instances(self.ctx.handle, plan.handle, C.byref(tmpl.node), count, n, idx, src,
-                                                        u64_array([self.block_elems] * n)))
+            plan._stage_instances(tmpl, rows.shape[0], self.leaf_index, self._gate_ptrs(rows),
+                                  [self.block_elems] * len(self.leaf_index))
         finally:
             rows.free()
-        plan.n_staged = count
 
     def __del__(self):
         try:

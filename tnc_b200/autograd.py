@@ -19,17 +19,16 @@ Forward mode (torch.autograd.forward_ad, torch.func.jvp) runs on a tangent plan 
 pass through the network from Hessian-vector products of a forward-over-reverse plan (NetworkPlan.for_hvp)."""
 from __future__ import annotations
 
-import ctypes
 import math
 from typing import Optional, Sequence
 
 import torch
 
-from . import Context, DeviceTensor, check_cuda_tensor, default_context
-from ._lib import check
+from . import Context, check_cuda_tensor, default_context
 from .contractionpath import ContractionPath
 from .contractionpath.slicing import SlicedPlan
 from .tensornetwork import NetworkPlan, PreparedNetwork, Tensor, leaves
+from .tensornetwork.contraction import _download
 from .tensornetwork.tensordata import TensorData
 
 
@@ -144,16 +143,6 @@ class _HessFn(torch.autograd.Function):
             tans = {i: torch.conj_physical(t) for i, t in zip(runner.wrt, b) if t is not None}
             _, gdot = runner._hvp(xs, seed, tans, None if a is None else torch.conj_physical(a), want_rdot=False)
         return (None, None) + (None,) * len(xs) + tuple(torch.conj_physical(g) for g in gdot)
-
-
-def _to_torch(blocks) -> list:
-    """the DeviceTensors `blocks` as torch CUDA tensors, each freed; None stays None"""
-    out = []
-    for b in blocks:
-        out.append(None if b is None else b.to_torch())
-        if b is not None:
-            b.free()
-    return out
 
 
 class NetworkFunction:
@@ -278,29 +267,25 @@ class NetworkFunction:
             vals = self.plan.vjp_batch_blocks(0, None, rows=False, sum=False, values=True)[0]
         else:
             vals = self.plan.run().tensordata.matrix
-        (res,) = _to_torch([vals])
+        (res,) = _download([vals], "to_torch")
         return res if self.on_device else res.cpu()
 
     def _backward(self, fctx, grad_out, xs):
         """the gradients of batched or sliced inputs (torch's convention, conj of the holomorphic vjp), None for batched
         inputs not in wrt: per-instance rows for batched inputs, their sum over the instances for shared ones"""
-        (s,) = self._to_ctx([torch.conj_physical(grad_out)], ["the seed"])
-        seed = DeviceTensor.from_torch(self._ctx, s)
-        try:
-            # vjp_batch and vjp_sliced re-run every forward: they only need these inputs staged
-            if self._token != fctx.token:
-                self._stage(self.plan, xs)
-                fctx.token = self._token = object()
-            if self.batched:
-                _, rows, total = self.plan.vjp_batch_blocks(0, None, seeds=seed, rows=any(i in self.batched for i in self.wrt),
-                                                            sum=any(i not in self.batched for i in self.wrt), values=False)
-            else:
-                value, total = self.plan.vjp_blocks(seed)
-                value.free()
-                rows = None
-        finally:
-            seed.free()
-        rows, total = (None if b is None else torch.conj_physical(b) for b in _to_torch([rows, total]))
+        (seed,) = self._to_ctx([torch.conj_physical(grad_out)], ["the seed"])
+        # vjp_batch and vjp_sliced re-run every forward: they only need these inputs staged
+        if self._token != fctx.token:
+            self._stage(self.plan, xs)
+            fctx.token = self._token = object()
+        if self.batched:
+            _, rows, total = self.plan.vjp_batch_blocks(0, None, seeds=seed, rows=any(i in self.batched for i in self.wrt),
+                                                        sum=any(i not in self.batched for i in self.wrt), values=False)
+        else:
+            value, total = self.plan.vjp_blocks(seed)
+            value.free()
+            rows = None
+        rows, total = (None if b is None else torch.conj_physical(b) for b in _download([rows, total], "to_torch"))
         wrt = dict(zip(self.wrt, xs))
         g = {}
         if rows is not None:
@@ -313,15 +298,11 @@ class NetworkFunction:
         """G_i = sum_r seed[r] dR[r]/dx_i (holomorphic, no conjugation) of the unbatched, unsliced plan, one per wrt input:
         the forward of the _NetworkFn call `fctx` (re-run when another call used the plan's state since), then vjp"""
         (s,) = self._to_ctx([seed], ["the seed"])
-        s = DeviceTensor.from_torch(self._ctx, s)
-        try:
-            if self._token != fctx.token:
-                self._forward(xs)
-                fctx.token = self._token
-            self._token = None           # the backward levels overwrite the forward state
-            (flat,) = _to_torch([self.plan.vjp_block(s)])
-        finally:
-            s.free()
+        if self._token != fctx.token:
+            self._forward(xs)
+            fctx.token = self._token
+        self._token = None               # the backward levels overwrite the forward state
+        (flat,) = _download([self.plan.vjp_block(s)], "to_torch")
         return tuple(self._split(flat, dict(zip(self.wrt, xs))).values())
 
     # ---- second order (create_graph=True, torch.autograd.functional.hvp / hessian, torch.func.jvp of torch.func.grad):
@@ -338,7 +319,7 @@ class NetworkFunction:
                           [f"tangent for leaf {i}" for i in tangents] + ["the seed", "the seed tangent"])
         _, rdot, _, gdot = self._hplan.hvp_blocks(dict(zip(tangents, ts[:n])), ts[n], ts[n + 1] if seed_tangent is not None else None,
                                                   (False, want_rdot, False, True))
-        rdot, gdot = _to_torch([rdot, gdot])
+        rdot, gdot = _download([rdot, gdot], "to_torch")
         g = self._split(gdot, dict(zip(self.wrt, xs)))
         return None if rdot is None else rdot.to(seed.device), tuple(g.values())
 
@@ -362,7 +343,7 @@ class NetworkFunction:
         else:
             val, tan = self._tplan.jvp_block(tans)
             val.free()
-        return _to_torch([tan])[0].to(device)
+        return _download([tan], "to_torch")[0].to(device)
 
     def __call__(self, *xs: torch.Tensor) -> torch.Tensor:
         if len(xs) != len(self.inputs):
@@ -493,23 +474,20 @@ class CircuitFunction:
 
     def _backward(self, theta, grad_out):
         B = self._theta(theta)
-        seed = DeviceTensor.from_torch(self.ctx, torch.conj_physical(grad_out.to(torch.complex128)))
-        try:
-            if B:
-                self.angles.stage_instances(self.plan, self.template, theta)
-                G = self.plan.vjp_batch_blocks(0, B, seeds=seed, rows=True, sum=False, values=False)[1]
+        seed = torch.conj_physical(grad_out.to(torch.complex128))
+        if B:
+            self.angles.stage_instances(self.plan, self.template, theta)
+            G = self.plan.vjp_batch_blocks(0, B, seeds=seed, rows=True, sum=False, values=False)[1]
+        else:
+            self.angles.set_leaves(self.plan, theta)
+            if self.sliced_legs:
+                value, G = self.plan.vjp_blocks(seed)
+                value.free()
             else:
-                self.angles.set_leaves(self.plan, theta)
-                if self.sliced_legs:
-                    value, G = self.plan.vjp_blocks(seed)
-                    value.free()
-                else:
-                    self.plan.run()
-                    G = self.plan.vjp_block(seed)
-            rows = self.angles.pullback(theta, G)[0]
-            G.free()
-        finally:
-            seed.free()
+                self.plan.run()
+                G = self.plan.vjp_block(seed)
+        rows = self.angles.pullback(theta, G)[0]
+        G.free()
         g = rows.to_torch().real
         rows.free()
         return g if B else g[0]
@@ -526,22 +504,17 @@ class CircuitFunction:
             self._tplan.stage(self.tn)
             self._tangles = Angles(self.ctx, self.tn, self.map, self._tplan)
         tdot = theta_dot.detach().to(torch.float64)
-        l, plan = self.ctx._l, self._tplan
-        out = ctypes.c_void_p()
+        plan = self._tplan
         if B:
             self._tangles.stage_instances(plan, self.template, theta)
-            tan = self._tangles.tangents(theta, tdot)
-            rc = l.tncb_plan_jvp_batch(self.ctx.handle, plan.handle, 0, B, tan.handle, None, ctypes.byref(out))
         else:
             self._tangles.set_leaves(plan, theta)
-            tan = self._tangles.tangents(theta, tdot)
-            rc = l.tncb_plan_jvp(self.ctx.handle, plan.handle, tan.handle, None, ctypes.byref(out))
-        tan.free()
-        check(rc)
-        rdot = DeviceTensor.adopt(self.ctx, out)
-        res = rdot.to_torch()
-        rdot.free()
-        return res
+        tan = self._tangles.tangents(theta, tdot)
+        try:
+            rdot = plan.jvp_batch_blocks(0, B, tan, values=False)[1] if B else plan._jvp_tangent(tan)
+        finally:
+            tan.free()
+        return _download([rdot], "to_torch")[0]
 
     def __call__(self, theta: torch.Tensor) -> torch.Tensor:
         return _CircuitFn.apply(self, theta)

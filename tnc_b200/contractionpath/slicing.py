@@ -198,7 +198,6 @@ class SlicedPlan:
         self.sn = None
         legs = [int(l) for l in legs]
         self.plan = NetworkPlan._derivative_plan(create, tn, path, wrt, self.ctx, len(legs), u64_array(legs or [0]))
-        self._legs = None
         dim = {l: int(d) for t in leaves(tn) for l, d in zip(t.legs, t.bond_dims)}
         self.n_slices = int(np.prod([dim[l] for l in legs], dtype=object)) if legs else 1
         return self
@@ -216,36 +215,18 @@ class SlicedPlan:
 
     def vjp(self, seed=None, rank: int = 0, world: int = 1, allreduce: bool = True):
         """(value, {leaf index: G}) summed over the slices rank, rank + world, ...: value is bit-identical to `run`, G has
-        the full leaf's shape with G[e] = sum_r seed[r] dR[r]/dX[e] (no conjugation).  seed: array or DeviceTensor with
-        the result's shape, None for a scalar result.  With world > 1 and allreduce, both are summed over the ranks."""
-        from ..tensornetwork.contraction import _download
-        from ..tensornetwork.tensordata import TensorData
+        the full leaf's shape with G[e] = sum_r seed[r] dR[r]/dX[e] (no conjugation).  seed: array, torch CUDA tensor or
+        DeviceTensor with the result's shape, None for a scalar result.  With world > 1 and allreduce, both are summed
+        over the ranks."""
+        from ..tensornetwork.contraction import _download, _leaf
         value, block = self.vjp_blocks(seed, rank, world, allreduce)
         (flat,) = _download([block])
-        grads = self.plan._unpack(self.plan.grad_offsets(), flat, ())
-        if self._legs is None:        # the result's leg order: an empty slice range returns it without running a kernel
-            self._legs = list(self.plan.run_slices(self.n_slices, 1).legs)
-        res = Tensor(self._legs, value.shape)
-        res.set_tensor_data(TensorData.Matrix(value))
-        return res, grads
+        return _leaf(list(self.plan.result_legs), value), self.plan._unpack(self.plan.grad_offsets(), flat, ())
 
     def vjp_blocks(self, seed=None, rank: int = 0, world: int = 1, allreduce: bool = True):
         """`vjp` left on the device: (value, rank-1 gradient block at grad_offsets()) as DeviceTensors"""
-        import ctypes as C
-        from .. import DeviceTensor
-        from .._lib import check
-        ctx = self.ctx
-        tmp = None
-        if seed is not None and not isinstance(seed, DeviceTensor):
-            seed = tmp = DeviceTensor.from_numpy(ctx, np.asarray(seed, dtype=np.complex128))
-        val, out = C.c_void_p(), C.c_void_p()
-        try:
-            check(ctx._l.tncb_plan_vjp_sliced(ctx.handle, self.plan.handle, int(rank), int(world),
-                                              seed.handle if seed is not None else None, C.byref(val), C.byref(out)))
-        finally:
-            if tmp is not None:
-                tmp.free()
-        return tuple(self._allreduce((DeviceTensor.adopt(ctx, val), DeviceTensor.adopt(ctx, out)), world, allreduce))
+        return tuple(self._allreduce(self.plan._call("tncb_plan_vjp_sliced", int(rank), int(world), inputs=[(seed, "seed", None)],
+                                                     outputs=(True, True)), world, allreduce))
 
     def _allreduce(self, blocks, world: int, allreduce: bool):
         from .._lib import check
@@ -255,62 +236,33 @@ class SlicedPlan:
                     check(self.ctx._l.tncb_comm_allreduce_sum(self.ctx.handle, b.handle))
         return blocks
 
-    def jvp_block(self, tangents: dict, rank: int = 0, world: int = 1, allreduce: bool = True):
+    def jvp_block(self, tangents, rank: int = 0, world: int = 1, allreduce: bool = True):
         """A sliced tangent plan's forward-mode pass over the slices rank, rank + world, ... (tncb_plan_jvp_sliced), left on
         the device: (value, tangent) DeviceTensors with the result's shape.  tangents: {leaf index: array or torch CUDA
-        tensor shaped like the FULL leaf}; requested leaves left out have zero tangent.  value equals `run` bit for bit.
-        With world > 1 and allreduce, both are summed over the ranks."""
-        import ctypes as C
-        from .. import DeviceTensor
-        from .._lib import check
-        block = self.plan._tangent_block(tangents)
-        val, tan = C.c_void_p(), C.c_void_p()
-        try:
-            check(self.ctx._l.tncb_plan_jvp_sliced(self.ctx.handle, self.plan.handle, int(rank), int(world), block.handle,
-                                                   C.byref(val), C.byref(tan)))
-        finally:
-            block.free()
-        return tuple(self._allreduce((DeviceTensor.adopt(self.ctx, val), DeviceTensor.adopt(self.ctx, tan)), world, allreduce))
+        tensor shaped like the FULL leaf}, requested leaves left out having zero tangent, or the tangents already packed
+        at grad_offsets() (see NetworkPlan.jvp_block).  value equals `run` bit for bit.  With world > 1 and allreduce,
+        both are summed over the ranks."""
+        return tuple(self._allreduce(self.plan._call("tncb_plan_jvp_sliced", int(rank), int(world),
+                                                     inputs=[(tangents, "tangents", None)], outputs=(True, True)), world, allreduce))
 
-    def jvp(self, tangents: dict, rank: int = 0, world: int = 1, allreduce: bool = True):
+    def jvp(self, tangents, rank: int = 0, world: int = 1, allreduce: bool = True):
         """`jvp_block` with the derivative downloaded: (value Tensor on the device with the result's legs, tangent
         ndarray), tangent[r] = sum_l sum_e dR[r]/dX_l[e] tangents[l][e] over the full leaves (no conjugation)."""
-        from ..tensornetwork.contraction import _download
-        from ..tensornetwork.tensordata import TensorData
+        from ..tensornetwork.contraction import _download, _leaf
         val, tan = self.jvp_block(tangents, rank, world, allreduce)
-        res = Tensor(list(self.plan.result_legs), val.shape)
-        res.set_tensor_data(TensorData.Matrix(val))
-        return res, _download([tan])[0]
+        return _leaf(list(self.plan.result_legs), val), _download([tan])[0]
 
-    def hvp_blocks(self, tangents: dict, seed=None, seed_tangent=None, rank: int = 0, world: int = 1, allreduce: bool = True,
+    def hvp_blocks(self, tangents, seed=None, seed_tangent=None, rank: int = 0, world: int = 1, allreduce: bool = True,
                    outputs=(True, True, True, True)):
         """A sliced Hessian-vector plan's forward-over-reverse pass over the slices rank, rank + world, ...
         (tncb_plan_hvp_sliced), left on the device: [value, tangent, grads, grad_tangents] as DeviceTensors, None where
         `outputs` is False; grads and grad_tangents are full-shape blocks at grad_offsets().  Arguments as
-        NetworkPlan.hvp_blocks, with tangents shaped like the FULL leaves.  With world > 1 and allreduce, every returned
-        block is summed over the ranks."""
-        import ctypes as C
-        from .. import DeviceTensor
-        from .._lib import check
-        block = self.plan._tangent_block(tangents)
-        tmp = []
-        try:
-            s, t = self.plan._result_input(seed, "seed")
-            tmp.append(t)
-            ds, t = self.plan._result_input(seed_tangent, "seed tangent")
-            tmp.append(t)
-            outs = [C.c_void_p() if want else None for want in outputs]
-            check(self.ctx._l.tncb_plan_hvp_sliced(self.ctx.handle, self.plan.handle, int(rank), int(world), block.handle,
-                                                   s.handle if s is not None else None, ds.handle if ds is not None else None,
-                                                   *[C.byref(o) if o is not None else None for o in outs]))
-        finally:
-            block.free()
-            for t in tmp:
-                if t is not None:
-                    t.free()
-        return self._allreduce([None if o is None else DeviceTensor.adopt(self.ctx, o) for o in outs], world, allreduce)
+        NetworkPlan.hvp_blocks, with tangents shaped like the FULL leaves, or already packed.  With world > 1 and
+        allreduce, every returned block is summed over the ranks."""
+        return self._allreduce(self.plan._hvp("tncb_plan_hvp_sliced", (int(rank), int(world)), tangents, seed, seed_tangent,
+                                              outputs), world, allreduce)
 
-    def hvp(self, tangents: dict, seed=None, seed_tangent=None, rank: int = 0, world: int = 1, allreduce: bool = True):
+    def hvp(self, tangents, seed=None, seed_tangent=None, rank: int = 0, world: int = 1, allreduce: bool = True):
         """`hvp_blocks` downloaded: (value, tangent, {leaf: G}, {leaf: Ġ}) as host arrays, G and Ġ shaped like the full
         leaf, for every requested leaf (see NetworkPlan.hvp)."""
         from ..tensornetwork.contraction import _download
@@ -327,10 +279,8 @@ class SlicedPlan:
         self.plan.set_leaves(payloads)
 
     def run(self, rank: int = 0, world: int = 1, allreduce: bool = True) -> Tensor:
-        from .._lib import check
         total = self.plan.run_slices(rank, world)
-        if world > 1 and allreduce:
-            check(self.ctx._l.tncb_comm_allreduce_sum(self.ctx.handle, total.tensordata.matrix.handle))
+        self._allreduce([total.tensordata.matrix], world, allreduce)
         return total
 
 

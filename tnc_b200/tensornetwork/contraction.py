@@ -153,17 +153,25 @@ def contract_tensor_network(tn: Tensor, contract_path: ContractionPath, ctx: Opt
     m = _Marshal()
     c_tn = m.tn(tn)
     c_path = m.path(contract_path)
-    out = C.c_void_p()
-    n_out = C.c_int()
-    legs = u64_array([0] * 64)
-    rc = ctx._l.tncb_contract_tensor_network(ctx.handle, C.byref(c_tn), C.byref(c_path), C.byref(out), C.byref(n_out), legs)
-    check(rc)
-    for d in m.device_inputs:  # consumed by the call
+    return _leaf(*_contracted(ctx, "tncb_contract_tensor_network", C.byref(c_tn), C.byref(c_path), consumed=m.device_inputs))
+
+
+def _contracted(ctx: Context, fn: str, *args, consumed=()):
+    """ctx._l.<fn>(context, *args, out, n_out, legs), checked, for the entries that return a contracted tensor; the
+    device leaves `consumed` are then given up (the call consumed them).  Returns (the result's legs, DeviceTensor or None
+    when nothing is left)."""
+    out, n_out, legs = C.c_void_p(), C.c_int(), u64_array([0] * 64)
+    check(getattr(ctx._l, fn)(ctx.handle, *args, C.byref(out), C.byref(n_out), legs))
+    for d in consumed:
         d.release()
-    if not out.value:
+    return [legs[i] for i in range(n_out.value)], (DeviceTensor.adopt(ctx, out) if out.value else None)
+
+
+def _leaf(legs, dt: Optional[DeviceTensor]) -> Tensor:
+    """the leaf Tensor with legs `legs` holding `dt`; an empty Tensor for None"""
+    if dt is None:
         return Tensor()  # nothing left (empty network)
-    dt = DeviceTensor.adopt(ctx, out)
-    res = Tensor([legs[i] for i in range(n_out.value)], dt.shape)
+    res = Tensor(legs, dt.shape)
     res.set_tensor_data(TensorData.Matrix(dt))
     return res
 
@@ -222,14 +230,20 @@ def _device_sources(ctx: Context, shapes, payloads: dict, count: Optional[int] =
     return idx, ptrs, strides, keep
 
 
-def _download(blocks) -> list:
-    """the DeviceTensors `blocks` as host arrays, each freed; None stays None"""
+def _download(blocks, convert: str = "to_numpy") -> list:
+    """the DeviceTensors `blocks` converted by their method `convert` (host arrays; "to_torch": torch CUDA tensors), each
+    freed; None stays None"""
     out = []
     for b in blocks:
-        out.append(None if b is None else b.to_numpy())
+        out.append(None if b is None else getattr(b, convert)())
         if b is not None:
             b.free()
     return out
+
+
+def _addresses(ptrs):
+    """device addresses as a C array (one null entry when there are none)"""
+    return (C.c_void_p * max(len(ptrs), 1))(*ptrs)
 
 
 def _call_after_torch(ctx: Context, keep, call) -> None:
@@ -246,17 +260,28 @@ def _call_after_torch(ctx: Context, keep, call) -> None:
         cur.wait_stream(ext)
 
 
+def _library_call(ctx: Context, fn: str, args, outputs=(), keep=None, temps=()) -> list:
+    """ctx._l.<fn>(*args, output pointers), checked; then `temps` are freed, whatever happened.  outputs: a flag per
+    output pointer; the outputs come back as DeviceTensors, None where the flag is False.  keep: the torch tensors the call
+    reads; the call is then ordered after torch's current stream (_call_after_torch)."""
+    outs = [C.c_void_p() if want else None for want in outputs]
+    call = lambda: getattr(ctx._l, fn)(*args, *[C.byref(o) if o is not None else None for o in outs])
+    try:
+        if keep is None:
+            check(call())
+        else:
+            _call_after_torch(ctx, keep, call)
+    finally:
+        for t in temps:
+            t.free()
+    return [None if o is None else DeviceTensor.adopt(ctx, o) for o in outs]
+
+
 class NetworkPlan:
     """Compile once / execute many (tncb_plan_*): same structure, new payloads."""
 
     def __init__(self, tn: Tensor, contract_path: ContractionPath, ctx: Optional[Context] = None):
-        self.ctx = ctx or default_context()
-        m = _Marshal()
-        c_tn, c_path = m.tn(tn), m.path(contract_path)
-        h = C.c_void_p()
-        check(self.ctx._l.tncb_plan_create(self.ctx.handle, C.byref(c_tn), C.byref(c_path), C.byref(h)))
-        self.handle = h
-        self.leaf_shapes = [tuple(int(d) for d in leaf.bond_dims) for leaf in leaves(tn)]
+        self._create("tncb_plan_create", tn, contract_path, ctx)
 
     @classmethod
     def for_gradients(cls, tn: Tensor, contract_path: ContractionPath, wrt=None, ctx: Optional[Context] = None) -> "NetworkPlan":
@@ -283,29 +308,91 @@ class NetworkPlan:
 
     @classmethod
     def _derivative_plan(cls, create: str, tn: Tensor, contract_path: ContractionPath, wrt, ctx, *extra) -> "NetworkPlan":
-        """a plan from the creator `create`, called with `extra` (a sliced creator's legs) between the path and the mask"""
+        """a plan from the derivative creator `create`, called with `extra` (a sliced creator's legs) between the path and
+        the mask of `wrt`"""
         self = cls.__new__(cls)
+        self._create(create, tn, contract_path, ctx, *extra, wrt=wrt, masked=True)
+        return self
+
+    def _create(self, create: str, tn: Tensor, contract_path: ContractionPath, ctx, *extra, wrt=None, masked=False) -> None:
+        """the plan from the creator `create`, called with `extra` after the path and, when `masked` (the derivative
+        creators), the mask of the leaves `wrt` (None: no mask); then the result's legs and dims"""
         self.handle = None
         self.ctx = ctx or default_context()
-        shapes = [tuple(int(d) for d in leaf.bond_dims) for leaf in leaves(tn)]
+        self.leaf_shapes = [tuple(int(d) for d in leaf.bond_dims) for leaf in leaves(tn)]
         mask = None
         if wrt is not None:
-            mask = (C.c_uint8 * max(len(shapes), 1))()
+            mask = (C.c_uint8 * max(len(self.leaf_shapes), 1))()
             for i in wrt:
-                if not 0 <= int(i) < len(shapes):
-                    raise IndexError(f"leaf index {i} out of range ({len(shapes)} leaves)")
+                if not 0 <= int(i) < len(self.leaf_shapes):
+                    raise IndexError(f"leaf index {i} out of range ({len(self.leaf_shapes)} leaves)")
                 mask[int(i)] = 1
         m = _Marshal()
         c_tn, c_path = m.tn(tn), m.path(contract_path)
         h = C.c_void_p()
-        check(getattr(self.ctx._l, create)(self.ctx.handle, C.byref(c_tn), C.byref(c_path), *extra, mask, C.byref(h)))
+        check(getattr(self.ctx._l, create)(self.ctx.handle, C.byref(c_tn), C.byref(c_path), *extra, *([mask] if masked else []),
+                                           C.byref(h)))
         self.handle = h
-        self.leaf_shapes = shapes
         n_out, legs, dims = C.c_int(), u64_array([0] * 64), u64_array([0] * 64)
         check(self.ctx._l.tncb_network_out_legs(C.byref(c_tn), C.byref(c_path), C.byref(n_out), legs, dims))
         self.result_legs = [legs[i] for i in range(n_out.value)]
         self.result_dims = tuple(int(dims[i]) for i in range(n_out.value))
-        return self
+
+    def _call(self, fn: str, *args, inputs=(), payloads=None, outputs=(), keep=None) -> list:
+        """_library_call of self.ctx._l.<fn>(context, plan, *args, *inputs, output pointers); DeviceTensors among `args`
+        are passed as their handles.  inputs: (value, what, count) of the tensor arguments, converted in order by
+        `_input`; what they upload is freed after the call, or when a later argument is refused.  payloads: ({leaf: torch
+        CUDA tensor} or None, count) of a batched pass, checked after the inputs and passed before them as (n, leaf
+        indices, addresses, instance strides), the call then ordered after torch's current stream."""
+        tmp = []
+        try:
+            ts = [self._input(x, what, count, tmp) for x, what, count in inputs]
+            if payloads is not None:
+                p, count = payloads
+                idx, ptrs, strides, keep = _device_sources(self.ctx, self.leaf_shapes, p, count) if p else ([], [], [], None)
+                args += (len(idx), u64_array(idx), _addresses(ptrs), u64_array(strides))
+        except BaseException:
+            for t in tmp:
+                t.free()
+            raise
+        return _library_call(self.ctx, fn, [self.ctx.handle, self.handle] + [a.handle if isinstance(a, DeviceTensor) else a
+                                                                             for a in (*args, *ts)], outputs, keep, tmp)
+
+    def _input(self, x, what: str, count: Optional[int], tmp: list):
+        """The tensor argument `what` ("tangents", "seed", "seeds", "seed tangent" or "seed tangents") of a plan call as a
+        DeviceTensor; None and DeviceTensors as they are (a DeviceTensor is checked by the library).  Tangents may be
+        {leaf index: tangent}, packed by _tangent_block; else an array or torch CUDA tensor shaped like the tangent block
+        [grad_elems] or like the result, after a leading `count` unless count is None, refused with ValueError before it
+        is uploaded.  What is uploaded is appended to `tmp`."""
+        one_pass_tangents = what == "tangents" and count is None
+        if isinstance(x, DeviceTensor) or x is None and not one_pass_tangents:
+            return x
+        if isinstance(x, dict) or x is None:      # None as the tangents of one pass fails in the packing
+            t = self._tangent_block(x, count)
+        else:
+            if what == "tangents":
+                dims = (sum(math.prod(s) for off, s in zip(self.grad_offsets(), self.leaf_shapes) if off >= 0),)
+            else:
+                dims = tuple(self.result_dims)
+            shape = dims if count is None else (int(count),) + dims
+            on_device = type(x).__module__.split(".")[0] == "torch"
+            if not on_device:
+                x = np.asarray(x, dtype=np.complex128)
+            if tuple(x.shape) != shape:
+                raise ValueError(f"the {what} have shape {tuple(x.shape)}, expected {shape}" if what.endswith("s") else
+                                 f"the {what} has shape {tuple(x.shape)}, the result {shape}")
+            t = DeviceTensor.from_torch(self.ctx, x) if on_device else DeviceTensor.from_numpy(self.ctx, x)
+        tmp.append(t)
+        return t
+
+    def _staged(self, count: int, fn: str, *args, keep=None) -> None:
+        """`fn` stages `count` networks of the plan's structure: the batched calls run them"""
+        self._call(fn, *args, keep=keep)
+        self.n_staged = count
+
+    def _count(self, first: int, count: Optional[int]) -> int:
+        """count, or for None the staged networks from `first` on"""
+        return max(0, getattr(self, "n_staged", 0) - int(first)) if count is None else int(count)
 
     def grad_offsets(self) -> List[int]:
         """Element offset of every leaf's gradient in the block `vjp` downloads, -1 for leaves not requested."""
@@ -315,23 +402,14 @@ class NetworkPlan:
 
     def vjp(self, seed=None) -> dict:
         """After a forward `run`/`execute` of a gradient plan: {leaf index: G} for every requested leaf, G shaped like
-        the leaf with G[e] = sum_r seed[r] dR[r]/dX[e] (no conjugation).  seed: array or DeviceTensor with the result's
-        shape; None for a scalar result (seed 1).  One device-to-host copy of the whole gradient block."""
+        the leaf with G[e] = sum_r seed[r] dR[r]/dX[e] (no conjugation).  seed: array, torch CUDA tensor or DeviceTensor
+        with the result's shape; None for a scalar result (seed 1).  One device-to-host copy of the whole gradient block."""
         (flat,) = _download([self.vjp_block(seed)])
         return self._unpack(self.grad_offsets(), flat, ())
 
     def vjp_block(self, seed=None) -> DeviceTensor:
         """`vjp` left on the device: the rank-1 block of every requested leaf's G at grad_offsets()"""
-        tmp = None
-        if seed is not None and not isinstance(seed, DeviceTensor):
-            seed = tmp = DeviceTensor.from_numpy(self.ctx, np.asarray(seed, dtype=np.complex128))
-        out = C.c_void_p()
-        try:
-            check(self.ctx._l.tncb_plan_vjp(self.ctx.handle, self.handle, seed.handle if seed is not None else None, C.byref(out)))
-        finally:
-            if tmp is not None:
-                tmp.free()
-        return DeviceTensor.adopt(self.ctx, out)
+        return self._call("tncb_plan_vjp", inputs=[(seed, "seed", None)], outputs=(True,))[0]
 
     def _tangent_block(self, tangents: dict, count: Optional[int] = None) -> DeviceTensor:
         """{leaf index: tangent} packed at grad_offsets() into a [tangent_elems] (count=None) or [count, tangent_elems]
@@ -372,85 +450,47 @@ class NetworkPlan:
             block[..., offs[leaf]:offs[leaf] + sizes[leaf]] = x.reshape(lead + (sizes[leaf],) if got != shape else (sizes[leaf],))
         return DeviceTensor.from_torch(self.ctx, block) if on_device else DeviceTensor.from_numpy(self.ctx, block)
 
-    def jvp_block(self, tangents: dict):
+    def jvp_block(self, tangents):
         """One forward-mode pass on the staged leaves (tncb_plan_jvp), left on the device: (value, tangent) DeviceTensors
-        with the result's shape.  tangents: {leaf index: array or torch CUDA tensor shaped like the leaf}; requested
-        leaves left out have zero tangent.  The value equals a plain plan's run bit for bit; a call repeats bit for bit."""
-        block = self._tangent_block(tangents)
-        val, tan = C.c_void_p(), C.c_void_p()
-        try:
-            check(self.ctx._l.tncb_plan_jvp(self.ctx.handle, self.handle, block.handle, C.byref(val), C.byref(tan)))
-        finally:
-            block.free()
-        return DeviceTensor.adopt(self.ctx, val), DeviceTensor.adopt(self.ctx, tan)
+        with the result's shape.  tangents: {leaf index: array or torch CUDA tensor shaped like the leaf}, requested
+        leaves left out having zero tangent, or the tangents already packed at grad_offsets(): a [grad_elems] array,
+        torch CUDA tensor or DeviceTensor (Angles.tangents).  The value equals a plain plan's run bit for bit; a call
+        repeats bit for bit."""
+        return tuple(self._call("tncb_plan_jvp", inputs=[(tangents, "tangents", None)], outputs=(True, True)))
 
-    def jvp(self, tangents: dict):
+    def _jvp_tangent(self, tangents) -> DeviceTensor:
+        """jvp_block's tangent alone: the library is given no value output to fill"""
+        return self._call("tncb_plan_jvp", inputs=[(tangents, "tangents", None)], outputs=(False, True))[1]
+
+    def jvp(self, tangents):
         """`jvp_block` with the derivative downloaded: (value Tensor on the device with the result's legs, tangent
         ndarray), tangent[r] = sum_l sum_e dR[r]/dX_l[e] tangents[l][e] (no conjugation)."""
         val, tan = self.jvp_block(tangents)
-        res = Tensor(list(self.result_legs), val.shape)
-        res.set_tensor_data(TensorData.Matrix(val))
-        return res, _download([tan])[0]
+        return _leaf(list(self.result_legs), val), _download([tan])[0]
 
-    def _result_input(self, x, what: str):
-        """(DeviceTensor, temporary to free) for an array, a torch CUDA tensor or a DeviceTensor with the result's shape"""
-        if x is None or isinstance(x, DeviceTensor):
-            return x, None
-        if type(x).__module__.split(".")[0] == "torch":
-            if tuple(x.shape) != tuple(self.result_dims):
-                raise ValueError(f"the {what} has shape {tuple(x.shape)}, the result {tuple(self.result_dims)}")
-            t = DeviceTensor.from_torch(self.ctx, x)
-        else:
-            t = DeviceTensor.from_numpy(self.ctx, np.asarray(x, dtype=np.complex128))
-        return t, t
-
-    def hvp_blocks(self, tangents: dict, seed=None, seed_tangent=None, outputs=(True, True, True, True)):
+    def hvp_blocks(self, tangents, seed=None, seed_tangent=None, outputs=(True, True, True, True)):
         """One forward-over-reverse pass on the staged leaves of a Hessian-vector plan (tncb_plan_hvp), left on the
         device: [value, tangent, grads, grad_tangents] as DeviceTensors, None where `outputs` is False.  value and
         tangent have the result's shape (R and Ṙ, as jvp_block); grads and grad_tangents are [grad_elems] blocks at
         grad_offsets() (G = vjp(seed) and Ġ, its derivative along the leaf tangents and the seed tangent).
-        tangents: {leaf index: array or torch CUDA tensor shaped like the leaf}, requested leaves left out have zero
-        tangent; seed / seed_tangent: array, torch CUDA tensor or DeviceTensor with the result's shape, seed None for a
-        scalar result (seed 1), seed_tangent None = zero.  No conjugation anywhere; a call repeats bit for bit."""
-        block = self._tangent_block(tangents)
-        tmp = []
-        try:
-            s, t = self._result_input(seed, "seed")
-            tmp.append(t)
-            ds, t = self._result_input(seed_tangent, "seed tangent")
-            tmp.append(t)
-            outs = [C.c_void_p() if want else None for want in outputs]
-            check(self.ctx._l.tncb_plan_hvp(self.ctx.handle, self.handle, block.handle,
-                                            s.handle if s is not None else None, ds.handle if ds is not None else None,
-                                            *[C.byref(o) if o is not None else None for o in outs]))
-        finally:
-            block.free()
-            for t in tmp:
-                if t is not None:
-                    t.free()
-        return [None if o is None else DeviceTensor.adopt(self.ctx, o) for o in outs]
+        tangents: {leaf index: array or torch CUDA tensor shaped like the leaf}, requested leaves left out having zero
+        tangent, or a packed [grad_elems] block as jvp_block takes it; seed / seed_tangent: array, torch CUDA tensor or
+        DeviceTensor with the result's shape, seed None for a scalar result (seed 1), seed_tangent None = zero.  No
+        conjugation anywhere; a call repeats bit for bit."""
+        return self._hvp("tncb_plan_hvp", (), tangents, seed, seed_tangent, outputs)
 
-    def hvp(self, tangents: dict, seed=None, seed_tangent=None):
+    def _hvp(self, fn: str, lead, tangents, seed, seed_tangent, outputs) -> list:
+        """the forward-over-reverse pass `fn` (tncb_plan_hvp, or a sliced one with lead = (rank, world))"""
+        return self._call(fn, *lead, inputs=[(tangents, "tangents", None), (seed, "seed", None),
+                                             (seed_tangent, "seed tangent", None)], outputs=outputs)
+
+    def hvp(self, tangents, seed=None, seed_tangent=None):
         """`hvp_blocks` downloaded: (value, tangent, {leaf: G}, {leaf: Ġ}) as host arrays, value and tangent with the
         result's shape, G and Ġ shaped like their leaf, for every requested leaf.  Ġ_l = sum_r Ṡ[r] dR[r]/dX_l +
         sum_r S[r] sum_m d²R[r]/dX_l dX_m · Ẋ_m: with Ṡ = 0 that is the Hessian of sum_r S[r] R[r] times the tangents."""
         value, tangent, g, dg = _download(self.hvp_blocks(tangents, seed, seed_tangent))
         offs = self.grad_offsets()
         return value, tangent, self._unpack(offs, g, ()), self._unpack(offs, dg, ())
-
-    def _rows_input(self, x, shape, what: str):
-        """(DeviceTensor, temporary to free) for an array, a torch CUDA tensor or a DeviceTensor shaped `shape`; an array
-        or torch tensor of another shape raises ValueError before anything reaches the device (a DeviceTensor is checked
-        by the library)"""
-        if x is None or isinstance(x, DeviceTensor):
-            return x, None
-        on_device = type(x).__module__.split(".")[0] == "torch"
-        if not on_device:
-            x = np.asarray(x, dtype=np.complex128)
-        if tuple(x.shape) != tuple(shape):
-            raise ValueError(f"the {what} have shape {tuple(x.shape)}, expected {tuple(shape)}")
-        t = DeviceTensor.from_torch(self.ctx, x) if on_device else DeviceTensor.from_numpy(self.ctx, x)
-        return t, t
 
     def hvp_batch_blocks(self, count: int, tangents, seeds=None, seed_tangents=None, payloads: Optional[dict] = None,
                          outputs=(True,) * 6):
@@ -466,37 +506,9 @@ class NetworkPlan:
         result (every seed 1), seed_tangents None = zero.  Row i equals set_leaves(instance i's payloads) + hvp(tangent
         row i, seed i, seed tangent i) bit for bit; the plan's staged leaves are left as they are."""
         count = int(count)
-        offs = self.grad_offsets()
-        te = sum(int(np.prod(s, dtype=np.int64)) for off, s in zip(offs, self.leaf_shapes) if off >= 0)
-        rdims = (count,) + tuple(self.result_dims)
-        tmp = []
-        try:
-            if isinstance(tangents, dict):
-                block = self._tangent_block(tangents, count)
-                tmp.append(block)
-            else:
-                block, t = self._rows_input(tangents, (count, te), "tangents")
-                tmp.append(t)
-            s, t = self._rows_input(seeds, rdims, "seeds")
-            tmp.append(t)
-            ds, t = self._rows_input(seed_tangents, rdims, "seed tangents")
-            tmp.append(t)
-            idx, ptrs, strides, keep = _device_sources(self.ctx, self.leaf_shapes, payloads, count) if payloads else ([], [], [], [])
-            c_ptrs = (C.c_void_p * max(len(ptrs), 1))(*ptrs)
-            outs = [C.c_void_p() if want else None for want in outputs]
-            h = lambda x: x.handle if x is not None else None
-            call = lambda: self.ctx._l.tncb_plan_hvp_batch(
-                self.ctx.handle, self.handle, count, len(idx), u64_array(idx), c_ptrs, u64_array(strides), h(block), h(s), h(ds),
-                *[C.byref(o) if o is not None else None for o in outs])
-            if keep:
-                _call_after_torch(self.ctx, keep, call)
-            else:
-                check(call())
-        finally:
-            for t in tmp:
-                if t is not None:
-                    t.free()
-        return [None if o is None else DeviceTensor.adopt(self.ctx, o) for o in outs]
+        return self._call("tncb_plan_hvp_batch", count, inputs=[(tangents, "tangents", count), (seeds, "seeds", count),
+                                                                (seed_tangents, "seed tangents", count)],
+                          payloads=(payloads, count), outputs=outputs)
 
     def hvp_batch(self, count: int, tangents, seeds=None, seed_tangents=None, payloads: Optional[dict] = None,
                   outputs=(True,) * 6):
@@ -509,27 +521,20 @@ class NetworkPlan:
         return (list(self.result_legs), host[0], host[1], self._unpack(offs, host[2], rows), self._unpack(offs, host[3], one),
                 self._unpack(offs, host[4], rows), self._unpack(offs, host[5], one))
 
-    def jvp_batch_blocks(self, first: int = 0, count: Optional[int] = None, tangents: Optional[dict] = None,
-                         values: bool = True):
+    def jvp_batch_blocks(self, first: int = 0, count: Optional[int] = None, tangents=None, values: bool = True):
         """`jvp_batch` left on the device: [values [count, *dims] or None, tangents [count, *dims]] as DeviceTensors"""
-        if count is None:
-            count = max(0, getattr(self, "n_staged", 0) - int(first))
-        block = self._tangent_block(tangents or {}, int(count))
-        outs = [C.c_void_p() if values else None, C.c_void_p()]
-        try:
-            check(self.ctx._l.tncb_plan_jvp_batch(self.ctx.handle, self.handle, int(first), int(count), block.handle,
-                                                  *[C.byref(o) if o is not None else None for o in outs]))
-        finally:
-            block.free()
-        return [None if o is None else DeviceTensor.adopt(self.ctx, o) for o in outs]
+        count = self._count(first, count)
+        return self._call("tncb_plan_jvp_batch", int(first), count, inputs=[({} if tangents is None else tangents, "tangents", count)],
+                          outputs=(values, True))
 
-    def jvp_batch(self, first: int = 0, count: Optional[int] = None, tangents: Optional[dict] = None, values: bool = True):
+    def jvp_batch(self, first: int = 0, count: Optional[int] = None, tangents=None, values: bool = True):
         """Forward mode over the staged networks first .. first + count - 1 (stage_batch / stage_instances), each with
         its own tangents, the instances a grid dimension of every kernel (tncb_plan_jvp_batch).  tangents: {leaf index:
-        [count, *leaf shape] (a row per instance) or [*leaf shape] (the same for every instance)}.  Returns (legs of one
-        instance, values [count, *dims] or None, tangents [count, *dims]); row i equals jvp of instance i with its
-        tangent rows, bit for bit.  Many directions of one network: stage_instances of it with count copies, one
-        tangent row per direction."""
+        [count, *leaf shape] (a row per instance) or [*leaf shape] (the same for every instance)}, or the tangent rows
+        already packed at grad_offsets(): a [count, grad_elems] array, torch CUDA tensor or DeviceTensor
+        (Angles.tangents).  Returns (legs of one instance, values [count, *dims] or None, tangents [count, *dims]); row i
+        equals jvp of instance i with its tangent rows, bit for bit.  Many directions of one network: stage_instances of
+        it with count copies, one tangent row per direction."""
         vals, tans = _download(self.jvp_batch_blocks(first, count, tangents, values))
         return list(self.result_legs), vals, tans
 
@@ -539,9 +544,11 @@ class NetworkPlan:
         One copy kernel on the context stream, after torch's current stream; the next run / vjp reads them.  A gradient
         plan needs a new run before vjp."""
         idx, ptrs, _, keep = _device_sources(self.ctx, self.leaf_shapes, payloads)
-        c_ptrs = (C.c_void_p * max(len(ptrs), 1))(*ptrs)
-        _call_after_torch(self.ctx, keep, lambda: self.ctx._l.tncb_plan_set_leaves(
-            self.ctx.handle, self.handle, len(idx), u64_array(idx), c_ptrs))
+        self._set_leaves(idx, ptrs, keep)
+
+    def _set_leaves(self, idx, ptrs, keep=None) -> None:
+        """tncb_plan_set_leaves: the leaves `idx` from the device addresses `ptrs`; keep: the torch tensors they lie in"""
+        self._call("tncb_plan_set_leaves", len(idx), u64_array(idx), _addresses(ptrs), keep=keep)
 
     def stage_instances(self, template, payloads: dict, count: int) -> None:
         """Stage `count` networks of the plan's structure from device memory (tncb_plan_stage_instances): every leaf from
@@ -550,11 +557,13 @@ class NetworkPlan:
         by all.  The host work does not grow with count.  Plain plans: feeds run_slices / run_batch, as stage_slices does;
         gradient plans: feeds vjp_batch, as stage_batch does."""
         tmpl = template if isinstance(template, PreparedNetwork) else PreparedNetwork(template)
-        idx, ptrs, strides, keep = _device_sources(self.ctx, self.leaf_shapes, payloads, int(count))
-        c_ptrs = (C.c_void_p * max(len(ptrs), 1))(*ptrs)
-        _call_after_torch(self.ctx, keep, lambda: self.ctx._l.tncb_plan_stage_instances(
-            self.ctx.handle, self.handle, C.byref(tmpl.node), int(count), len(idx), u64_array(idx), c_ptrs, u64_array(strides)))
-        self.n_staged = int(count)
+        self._stage_instances(tmpl, int(count), *_device_sources(self.ctx, self.leaf_shapes, payloads, int(count)))
+
+    def _stage_instances(self, template: PreparedNetwork, count: int, idx, ptrs, strides, keep=None) -> None:
+        """tncb_plan_stage_instances: `count` copies of `template` with the leaves `idx` from the device addresses `ptrs`,
+        instance i at ptr + i * stride elements; keep: the torch tensors they lie in"""
+        self._staged(count, "tncb_plan_stage_instances", C.byref(template.node), count, len(idx), u64_array(idx),
+                     _addresses(ptrs), u64_array(strides), keep=keep)
 
     def stage_batch(self, nets) -> None:
         """Materialise + upload the leaves of many networks of a gradient plan's structure once (tncb_plan_stage_batch):
@@ -562,22 +571,20 @@ class NetworkPlan:
         m = _Marshal()
         nodes = [m.tn(t) for t in nets]
         ptrs = (C.POINTER(TncbTn) * max(len(nodes), 1))(*[C.pointer(n) for n in nodes])
-        check(self.ctx._l.tncb_plan_stage_batch(self.ctx.handle, self.handle, len(nodes), ptrs))
-        self.n_staged = len(nodes)
+        self._staged(len(nodes), "tncb_plan_stage_batch", len(nodes), ptrs)
 
     def vjp_batch(self, first: int = 0, count: Optional[int] = None, seeds=None, rows: bool = True, sum: bool = False,
                   values: bool = True):
         """Forward and backward of the staged networks first .. first + count - 1, each on its own, the instances as a
         grid dimension of every kernel (tncb_plan_vjp_batch).  count=None: every staged network from `first` on.
-        seeds: [count, *result dims] array or DeviceTensor; None for a scalar result (seed 1) or without gradients.
-        Returns (legs of one instance, values [count, *dims] or None, {leaf: [count, *leaf shape]} or None,
-        {leaf: leaf-shaped sum over the instances} or None).  Row i equals stage(net_i) + run + vjp(seed_i) bit for bit;
-        the sum is the left fold of the rows in instance order, also bit for bit."""
-        if count is None:
-            count = max(0, getattr(self, "n_staged", 0) - int(first))
+        seeds: [count, *result dims] array, torch CUDA tensor or DeviceTensor; None for a scalar result (seed 1) or
+        without gradients.  Returns (legs of one instance, values [count, *dims] or None, {leaf: [count, *leaf shape]} or
+        None, {leaf: leaf-shaped sum over the instances} or None).  Row i equals stage(net_i) + run + vjp(seed_i) bit for
+        bit; the sum is the left fold of the rows in instance order, also bit for bit."""
+        count = self._count(first, count)
         vals, row_block, sum_block = _download(self.vjp_batch_blocks(first, count, seeds, rows, sum, values))
         offs = self.grad_offsets()
-        return (list(self.result_legs), vals, self._unpack(offs, row_block, (int(count),)), self._unpack(offs, sum_block, ()))
+        return (list(self.result_legs), vals, self._unpack(offs, row_block, (count,)), self._unpack(offs, sum_block, ()))
 
     def _unpack(self, offs, block, lead):
         """{leaf: lead + leaf shape} views of a host block [*lead, grad_elems] at the offsets `offs`; None stays None"""
@@ -594,20 +601,8 @@ class NetworkPlan:
                          sum: bool = False, values: bool = True):
         """`vjp_batch` left on the device: [values [count, *dims], rows [count, grad_elems], sum [grad_elems]] as
         DeviceTensors, None where not requested"""
-        if count is None:
-            count = max(0, getattr(self, "n_staged", 0) - int(first))
-        tmp = None
-        if seeds is not None and not isinstance(seeds, DeviceTensor):
-            seeds = tmp = DeviceTensor.from_numpy(self.ctx, np.asarray(seeds, dtype=np.complex128))
-        outs = [C.c_void_p() if want else None for want in (values, rows, sum)]
-        try:
-            check(self.ctx._l.tncb_plan_vjp_batch(self.ctx.handle, self.handle, int(first), int(count),
-                                                  seeds.handle if seeds is not None else None,
-                                                  *[C.byref(o) if o is not None else None for o in outs]))
-        finally:
-            if tmp is not None:
-                tmp.free()
-        return [None if o is None else DeviceTensor.adopt(self.ctx, o) for o in outs]
+        count = self._count(first, count)
+        return self._call("tncb_plan_vjp_batch", int(first), count, inputs=[(seeds, "seeds", count)], outputs=(values, rows, sum))
 
     def info(self) -> dict:
         n, k = C.c_uint64(), C.c_uint64()
@@ -620,17 +615,10 @@ class NetworkPlan:
         """Materialise + upload the leaves once (tncb_plan_stage); `run()` then needs no host data."""
         m = _Marshal()
         c_tn = m.tn(tn)
-        check(self.ctx._l.tncb_plan_stage(self.ctx.handle, self.handle, C.byref(c_tn)))
+        self._call("tncb_plan_stage", C.byref(c_tn))
 
     def run(self) -> Tensor:
-        out, n_out, legs = C.c_void_p(), C.c_int(), u64_array([0] * 64)
-        check(self.ctx._l.tncb_plan_run(self.ctx.handle, self.handle, C.byref(out), C.byref(n_out), legs))
-        if not out.value:
-            return Tensor()
-        dt = DeviceTensor.adopt(self.ctx, out)
-        res = Tensor([legs[i] for i in range(n_out.value)], dt.shape)
-        res.set_tensor_data(TensorData.Matrix(dt))
-        return res
+        return _leaf(*_contracted(self.ctx, "tncb_plan_run", self.handle))
 
     def stage_slices(self, slice_tns) -> None:
         """Materialise + upload the leaf blocks of many networks of the plan's structure once (tncb_plan_stage_slices):
@@ -638,41 +626,22 @@ class NetworkPlan:
         m = _Marshal()
         nodes = [m.tn(t) for t in slice_tns]
         ptrs = (C.POINTER(TncbTn) * len(nodes))(*[C.pointer(n) for n in nodes])
-        check(self.ctx._l.tncb_plan_stage_slices(self.ctx.handle, self.handle, len(nodes), ptrs))
-        self.n_staged = len(nodes)
+        self._staged(len(nodes), "tncb_plan_stage_slices", len(nodes), ptrs)
 
     def run_batch(self, first: int = 0, count: Optional[int] = None):
         """Contract the staged networks first .. first + count - 1 each on its own, the instances as a grid dimension of
         every kernel (tncb_plan_run_batch).  count=None: every staged network from `first` on.  Returns (legs of one
         instance, DeviceTensor of shape (count, *dims)); row i is bit-identical to run_slices(first + i, n_staged)."""
-        if count is None:
-            count = max(0, getattr(self, "n_staged", 0) - int(first))
-        out, n_out, legs = C.c_void_p(), C.c_int(), u64_array([0] * 64)
-        check(self.ctx._l.tncb_plan_run_batch(self.ctx.handle, self.handle, int(first), int(count), C.byref(out), C.byref(n_out), legs))
-        return [legs[i] for i in range(n_out.value)], DeviceTensor.adopt(self.ctx, out)
+        return _contracted(self.ctx, "tncb_plan_run_batch", self.handle, int(first), self._count(first, count))
 
     def run_slices(self, first: int = 0, stride: int = 1) -> Tensor:
         """Sum of the slices first, first + stride, ... on the device, no host work per slice."""
-        out, n_out, legs = C.c_void_p(), C.c_int(), u64_array([0] * 64)
-        check(self.ctx._l.tncb_plan_run_slices(self.ctx.handle, self.handle, int(first), int(stride), C.byref(out), C.byref(n_out), legs))
-        dt = DeviceTensor.adopt(self.ctx, out)
-        res = Tensor([legs[i] for i in range(n_out.value)], dt.shape)
-        res.set_tensor_data(TensorData.Matrix(dt))
-        return res
+        return _leaf(*_contracted(self.ctx, "tncb_plan_run_slices", self.handle, int(first), int(stride)))
 
     def execute(self, tn: Tensor) -> Tensor:
         m = _Marshal()
         c_tn = m.tn(tn)
-        out, n_out, legs = C.c_void_p(), C.c_int(), u64_array([0] * 64)
-        check(self.ctx._l.tncb_plan_execute(self.ctx.handle, self.handle, C.byref(c_tn), C.byref(out), C.byref(n_out), legs))
-        for d in m.device_inputs:
-            d.release()
-        if not out.value:
-            return Tensor()
-        dt = DeviceTensor.adopt(self.ctx, out)
-        res = Tensor([legs[i] for i in range(n_out.value)], dt.shape)
-        res.set_tensor_data(TensorData.Matrix(dt))
-        return res
+        return _leaf(*_contracted(self.ctx, "tncb_plan_execute", self.handle, C.byref(c_tn), consumed=m.device_inputs))
 
     def __del__(self):
         try:
