@@ -23,8 +23,8 @@
 // implementation for complex operands with the TTGT gather fused in.
 //
 // GEMM kernel (crt_gemm_kernel, main loop in sm90.h): persistent CTAs of three warpgroups, work item = (modulus, K chunk,
-// 128 x 128 complex tile; three products: 128 x 256 of one product), items ordered modulus-major with a grouped tile
-// raster so that the CTAs resident at any time share a few operand row bands of ONE modulus in L2.
+// 128 x 128 complex tile; three products: 128 x 256 of one product), items ordered modulus-major with a banded tile
+// raster so that the Bt tiles of a band of ONE modulus stay in L2 while its At tiles stream from HBM once.
 #include "internal.h"
 #include "sm90.h"
 #include <cuda.h>
@@ -219,8 +219,10 @@ crt_rowmax_kernel(const double2* __restrict__ src, const long long* __restrict__
 }
 
 // Tile of 32 rows x 128 k: load (coalesced along whichever index is contiguous in the source), scale +
-// truncate to integer-valued doubles in shared memory, then every thread reduces 2 x 8 consecutive k of one row
-// modulo every m_i and writes 8 bytes per plane and pass.
+// truncate to integer-valued doubles in shared memory, then every thread reduces 4 consecutive k of each of four rows
+// modulo every m_i and writes 4 bytes per plane and row; the 32 lanes of a warp write a row's 128 bytes of a plane in one
+// instruction, so every plane line is written whole.  At 4 k per thread the integers x mod 2^32 stay in registers within
+// the 80-register budget of 3 CTAs per SM (at 8 the compiler converted them again for every modulus).
 // planes: [((mod * NPL + plane) * rowsP + row) * Kp + k];
 //   four-product form:  COMPS == 2 (Bt side): NPL = 2 planes (re, im);  COMPS == 3 (At side): NPL = 3 planes (-im, re, im)
 //   three-product form (KARA, see crt_gemm_kernel): NPL = 3 on both sides, (re, im, re + im); plane p of Bt meets plane p
@@ -280,30 +282,30 @@ crt_residue_kernel(const double2* __restrict__ src, const long long* __restrict_
     tile[r * RES_RS + k + (k >> 3)] = v;
   }
   __syncthreads();
-  const int r = tid >> 3;
-  if (row0 + r >= rows) return;
   const double RMAGIC = 6755399441055744.0;   // 1.5 * 2^52: the low word of (x + RMAGIC) is rint(x) mod 2^32
   const long long plane_stride = rowsP * Kp;
+  const int g = tid & 31;                      // group of 4 consecutive k: a warp stores a whole 128-byte row of a plane
+  const int nmod = T.nmod;
 #pragma unroll 1
-  for (int pass = 0; pass < 2; pass++) {
-    const int g = (tid & 7) + 8 * pass;        // group of 8 consecutive k
-    double xr[8], xi[8];
-    int lr[8], li[8];                           // the integers x mod 2^32
+  for (int pass = 0; pass < RES_ROWS / 8; pass++) {
+    const int r = (tid >> 5) + 8 * pass;
+    if (row0 + r >= rows) return;
+    double xr[4], xi[4];
+    int lr[4], li[4];                           // the integers x mod 2^32
 #pragma unroll
-    for (int j = 0; j < 8; j++) {
-      const double2 v = tile[r * RES_RS + g * 9 + j];
+    for (int j = 0; j < 4; j++) {
+      const double2 v = tile[r * RES_RS + g * 4 + j + (g >> 1)];
       xr[j] = v.x; xi[j] = v.y;
       lr[j] = (int)__double2ll_rn(v.x); li[j] = (int)__double2ll_rn(v.y);
     }
-    int8_t* dst = planes + (row0 + r) * Kp + k0 + g * 8;
-    const int nmod = T.nmod;
+    int8_t* dst = planes + (row0 + r) * Kp + k0 + g * 4;
 #pragma unroll 1
     for (int i = 0; i < nmod; i++) {
       const int m = s_mod[i];
       const double inv = s_inv[i];
-      uint32_t wr[2] = {0, 0}, wi[2] = {0, 0}, ws[2] = {0, 0};
+      uint32_t wr = 0, wi = 0, ws = 0;
 #pragma unroll
-      for (int j = 0; j < 8; j++) {
+      for (int j = 0; j < 4; j++) {
         // q = rint(x / m): ONE rounding (the product is exact inside the FMA, the sum has ulp 1); its low 32 bits are
         // the low word of the sum.  r = x - q m is tiny, so computing it modulo 2^32 in int32 is exact.
         // |x inv - x/m| <= 2^53/m * 2^-53 < 0.006  =>  |r| <= 0.506 m: <= 127 for every odd m <= 253, and for
@@ -311,24 +313,20 @@ crt_residue_kernel(const double2* __restrict__ src, const long long* __restrict_
         const int qr = __double2loint(fma(xr[j], inv, RMAGIC));
         const int qi = __double2loint(fma(xi[j], inv, RMAGIC));
         const int rr = lr[j] - qr * m, ri = li[j] - qi * m;
-        constexpr uint32_t sel[4] = {0x3214u, 0x3240u, 0x3410u, 0x4210u};   // low byte of the 2nd operand into byte j & 3
-        wr[j >> 2] = __byte_perm(wr[j >> 2], (uint32_t)rr, sel[j & 3]);
-        wi[j >> 2] = __byte_perm(wi[j >> 2], (uint32_t)ri, sel[j & 3]);
-        if (KARA) ws[j >> 2] = __byte_perm(ws[j >> 2], (uint32_t)crt_fix_byte(rr + ri, m), sel[j & 3]);
+        constexpr uint32_t sel[4] = {0x3214u, 0x3240u, 0x3410u, 0x4210u};   // low byte of the 2nd operand into byte j
+        wr = __byte_perm(wr, (uint32_t)rr, sel[j]);
+        wi = __byte_perm(wi, (uint32_t)ri, sel[j]);
+        if (KARA) ws = __byte_perm(ws, (uint32_t)crt_fix_byte(rr + ri, m), sel[j]);
       }
-      int8_t* d = dst + (long long)i * (KARA ? 3 : COMPS) * plane_stride;
+      uint32_t* d = reinterpret_cast<uint32_t*>(dst + (long long)i * (KARA ? 3 : COMPS) * plane_stride);
+      const long long ps = plane_stride / 4;
       if (KARA) {
-        *reinterpret_cast<uint2*>(d) = make_uint2(wr[0], wr[1]);
-        *reinterpret_cast<uint2*>(d + plane_stride) = make_uint2(wi[0], wi[1]);
-        *reinterpret_cast<uint2*>(d + 2 * plane_stride) = make_uint2(ws[0], ws[1]);
+        d[0] = wr; d[ps] = wi; d[2 * ps] = ws;
       } else if (COMPS == 2) {
-        *reinterpret_cast<uint2*>(d) = make_uint2(wr[0], wr[1]);
-        *reinterpret_cast<uint2*>(d + plane_stride) = make_uint2(wi[0], wi[1]);
+        d[0] = wr; d[ps] = wi;
       } else {
         // byte-wise negation: |ri| <= 127 for odd m; for m = 256 the wrap -(-128) = -128 is again == 128 (mod 256)
-        *reinterpret_cast<uint2*>(d) = make_uint2(__vneg4(wi[0]), __vneg4(wi[1]));
-        *reinterpret_cast<uint2*>(d + plane_stride) = make_uint2(wr[0], wr[1]);
-        *reinterpret_cast<uint2*>(d + 2 * plane_stride) = make_uint2(wi[0], wi[1]);
+        d[0] = __vneg4(wi); d[ps] = wr; d[2 * ps] = wi;
       }
     }
   }
@@ -356,7 +354,7 @@ __device__ __forceinline__ CrtItem crt_decode(const CrtGemmArgs& p, int item) {
   const int mp = mk / p.nkc;            // (modulus, product) major, K chunk minor
   it.kc = mk - mp * p.nkc;
   it.mod_i = KARA ? mp / 3 : mp; it.prod = KARA ? mp - it.mod_i * 3 : 0;
-  // grouped raster: bands of `group` n-tiles x all m-tiles; concurrently running CTAs (consecutive items)
+  // banded raster: bands of `group` n-tiles x all m-tiles; concurrently running CTAs (consecutive items)
   // share `group` Bt row bands and ~(#CTAs / group) At tiles
   const int per_band = p.group * p.tiles_m;
   const int band = t / per_band, first = band * p.group;
@@ -367,7 +365,7 @@ __device__ __forceinline__ CrtItem crt_decode(const CrtGemmArgs& p, int item) {
   return it;
 }
 
-// Persistent CTAs, work item = (modulus, K chunk, 128 x 128 complex tile), items ordered modulus-major with a grouped tile
+// Persistent CTAs, work item = (modulus, K chunk, 128 x 128 complex tile), items ordered modulus-major with a banded tile
 // raster.  Warpgroup 0 streams the operand tiles (TMA), warpgroups 1-2 run the wgmma main loop (sm90.h) on 64 Bt rows each
 // and then their epilogue: accumulator mod m_i -> one offset byte -> a transpose of 32-bit words inside each lane quad
 // (shuffles, no shared memory) -> 16-byte stores.  The producer runs ahead into the next item, up to the ring's depth,
@@ -505,15 +503,17 @@ struct CrtReconArgs {
   int nkc;
 };
 
-// one thread: 4 consecutive m of one row n (56 registers -> 4 resident CTAs per SM: the kernel is bound by the latency of
-// its residue loads, ncu r02: 52 % long_scoreboard at 25 % occupancy with 8 m per thread).  No conversion-pipe
-// instruction in the inner loop: a residue byte u = y + 128 becomes the double 2^52 + u by a byte permute into the low
-// mantissa word, one DADD removes 2^52 + 128 nkc.
+// one thread: 4 consecutive m of one row n.  The kernel is bound by the latency of its residue loads, so with one K chunk the
+// words of RB moduli (RB x 3 or RB x 2 independent loads) are all in flight before the first is used: 3 (three products) or
+// 4 resident CTAs per SM keep 24 x 24 or 32 x 16 loads of 128 bytes per warp outstanding.
+// No conversion-pipe instruction in the inner loop: a residue byte u = y + 128 becomes the double 2^52 + u by a byte
+// permute into the low mantissa word, one DADD removes 2^52 + 128 nkc.
 // KARA (three products): the planes hold k1, k2, k3 (+128 each); re = k1 - k2 and im = k3 - k1 - k2 are formed here from the
 // bytes (the CRT sum is linear, no reduction mod m_i needed: |y| <= 3 * 128 * 32 < 2^13.6 keeps S1 exact, 13.6 + 34 + 4.4 bits).
 template <bool ONE_CHUNK, bool KARA>
-__global__ void __launch_bounds__(256, 4)
+__global__ void __launch_bounds__(256, KARA ? 3 : 4)
 crt_reconstruct_kernel(const __grid_constant__ CrtReconArgs a, const __grid_constant__ CrtTables T) {
+  constexpr int NPR = KARA ? 3 : 2, RB = 8;
   const long long cols4 = a.Mp >> 2;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long n = idx / cols4, m4 = (idx - n * cols4) * 4;
@@ -527,48 +527,56 @@ crt_reconstruct_kernel(const __grid_constant__ CrtReconArgs a, const __grid_cons
   // im = (u3 - u1 - u2 + 512) - 384 per chunk (the +256 / +512 keep the running sums non-negative for the conversion below)
   const double bias = 4503599627370496.0 + (KARA ? 256.0 : 128.0) * (double)a.nkc;   // 2^52 + ...
   const double bias_i = 4503599627370496.0 + (KARA ? 384.0 : 128.0) * (double)a.nkc;
-#pragma unroll 8
-  for (int i = 0; i < T.nmod; i++) {
-    uint32_t ur[4], ui[4];     // byte sums over the K chunks (still == C' + 128 nkc mod m_i)
-    if (KARA) {
+  const int nmod = T.nmod;
+#pragma unroll 1
+  for (int i0 = 0; i0 < nmod; i0 += RB) {
+    uint32_t w[RB][NPR];       // one K chunk: the residue words of moduli i0 .. i0 + RB - 1
+    if (ONE_CHUNK) {
+#pragma unroll
+      for (int u = 0; u < RB; u++) {
+        if (i0 + u < nmod) {
+#pragma unroll
+          for (int p = 0; p < NPR; p++) w[u][p] = __ldg(reinterpret_cast<const uint32_t*>(base + (long long)((i0 + u) * NPR + p) * plane));
+        }
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < RB; u++) {
+      const int i = i0 + u;
+      if (i >= nmod) break;
+      uint32_t ur[4], ui[4];     // byte sums over the K chunks (still == C' + 128 nkc mod m_i)
 #pragma unroll
       for (int j = 0; j < 4; j++) { ur[j] = 0; ui[j] = 0; }
       for (int c = 0; c < (ONE_CHUNK ? 1 : a.nkc); c++) {
-        const int8_t* pk = base + (long long)((i * a.nkc + c) * 3) * plane;
-        const uint32_t w1 = __ldg(reinterpret_cast<const uint32_t*>(pk));
-        const uint32_t w2 = __ldg(reinterpret_cast<const uint32_t*>(pk + plane));
-        const uint32_t w3 = __ldg(reinterpret_cast<const uint32_t*>(pk + 2 * plane));
+        uint32_t x[NPR];
+        if (ONE_CHUNK) {
+#pragma unroll
+          for (int p = 0; p < NPR; p++) x[p] = w[u][p];
+        } else {
+          const int8_t* pk = base + (long long)((i * a.nkc + c) * NPR) * plane;
+#pragma unroll
+          for (int p = 0; p < NPR; p++) x[p] = __ldg(reinterpret_cast<const uint32_t*>(pk + p * plane));
+        }
 #pragma unroll
         for (int j = 0; j < 4; j++) {
-          const uint32_t k1 = __byte_perm(w1, 0, 0x4440 + j), k2 = __byte_perm(w2, 0, 0x4440 + j);
-          ur[j] += 256u + k1 - k2;
-          ui[j] += 512u + __byte_perm(w3, 0, 0x4440 + j) - k1 - k2;
+          const uint32_t k1 = __byte_perm(x[0], 0, 0x4440 + j), k2 = __byte_perm(x[1], 0, 0x4440 + j);
+          if (KARA) {
+            ur[j] += 256u + k1 - k2;
+            ui[j] += 512u + __byte_perm(x[NPR - 1], 0, 0x4440 + j) - k1 - k2;
+          } else {
+            ur[j] += k1; ui[j] += k2;
+          }
         }
       }
-    } else if (ONE_CHUNK) {
-      const uint32_t wr = __ldg(reinterpret_cast<const uint32_t*>(base + (long long)(i * 2) * plane));
-      const uint32_t wi = __ldg(reinterpret_cast<const uint32_t*>(base + (long long)(i * 2 + 1) * plane));
+      const double r1 = T.rho1[i], r2 = T.rho2[i];
 #pragma unroll
-      for (int j = 0; j < 4; j++) { ur[j] = __byte_perm(wr, 0, 0x4440 + j); ui[j] = __byte_perm(wi, 0, 0x4440 + j); }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 4; j++) { ur[j] = 0; ui[j] = 0; }
-      for (int c = 0; c < a.nkc; c++) {
-        const int8_t* pr = base + (long long)((i * a.nkc + c) * 2) * plane;
-        const uint32_t wr = __ldg(reinterpret_cast<const uint32_t*>(pr));
-        const uint32_t wi = __ldg(reinterpret_cast<const uint32_t*>(pr + plane));
-#pragma unroll
-        for (int j = 0; j < 4; j++) { ur[j] += __byte_perm(wr, 0, 0x4440 + j); ui[j] += __byte_perm(wi, 0, 0x4440 + j); }
+      for (int j = 0; j < 4; j++) {
+        // y * rho1 is exact (|y| <= 2^13, rho1 on a 2^-34 grid) and so is the sum over <= 20 moduli (|S1| < 2^18)
+        const double dr = __hiloint2double(0x43300000, (int)ur[j]) - bias;
+        const double di = __hiloint2double(0x43300000, (int)ui[j]) - bias_i;
+        s1r[j] = fma(dr, r1, s1r[j]); s2r[j] = fma(dr, r2, s2r[j]);
+        s1i[j] = fma(di, r1, s1i[j]); s2i[j] = fma(di, r2, s2i[j]);
       }
-    }
-    const double r1 = T.rho1[i], r2 = T.rho2[i];
-#pragma unroll
-    for (int j = 0; j < 4; j++) {
-      // y * rho1 is exact (|y| <= 2^13, rho1 on a 2^-34 grid) and so is the sum over <= 20 moduli (|S1| < 2^18)
-      const double dr = __hiloint2double(0x43300000, (int)ur[j]) - bias;
-      const double di = __hiloint2double(0x43300000, (int)ui[j]) - bias_i;
-      s1r[j] = fma(dr, r1, s1r[j]); s2r[j] = fma(dr, r2, s2r[j]);
-      s1i[j] = fma(di, r1, s1i[j]); s2i[j] = fma(di, r2, s2i[j]);
     }
   }
   const int en = crt_exp_from_bits(a.max_n[n]);
@@ -588,7 +596,7 @@ crt_reconstruct_kernel(const __grid_constant__ CrtReconArgs a, const __grid_cons
       const double fr = (s1r[j] - qr) + s2r[j], fi = (s1i[j] - qi) + s2i[j];
       out = make_double2(scalbn(fr * T.p_scaled, en + em), scalbn(fi * T.p_scaled, en + em));
     }
-    dst[j] = out;
+    __stcs(dst + j, out);   // C is not read again by this pair: stream it past the L2
   }
 }
 
@@ -751,7 +759,11 @@ int launch_k1_crt(tncb_ctx* ctx, const PairPlan& P, const double2* A, const doub
       const long long items = (long long)g.tiles_n * g.tiles_m * nmod * nkc * (kara ? 3 : 1);
       if (items > 0x7fffffffLL) { cleanup(); return fail(TNCB_ERR_UNSUPPORTED, "too many work items"); }
       g.total_items = (int)items;
-      g.group = ctx->crt_group;
+      // raster band (n-tiles): the Bt tiles of a whole band stay in L2 while the At tiles stream past them, so a band over
+      // all n-tiles reads every At tile from HBM once per (modulus, product) instead of once per band.  The band takes at
+      // most half of the L2, so that the streamed At tiles do not evict it.
+      const long long bt_tile_bytes = (long long)CRT_BT * Kp * (kara ? 1 : 2);   // three products: plane `prod`; four: Br, Bi
+      g.group = (int)std::max<long long>(1, std::min<long long>(g.tiles_n, ctx->l2_bytes / 2 / bt_tile_bytes));
       for (int i = 0; i < CRT_MAX_MOD; i++) { g.negmod[i] = -T.mod[i]; g.magic[i] = T.magic[i]; }
       const unsigned grid = (unsigned)std::min<long long>(ctas_max, items);
       const double ops = 2.0 * (kara ? 3.0 : 4.0) * (double)nmod * (double)Np * (double)Mp * (double)Kp;

@@ -84,7 +84,7 @@ struct tncb_ctx {
   // CRT engine: operand bits (53 = full mantissa) or a requested tolerance, forced modulus count, thresholds, workspace
   int crt_bits = 53; double crt_tol = 0.0; int crt_nmod_force = 0;
   long long crt_min_k = 256; double crt_min_mnk = 268435456.0;   // K >= 256 and M*N*K >= 2^28
-  size_t crt_ws_bytes = (size_t)12 << 30; int crt_group = 8;
+  size_t crt_ws_bytes = (size_t)12 << 30;
   double last_int8_ops = 0.0; int last_nmod = 0; int last_products = 0;
   int crt_products = 0;            // real int8 products per complex product: 0 = auto (3 when K >= crt_kara_min_k), 3, 4
   long long crt_kara_min_k = 2048;
@@ -93,6 +93,7 @@ struct tncb_ctx {
   int time_gemm = 0; cudaEvent_t gemm_ev0 = nullptr, gemm_ev1 = nullptr; bool gemm_ev_valid = false;
   std::vector<cudaEvent_t> gemm_pool; size_t gemm_used = 0; std::vector<double> gemm_ops;
   int sm_count = 132;
+  long long l2_bytes = 50LL << 20;
   // pinned staging for leaf uploads
   void* stage_host = nullptr; size_t stage_bytes = 0;
   // K1 offset-table workspace (grown on demand, stream-ordered reuse)

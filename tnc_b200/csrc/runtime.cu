@@ -148,13 +148,13 @@ int tncb_ctx_create(int device, size_t arena_bytes, tncb_ctx** out) {
   tncb_ctx* ctx = new tncb_ctx();
   ctx->device = device;
   ctx->sm_count = prop.multiProcessorCount;
+  ctx->l2_bytes = prop.l2CacheSize;
   ctx->arena.capacity_limit = arena_bytes;
   if (const char* e = std::getenv("TNCB_OZAKI_SLICES")) ctx->oz_slices = std::max(0, std::min(8, atoi(e)));
   if (const char* e = std::getenv("TNCB_TCGEN05_ENGINE")) ctx->oz_engine = atoi(e) == 1 ? 1 : 0;
   if (const char* e = std::getenv("TNCB_CRT_MODULI")) ctx->crt_nmod_force = std::max(0, std::min(20, atoi(e)));
   if (const char* e = std::getenv("TNCB_CRT_PRODUCTS")) { const int v = atoi(e); ctx->crt_products = (v == 3 || v == 4) ? v : 0; }
   if (const char* e = std::getenv("TNCB_CRT_MIN_K3")) ctx->crt_kara_min_k = std::max(1, atoi(e));
-  if (const char* e = std::getenv("TNCB_CRT_GROUP")) ctx->crt_group = std::max(1, atoi(e));
   if (const char* e = std::getenv("TNCB_CRT_WS_GB")) ctx->crt_ws_bytes = (size_t)std::max(1, atoi(e)) << 30;
   cudaError_t se = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking);
   if (se != cudaSuccess) { delete ctx; return fail(TNCB_ERR_CUDA, cudaGetErrorString(se)); }

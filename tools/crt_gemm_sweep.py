@@ -1,5 +1,6 @@
 """Kernel time of crt_gemm_kernel alone (CUDA events around each launch, tncb_ctx_time_gemm accumulate mode) at the six
-int8 pairs of the benchmark network, for ring variants of the GEMM's stage ring.
+int8 pairs of the benchmark network, for ring variants of the GEMM's stage ring; with --passes, the time of every kernel
+of an int8 pair instead.
 
 The ring (slots x K bytes per slot, one configuration per product form) is a compile-time constant of csrc/crt.cu.  Each
 variant is a separate copy of the library: crt.cu compiled with -D overrides of CRT_RING3_* / CRT_RING4_*, linked with the
@@ -12,7 +13,13 @@ does inside the network (default context).  Per pair and variant one JSON line: 
 call, the rate, and the SM clock sampled by nvidia-smi during the timed window.  The output starts with the card's name,
 power limit and maximum SM clock, and the tools/i8_peak lines (what the tensor pipe sustains on this card).
 
-usage: python tools/crt_gemm_sweep.py [--variant NAME=S3xBK3,S4xBK4 ...] [--lib NAME=PATH ...] [--build-only] [--out FILE]
+--passes times each kernel of the pair (row maxima and residues of Bt and At, GEMM, reconstruction) with torch.profiler
+(CUDA activities, a run of its own, no GEMM events) and prints per kernel its HBM bytes from the shape model below, the
+rate and the fraction of the H100 SXM data sheet's 3.35 TB/s.  Only the libraries given with --lib run (the tree's own
+build when there is none); no ring variant is built.
+
+usage: python tools/crt_gemm_sweep.py [--variant NAME=S3xBK3,S4xBK4 ...] [--lib NAME=PATH ...] [--build-only] [--passes]
+                                      [--out FILE]
 """
 import argparse
 import json
@@ -37,6 +44,35 @@ VARIANTS = {
     "r9x64_3x64": "9x64,3x64",
 }
 SWEEP_DIR = os.path.join(ROOT, "build", "crt_sweep")
+HBM_BYTES_PER_S = 3.35e12   # H100 SXM data sheet
+
+
+def pass_bytes(M, N, K, products, nmod, nkc):
+    """Compulsory HBM bytes per kernel and call (all panels): operands are complex128 (16 B), planes and residues one byte.
+    rowmax reads its operand; residue reads it and writes NPL planes per modulus (three products: 3 per side, four: 2 for
+    Bt and 3 for At); the GEMM reads every plane once and writes the residues; the reconstruction reads the residues
+    (three or two planes per modulus and K chunk) and writes complex128 C."""
+    npb, npr = (3, 3) if products == 3 else (2, 2)
+    planes_b, planes_a = nmod * npb * N * K, nmod * 3 * M * K
+    residues = nmod * nkc * npr * N * M
+    return {"rowmax_bt": 16 * N * K, "rowmax_at": 16 * M * K,
+            "residue_bt": 16 * N * K + planes_b, "residue_at": 16 * M * K + planes_a,
+            "gemm": planes_b + planes_a + residues, "reconstruct": residues + 16 * N * M}
+
+
+def pass_of(kernel, following):
+    """the pass a kernel name belongs to; a row-max kernel takes its side from the residue kernel that follows it"""
+    if "crt_residue_kernel<2" in kernel:
+        return "residue_bt"
+    if "crt_residue_kernel<3" in kernel:
+        return "residue_at"
+    if "crt_rowmax_kernel" in kernel:
+        return None if following is None else "rowmax_" + pass_of(following, None).split("_")[1]
+    if "crt_gemm_kernel" in kernel:
+        return "gemm"
+    if "crt_reconstruct_kernel" in kernel:
+        return "reconstruct"
+    return None
 
 
 def defines(spec):
@@ -101,7 +137,36 @@ class ClockSampler:
         return False
 
 
-def child(name, lib_path, min_window_s):
+def profile_passes(ctx, tb, a, b, c, reps):
+    """device ms per call of each pass, from one torch.profiler run of `reps` calls; nkc from the reconstruction's name"""
+    import tempfile
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(reps):
+            tb.contract_pair_into(ctx, [0, 1], a, [2, 0], b, c)
+        ctx.synchronize()
+        torch.cuda.synchronize()
+    with tempfile.TemporaryDirectory() as d:
+        path = os.path.join(d, "trace.json")
+        prof.export_chrome_trace(path)
+        with open(path) as f:
+            events = json.load(f)["traceEvents"]
+    kernels = sorted((e for e in events if e.get("cat") == "kernel"), key=lambda e: e["ts"])
+    us, count, one_chunk = {}, {}, None
+    for i, e in enumerate(kernels):
+        nxt = kernels[i + 1]["name"] if i + 1 < len(kernels) else None
+        p = pass_of(e["name"], nxt)
+        if p is None:
+            continue
+        if p == "reconstruct":
+            one_chunk = "crt_reconstruct_kernel<true" in e["name"]
+        us[p] = us.get(p, 0.0) + e["dur"]
+        count[p] = count.get(p, 0) + 1
+    return {p: v / 1e3 / reps for p, v in us.items()}, {p: v // reps for p, v in count.items()}, one_chunk
+
+
+def child(name, lib_path, min_window_s, passes=False):
     import torch
     import tnc_b200 as tb
     import tnc_b200._lib as tl
@@ -119,6 +184,29 @@ def child(name, lib_path, min_window_s):
         for t, shape in ((a, (K, M)), (b, (N, K))):
             torch.as_tensor(_DevView(t.device_ptr(), shape), device="cuda").normal_(generator=gen)
         torch.cuda.synchronize()
+        if passes:
+            for _ in range(2):   # warm-up: module load, arena growth
+                tb.contract_pair_into(ctx, [0, 1], a, [2, 0], b, c)
+            ctx.synchronize()
+            reps = 5
+            with ClockSampler() as clk:
+                ms, launches, one_chunk = profile_passes(ctx, tb, a, b, c, reps)
+            info = ctx.last_tcgen05_info()
+            assert one_chunk, "the byte model below takes one K chunk"
+            model = pass_bytes(M, N, K, info["products"], info["n_moduli"], 1)
+            rec = {"variant": name, "step": step, "M": M, "N": N, "K": K, "products": info["products"],
+                   "n_moduli": info["n_moduli"], "k_chunks": 1, "reps": reps,
+                   "sm_clock_mhz_median": statistics.median(clk.mhz) if clk.mhz else None,
+                   "sm_clock_mhz_min": min(clk.mhz) if clk.mhz else None, "passes": {}}
+            for p, nbytes in model.items():
+                rate = nbytes / (ms[p] * 1e-3)
+                rec["passes"][p] = {"ms": round(ms[p], 4), "launches": launches[p], "gb": round(nbytes / 1e9, 3),
+                                    "gb_per_s": round(rate / 1e9, 1), "of_hbm_peak": round(rate / HBM_BYTES_PER_S, 3)}
+            rec["total_ms"] = round(sum(ms[p] for p in model), 4)
+            print(json.dumps(rec), flush=True)
+            for t in (a, b, c):
+                t.free()
+            continue
         ctx.time_gemm(2)
         t0 = time.perf_counter()
         for _ in range(2):   # warm-up: module load, arena growth
@@ -151,14 +239,20 @@ def main():
                     help="ring variant (default: the built-in list)")
     ap.add_argument("--lib", action="append", default=[], metavar="NAME=PATH", help="an already built libtncb200.so")
     ap.add_argument("--build-only", action="store_true")
+    ap.add_argument("--passes", action="store_true", help="per-kernel times and HBM rates of every pass (--lib builds only)")
     ap.add_argument("--window", type=float, default=0.4, help="seconds of GEMM calls per pair and variant (at least 3 calls)")
     ap.add_argument("--out", default=None, help="also write the records to this file")
     ap.add_argument("--child", nargs=2, metavar=("NAME", "LIB"), help=argparse.SUPPRESS)
     a = ap.parse_args()
     if a.child:
-        return child(a.child[0], a.child[1], a.window)
+        return child(a.child[0], a.child[1], a.window, a.passes)
     variants = dict(v.split("=", 1) for v in a.variant) if a.variant else dict(VARIANTS)
     libs = {k: os.path.abspath(v) for k, v in (x.split("=", 1) for x in a.lib)}
+    if a.passes:
+        variants = {}
+        if not libs:
+            import tnc_b200._lib as tl
+            libs["tree"] = tl.LIB_PATH
     libs.update(build_variants(variants))
     if a.build_only:
         return
@@ -169,8 +263,8 @@ def main():
     for ln in lines:
         print(ln, flush=True)
     for name, lib in libs.items():
-        r = subprocess.run([sys.executable, os.path.abspath(__file__), "--window", str(a.window), "--child", name, lib],
-                           stdout=subprocess.PIPE, text=True)
+        r = subprocess.run([sys.executable, os.path.abspath(__file__), "--window", str(a.window), "--child", name, lib]
+                           + (["--passes"] if a.passes else []), stdout=subprocess.PIPE, text=True)
         for ln in r.stdout.strip().splitlines():
             rec = json.loads(ln)
             rec["ring"] = variants.get(name, "library as built")
