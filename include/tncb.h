@@ -292,7 +292,8 @@ int tncb_network_out_legs(const tncb_tn* tn, const tncb_path* path, int* n_out, 
  *   hvp_sliced             I     I    I    I       I           I           .
  *   stage_instances        .     .    .    U       U           U           U
  *   set_leaves             .     .    .    .       .           U           U
- *   grad_offsets           I     .    .    .       .           .           .          */
+ *   grad_offsets           I     .    .    .       .           .           .
+ *   sample                 .     U    U    U       U           U           U          */
 int tncb_plan_create(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, tncb_plan** out);
 /* `tn` must have the structure the plan was compiled from: every leaf is re-validated (kind, rank,
  * dims, non-null payload, live device handle) -> TNCB_ERR_INVALID / TNCB_ERR_SHAPE /
@@ -525,6 +526,56 @@ int tncb_plan_hvp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t count, size_t n, 
                         const tncb_tensor* seeds, const tncb_tensor* seed_tangents, tncb_tensor** values,
                         tncb_tensor** tangent_rows, tncb_tensor** grad_rows, tncb_tensor** grad_sum,
                         tncb_tensor** grad_tangent_rows, tncb_tensor** grad_tangent_sum);
+/* ---- sampling bitstrings from a circuit's output distribution ----
+ * A circuit on n <= 64 qubits, its amplitude network with the bras of the closed qubits Q (n - k of them) as leaves and
+ * the k open qubits O as the plan's result legs: for a closed assignment c the plan contracts to the 2^k amplitudes
+ * a_c(y) = <c, y| C |init>.  With p(c, y) = |a_c(y)|^2 and the exact marginal q(c) = sum_y p(c, y), candidate i carries
+ * (c_i, u_i, v_i) from the random stream below and is accepted iff u_i < r_i = q(c_i) 2^(n-k) / m.  An accepted candidate's
+ * open bits y_i are the first y, in the row-major order of the result, whose inclusive prefix sum of p exceeds v_i q(c_i),
+ * q being the last value of that same fixed-order prefix sum (so such a y exists and p(c_i, y_i) > 0).  The sample is
+ * (c_i, y_i) with its p(c_i, y_i).  The prefix sum runs over T = min(256, 2^k) chunks of consecutive outcomes, left to
+ * right inside a chunk and over the chunk sums.
+ *   Exact when nothing is clipped: if r <= 1 for every c, the samples are i.i.d. with law p / sum p, because a candidate
+ *     is accepted with value x with probability p(x) / m (the network need not be normalised).
+ *   Clipping biases the result: where r > 1 the assignment c is under-sampled; stats report how many consumed candidates
+ *     were clipped and the largest ratio seen, so that m can be raised.
+ *   Limiting cases: k = 0 is frugal rejection sampling (Markov et al.); k = n with m = 1 samples the state vector directly.
+ *   Open qubits help: q(c) 2^(n-k) is a mean over 2^k outcomes and concentrates near 1, so a larger k allows m close to 1
+ *     (nearly every contraction yields a sample) at a higher cost per contraction.  Which qubits are open changes the
+ *     contraction's cost a great deal: choose them, or the path, with the open legs in mind (tncb_plan_info).
+ * Random stream: candidate i of seed s is the Philox4x64-10 block (Random123 constants) of key (s, 0) and counter
+ * (i, 0, 0, 0), words w0..w3; bit j of w0 is the value of closed qubit closed_qubit[j]; u = (w1 >> 11) 2^-53 and
+ * v = (w2 >> 11) 2^-53.  Samples come out in candidate order, and a call's output depends only on (seed, first, the
+ * candidates consumed): not on the pass size, nor on how the work is split into calls.  Ranks of a multi-GPU job take
+ * disjoint candidate ranges through `first`. */
+typedef struct tncb_sample_spec {
+  int n_qubits;                 /* 1..64 */
+  size_t n_closed;
+  const uint64_t* closed_leaf;  /* leaf index (collect order) of the bra of closed qubit closed_qubit[j] */
+  const int* closed_qubit;
+  const int* result_qubit;      /* the qubit of each result leg of the plan, in result-leg order */
+} tncb_sample_spec;
+typedef struct tncb_sample_stats { uint64_t candidates, samples, clipped, passes; double max_ratio; } tncb_sample_stats;
+/* Candidates first, first + 1, ... in passes of `batch` (0: as many workspace copies as fit, as tncb_plan_run_batch)
+ * until max_samples are accepted or max_candidates are consumed.  The plan is a static plain plan staged on ctx
+ * (tncb_plan_stage): its staged block supplies every leaf except the closed bras, which the device writes per candidate,
+ * and it is left untouched.  Per pass: one kernel writes the candidates' bras, u and v; the batched forward levels
+ * (tncb_plan_run_batch's launches); one kernel per candidate reads its amplitudes in place and decides; one kernel writes
+ * the accepted samples in candidate order; one small device-to-host copy of the pass's counts.  When the target is
+ * reached inside a pass, its later candidates are not consumed and do not count, so a call resumed at
+ * first + stats->candidates continues the same stream.
+ *   bits:  device, max_samples words; sample s at bits[s], bit q = qubit q
+ *   probs: device, max_samples doubles, p of each sample; NULL = not written
+ *   stats: candidates consumed, samples written, clipped candidates among those consumed, passes, the largest ratio r
+ * Every refusal happens before any device work and leaves the arena as it found it.  TNCB_ERR_INVALID: a null argument;
+ * n_qubits outside 1..64; a closed leaf out of range, listed twice, or not a rank-1, dimension-2 leaf with a payload; a
+ * qubit missing from, or listed twice across, closed_qubit and result_qubit; a result leg whose dimension is not 2; m
+ * not finite or not > 0; max_samples == 0; bits / probs not 8-byte aligned device memory of the ctx's device, or running
+ * past the end of their allocation (cuMemGetAddressRange); not staged on this context.  TNCB_ERR_UNSUPPORTED: a plan of
+ * another kind or without a static layout.  TNCB_ERR_OOM: not even one workspace copy fits. */
+int tncb_plan_sample(tncb_ctx* ctx, tncb_plan* plan, const tncb_sample_spec* spec, uint64_t seed, uint64_t first,
+                     uint64_t max_candidates, uint64_t max_samples, double m, size_t batch, uint64_t* bits, double* probs,
+                     tncb_sample_stats* stats);
 /* ---- sliced tangents and Hessian-vector products: networks whose tangent or Hessian-vector workspace does not fit ----
  * By linearity, as for sliced gradients: R = sum_q R_q, so Ṙ = sum_q Ṙ_q; slice q's leaf (and its tangent) is q's
  * fixed-index sub-block of the full leaf (and of its full-shape tangent), and q's G_l and Ġ_l add into q's sub-block of

@@ -16,7 +16,8 @@ import numpy as np
 
 from ._lib import TncbError, check, lib, u64_array
 
-__all__ = ["Context", "DeviceTensor", "TncbError", "contract_pair", "contract_pair_into", "default_context", "lib"]
+__all__ = ["Context", "DeviceTensor", "Sampler", "Samples", "TncbError", "contract_pair", "contract_pair_into", "default_context",
+           "lib"]
 
 
 class Context:
@@ -297,3 +298,6 @@ def upload_into(ctx: Context, host: np.ndarray, dst: DeviceTensor) -> None:
 def download_into(ctx: Context, src: DeviceTensor, host: np.ndarray) -> None:
     """Asynchronous D2H into a (pinned) host array; synchronise the context before reading."""
     check(ctx._l.tncb_tensor_read(ctx.handle, src.handle, host.ctypes.data_as(C.c_void_p)))
+
+
+from .sampling import Sampler, Samples  # noqa: E402  (needs Context and DeviceTensor above)

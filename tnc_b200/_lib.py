@@ -49,6 +49,17 @@ TncbPath._fields_ = [
     ("nested", C.POINTER(TncbPath)),
 ]
 
+
+class TncbSampleSpec(C.Structure):
+    _fields_ = [("n_qubits", C.c_int), ("n_closed", C.c_size_t), ("closed_leaf", u64p), ("closed_qubit", i32p),
+                ("result_qubit", i32p)]
+
+
+class TncbSampleStats(C.Structure):
+    _fields_ = [("candidates", C.c_uint64), ("samples", C.c_uint64), ("clipped", C.c_uint64), ("passes", C.c_uint64),
+                ("max_ratio", C.c_double)]
+
+
 # every symbol include/tncb.h declares: (restype, argtypes)
 SIGNATURES = {
     "tncb_strerror": (C.c_char_p, [C.c_int]),
@@ -133,6 +144,8 @@ SIGNATURES = {
                                               C.POINTER(C.c_uint8), vpp]),
     "tncb_plan_hvp_sliced": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
                                        vpp, vpp, vpp, vpp]),
+    "tncb_plan_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(TncbSampleSpec), C.c_uint64, C.c_uint64, C.c_uint64,
+                                   C.c_uint64, C.c_double, C.c_size_t, C.c_void_p, C.c_void_p, C.POINTER(TncbSampleStats)]),
     "tncb_plan_destroy": (None, [C.c_void_p]),
     "tncb_angles_create": (C.c_int, [C.POINTER(TncbTn), C.c_size_t, C.c_size_t, C.c_void_p, C.POINTER(C.c_int64), C.c_size_t, vpp]),
     "tncb_angles_destroy": (C.c_int, [C.c_void_p]),

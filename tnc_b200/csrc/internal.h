@@ -241,6 +241,26 @@ struct TangentSumItem { long long t1, t2, out, elems; };   // byte offsets in th
 int launch_tangent_sum(tncb_ctx* ctx, const TangentSumItem* d_items, const long long* d_block_start, int n_items,
                        long long total_blocks, char* ws, int count, long long stride);
 
+// ---- sampling (tncb_plan_sample, sample.cu): the kernels of one pass of c candidate slots ----
+struct SampleMap {
+  int n_qubits, n_closed, k, _pad;
+  unsigned char closed_qubit[64];   // closed bit j (bit j of w0) is qubit closed_qubit[j]
+  unsigned char result_qubit[64];   // result leg r (row-major, leg 0 outermost) is qubit result_qubit[r]
+};
+struct SampleCand { unsigned long long bits; double p, ratio; int accept, clipped; };   // one candidate after selection
+struct SampleCounts { unsigned long long consumed, accepted, clipped; double max_ratio; };   // one pass, after the cut
+// candidates first .. first + n - 1: the one-hot bras of the closed bits, closed bra j of slot i at bras + (j c + i) * 2,
+// u and v at uv[i], the closed bits deposited on their qubits at closed_bits[i]
+int launch_sample_candidates(tncb_ctx* ctx, unsigned long long seed, unsigned long long first, size_t n, size_t c,
+                             const SampleMap& map, double2* bras, double2* uv, unsigned long long* closed_bits);
+// one block per slot i < n: the 2^k amplitudes at ws + i * stride + res_off, accept / reject, the pick (SampleCand)
+int launch_sample_select(tncb_ctx* ctx, const char* ws, long long stride, long long res_off, size_t n, double m,
+                         const SampleMap& map, const double2* uv, const unsigned long long* closed_bits, SampleCand* cand);
+// the accepted candidates of slots 0 .. n - 1, in slot order, up to `remaining` of them, into bits / probs (NULL: not
+// written); the pass's counts into *counts
+int launch_sample_compact(tncb_ctx* ctx, const SampleCand* cand, size_t n, unsigned long long remaining,
+                          unsigned long long* bits, double* probs, SampleCounts* counts);
+
 int tensor_new(tncb_ctx* ctx, int rank, const uint64_t* dims, tncb_tensor** out);
 
 // TensorData::File leaf (hdf5io.cpp): first member of /tensors, optionally adjointed, checked against the leaf's dims

@@ -13,7 +13,9 @@
 #include <complex>
 #include <cstdio>
 #include <cstdlib>
+#include <cmath>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <memory>
 
@@ -435,7 +437,7 @@ static size_t device_bytes(tncb_ctx* ctx) {
 // ---- which call takes which plan kind (the table in tncb.h) ----
 // The calls that take a plan, in the order of kRoutes' rows
 enum class Call { stage, run, execute, stage_slices, run_slices, run_batch, vjp, vjp_sliced, stage_batch, vjp_batch, jvp,
-                  jvp_batch, jvp_sliced, hvp, hvp_batch, hvp_sliced, stage_instances, set_leaves, grad_offsets, count };
+                  jvp_batch, jvp_sliced, hvp, hvp_batch, hvp_sliced, stage_instances, set_leaves, grad_offsets, sample, count };
 struct Refusal { int status; const char* msg; };
 static const Refusal
     kHvpRuns{TNCB_ERR_UNSUPPORTED, "a Hessian-vector plan runs through tncb_plan_hvp"},
@@ -458,7 +460,8 @@ static const Refusal
     kNotSlJvp{TNCB_ERR_INVALID, "not a sliced tangent plan (tncb_plan_create_jvp_sliced)"},
     kNotSlHvp{TNCB_ERR_INVALID, "not a sliced Hessian-vector plan (tncb_plan_create_hvp_sliced)"},
     kNotDerivStage{TNCB_ERR_INVALID, "not a gradient or tangent plan (plain plans stage many networks with tncb_plan_stage_slices)"},
-    kNotDeriv{TNCB_ERR_INVALID, "not a gradient or tangent plan (tncb_plan_create_vjp / _jvp)"};
+    kNotDeriv{TNCB_ERR_INVALID, "not a gradient or tangent plan (tncb_plan_create_vjp / _jvp)"},
+    kSamplePlain{TNCB_ERR_UNSUPPORTED, "tncb_plan_sample takes a plain plan (tncb_plan_create)"};
 static const Refusal* const kTakes = nullptr;
 static const Refusal* const kRoutes[(int)Call::count][7] = {
   //                    plain            vjp             jvp           hvp          sliced vjp      sliced jvp    sliced hvp
@@ -481,6 +484,7 @@ static const Refusal* const kRoutes[(int)Call::count][7] = {
   /* stage_instances */ {kTakes,          kTakes,         kTakes,       &kHvpRuns,   &kSlVjpLeaves,  &kSlJvpRuns,  &kSlHvpRuns},
   /* set_leaves */      {kTakes,          kTakes,         kTakes,       kTakes,      kTakes,         &kSlJvpRuns,  &kSlHvpRuns},
   /* grad_offsets */    {&kNotDeriv,      kTakes,         kTakes,       kTakes,      kTakes,         kTakes,       kTakes},
+  /* sample */          {kTakes,          &kSamplePlain,  &kSamplePlain, &kSamplePlain, &kSamplePlain, &kSamplePlain, &kSamplePlain},
 };
 
 // TNCB_OK if `c` takes P's kind, else the cell's refusal.  Every plan-taking call asks first, right after its null checks.
@@ -1352,45 +1356,67 @@ MemRangeFn get_mem_range() {
   return fn;
 }
 
+// payload elements of every leaf of S, -1 = no payload
+static std::vector<long long> leaf_elems(const Schedule& S) {
+  std::vector<long long> elems(S.n_leaves_total, -1);
+  for (const SlotMeta& m : S.slots) if (m.leaf_index >= 0) elems[m.leaf_index] = (long long)m.elems;
+  return elems;
+}
+// leaf li of a caller's list (`seen`: the leaves listed so far): in range, listed once, with a payload
+static int listed_leaf(const std::vector<long long>& elems, std::vector<char>& seen, uint64_t li, const std::string& name) {
+  if (li >= elems.size()) return fail(TNCB_ERR_INVALID, name + " is out of range (" + std::to_string(elems.size()) + " leaves)");
+  if (seen[li]) return fail(TNCB_ERR_INVALID, name + " is listed twice");
+  seen[li] = 1;
+  if (elems[li] < 0) return fail(TNCB_ERR_INVALID, name + " has no payload");
+  return TNCB_OK;
+}
+
+// Memory a launch will read or write at p, named `noun` in the messages after `name`: device or managed memory of the
+// ctx's device (device_memory), and its `bytes` inside the allocation that holds p (in_allocation)
+static int device_memory(const tncb_ctx* ctx, const void* p, const std::string& name, const char* noun) {
+  cudaPointerAttributes a{};
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return fail(TNCB_ERR_INVALID, name + ": " + noun + " is not device memory"); }
+  if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) return fail(TNCB_ERR_INVALID, name + ": " + noun + " is not device memory");
+  if (a.device != ctx->device)
+    return fail(TNCB_ERR_INVALID, name + ": " + noun + " is on device " + std::to_string(a.device) + ", the context on device " + std::to_string(ctx->device));
+  return TNCB_OK;
+}
+static int in_allocation(const void* p, unsigned long long bytes, const std::string& name, const char* noun) {
+  const MemRangeFn range = get_mem_range();
+  if (!range) return fail(TNCB_ERR_CUDA, "cuMemGetAddressRange is not available");
+  CUdeviceptr base = 0;
+  size_t size = 0;
+  if (range(&base, &size, (CUdeviceptr)p) != CUDA_SUCCESS) return fail(TNCB_ERR_INVALID, name + ": no device allocation holds " + noun);
+  if ((unsigned long long)((CUdeviceptr)p - base) + bytes > size)
+    return fail(TNCB_ERR_INVALID, name + ": " + noun + "'s " + std::to_string(bytes) + " bytes run past the end of its allocation");
+  return TNCB_OK;
+}
+
 // The stage items of the leaves leaf_index[0..n) of S, leaf k read from src[k] + i * stride[k] elements for instance
 // i < n_inst (stride == NULL: one instance).  Everything a launch could trip over is checked here, on the host, before
 // any copy: the leaf (in range, listed once, with a payload), the stride, and the source (non-null, 16-byte aligned,
 // device or managed memory of the ctx's device, every byte it reads inside one allocation).
 static int device_items(const tncb_ctx* ctx, const Schedule& S, size_t n_inst, size_t n, const uint64_t* leaf_index,
                         const void* const* src, const uint64_t* stride, std::vector<LeafStageItem>& items) {
-  std::vector<long long> elems(S.n_leaves_total, -1);   // payload elements per leaf, -1 = no payload
-  for (const SlotMeta& m : S.slots) if (m.leaf_index >= 0) elems[m.leaf_index] = (long long)m.elems;
+  const std::vector<long long> elems = leaf_elems(S);
   std::vector<char> seen(elems.size(), 0);
   items.clear();
   for (size_t k = 0; k < n; k++) {
     const uint64_t li = leaf_index[k];
     const std::string name = "leaf " + std::to_string(li);
-    if (li >= elems.size()) return fail(TNCB_ERR_INVALID, name + " is out of range (" + std::to_string(elems.size()) + " leaves)");
-    if (seen[li]) return fail(TNCB_ERR_INVALID, name + " is listed twice");
-    seen[li] = 1;
-    if (elems[li] < 0) return fail(TNCB_ERR_INVALID, name + " has no payload");
+    if (int rc = listed_leaf(elems, seen, li, name)) return rc;
     const unsigned long long e = (unsigned long long)elems[li], st = stride ? stride[k] : 0;
     if (st != 0 && st < e)
       return fail(TNCB_ERR_INVALID, name + ": instance stride " + std::to_string(st) + " is below its " + std::to_string(e) + " elements");
     const void* p = src[k];
     if (!p) return fail(TNCB_ERR_INVALID, name + ": the source is null");
     if ((uintptr_t)p % 16) return fail(TNCB_ERR_INVALID, name + ": the source is not 16-byte aligned");
-    cudaPointerAttributes a{};
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return fail(TNCB_ERR_INVALID, name + ": the source is not device memory"); }
-    if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) return fail(TNCB_ERR_INVALID, name + ": the source is not device memory");
-    if (a.device != ctx->device)
-      return fail(TNCB_ERR_INVALID, name + ": the source is on device " + std::to_string(a.device) + ", the context on device " + std::to_string(ctx->device));
+    if (int rc = device_memory(ctx, p, name, "the source")) return rc;
     unsigned long long span = 0, bytes = 0;        // [p, p + ((n_inst - 1) * stride + elems) * 16)
     if (__builtin_mul_overflow((unsigned long long)(n_inst - 1), st, &span) || __builtin_add_overflow(span, e, &span) ||
         __builtin_mul_overflow(span, 16ull, &bytes))
       return fail(TNCB_ERR_INVALID, name + ": the source range overflows 64 bits");
-    const MemRangeFn range = get_mem_range();
-    if (!range) return fail(TNCB_ERR_CUDA, "cuMemGetAddressRange is not available");
-    CUdeviceptr base = 0;
-    size_t size = 0;
-    if (range(&base, &size, (CUdeviceptr)p) != CUDA_SUCCESS) return fail(TNCB_ERR_INVALID, name + ": no device allocation holds the source");
-    if ((unsigned long long)((CUdeviceptr)p - base) + bytes > size)
-      return fail(TNCB_ERR_INVALID, name + ": the source's " + std::to_string(bytes) + " bytes run past the end of its allocation");
+    if (int rc = in_allocation(p, bytes, name, "the source")) return rc;
     items.push_back({(const double2*)p, st, (long long)S.leaf_offset[li], (long long)e});
   }
   return TNCB_OK;
@@ -1546,10 +1572,21 @@ struct InstanceFill {
 };
 // The inputs (rows of the instances: a tangent plan's tangents, seeds, seed tangents; NULL seeds: 1, NULL seed tangents:
 // zero) and the outputs, each made if its destination is non-null
+// A caller's work around every pass (tncb_plan_sample): at most `width` instances per pass (0: as many as fit); begin(c)
+// once the pass size c is known; fill(done, n) before the leaf blocks of instances done .. done + n - 1 are filled, to
+// write their device payloads (InstanceFill::dev then holds one pass: instance i of a pass reads src + i * src_stride);
+// end(base, ws, n, &stop) after the forward levels, to read the pass's workspaces; stop = true ends the call.
+struct PassHook {
+  size_t width = 0;
+  std::function<int(size_t c)> begin;
+  std::function<int(size_t done, size_t n)> fill;
+  std::function<int(const char* base, size_t ws, size_t n, bool* stop)> end;
+};
 struct InstanceIO {
   const tncb_tensor *tangents = nullptr, *seeds = nullptr, *seed_tangents = nullptr;
   tncb_tensor **values = nullptr, **tangent_rows = nullptr, **grad_rows = nullptr, **grad_sum = nullptr,
               **grad_tangent_rows = nullptr, **grad_tangent_sum = nullptr;
+  const PassHook* hook = nullptr;
 };
 
 // rows[0] instances with value rows of dims `rows` (result_rows), in passes of c instances on c copies of the plan's
@@ -1565,7 +1602,7 @@ static int run_instances(tncb_ctx* ctx, tncb_plan* P, const std::vector<uint64_t
   const bool backward = io.grad_rows || io.grad_sum || io.grad_tangent_rows || io.grad_tangent_sum;
   TNCB_CUDA(cudaSetDevice(ctx->device));
   BatchBlock B;
-  int rc = batch_size(ctx, P, count, &B);
+  int rc = batch_size(ctx, P, io.hook && io.hook->width ? std::min(count, io.hook->width) : count, &B);
   if (rc) return rc;
   Outputs out{ctx};
   tncb_tensor* v = out.add(io.values, (int)rows.size(), rows.data());
@@ -1576,6 +1613,7 @@ static int run_instances(tncb_ctx* ctx, tncb_plan* P, const std::vector<uint64_t
   tncb_tensor* dgs = out.add(io.grad_tangent_sum, 1, &ge);
   if (!(rc = out.rc)) rc = batch_alloc(ctx, &B);
   const size_t ws = B.ws, c = B.c;
+  if (!rc && io.hook) rc = io.hook->begin(c);
   void* aux = nullptr;                 // the seed 1 of every copy (scalar result, NULL seeds), the K3 scratch of the sums
   const size_t ones = backward && !io.seeds ? c : 0;
   size_t scratch = 0;
@@ -1602,15 +1640,18 @@ static int run_instances(tncb_ctx* ctx, tncb_plan* P, const std::vector<uint64_t
   const size_t block_bytes = std::max<size_t>(S.leaf_block_elems, 1) * sizeof(double2);
   const size_t res_bytes = S.slots[S.result_slot].elems * sizeof(double2);
   std::vector<LeafStageItem> items;
-  for (size_t done = 0; done < count && !rc; done += c) {
+  bool stop = false;
+  for (size_t done = 0; done < count && !rc && !stop; done += c) {
     const size_t n = std::min(c, count - done);
+    if (io.hook && (rc = io.hook->fill(done, n))) break;
     if (!fill.dev) {
       const char* src = (const char*)P->slices_dev + (fill.first + done) * block_bytes;
       if ((rc = batch_copy(ctx, B, base + P->leaf_off, ws, src, block_bytes, block_bytes, n))) break;
     } else {          // every copy's leaf block: the device payloads of instances done .. done+n-1, the staged block between
       const double2* staged = (const double2*)((const char*)P->ws + P->leaf_off);
       items.clear();
-      for (const LeafStageItem& it : *fill.dev) items.push_back({it.src + done * it.src_stride, it.src_stride, it.dst, it.elems});
+      const size_t at = io.hook ? 0 : done;
+      for (const LeafStageItem& it : *fill.dev) items.push_back({it.src + at * it.src_stride, it.src_stride, it.dst, it.elems});
       for (const LeafRun& lr : *fill.runs) items.push_back({staged + lr.start, 0, lr.start, lr.len});
       if ((rc = launch_leaf_stage(ctx, items.data(), items.size(), (double2*)(base + P->leaf_off), (long long)(ws / sizeof(double2)), n))) break;
     }
@@ -1618,6 +1659,7 @@ static int run_instances(tncb_ctx* ctx, tncb_plan* P, const std::vector<uint64_t
     if ((rc = enqueue_static(ctx, P, base, (int)n, (long long)ws, 0, P->n_fwd_levels))) break;
     for (auto [x, slot] : {std::pair<tncb_tensor*, int>{v, S.result_slot}, {t, P->tan_result}})
       if (!rc && x && res_bytes) rc = batch_copy(ctx, B, (char*)x->ptr + done * res_bytes, res_bytes, base + P->slot_off[slot], ws, res_bytes, n);
+    if (!rc && io.hook) rc = io.hook->end(base, ws, n, &stop);
     if (rc || !backward) continue;
     // the seed slots may reuse memory the forward levels freed: written after them, on the stream
     char* seed_dst = base + P->slot_off[P->seed_slot];
@@ -2215,6 +2257,132 @@ int tncb_plan_hvp_batch(tncb_ctx* ctx, tncb_plan* plan, size_t count, size_t n, 
   io.values = values; io.tangent_rows = tangent_rows; io.grad_rows = grad_rows; io.grad_sum = grad_sum;
   io.grad_tangent_rows = grad_tangent_rows; io.grad_tangent_sum = grad_tangent_sum;
   return run_instances(ctx, plan, rows, {0, &dev_items, &runs}, io);
+}
+
+namespace tncb {
+// The qubits of a sampling spec against the plan: every closed leaf a listed, rank-1, dimension-2 leaf with a payload, every
+// result leg of dimension 2, and the closed qubits and result legs' qubits together each qubit 0 .. n_qubits - 1 once
+static int sample_map(const Schedule& S, const tncb_sample_spec& sp, SampleMap* map) {
+  if (sp.n_qubits < 1 || sp.n_qubits > 64) return fail(TNCB_ERR_INVALID, "n_qubits " + std::to_string(sp.n_qubits) + " is outside 1..64");
+  const SlotMeta& rm = S.slots[S.result_slot];
+  const size_t k = rm.dims.size();
+  if ((sp.n_closed && (!sp.closed_leaf || !sp.closed_qubit)) || (k && !sp.result_qubit)) return fail(TNCB_ERR_INVALID, "null argument");
+  for (size_t r = 0; r < k; r++)
+    if (rm.dims[r] != 2) return fail(TNCB_ERR_INVALID, "result leg " + std::to_string(r) + " has dimension " + std::to_string(rm.dims[r]) + ", not 2");
+  const std::vector<long long> elems = leaf_elems(S);
+  std::vector<const SlotMeta*> meta(elems.size(), nullptr);
+  for (const SlotMeta& m : S.slots) if (m.leaf_index >= 0) meta[m.leaf_index] = &m;
+  std::vector<char> seen(elems.size(), 0), taken(sp.n_qubits, 0);
+  auto qubit = [&](int q, const std::string& what) -> int {
+    if (q < 0 || q >= sp.n_qubits) return fail(TNCB_ERR_INVALID, what + " is qubit " + std::to_string(q) + ", outside 0.." + std::to_string(sp.n_qubits - 1));
+    if (taken[q]) return fail(TNCB_ERR_INVALID, "qubit " + std::to_string(q) + " is listed twice (" + what + ")");
+    taken[q] = 1;
+    return TNCB_OK;
+  };
+  for (size_t j = 0; j < sp.n_closed; j++) {
+    const uint64_t li = sp.closed_leaf[j];
+    const std::string name = "closed leaf " + std::to_string(li);
+    if (int rc = listed_leaf(elems, seen, li, name)) return rc;
+    if (meta[li]->dims.size() != 1 || meta[li]->dims[0] != 2) return fail(TNCB_ERR_INVALID, name + " is not a rank-1 leaf of dimension 2");
+    if (int rc = qubit(sp.closed_qubit[j], "closed qubit " + std::to_string(j))) return rc;
+    map->closed_qubit[j] = (unsigned char)sp.closed_qubit[j];
+  }
+  for (size_t r = 0; r < k; r++) {
+    if (int rc = qubit(sp.result_qubit[r], "result leg " + std::to_string(r))) return rc;
+    map->result_qubit[r] = (unsigned char)sp.result_qubit[r];
+  }
+  for (int q = 0; q < sp.n_qubits; q++)
+    if (!taken[q]) return fail(TNCB_ERR_INVALID, "qubit " + std::to_string(q) + " is neither closed nor on a result leg");
+  map->n_qubits = sp.n_qubits; map->n_closed = (int)sp.n_closed; map->k = (int)k;
+  return TNCB_OK;
+}
+
+// the output buffer `name` of tncb_plan_sample: 8-byte aligned device memory of the ctx's device holding max_samples words
+static int sample_output(const tncb_ctx* ctx, const void* p, uint64_t max_samples, const char* name) {
+  unsigned long long bytes = 0;
+  if ((uintptr_t)p % 8) return fail(TNCB_ERR_INVALID, std::string(name) + ": the buffer is not 8-byte aligned");
+  if (__builtin_mul_overflow((unsigned long long)max_samples, 8ull, &bytes)) return fail(TNCB_ERR_INVALID, std::string(name) + ": max_samples words overflow 64 bits");
+  int rc = device_memory(ctx, p, name, "the buffer");
+  return rc ? rc : in_allocation(p, bytes, name, "the buffer");
+}
+} // namespace tncb
+
+// Sampling (tncb.h, DESIGN §5) on the instance-batched path of tncb_plan_hvp_batch: per pass of c candidates the candidate
+// kernel writes the closed bras, run_instances stages them as device payloads (the staged block's other leaves at
+// stride 0) and runs the forward levels, the select kernel reads every candidate's amplitudes in place and the compact
+// kernel writes the accepted samples in candidate order; one device-to-host copy of the pass's counts decides whether
+// another pass runs.  No leaf bytes come from the host.
+int tncb_plan_sample(tncb_ctx* ctx, tncb_plan* plan, const tncb_sample_spec* spec, uint64_t seed, uint64_t first,
+                     uint64_t max_candidates, uint64_t max_samples, double m, size_t batch, uint64_t* bits, double* probs,
+                     tncb_sample_stats* stats) {
+  using namespace tncb;
+  if (!ctx || !plan || !spec || !bits || !stats) return fail(TNCB_ERR_INVALID, "null argument");
+  int rc = route(plan, Call::sample);
+  if (rc) return rc;
+  if (!plan->is_static) return fail(TNCB_ERR_UNSUPPORTED, "sampling needs a plan with a static layout (no device leaves)");
+  if (plan->ctx != ctx || !plan->leaves_resident) return fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this plan and context");
+  const Schedule& S = plan->S;
+  SampleMap map{};
+  if ((rc = sample_map(S, *spec, &map))) return rc;
+  if (!std::isfinite(m) || !(m > 0)) return fail(TNCB_ERR_INVALID, "m must be finite and > 0, got " + std::to_string(m));
+  if (max_samples == 0) return fail(TNCB_ERR_INVALID, "max_samples is 0");
+  TNCB_CUDA(cudaSetDevice(ctx->device));
+  if ((rc = sample_output(ctx, bits, max_samples, "bits")) || (probs && (rc = sample_output(ctx, probs, max_samples, "probs")))) return rc;
+  tncb_sample_stats st{};
+  if (max_candidates == 0) { *stats = st; return TNCB_OK; }
+  const size_t nc = spec->n_closed;
+  // the closed bras as device payloads, two elements apart from candidate to candidate; their sources are set once the
+  // pass size is known
+  std::vector<LeafStageItem> dev_items;
+  std::vector<long long> closed_dst(nc);
+  for (size_t j = 0; j < nc; j++) {
+    closed_dst[j] = (long long)S.leaf_offset[spec->closed_leaf[j]];
+    dev_items.push_back({nullptr, 2, closed_dst[j], 2});
+  }
+  const std::vector<LeafRun> runs = leaf_runs(dev_items, (long long)std::max<size_t>(S.leaf_block_elems, 1));
+  void* blk = nullptr;
+  size_t blk_bytes = 0, c = 0;
+  double2 *bras = nullptr, *uv = nullptr;
+  unsigned long long* closed_bits = nullptr;
+  SampleCand* cand = nullptr;
+  SampleCounts* d_counts = nullptr;
+  PassHook hook;
+  hook.width = batch;
+  hook.begin = [&](size_t pass) -> int {
+    auto up = [](size_t b) { return (b + 255) / 256 * 256; };
+    c = pass;
+    const size_t o_uv = up(nc * c * 2 * sizeof(double2)), o_bits = o_uv + up(c * sizeof(double2));
+    const size_t o_cand = o_bits + up(c * sizeof(unsigned long long)), o_counts = o_cand + up(c * sizeof(SampleCand));
+    blk_bytes = o_counts + sizeof(SampleCounts);
+    if (int r = ctx->arena.alloc(blk_bytes, &blk)) return r;
+    char* b = (char*)blk;
+    bras = (double2*)b; uv = (double2*)(b + o_uv); closed_bits = (unsigned long long*)(b + o_bits);
+    cand = (SampleCand*)(b + o_cand); d_counts = (SampleCounts*)(b + o_counts);
+    for (LeafStageItem& it : dev_items)
+      it.src = bras + (size_t)(std::find(closed_dst.begin(), closed_dst.end(), it.dst) - closed_dst.begin()) * c * 2;
+    return TNCB_OK;
+  };
+  hook.fill = [&](size_t done, size_t n) -> int { return launch_sample_candidates(ctx, seed, first + done, n, c, map, bras, uv, closed_bits); };
+  hook.end = [&](const char* base, size_t ws, size_t n, bool* stop) -> int {
+    int r = launch_sample_select(ctx, base, (long long)ws, (long long)plan->slot_off[S.result_slot], n, m, map, uv, closed_bits, cand);
+    if (!r) r = launch_sample_compact(ctx, cand, n, max_samples - st.samples, (unsigned long long*)bits + st.samples,
+                                      probs ? probs + st.samples : nullptr, d_counts);
+    if (r) return r;
+    SampleCounts h{};
+    TNCB_CUDA(cudaMemcpyAsync(&h, d_counts, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
+    TNCB_CUDA(cudaStreamSynchronize(ctx->stream));
+    st.candidates += h.consumed; st.samples += h.accepted; st.clipped += h.clipped; st.passes++;
+    st.max_ratio = std::max(st.max_ratio, h.max_ratio);
+    *stop = st.samples == max_samples;
+    return TNCB_OK;
+  };
+  InstanceIO io;
+  io.hook = &hook;
+  rc = run_instances(ctx, plan, std::vector<uint64_t>{max_candidates}, {0, &dev_items, &runs}, io);
+  if (blk) ctx->arena.free(blk, blk_bytes);
+  if (rc) return rc;
+  *stats = st;
+  return TNCB_OK;
 }
 
 namespace tncb {
