@@ -293,7 +293,8 @@ int tncb_network_out_legs(const tncb_tn* tn, const tncb_path* path, int* n_out, 
  *   stage_instances        .     .    .    U       U           U           U
  *   set_leaves             .     .    .    .       .           U           U
  *   grad_offsets           I     .    .    .       .           .           .
- *   sample                 .     U    U    U       U           U           U          */
+ *   sample                 .     U    U    U       U           U           U
+ *   sample_slices          .     U    U    U       U           U           U          */
 int tncb_plan_create(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, tncb_plan** out);
 /* `tn` must have the structure the plan was compiled from: every leaf is re-validated (kind, rank,
  * dims, non-null payload, live device handle) -> TNCB_ERR_INVALID / TNCB_ERR_SHAPE /
@@ -576,6 +577,28 @@ typedef struct tncb_sample_stats { uint64_t candidates, samples, clipped, passes
 int tncb_plan_sample(tncb_ctx* ctx, tncb_plan* plan, const tncb_sample_spec* spec, uint64_t seed, uint64_t first,
                      uint64_t max_candidates, uint64_t max_samples, double m, size_t batch, uint64_t* bits, double* probs,
                      tncb_sample_stats* stats);
+/* Sampling a circuit whose amplitude network only contracts sliced: the networks staged by tncb_plan_stage_slices on
+ * ctx are the S slices of one open amplitude network, each with the closed bras at the same leaf indices (their staged
+ * payloads are ignored), and candidate c's amplitudes are a_c(y) = sum_q R_q(c, y) over q = 0 .. S-1, formed as
+ * tncb_plan_run_slices(0, 1) forms its sum: R_0 copied, then R_1, R_2, ... added in slice order, so that a_c is
+ * bit-identical to that call on c's sliced networks.  Everything else -- the random stream, acceptance, the pick, the
+ * clipping stats, candidate order, resuming at first + stats->candidates -- is tncb_plan_sample's contract.  Ranks of a
+ * multi-GPU job split candidates through `first`, never slices: a candidate needs every slice.
+ * Per pass: the candidate kernel once; for each slice, one leaf staging launch from that slice's staged block, the
+ * batched forward levels and one launch that folds every candidate's result into its row of a [c, 2^k] accumulator;
+ * then the select and compact kernels on the accumulator and the counts read-back, as tncb_plan_sample.
+ * Memory: `batch` (0: as many as fit) workspace copies beside the plan's own, leaving 1 GiB and the int8 engine's plane
+ * budget free, as tncb_plan_run_batch.  When the device has no room for even one copy, the call does not fail: it runs
+ * one candidate per pass in the plan's own workspace and clears the leaves tncb_plan_stage put there, so a later
+ * tncb_plan_run or tncb_plan_sample needs tncb_plan_stage again (until then they return TNCB_ERR_INVALID).  tncb_plan_run_slices and
+ * tncb_plan_run_batch stage their leaves on every call and are unaffected; the staged slices are never written.  The
+ * stats do not say which way a call ran, and the bits are the same either way.
+ * Refusals: every refusal of tncb_plan_sample, with the same messages, except that "not staged" means nothing staged by
+ * tncb_plan_stage_slices on ctx (TNCB_ERR_INVALID).  A slice whose closed bra is not a rank-1, dimension-2 leaf (a
+ * sliced leg on a closed bra makes one) is refused as a closed leaf of the wrong shape. */
+int tncb_plan_sample_slices(tncb_ctx* ctx, tncb_plan* plan, const tncb_sample_spec* spec, uint64_t seed, uint64_t first,
+                            uint64_t max_candidates, uint64_t max_samples, double m, size_t batch, uint64_t* bits,
+                            double* probs, tncb_sample_stats* stats);
 /* ---- sliced tangents and Hessian-vector products: networks whose tangent or Hessian-vector workspace does not fit ----
  * By linearity, as for sliced gradients: R = sum_q R_q, so Ṙ = sum_q Ṙ_q; slice q's leaf (and its tangent) is q's
  * fixed-index sub-block of the full leaf (and of its full-shape tangent), and q's G_l and Ġ_l add into q's sub-block of

@@ -146,6 +146,9 @@ SIGNATURES = {
                                        vpp, vpp, vpp, vpp]),
     "tncb_plan_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(TncbSampleSpec), C.c_uint64, C.c_uint64, C.c_uint64,
                                    C.c_uint64, C.c_double, C.c_size_t, C.c_void_p, C.c_void_p, C.POINTER(TncbSampleStats)]),
+    "tncb_plan_sample_slices": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(TncbSampleSpec), C.c_uint64, C.c_uint64,
+                                          C.c_uint64, C.c_uint64, C.c_double, C.c_size_t, C.c_void_p, C.c_void_p,
+                                          C.POINTER(TncbSampleStats)]),
     "tncb_plan_destroy": (None, [C.c_void_p]),
     "tncb_angles_create": (C.c_int, [C.POINTER(TncbTn), C.c_size_t, C.c_size_t, C.c_void_p, C.POINTER(C.c_int64), C.c_size_t, vpp]),
     "tncb_angles_destroy": (C.c_int, [C.c_void_p]),

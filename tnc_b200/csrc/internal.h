@@ -256,6 +256,10 @@ int launch_sample_candidates(tncb_ctx* ctx, unsigned long long seed, unsigned lo
 // one block per slot i < n: the 2^k amplitudes at ws + i * stride + res_off, accept / reject, the pick (SampleCand)
 int launch_sample_select(tncb_ctx* ctx, const char* ws, long long stride, long long res_off, size_t n, double m,
                          const SampleMap& map, const double2* uv, const unsigned long long* closed_bits, SampleCand* cand);
+// tncb_plan_sample_slices: slot i's result (ws + i * stride + res_off, `elems` elements) into row i of acc ([n, elems]),
+// copied (first) or added, the arithmetic of launch_add
+int launch_sample_accumulate(tncb_ctx* ctx, const char* ws, long long stride, long long res_off, size_t n, size_t elems,
+                             bool first, double2* acc);
 // the accepted candidates of slots 0 .. n - 1, in slot order, up to `remaining` of them, into bits / probs (NULL: not
 // written); the pass's counts into *counts
 int launch_sample_compact(tncb_ctx* ctx, const SampleCand* cand, size_t n, unsigned long long remaining,

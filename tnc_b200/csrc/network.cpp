@@ -437,7 +437,8 @@ static size_t device_bytes(tncb_ctx* ctx) {
 // ---- which call takes which plan kind (the table in tncb.h) ----
 // The calls that take a plan, in the order of kRoutes' rows
 enum class Call { stage, run, execute, stage_slices, run_slices, run_batch, vjp, vjp_sliced, stage_batch, vjp_batch, jvp,
-                  jvp_batch, jvp_sliced, hvp, hvp_batch, hvp_sliced, stage_instances, set_leaves, grad_offsets, sample, count };
+                  jvp_batch, jvp_sliced, hvp, hvp_batch, hvp_sliced, stage_instances, set_leaves, grad_offsets, sample, sample_slices,
+                  count };
 struct Refusal { int status; const char* msg; };
 static const Refusal
     kHvpRuns{TNCB_ERR_UNSUPPORTED, "a Hessian-vector plan runs through tncb_plan_hvp"},
@@ -461,7 +462,8 @@ static const Refusal
     kNotSlHvp{TNCB_ERR_INVALID, "not a sliced Hessian-vector plan (tncb_plan_create_hvp_sliced)"},
     kNotDerivStage{TNCB_ERR_INVALID, "not a gradient or tangent plan (plain plans stage many networks with tncb_plan_stage_slices)"},
     kNotDeriv{TNCB_ERR_INVALID, "not a gradient or tangent plan (tncb_plan_create_vjp / _jvp)"},
-    kSamplePlain{TNCB_ERR_UNSUPPORTED, "tncb_plan_sample takes a plain plan (tncb_plan_create)"};
+    kSamplePlain{TNCB_ERR_UNSUPPORTED, "tncb_plan_sample takes a plain plan (tncb_plan_create)"},
+    kSampleSlPlain{TNCB_ERR_UNSUPPORTED, "tncb_plan_sample_slices takes a plain plan (tncb_plan_create)"};
 static const Refusal* const kTakes = nullptr;
 static const Refusal* const kRoutes[(int)Call::count][7] = {
   //                    plain            vjp             jvp           hvp          sliced vjp      sliced jvp    sliced hvp
@@ -485,6 +487,8 @@ static const Refusal* const kRoutes[(int)Call::count][7] = {
   /* set_leaves */      {kTakes,          kTakes,         kTakes,       kTakes,      kTakes,         &kSlJvpRuns,  &kSlHvpRuns},
   /* grad_offsets */    {&kNotDeriv,      kTakes,         kTakes,       kTakes,      kTakes,         kTakes,       kTakes},
   /* sample */          {kTakes,          &kSamplePlain,  &kSamplePlain, &kSamplePlain, &kSamplePlain, &kSamplePlain, &kSamplePlain},
+  /* sample_slices */   {kTakes,          &kSampleSlPlain, &kSampleSlPlain, &kSampleSlPlain, &kSampleSlPlain, &kSampleSlPlain,
+                         &kSampleSlPlain},
 };
 
 // TNCB_OK if `c` takes P's kind, else the cell's refusal.  Every plan-taking call asks first, right after its null checks.
@@ -1272,6 +1276,7 @@ static int stage_networks(tncb_ctx* ctx, tncb_plan* P, size_t n, const tncb_tn* 
 struct BatchBlock {
   size_t ws = 0, c = 0;         // bytes per copy, copies per pass
   bool strided = true;          // the copies fit the device's largest copy pitch (2 GiB): one 2D copy per pass
+  bool no_room = false;         // batch_size refused because the device had no room for one copy
   void* blk = nullptr;
 };
 
@@ -1292,6 +1297,7 @@ static int batch_size(tncb_ctx* ctx, const tncb_plan* P, size_t count, BatchBloc
   const size_t keep = ((size_t)1 << 30) + (int8 ? ctx->crt_ws_bytes : 0);
   const size_t room = dev_free + (ctx->arena.reserved - ctx->arena.live);
   B->c = std::min(B->c, room > keep ? (room - keep) / B->ws : 0);
+  B->no_room = B->c == 0;
   if (B->c == 0) return fail(TNCB_ERR_OOM, "no room on the device for the workspace of one instance");
   return TNCB_OK;
 }
@@ -1565,10 +1571,13 @@ static int gather_set(tncb_ctx* ctx, const tncb_plan* P, const std::vector<GradI
 // ---- instance-batched passes (tncb_plan_run_batch / _vjp_batch / _jvp_batch / _hvp_batch) ----
 // Where a pass's leaf blocks come from: the staged instance blocks from `first` on (dev == nullptr), or the device
 // payloads `dev` (sorted by leaf_runs) with the `runs` between them from the plan's staged leaf block, at stride 0
+// (slices > 0, with dev: the runs come from the first `slices` staged instance blocks in turn, and every pass contracts
+// once per block, PassHook::fold after each)
 struct InstanceFill {
   size_t first = 0;
   const std::vector<LeafStageItem>* dev = nullptr;
   const std::vector<LeafRun>* runs = nullptr;
+  size_t slices = 0;
 };
 // The inputs (rows of the instances: a tangent plan's tangents, seeds, seed tangents; NULL seeds: 1, NULL seed tangents:
 // zero) and the outputs, each made if its destination is non-null
@@ -1576,10 +1585,16 @@ struct InstanceFill {
 // once the pass size c is known; fill(done, n) before the leaf blocks of instances done .. done + n - 1 are filled, to
 // write their device payloads (InstanceFill::dev then holds one pass: instance i of a pass reads src + i * src_stride);
 // end(base, ws, n, &stop) after the forward levels, to read the pass's workspaces; stop = true ends the call.
+// fold(q, base, ws, n) after the forward levels of staged block q (InstanceFill::slices).  in_place: when the device has
+// no room for one copy beside the plan's workspace, run one instance per pass in that workspace instead; its staged
+// leaves are then gone (leaves_resident is cleared before the first launch).  Only for fills whose runs do not come
+// from the plan's own staged block.
 struct PassHook {
   size_t width = 0;
+  bool in_place = false;
   std::function<int(size_t c)> begin;
   std::function<int(size_t done, size_t n)> fill;
+  std::function<int(size_t q, const char* base, size_t ws, size_t n)> fold;
   std::function<int(const char* base, size_t ws, size_t n, bool* stop)> end;
 };
 struct InstanceIO {
@@ -1603,6 +1618,9 @@ static int run_instances(tncb_ctx* ctx, tncb_plan* P, const std::vector<uint64_t
   TNCB_CUDA(cudaSetDevice(ctx->device));
   BatchBlock B;
   int rc = batch_size(ctx, P, io.hook && io.hook->width ? std::min(count, io.hook->width) : count, &B);
+  const bool may_borrow = io.hook && io.hook->in_place;
+  bool in_place = rc == TNCB_ERR_OOM && B.no_room && may_borrow;
+  if (in_place) rc = TNCB_OK;
   if (rc) return rc;
   Outputs out{ctx};
   tncb_tensor* v = out.add(io.values, (int)rows.size(), rows.data());
@@ -1611,7 +1629,11 @@ static int run_instances(tncb_ctx* ctx, tncb_plan* P, const std::vector<uint64_t
   tncb_tensor* gs = out.add(io.grad_sum, 1, &ge);
   tncb_tensor* dgr = out.add(io.grad_tangent_rows, 2, row_dims);
   tncb_tensor* dgs = out.add(io.grad_tangent_sum, 1, &ge);
-  if (!(rc = out.rc)) rc = batch_alloc(ctx, &B);
+  if (!(rc = out.rc) && !in_place && (rc = batch_alloc(ctx, &B)) == TNCB_ERR_OOM && may_borrow) { in_place = true; rc = TNCB_OK; }
+  if (!rc && in_place) {         // the plan's own workspace is the one copy
+    B.c = 1; B.blk = nullptr;
+    P->leaves_resident = false; P->fwd_ready = false;
+  }
   const size_t ws = B.ws, c = B.c;
   if (!rc && io.hook) rc = io.hook->begin(c);
   void* aux = nullptr;                 // the seed 1 of every copy (scalar result, NULL seeds), the K3 scratch of the sums
@@ -1634,7 +1656,7 @@ static int run_instances(tncb_ctx* ctx, tncb_plan* P, const std::vector<uint64_t
     cudaError_t e = cudaMemsetAsync(x->ptr, 0, std::max<uint64_t>(ge, 1) * sizeof(double2), ctx->stream);
     if (e != cudaSuccess) rc = fail(TNCB_ERR_CUDA, std::string("gradient sum: ") + cudaGetErrorString(e));
   }
-  char* base = (char*)B.blk;
+  char* base = in_place ? (char*)P->ws : (char*)B.blk;
   const double2* d_one = (const double2*)aux;
   double2* d_scratch = (double2*)aux + ones;
   const size_t block_bytes = std::max<size_t>(S.leaf_block_elems, 1) * sizeof(double2);
@@ -1644,19 +1666,24 @@ static int run_instances(tncb_ctx* ctx, tncb_plan* P, const std::vector<uint64_t
   for (size_t done = 0; done < count && !rc && !stop; done += c) {
     const size_t n = std::min(c, count - done);
     if (io.hook && (rc = io.hook->fill(done, n))) break;
-    if (!fill.dev) {
-      const char* src = (const char*)P->slices_dev + (fill.first + done) * block_bytes;
-      if ((rc = batch_copy(ctx, B, base + P->leaf_off, ws, src, block_bytes, block_bytes, n))) break;
-    } else {          // every copy's leaf block: the device payloads of instances done .. done+n-1, the staged block between
-      const double2* staged = (const double2*)((const char*)P->ws + P->leaf_off);
-      items.clear();
-      const size_t at = io.hook ? 0 : done;
-      for (const LeafStageItem& it : *fill.dev) items.push_back({it.src + at * it.src_stride, it.src_stride, it.dst, it.elems});
-      for (const LeafRun& lr : *fill.runs) items.push_back({staged + lr.start, 0, lr.start, lr.len});
-      if ((rc = launch_leaf_stage(ctx, items.data(), items.size(), (double2*)(base + P->leaf_off), (long long)(ws / sizeof(double2)), n))) break;
+    for (size_t q = 0; q < std::max<size_t>(fill.slices, 1) && !rc; q++) {
+      if (!fill.dev) {
+        const char* src = (const char*)P->slices_dev + (fill.first + done) * block_bytes;
+        rc = batch_copy(ctx, B, base + P->leaf_off, ws, src, block_bytes, block_bytes, n);
+      } else {        // every copy's leaf block: the device payloads of instances done .. done+n-1, the staged block between
+        const char* block = fill.slices ? (const char*)P->slices_dev + q * block_bytes : (const char*)P->ws + P->leaf_off;
+        const double2* staged = (const double2*)block;
+        items.clear();
+        const size_t at = io.hook ? 0 : done;
+        for (const LeafStageItem& it : *fill.dev) items.push_back({it.src + at * it.src_stride, it.src_stride, it.dst, it.elems});
+        for (const LeafRun& lr : *fill.runs) items.push_back({staged + lr.start, 0, lr.start, lr.len});
+        rc = launch_leaf_stage(ctx, items.data(), items.size(), (double2*)(base + P->leaf_off), (long long)(ws / sizeof(double2)), n);
+      }
+      if (!rc && P->tangent()) rc = stage_tangents(ctx, P, io.tangents->ptr + done * ge, ge, base, (long long)ws, n);
+      if (!rc) rc = enqueue_static(ctx, P, base, (int)n, (long long)ws, 0, P->n_fwd_levels);
+      if (!rc && fill.slices) rc = io.hook->fold(q, base, ws, n);
     }
-    if (P->tangent() && (rc = stage_tangents(ctx, P, io.tangents->ptr + done * ge, ge, base, (long long)ws, n))) break;
-    if ((rc = enqueue_static(ctx, P, base, (int)n, (long long)ws, 0, P->n_fwd_levels))) break;
+    if (rc) break;
     for (auto [x, slot] : {std::pair<tncb_tensor*, int>{v, S.result_slot}, {t, P->tan_result}})
       if (!rc && x && res_bytes) rc = batch_copy(ctx, B, (char*)x->ptr + done * res_bytes, res_bytes, base + P->slot_off[slot], ws, res_bytes, n);
     if (!rc && io.hook) rc = io.hook->end(base, ws, n, &stop);
@@ -2305,22 +2332,28 @@ static int sample_output(const tncb_ctx* ctx, const void* p, uint64_t max_sample
   int rc = device_memory(ctx, p, name, "the buffer");
   return rc ? rc : in_allocation(p, bytes, name, "the buffer");
 }
-} // namespace tncb
 
 // Sampling (tncb.h, DESIGN §5) on the instance-batched path of tncb_plan_hvp_batch: per pass of c candidates the candidate
 // kernel writes the closed bras, run_instances stages them as device payloads (the staged block's other leaves at
 // stride 0) and runs the forward levels, the select kernel reads every candidate's amplitudes in place and the compact
 // kernel writes the accepted samples in candidate order; one device-to-host copy of the pass's counts decides whether
 // another pass runs.  No leaf bytes come from the host.
-int tncb_plan_sample(tncb_ctx* ctx, tncb_plan* plan, const tncb_sample_spec* spec, uint64_t seed, uint64_t first,
-                     uint64_t max_candidates, uint64_t max_samples, double m, size_t batch, uint64_t* bits, double* probs,
-                     tncb_sample_stats* stats) {
-  using namespace tncb;
+// sliced (tncb_plan_sample_slices): the other leaves come from each network staged by tncb_plan_stage_slices in turn,
+// and after each one's forward levels the accumulate kernel folds every candidate's result into its row of a [c, 2^k]
+// block, which the select kernel then reads instead of the workspaces.  When no copy fits beside the plan's workspace
+// the pass runs one candidate in that workspace (PassHook::in_place).
+static int sample_call(tncb_ctx* ctx, tncb_plan* plan, const tncb_sample_spec* spec, uint64_t seed, uint64_t first,
+                       uint64_t max_candidates, uint64_t max_samples, double m, size_t batch, uint64_t* bits, double* probs,
+                       tncb_sample_stats* stats, bool sliced) {
   if (!ctx || !plan || !spec || !bits || !stats) return fail(TNCB_ERR_INVALID, "null argument");
-  int rc = route(plan, Call::sample);
+  int rc = route(plan, sliced ? Call::sample_slices : Call::sample);
   if (rc) return rc;
   if (!plan->is_static) return fail(TNCB_ERR_UNSUPPORTED, "sampling needs a plan with a static layout (no device leaves)");
-  if (plan->ctx != ctx || !plan->leaves_resident) return fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this plan and context");
+  if (sliced) {
+    if (!plan->slices_dev || plan->ctx != ctx) return fail(TNCB_ERR_INVALID, "tncb_plan_stage_slices has not been called on this context");
+  } else if (plan->ctx != ctx || !plan->leaves_resident) {
+    return fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this plan and context");
+  }
   const Schedule& S = plan->S;
   SampleMap map{};
   if ((rc = sample_map(S, *spec, &map))) return rc;
@@ -2331,6 +2364,7 @@ int tncb_plan_sample(tncb_ctx* ctx, tncb_plan* plan, const tncb_sample_spec* spe
   tncb_sample_stats st{};
   if (max_candidates == 0) { *stats = st; return TNCB_OK; }
   const size_t nc = spec->n_closed;
+  const size_t res_elems = std::max<size_t>(S.slots[S.result_slot].elems, 1);
   // the closed bras as device payloads, two elements apart from candidate to candidate; their sources are set once the
   // pass size is known
   std::vector<LeafStageItem> dev_items;
@@ -2342,29 +2376,36 @@ int tncb_plan_sample(tncb_ctx* ctx, tncb_plan* plan, const tncb_sample_spec* spe
   const std::vector<LeafRun> runs = leaf_runs(dev_items, (long long)std::max<size_t>(S.leaf_block_elems, 1));
   void* blk = nullptr;
   size_t blk_bytes = 0, c = 0;
-  double2 *bras = nullptr, *uv = nullptr;
+  double2 *bras = nullptr, *uv = nullptr, *acc = nullptr;
   unsigned long long* closed_bits = nullptr;
   SampleCand* cand = nullptr;
   SampleCounts* d_counts = nullptr;
   PassHook hook;
   hook.width = batch;
+  hook.in_place = sliced;
   hook.begin = [&](size_t pass) -> int {
     auto up = [](size_t b) { return (b + 255) / 256 * 256; };
     c = pass;
-    const size_t o_uv = up(nc * c * 2 * sizeof(double2)), o_bits = o_uv + up(c * sizeof(double2));
+    const size_t o_bras = sliced ? up(c * res_elems * sizeof(double2)) : 0;
+    const size_t o_uv = o_bras + up(nc * c * 2 * sizeof(double2)), o_bits = o_uv + up(c * sizeof(double2));
     const size_t o_cand = o_bits + up(c * sizeof(unsigned long long)), o_counts = o_cand + up(c * sizeof(SampleCand));
     blk_bytes = o_counts + sizeof(SampleCounts);
     if (int r = ctx->arena.alloc(blk_bytes, &blk)) return r;
     char* b = (char*)blk;
-    bras = (double2*)b; uv = (double2*)(b + o_uv); closed_bits = (unsigned long long*)(b + o_bits);
+    if (sliced) acc = (double2*)b;
+    bras = (double2*)(b + o_bras); uv = (double2*)(b + o_uv); closed_bits = (unsigned long long*)(b + o_bits);
     cand = (SampleCand*)(b + o_cand); d_counts = (SampleCounts*)(b + o_counts);
     for (LeafStageItem& it : dev_items)
       it.src = bras + (size_t)(std::find(closed_dst.begin(), closed_dst.end(), it.dst) - closed_dst.begin()) * c * 2;
     return TNCB_OK;
   };
   hook.fill = [&](size_t done, size_t n) -> int { return launch_sample_candidates(ctx, seed, first + done, n, c, map, bras, uv, closed_bits); };
+  hook.fold = [&](size_t q, const char* base, size_t ws, size_t n) -> int {
+    return launch_sample_accumulate(ctx, base, (long long)ws, (long long)plan->slot_off[S.result_slot], n, res_elems, q == 0, acc);
+  };
   hook.end = [&](const char* base, size_t ws, size_t n, bool* stop) -> int {
-    int r = launch_sample_select(ctx, base, (long long)ws, (long long)plan->slot_off[S.result_slot], n, m, map, uv, closed_bits, cand);
+    int r = sliced ? launch_sample_select(ctx, (const char*)acc, (long long)(res_elems * sizeof(double2)), 0, n, m, map, uv, closed_bits, cand)
+                   : launch_sample_select(ctx, base, (long long)ws, (long long)plan->slot_off[S.result_slot], n, m, map, uv, closed_bits, cand);
     if (!r) r = launch_sample_compact(ctx, cand, n, max_samples - st.samples, (unsigned long long*)bits + st.samples,
                                       probs ? probs + st.samples : nullptr, d_counts);
     if (r) return r;
@@ -2378,11 +2419,26 @@ int tncb_plan_sample(tncb_ctx* ctx, tncb_plan* plan, const tncb_sample_spec* spe
   };
   InstanceIO io;
   io.hook = &hook;
-  rc = run_instances(ctx, plan, std::vector<uint64_t>{max_candidates}, {0, &dev_items, &runs}, io);
+  rc = run_instances(ctx, plan, std::vector<uint64_t>{max_candidates}, {0, &dev_items, &runs, sliced ? plan->n_slices : 0}, io);
   if (blk) ctx->arena.free(blk, blk_bytes);
   if (rc) return rc;
   *stats = st;
   return TNCB_OK;
+}
+} // namespace tncb
+
+int tncb_plan_sample(tncb_ctx* ctx, tncb_plan* plan, const tncb_sample_spec* spec, uint64_t seed, uint64_t first,
+                     uint64_t max_candidates, uint64_t max_samples, double m, size_t batch, uint64_t* bits, double* probs,
+                     tncb_sample_stats* stats) {
+  return tncb::sample_call(ctx, plan, spec, seed, first, max_candidates, max_samples, m, batch, bits, probs, stats, false);
+}
+
+// A candidate's amplitudes are the sum over the S staged slices, R_0 copied, then R_1, R_2, ... added: the fold
+// tncb_plan_run_slices(0, 1) forms.
+int tncb_plan_sample_slices(tncb_ctx* ctx, tncb_plan* plan, const tncb_sample_spec* spec, uint64_t seed, uint64_t first,
+                            uint64_t max_candidates, uint64_t max_samples, double m, size_t batch, uint64_t* bits,
+                            double* probs, tncb_sample_stats* stats) {
+  return tncb::sample_call(ctx, plan, spec, seed, first, max_candidates, max_samples, m, batch, bits, probs, stats, true);
 }
 
 namespace tncb {

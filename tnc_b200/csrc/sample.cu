@@ -1,6 +1,6 @@
-// Sampling bitstrings from a circuit's output distribution (tncb_plan_sample): the three kernels of one pass around the
-// batched contraction of the candidates' networks.  The algorithm and the random stream are described in tncb.h and
-// DESIGN §5.  Nothing here uses atomics, so a pass's output repeats bit for bit.
+// Sampling bitstrings from a circuit's output distribution (tncb_plan_sample, tncb_plan_sample_slices): the kernels of one
+// pass around the batched contraction of the candidates' networks.  The algorithm and the random stream are described in
+// tncb.h and DESIGN §5.  Nothing here uses atomics, so a pass's output repeats bit for bit.
 #include "internal.h"
 #include "philox.h"
 
@@ -9,6 +9,7 @@ namespace tncb {
 constexpr int kCandThreads = 128;
 constexpr int kSelectThreads = 256;
 constexpr int kCompactThreads = 512;
+constexpr int kAccThreads = 256;
 
 // |z|^2 and the prefix sums with explicit roundings: no contraction into FMAs, so that every sum of the selection is
 // formed the same way in each loop that forms it (and as numpy forms it)
@@ -108,6 +109,37 @@ int launch_sample_select(tncb_ctx* ctx, const char* ws, long long stride, long l
   if (n > 0x7fffffffull) return fail(TNCB_ERR_UNSUPPORTED, "too many candidates in one selection launch");
   const double scale = ldexp(1.0, map.n_qubits - map.k);    // 2^(n - k), exact
   sample_select_kernel<<<(unsigned)n, kSelectThreads, 0, ctx->stream>>>(ws, stride, res_off, scale, m, map, uv, closed_bits, cand);
+  ctx->launches++;
+  TNCB_CUDA(cudaGetLastError());
+  return TNCB_OK;
+}
+
+// ------------------------------------------------------------------------------------------
+// Slice sum (tncb_plan_sample_slices): row i of acc gets slot i's result, the instance blockIdx.y.  The first slice is
+// copied, every later one added with add_kernel's arithmetic, so that a row is the left fold tncb_plan_run_slices forms.
+// One 16-byte load (and store) per element and operand.
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kAccThreads)
+sample_accumulate_kernel(const char* __restrict__ ws, long long stride, long long res_off, long long elems, int first,
+                         double2* __restrict__ acc) {
+  const unsigned long long i = blockIdx.y;
+  const double2* r = reinterpret_cast<const double2*>(ws + (long long)i * stride + res_off);
+  double2* a = acc + (long long)i * elems;
+  for (long long o = (long long)blockIdx.x * kAccThreads + threadIdx.x; o < elems; o += (long long)gridDim.x * kAccThreads) {
+    const double2 v = r[o];
+    if (first) { a[o] = v; continue; }
+    double2 d = a[o];
+    d.x += v.x; d.y += v.y; a[o] = d;
+  }
+}
+
+int launch_sample_accumulate(tncb_ctx* ctx, const char* ws, long long stride, long long res_off, size_t n, size_t elems,
+                             bool first, double2* acc) {
+  if (n == 0 || elems == 0) return TNCB_OK;
+  if (n > 65535) return fail(TNCB_ERR_UNSUPPORTED, "too many candidates in one accumulate launch");
+  const unsigned blocks = (unsigned)std::min<long long>(((long long)elems + kAccThreads - 1) / kAccThreads, (long long)ctx->sm_count * 16);
+  sample_accumulate_kernel<<<dim3(blocks, (unsigned)n), kAccThreads, 0, ctx->stream>>>(ws, stride, res_off, (long long)elems,
+                                                                                      first ? 1 : 0, acc);
   ctx->launches++;
   TNCB_CUDA(cudaGetLastError());
   return TNCB_OK;
