@@ -294,7 +294,8 @@ int tncb_network_out_legs(const tncb_tn* tn, const tncb_path* path, int* n_out, 
  *   set_leaves             .     .    .    .       .           U           U
  *   grad_offsets           I     .    .    .       .           .           .
  *   sample                 .     U    U    U       U           U           U
- *   sample_slices          .     U    U    U       U           U           U          */
+ *   sample_slices          .     U    U    U       U           U           U
+ *   expect                 .     .    U    U       U           U           U          */
 int tncb_plan_create(tncb_ctx* ctx, const tncb_tn* tn, const tncb_path* path, tncb_plan** out);
 /* `tn` must have the structure the plan was compiled from: every leaf is re-validated (kind, rank,
  * dims, non-null payload, live device handle) -> TNCB_ERR_INVALID / TNCB_ERR_SHAPE /
@@ -599,6 +600,44 @@ int tncb_plan_sample(tncb_ctx* ctx, tncb_plan* plan, const tncb_sample_spec* spe
 int tncb_plan_sample_slices(tncb_ctx* ctx, tncb_plan* plan, const tncb_sample_spec* spec, uint64_t seed, uint64_t first,
                             uint64_t max_candidates, uint64_t max_samples, double m, size_t batch, uint64_t* bits,
                             double* probs, tncb_sample_stats* stats);
+/* ---- expectation values of Pauli sums: E = sum_k c_k <psi|P_k|psi> and its leaf gradient, every term in one pass ----
+ * The plan's network is <psi|L|psi> with one observable ("layer") leaf L_q per qubit q of the layer, legs [ket leg, bra
+ * leg]: the circuit's kept tensors, their adjoint mirror images, and the layer (Circuit.into_pauli_expectation_network
+ * builds it, light cone pruned).  Term k is P_k = (x) over q of sigma(bit q of x_mask[k], bit q of z_mask[k]), sigma(0,0) = I,
+ * (1,0) = X, (0,1) = Z, (1,1) = Y, with a real coefficient c_k.  Its layer payload on qubit q is the 2x2 matrix M = sigma^T
+ * (row-major, [ket, bra]): the network contracts to sum_ab psi_a M[a,b] conj(psi_b), so R_k = <psi|P_k|psi>; only Y
+ * differs from its transpose, and the transpose fixes the sign of every term with an odd number of Y's.  The payload
+ * staged with the plan (the identity, say) is ignored by this call. */
+typedef struct tncb_pauli_layer {
+  int n_qubits;                 /* 1..64: bit q of a term's masks is qubit q */
+  size_t n_layer;
+  const uint64_t* layer_leaf;   /* leaf index (collect order) of the observable leaf of qubit layer_qubit[j] */
+  const int* layer_qubit;
+} tncb_pauli_layer;
+/* Terms 0 .. n_terms - 1 (x_mask, z_mask, coeff: host arrays) in passes of `batch` terms (0: as many workspace copies
+ * as fit, as tncb_plan_run_batch).  The plan is a static plain or gradient plan staged on ctx (tncb_plan_stage, and
+ * tncb_plan_set_leaves for angles): its staged block supplies every leaf except the layer leaves, and it is left
+ * untouched, so tncb_plan_run before and after gives the same bits.  The term table goes to the device in one small
+ * host-to-device copy per call.  Per pass: one kernel writes the terms' layer payloads, the batched forward levels, the
+ * value rows out; with grad_sum the seeds (c_k, 0), the backward levels and the gather that folds sum_k c_k G_k.  One
+ * one-block kernel then forms the energy.  No atomics: results do not depend on `batch`, and calls repeat bit for bit.
+ *   values:   new [n_terms]; row k bit-identical to tncb_plan_run on the network with term k's layer payloads staged
+ *             from the host (for a gradient plan: to tncb_plan_vjp_batch's value row)
+ *   energy:   new rank-0; the left fold ((0 + c_0 R_0) + c_1 R_1) + ... in term order, c R formed as (c Re R, c Im R),
+ *             every operation rounded on its own (no FMA)
+ *   grad_sum: gradient plans only; new [grad_elems] at tncb_plan_grad_offsets, bit-identical to tncb_plan_vjp_batch
+ *             (seeds = c_k) over the per-term networks.  Requested layer leaves get sum_k c_k of their environments.
+ * Any output may be NULL, not all three.  Ranks of a multi-GPU job pass disjoint subsets of the terms and add their
+ * energy and grad_sum with tncb_comm_allreduce_sum.
+ * Every refusal happens before any device work and leaves the arena as it found it.  TNCB_ERR_INVALID: a null argument
+ * or n_terms == 0; n_qubits outside 1..64; a layer leaf out of range, listed twice, without a payload, or not rank 2 with
+ * dims [2, 2]; a layer qubit out of range or listed twice; a term acting on a qubit without a layer leaf (named); a
+ * non-finite coefficient (named); a result that is not a scalar; no output; grad_sum on a plain plan; not staged on this
+ * context.  TNCB_ERR_UNSUPPORTED: a plan of another kind or without a static layout.  TNCB_ERR_OOM: not even one
+ * workspace copy fits. */
+int tncb_plan_expect(tncb_ctx* ctx, tncb_plan* plan, const tncb_pauli_layer* layer, size_t n_terms,
+                     const uint64_t* x_mask, const uint64_t* z_mask, const double* coeff, size_t batch,
+                     tncb_tensor** values, tncb_tensor** energy, tncb_tensor** grad_sum);
 /* ---- sliced tangents and Hessian-vector products: networks whose tangent or Hessian-vector workspace does not fit ----
  * By linearity, as for sliced gradients: R = sum_q R_q, so Ṙ = sum_q Ṙ_q; slice q's leaf (and its tangent) is q's
  * fixed-index sub-block of the full leaf (and of its full-shape tangent), and q's G_l and Ġ_l add into q's sub-block of

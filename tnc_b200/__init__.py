@@ -16,7 +16,7 @@ import numpy as np
 
 from ._lib import TncbError, check, lib, u64_array
 
-__all__ = ["Context", "DeviceTensor", "Sampler", "Samples", "TncbError", "contract_pair", "contract_pair_into", "default_context",
+__all__ = ["Context", "DeviceTensor", "Expectation", "PauliSum", "Sampler", "Samples", "TncbError", "contract_pair", "contract_pair_into", "default_context",
            "lib"]
 
 
@@ -301,3 +301,4 @@ def download_into(ctx: Context, src: DeviceTensor, host: np.ndarray) -> None:
 
 
 from .sampling import Sampler, Samples  # noqa: E402  (needs Context and DeviceTensor above)
+from .observables import Expectation, PauliSum, pauli_layer_matrix  # noqa: E402

@@ -55,6 +55,10 @@ class TncbSampleSpec(C.Structure):
                 ("result_qubit", i32p)]
 
 
+class TncbPauliLayer(C.Structure):
+    _fields_ = [("n_qubits", C.c_int), ("n_layer", C.c_size_t), ("layer_leaf", u64p), ("layer_qubit", i32p)]
+
+
 class TncbSampleStats(C.Structure):
     _fields_ = [("candidates", C.c_uint64), ("samples", C.c_uint64), ("clipped", C.c_uint64), ("passes", C.c_uint64),
                 ("max_ratio", C.c_double)]
@@ -149,6 +153,8 @@ SIGNATURES = {
     "tncb_plan_sample_slices": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(TncbSampleSpec), C.c_uint64, C.c_uint64,
                                           C.c_uint64, C.c_uint64, C.c_double, C.c_size_t, C.c_void_p, C.c_void_p,
                                           C.POINTER(TncbSampleStats)]),
+    "tncb_plan_expect": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(TncbPauliLayer), C.c_size_t, u64p, u64p, f64p,
+                                   C.c_size_t, vpp, vpp, vpp]),
     "tncb_plan_destroy": (None, [C.c_void_p]),
     "tncb_angles_create": (C.c_int, [C.POINTER(TncbTn), C.c_size_t, C.c_size_t, C.c_void_p, C.POINTER(C.c_int64), C.c_size_t, vpp]),
     "tncb_angles_destroy": (C.c_int, [C.c_void_p]),

@@ -534,3 +534,64 @@ def circuit_function(tn: Tensor, path: ContractionPath, angle_map, ctx: Optional
     Angles.tangents and a tangent plan's jvp / jvp_batch, compiled on first use.  Second order (create_graph=True) and
     forward mode with sliced_legs raise NotImplementedError; vmap is not supported."""
     return CircuitFunction(tn, path, angle_map, ctx, sliced_legs)
+
+
+class _ExpectFn(torch.autograd.Function):
+    @staticmethod
+    def forward(runner, theta):
+        return runner._forward(theta)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        ctx.runner = inputs[0]
+        ctx.save_for_backward(inputs[1])
+
+    @staticmethod
+    def jvp(ctx, *tangents):
+        raise NotImplementedError("forward mode is not supported by expectation_function")
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        (theta,) = ctx.saved_tensors
+        if torch.is_grad_enabled():
+            raise NotImplementedError("second-order derivatives (create_graph=True) are not supported by expectation_function")
+        return None, grad_out * ctx.runner._grad(theta)
+
+
+class ExpectationFunction:
+    """See expectation_function."""
+
+    def __init__(self, exp):
+        if exp.angles is None:
+            raise ValueError("expectation_function needs an Expectation built with an angle_map")
+        self.exp = exp
+
+    def _check(self, theta) -> None:
+        check_cuda_tensor(self.exp.ctx, theta, "theta")
+        P = self.exp.angles.n_params
+        if theta.dtype != torch.float64:
+            raise ValueError(f"theta must be float64, got {theta.dtype}")
+        if theta.dim() == 2 and theta.shape[1] == P:
+            raise NotImplementedError("expectation_function takes one θ [P]; batches of θ are not supported")
+        if theta.dim() != 1 or theta.shape[0] != P:
+            raise ValueError(f"theta has shape {tuple(theta.shape)}, expected [{P}]")
+
+    def _forward(self, theta):
+        self._check(theta)
+        e, _ = self.exp.values(theta.detach())
+        return torch.tensor(e.real, dtype=torch.float64, device=theta.device)
+
+    def _grad(self, theta):
+        return self.exp.value_and_grad(theta.detach())[1]
+
+    def __call__(self, theta: torch.Tensor) -> torch.Tensor:
+        return _ExpectFn.apply(self, theta)
+
+
+def expectation_function(exp) -> ExpectationFunction:
+    """A torch.autograd.Function of the gate angles: the returned callable takes θ, a CUDA float64 tensor [P] (P =
+    the angle map's n_params of `exp`, an observables.Expectation built with an angle_map), and returns E(θ) =
+    sum_k c_k <psi(θ)|P_k|psi(θ)> as a float64 CUDA scalar (the real part of Expectation.values).  Backward:
+    grad_θ = grad_out * Re(dE/dθ) (Expectation.value_and_grad, which re-stages θ and runs the forward pass again).
+    Forward mode, second order (create_graph=True) and θ of shape [B, P] raise NotImplementedError."""
+    return ExpectationFunction(exp)

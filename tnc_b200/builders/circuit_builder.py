@@ -117,3 +117,99 @@ class Circuit:
             z.set_tensor_data(TensorData.Gate("z"))
             tensors.append(z)
         return Tensor.new_composite(tensors)
+
+    def tensor_qubits(self) -> List[List[int]]:
+        """The qubits of every tensor of `tensors`: a ket's qubit, a gate's qubits in argument order."""
+        qubit_of, out, kets = {}, [], 0
+        for t in self.tensors:
+            if len(t.legs) == 1:             # allocate_register's kets, in qubit order
+                qubit_of[t.legs[0]] = kets
+                out.append([kets])
+                kets += 1
+                continue
+            half = len(t.legs) // 2
+            qs = [qubit_of[l] for l in t.legs[:half]]
+            for q, l in zip(qs, t.legs[half:]):
+                qubit_of[l] = q
+            out.append(qs)
+        return out
+
+    def into_pauli_expectation_network(self, support: Sequence[int]) -> "PauliNetwork":
+        """<psi|L|psi> with one observable ("layer") leaf per qubit of `support`, pruned to the light cone of `support`.
+
+        Leaves: the kept circuit tensors, their adjoint mirror images (built as into_expectation_value_network builds
+        them: legs rotated by half, offset next_edge, TensorData.adjoint()), then per qubit q of `support`, ascending, a
+        layer leaf with legs [e, e + offset] (e = open_edges[q]) holding the 2x2 identity, so that a staged plan
+        contracts to <psi|psi>; tncb_plan_expect writes each term's payload there instead.
+        Light cone: the gates are walked from last to first; a gate touching a qubit already in the cone is kept and adds
+        its qubits to the cone.  A gate not kept cancels against its mirror image, and both are dropped.  A qubit of the
+        cone outside `support` loses its later gates: its ket wire is joined to its bra wire (the bra copy takes the ket's
+        leg id, no leaf is added).  Qubits never in the cone lose their ket and its mirror (<0|0> = 1).  With `support` =
+        every qubit nothing is pruned, and the network is into_expectation_value_network()'s with I in place of Z."""
+        n = self.num_qubits()
+        sup = sorted({int(q) for q in support})
+        if not sup or any(not 0 <= q < n for q in sup):
+            raise ValueError(f"support {list(support)} must be a non-empty set of qubits of the {n}-qubit circuit")
+        qubits = self.tensor_qubits()
+        cone, keep = set(sup), [False] * len(self.tensors)
+        for i in reversed(range(len(self.tensors))):
+            if len(self.tensors[i].legs) > 1 and cone.intersection(qubits[i]):
+                keep[i] = True
+                cone.update(qubits[i])
+        for i, t in enumerate(self.tensors):
+            if len(t.legs) == 1:
+                keep[i] = qubits[i][0] in cone
+        # the output wire of each cone qubit's last kept tensor: joined to its mirror unless the qubit is in the support
+        last = {}
+        for i, t in enumerate(self.tensors):
+            if keep[i]:
+                half = len(t.legs) // 2
+                for q, l in zip(qubits[i], t.legs[half:]):
+                    last[q] = l
+        joined = {l for q, l in last.items() if q not in set(sup)}
+        offset = self.next_edge
+        kept = [i for i in range(len(self.tensors)) if keep[i]]
+        tensors = [self.tensors[i] for i in kept]
+        for i in kept:
+            t = self.tensors[i]
+            half = len(t.legs) // 2
+            legs = [l if l in joined else l + offset for l in (t.legs[half:] + t.legs[:half])]
+            adj = Tensor(legs, t.bond_dims[half:] + t.bond_dims[:half])
+            adj.set_tensor_data(t.tensordata.adjoint())
+            tensors.append(adj)
+        layer_leaf = []
+        for q in sup:
+            e = self.open_edges[q]
+            layer = Tensor.new_from_const([e, e + offset], 2)
+            layer.set_tensor_data(TensorData.new_from_data([2, 2], [1, 0, 0, 1]))
+            layer_leaf.append(len(tensors))
+            tensors.append(layer)
+        k = len(kept)
+        return PauliNetwork(Tensor.new_composite(tensors), layer_leaf, sup, {k + j: j for j in range(k)}, kept)
+
+
+class PauliNetwork:
+    """The network of Circuit.into_pauli_expectation_network.
+
+    tn:          the network; its leaves are leaves(tn) in order
+    layer_leaf:  the leaf index of the layer leaf of qubit layer_qubit[j]
+    layer_qubit: the support, ascending
+    ket_of:      {bra-copy leaf: its ket leaf}
+    kept:        kept[i] is the index into circuit.tensors of ket leaf i"""
+
+    def __init__(self, tn: Tensor, layer_leaf: List[int], layer_qubit: List[int], ket_of: dict, kept: List[int]):
+        self.tn, self.layer_leaf, self.layer_qubit, self.ket_of, self.kept = tn, layer_leaf, layer_qubit, ket_of, kept
+
+    def angle_map(self, circuit_map):
+        """An AngleMap of this network from `circuit_map`, whose refs name circuit.tensors indices: each ref on a kept
+        gate becomes a ref on its ket copy and one on its bra copy, with the same param and scale; refs on pruned gates
+        are dropped, so their params get zero gradient.  n_params and theta0 stay the circuit's."""
+        from ..angles import AngleMap
+        leaf_of = {c: i for i, c in enumerate(self.kept)}
+        bra_of = {k: b for b, k in self.ket_of.items()}
+        refs = []
+        for leaf, slot, param, scale in circuit_map.refs:
+            if leaf in leaf_of:
+                i = leaf_of[leaf]
+                refs += [(i, slot, param, scale), (bra_of[i], slot, param, scale)]
+        return AngleMap(refs, circuit_map.n_params, circuit_map.theta0)

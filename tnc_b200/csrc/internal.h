@@ -265,6 +265,18 @@ int launch_sample_accumulate(tncb_ctx* ctx, const char* ws, long long stride, lo
 int launch_sample_compact(tncb_ctx* ctx, const SampleCand* cand, size_t n, unsigned long long remaining,
                           unsigned long long* bits, double* probs, SampleCounts* counts);
 
+// ---- expectation values of Pauli sums (tncb_plan_expect, expect.cu) ----
+struct ExpectLayer {
+  int n_layer, _pad;
+  unsigned char qubit[64];          // layer leaf j (in the caller's order) is qubit qubit[j]
+};
+// the layer payloads of terms first .. first + n - 1 (bit q of x_mask / z_mask picks qubit q's Pauli): layer leaf j of
+// slot i at out + (j c + i) * 4, the 2x2 matrix with legs [ket, bra]
+int launch_expect_layer(tncb_ctx* ctx, const unsigned long long* x_mask, const unsigned long long* z_mask,
+                        unsigned long long first, size_t n, size_t c, const ExpectLayer& layer, double2* out);
+// *energy = the left fold over k < n of (c_k Re R_k, c_k Im R_k), c_k = seeds[k].x, R_k = values[k]; one block
+int launch_expect_fold(tncb_ctx* ctx, const double2* values, const double2* seeds, size_t n, double2* energy);
+
 int tensor_new(tncb_ctx* ctx, int rank, const uint64_t* dims, tncb_tensor** out);
 
 // TensorData::File leaf (hdf5io.cpp): first member of /tensors, optionally adjointed, checked against the leaf's dims

@@ -438,7 +438,7 @@ static size_t device_bytes(tncb_ctx* ctx) {
 // The calls that take a plan, in the order of kRoutes' rows
 enum class Call { stage, run, execute, stage_slices, run_slices, run_batch, vjp, vjp_sliced, stage_batch, vjp_batch, jvp,
                   jvp_batch, jvp_sliced, hvp, hvp_batch, hvp_sliced, stage_instances, set_leaves, grad_offsets, sample, sample_slices,
-                  count };
+                  expect, count };
 struct Refusal { int status; const char* msg; };
 static const Refusal
     kHvpRuns{TNCB_ERR_UNSUPPORTED, "a Hessian-vector plan runs through tncb_plan_hvp"},
@@ -463,7 +463,8 @@ static const Refusal
     kNotDerivStage{TNCB_ERR_INVALID, "not a gradient or tangent plan (plain plans stage many networks with tncb_plan_stage_slices)"},
     kNotDeriv{TNCB_ERR_INVALID, "not a gradient or tangent plan (tncb_plan_create_vjp / _jvp)"},
     kSamplePlain{TNCB_ERR_UNSUPPORTED, "tncb_plan_sample takes a plain plan (tncb_plan_create)"},
-    kSampleSlPlain{TNCB_ERR_UNSUPPORTED, "tncb_plan_sample_slices takes a plain plan (tncb_plan_create)"};
+    kSampleSlPlain{TNCB_ERR_UNSUPPORTED, "tncb_plan_sample_slices takes a plain plan (tncb_plan_create)"},
+    kExpectPlain{TNCB_ERR_UNSUPPORTED, "tncb_plan_expect takes a plain or a gradient plan (tncb_plan_create / _vjp)"};
 static const Refusal* const kTakes = nullptr;
 static const Refusal* const kRoutes[(int)Call::count][7] = {
   //                    plain            vjp             jvp           hvp          sliced vjp      sliced jvp    sliced hvp
@@ -489,6 +490,7 @@ static const Refusal* const kRoutes[(int)Call::count][7] = {
   /* sample */          {kTakes,          &kSamplePlain,  &kSamplePlain, &kSamplePlain, &kSamplePlain, &kSamplePlain, &kSamplePlain},
   /* sample_slices */   {kTakes,          &kSampleSlPlain, &kSampleSlPlain, &kSampleSlPlain, &kSampleSlPlain, &kSampleSlPlain,
                          &kSampleSlPlain},
+  /* expect */          {kTakes,          kTakes,         &kExpectPlain, &kExpectPlain, &kExpectPlain, &kExpectPlain, &kExpectPlain},
 };
 
 // TNCB_OK if `c` takes P's kind, else the cell's refusal.  Every plan-taking call asks first, right after its null checks.
@@ -2439,6 +2441,123 @@ int tncb_plan_sample_slices(tncb_ctx* ctx, tncb_plan* plan, const tncb_sample_sp
                             uint64_t max_candidates, uint64_t max_samples, double m, size_t batch, uint64_t* bits,
                             double* probs, tncb_sample_stats* stats) {
   return tncb::sample_call(ctx, plan, spec, seed, first, max_candidates, max_samples, m, batch, bits, probs, stats, true);
+}
+
+namespace tncb {
+// The observable layer of tncb_plan_expect against the plan: every layer leaf a listed, rank-2 leaf of dims [2, 2] with a
+// payload, on a distinct qubit in 0 .. n_qubits - 1; *mask gets the layer's qubits
+static int expect_layer_map(const Schedule& S, const tncb_pauli_layer& L, ExpectLayer* map, uint64_t* mask) {
+  if (L.n_qubits < 1 || L.n_qubits > 64) return fail(TNCB_ERR_INVALID, "n_qubits " + std::to_string(L.n_qubits) + " is outside 1..64");
+  if (L.n_layer && (!L.layer_leaf || !L.layer_qubit)) return fail(TNCB_ERR_INVALID, "null argument");
+  const std::vector<long long> elems = leaf_elems(S);
+  std::vector<const SlotMeta*> meta(elems.size(), nullptr);
+  for (const SlotMeta& m : S.slots) if (m.leaf_index >= 0) meta[m.leaf_index] = &m;
+  std::vector<char> seen(elems.size(), 0);
+  *mask = 0;
+  for (size_t j = 0; j < L.n_layer; j++) {
+    const uint64_t li = L.layer_leaf[j];
+    const std::string name = "layer leaf " + std::to_string(li);
+    if (int rc = listed_leaf(elems, seen, li, name)) return rc;
+    const std::vector<uint64_t>& d = meta[li]->dims;
+    if (d.size() != 2 || d[0] != 2 || d[1] != 2) return fail(TNCB_ERR_INVALID, name + " is not a rank-2 leaf with dims [2, 2]");
+    const int q = L.layer_qubit[j];
+    if (q < 0 || q >= L.n_qubits)
+      return fail(TNCB_ERR_INVALID, "layer qubit " + std::to_string(j) + " is qubit " + std::to_string(q) + ", outside 0.." + std::to_string(L.n_qubits - 1));
+    if ((*mask >> q) & 1) return fail(TNCB_ERR_INVALID, "qubit " + std::to_string(q) + " is listed twice (layer qubit " + std::to_string(j) + ")");
+    *mask |= 1ull << q;
+    map->qubit[j] = (unsigned char)q;
+  }
+  map->n_layer = (int)L.n_layer;
+  return TNCB_OK;
+}
+} // namespace tncb
+
+// Expectation values of a Pauli sum (tncb.h, DESIGN §5) on the instance-batched path of tncb_plan_sample: the term table
+// goes to the device in one copy; per pass of c terms the layer kernel writes the terms' layer payloads, run_instances
+// stages them as device payloads (the staged block's other leaves at stride 0), runs the forward levels and copies the
+// value rows out, and with grad_sum writes the seeds c_k, runs the backward levels and folds Σ_k c_k G_k in term order.
+// The fold kernel forms the energy from the value rows after the last pass.  No leaf bytes come from the host.
+int tncb_plan_expect(tncb_ctx* ctx, tncb_plan* plan, const tncb_pauli_layer* layer, size_t n_terms, const uint64_t* x_mask,
+                     const uint64_t* z_mask, const double* coeff, size_t batch, tncb_tensor** values, tncb_tensor** energy,
+                     tncb_tensor** grad_sum) {
+  using namespace tncb;
+  if (!ctx || !plan || !layer || !x_mask || !z_mask || !coeff) return fail(TNCB_ERR_INVALID, "null argument");
+  int rc = route(plan, Call::expect);
+  if (rc) return rc;
+  if (!plan->is_static) return fail(TNCB_ERR_UNSUPPORTED, "expectation values need a plan with a static layout (no device leaves)");
+  if (plan->ctx != ctx || !plan->leaves_resident) return fail(TNCB_ERR_INVALID, "tncb_plan_stage has not been called on this plan and context");
+  if (n_terms == 0) return fail(TNCB_ERR_INVALID, "n_terms is 0");
+  if (!values && !energy && !grad_sum) return fail(TNCB_ERR_INVALID, "no output requested");
+  if (grad_sum && !plan->grad()) return fail(TNCB_ERR_INVALID, "grad_sum needs a gradient plan (tncb_plan_create_vjp)");
+  const Schedule& S = plan->S;
+  if (S.result_slot < 0 || !S.slots[S.result_slot].dims.empty())
+    return fail(TNCB_ERR_INVALID, "the network does not contract to a scalar (" + std::to_string(S.result_slot < 0 ? 0 : S.slots[S.result_slot].dims.size()) + " result legs)");
+  ExpectLayer map{};
+  uint64_t mask = 0;
+  if ((rc = expect_layer_map(S, *layer, &map, &mask))) return rc;
+  for (size_t k = 0; k < n_terms; k++) {
+    const uint64_t off = (x_mask[k] | z_mask[k]) & ~mask;
+    if (off) return fail(TNCB_ERR_INVALID, "term " + std::to_string(k) + " acts on qubit " + std::to_string(__builtin_ctzll(off)) + ", which has no layer leaf");
+    if (!std::isfinite(coeff[k])) return fail(TNCB_ERR_INVALID, "the coefficient of term " + std::to_string(k) + " is not finite");
+  }
+  TNCB_CUDA(cudaSetDevice(ctx->device));
+  // the term table, [x masks][z masks][seeds (c_k, 0)], in one host-to-device copy
+  const size_t o_z = n_terms * sizeof(uint64_t), o_seeds = 2 * o_z, table_bytes = o_seeds + n_terms * sizeof(double2);
+  std::vector<char> host(table_bytes);
+  std::memcpy(host.data(), x_mask, o_z);
+  std::memcpy(host.data() + o_z, z_mask, o_z);
+  for (size_t k = 0; k < n_terms; k++) ((double2*)(host.data() + o_seeds))[k] = make_double2(coeff[k], 0.0);
+  void* table = nullptr;
+  if ((rc = ctx->arena.alloc(table_bytes, &table))) return rc;
+  cudaError_t e = cudaMemcpyAsync(table, host.data(), table_bytes, cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);      // `host` dies with this scope
+  if (e != cudaSuccess) { ctx->arena.free(table, table_bytes); return fail(TNCB_ERR_CUDA, std::string("term table copy: ") + cudaGetErrorString(e)); }
+  const unsigned long long* d_x = (const unsigned long long*)table;
+  const unsigned long long* d_z = (const unsigned long long*)((char*)table + o_z);
+  const double2* d_seeds = (const double2*)((char*)table + o_seeds);
+  // the layer payloads as device payloads, four elements apart from term to term; their sources are set once the pass
+  // size is known
+  std::vector<LeafStageItem> dev_items;
+  std::vector<long long> layer_dst(layer->n_layer);
+  for (size_t j = 0; j < layer->n_layer; j++) {
+    layer_dst[j] = (long long)S.leaf_offset[layer->layer_leaf[j]];
+    dev_items.push_back({nullptr, 4, layer_dst[j], 4});
+  }
+  const std::vector<LeafRun> runs = leaf_runs(dev_items, (long long)std::max<size_t>(S.leaf_block_elems, 1));
+  void* blk = nullptr;
+  size_t blk_bytes = 0, c = 0;
+  PassHook hook;
+  hook.width = batch;
+  hook.begin = [&](size_t pass) -> int {
+    c = pass;
+    blk_bytes = std::max<size_t>(layer->n_layer * c * 4 * sizeof(double2), 16);
+    if (int r = ctx->arena.alloc(blk_bytes, &blk)) return r;
+    for (LeafStageItem& it : dev_items)
+      it.src = (const double2*)blk + (size_t)(std::find(layer_dst.begin(), layer_dst.end(), it.dst) - layer_dst.begin()) * c * 4;
+    return TNCB_OK;
+  };
+  hook.fill = [&](size_t done, size_t n) -> int { return launch_expect_layer(ctx, d_x, d_z, done, n, c, map, (double2*)blk); };
+  hook.end = [](const char*, size_t, size_t, bool*) -> int { return TNCB_OK; };
+  Outputs out{ctx};
+  tncb_tensor* en = out.add(energy, 0, nullptr);
+  tncb_tensor *vals = nullptr, *gs = nullptr;
+  tncb_tensor seeds;
+  seeds.ptr = (double2*)d_seeds; seeds.rank = 1; seeds.dims[0] = n_terms; seeds.elems = n_terms; seeds.owned = false;
+  InstanceIO io;
+  io.hook = &hook;
+  io.values = &vals;
+  if (grad_sum) { io.grad_sum = &gs; io.seeds = &seeds; }
+  if (!(rc = out.rc)) rc = run_instances(ctx, plan, std::vector<uint64_t>{n_terms}, {0, &dev_items, &runs}, io);
+  if (blk) ctx->arena.free(blk, blk_bytes);
+  if (!rc && en) rc = launch_expect_fold(ctx, vals->ptr, d_seeds, n_terms, en->ptr);
+  ctx->arena.free(table, table_bytes);          // stream-ordered: after the passes and the fold
+  if (rc) {
+    for (tncb_tensor* t : {vals, gs}) if (t) tncb_tensor_free(ctx, t);
+    return out.finish(rc);
+  }
+  if (values) *values = vals; else tncb_tensor_free(ctx, vals);
+  if (grad_sum) *grad_sum = gs;
+  return out.finish(TNCB_OK);
 }
 
 namespace tncb {
